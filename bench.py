@@ -2,7 +2,7 @@
 """bench.py - speech-tokens/s of the GPT decode hot path (BASELINE.json metric), one JSON line.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl ours|reference|torch-cuda]
-                    [--config c2|c3] [--path gpt|decoder]
+                    [--config c2|c3] [--path gpt|decoder] [--dump-outputs DIR]
 
 A "step" is one whole ``generate`` pass of the hot path over one batch: a 16-token prompt and
 ``--tokens`` (512) forced speech tokens per row, greedy + EOS excluded (BASELINE.json configs[1];
@@ -15,7 +15,9 @@ utterances sharded, one NCCL broadcast of the packed weights at load, no step-lo
 ``--config c3``: BASELINE configs[2] (batch 32, prompts of 8..128 tokens, refine-text pass then code pass, top-p 0.7 /
 top-k 20 / penalty 1.05).  ``--path decoder``: hot path 2 at BASELINE configs[3] (DVAE decoder + Vocos + iSTFT of
 64 x 10 s), audio-samples/s with a tensor-core roofline against a TF32 peak measured in the same run.
-``--impl torch-cuda``: the reference's own stack (HF LlamaModel, torch SDPA, eager PyTorch) on the same B200.
+``--impl torch-cuda``: the reference's own stack (HF LlamaModel, torch SDPA, eager PyTorch) on the same GPU.
+``--dump-outputs DIR``: after the timed steps, write what the timed path returned in its last step as DIR/<name>.npy
+(float64 token ids, float32 waveform rows); inputs are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -37,8 +39,7 @@ PROMPT_LEN = 16
 # SURVEY.md 8d: streamed weight elements per audio step (20 layers + 41 norms + 4 heads)
 W_ELEMS = 190_698_240
 KV_BYTES_PER_TOKEN_ROW = 20 * 2 * 768 * 4  # 122,880 B per row per context token (read), same per step (write)
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE single-step k_flow<1> launch (ncu --set full, round 2; see profiles/)
-TRAFFIC_K_FLOW_B1 = 771_000_000
+L2_NOTE = "50 MB L2 of the H100"
 
 
 def algorithmic_bytes_per_step(B: int, T: float) -> float:
@@ -50,7 +51,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3 (not measured)"
 
 
 class ClockSampler:
@@ -93,6 +94,18 @@ class ClockSampler:
         reasons = [n for i, n in enumerate(names) if any(len(r) > 3 + i and r[3 + i].lower().startswith("active") for r in self.rows)]
         return {"sm_mhz": sm[len(sm) // 2], "sm_max_mhz": int(self.rows[0][1]), "reasons": reasons,
                 "samples": len(sm)}
+
+
+def dump_outputs(path, arrays):
+    """Write {name: array} as path/<name>.npy (float32 stays float32, everything else becomes float64)."""
+    import numpy as np
+
+    if not path:
+        return
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
+        np.save(os.path.join(path, name + ".npy"), a.astype(np.float32 if a.dtype == np.float32 else np.float64))
 
 
 def build_inputs(B: int, tokens: int, seed: int):
@@ -177,6 +190,8 @@ def run_ours(args, rank: int, world: int, local_rank: int):
     launches = int(lib.ctb_launch_count() - l0)
     ms_per_step = ms / args.steps
     value = world * B * tokens / (ms_per_step / 1e3)
+    if rank == 0:
+        dump_outputs(args.dump_outputs, {"ids": ids_out})  # [B, tokens, 4] speech-token ids of the last timed step
 
     # ---- e2e through the public API with host buffers
     for _ in range(max(1, min(args.warmup, 2))):
@@ -211,10 +226,10 @@ def run_ours(args, rank: int, world: int, local_rank: int):
     t_avg = PROMPT_LEN + tokens / 2
     step_bytes = algorithmic_bytes_per_step(B, t_avg)
     step_us = ms_per_step * 1e3 / tokens  # `tokens` loop iterations per pass; the 16-token prompt is one batched prefill inside the first
-    one_kernel = B <= 4 and not os.environ.get("CTB_NO_FLOW")
+    one_kernel = B == 1 and not os.environ.get("CTB_NO_FLOW")
     kern = {}
     if one_kernel:
-        # B <= 4: the decode loop is the persistent dataflow kernel k_flow (csrc/flow.cuh): one launch = 16 decode
+        # B = 1: the decode loop is the persistent dataflow kernel k_flow (csrc/flow.cuh): one launch = 16 decode
         # iterations (20 layers + heads + sampling tail each).  Timed with CUDA events around single launches.
         roof_new = tokens + 112
         ids_big = torch.zeros(B, roof_new, 4, dtype=torch.int32, device=dev)
@@ -234,21 +249,18 @@ def run_ours(args, rank: int, world: int, local_rank: int):
         us = e0.elapsed_time(e1) * 1e3 / reps  # us per launch
         kbytes = sum(algorithmic_bytes_per_step(B, ctx0 + i) for i in range(reps * per)) / reps
         achieved = kbytes / (us * 1e-6) / 1e9
-        roofline = {"bound": "hbm", "kernel": f"k_flow<{1 if B == 1 else 2 if B == 2 else 4}> (one launch = {per} decode iterations: "
+        roofline = {"bound": "hbm", "kernel": f"k_flow<1> (one launch = {per} decode iterations: "
                                               "20 layers + heads + sampling tail each, no grid barriers)",
                     "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s", "frac": round(achieved / peak, 4),
-                    "traffic": TRAFFIC_K_FLOW_B1 * per if B == 1 else None, "peak_source": peak_src,
+                    "traffic": None, "peak_source": peak_src,
                     "bytes_per_launch": int(kbytes), "us_per_launch": round(us, 2), "steps_per_launch": per,
-                    "us_per_step_in_kernel": round(us / per, 2), "context_tokens": [ctx0, ctx0 + reps * per],
-                    "traffic_note": "dram__bytes_read+write of one single-step k_flow<1> launch from ncu --set full "
-                                    "(profiles/r02_k_flow_b1_full_raw.csv), times the steps per launch; a constant from "
-                                    "that capture, not measured in this run"}
+                    "us_per_step_in_kernel": round(us / per, 2), "context_tokens": [ctx0, ctx0 + reps * per]}
     else:
         for kind, name in ((3, "gateup"), (4, "down"), (0, "qkv"), (2, "oproj"), (1, "k_attn"), (5, "heads"), (6, "k_sample")):
             kern[name] = time_kind(kind, 20, 20 if kind < 5 else 1)
         gu_bytes = 2 * 3072 * 768 * 4 + B * 768 * 4 + B * 3072 * 4  # weights + x in + mlp out
         achieved = gu_bytes / (kern["gateup"] * 1e-6) / 1e9
-        kname = "k_tc_dec<DE_GATEUP> (tcgen05 3xTF32)" if B > 16 else "k_gemv<BT,EPI_GATEUP>"
+        kname = "k_tc_dec<DE_GATEUP> (wgmma 3xTF32)" if B >= 9 else "k_gemv<BT,EPI_GATEUP>"
         roofline = {"bound": "hbm", "kernel": kname, "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s",
                     "frac": round(achieved / peak, 4), "traffic": None, "peak_source": peak_src,
                     "bytes_per_launch": gu_bytes, "us_per_launch": round(kern["gateup"], 3),
@@ -297,7 +309,7 @@ def run_ours(args, rank: int, world: int, local_rank: int):
         "config": {"workload": f"GPT decode: batch {B}/GPU x (16-token prompt + {tokens} forced speech tokens), greedy "
                                "(BASELINE configs[1]); one step = one whole generate pass",
                    "batch_per_gpu": B, "tokens": tokens, "prompt_len": PROMPT_LEN, "parallelism": f"dp{world}",
-                   "l2_policy": "inputs larger than L2: every decode iteration streams 763 MB of fp32 weights (> 126 MB L2)"},
+                   "l2_policy": f"inputs larger than L2: every decode iteration streams 763 MB of fp32 weights (> {L2_NOTE})"},
         "rtf": round((ms_per_step / 1e3) / audio_s, 6),
         "e2e": {"value": round(e2e_value, 2), "unit": "speech-tokens/s", "h2d_bytes_per_step": int(h2d),
                 "d2h_bytes_per_step": int(d2h), "ms_per_step": round(ms_e2e, 3),
@@ -333,7 +345,7 @@ def bench_decoder(dev, B: int = 64, T: int = 469):
     ms = e0.elapsed_time(e1) / 3
     frames = B * 2 * T
     flops = frames * 78.7e6  # SURVEY.md 8d: 78.7 MFLOP per mel frame on the hidden path
-    return {"workload": f"DVAE decoder + Vocos + iSTFT, batch {B} x {T} tokens (10 s each), hidden path, tcgen05 3xTF32 GEMMs",
+    return {"workload": f"DVAE decoder + Vocos + iSTFT, batch {B} x {T} tokens (10 s each), hidden path, wgmma 3xTF32 GEMMs",
             "ms": round(ms, 2), "audio_samples_per_s": round(wav.numel() / (ms / 1e3), 1),
             "rtf": round((ms / 1e3) / (wav.numel() / 24000.0), 7), "tflops_fp32_equiv": round(flops / (ms / 1e3) / 1e12, 1)}
 
@@ -342,9 +354,7 @@ def bench_decoder(dev, B: int = 64, T: int = 469):
 DEC_B, DEC_T = 64, 469                      # BASELINE configs[3]: 64 utterances of 10 s (469 tokens = 938 mel frames)
 DEC_FLOP_PER_FRAME = 78.7e6                 # SURVEY.md 8d: hidden path, decoder 25.86 + vocos 13.50 + iDFT MMAC per frame
 DEC_ALGO_BYTES = 92.2e6 + 157.8e6 + 61.4e6  # hiddens in + fp32 weights + waveform out (SURVEY.md 8d, C4)
-# dram__bytes_read + dram__bytes_write summed over the 70 launches of one tokens_to_wav call at C4, from the ncu capture of
-# this round (tools/dec_profile.py -> profiles/r02_decoder_c4_dram.csv, _summary.txt); a constant from that capture
-DEC_TRAFFIC_C4 = 29_863_704_832
+DEC_DUMP_ROWS = slice(0, DEC_B, 4)          # --dump-outputs: every 4th utterance of the batch (15 MB)
 
 
 def measured_tf32_peak(dev):
@@ -451,6 +461,8 @@ def run_decoder(args, rank: int, world: int, local_rank: int):
     with ClockSampler(local_rank) as clk:
         ms = timed(step_resident, args.steps) / args.steps
     launches = int(lib.ctb_launch_count() - l0)
+    if rank == 0:
+        dump_outputs(args.dump_outputs, {"wav": step_resident()[DEC_DUMP_ROWS]})  # same inputs as the timed steps
     samples = DEC_B * (512 * DEC_T - 256)
     value = world * samples / (ms / 1e3)
     step_e2e()
@@ -489,23 +501,20 @@ def run_decoder(args, rank: int, world: int, local_rank: int):
                                "states -> mel -> waveform; one step = one whole batch", "batch_per_gpu": DEC_B, "tokens": DEC_T,
                    "parallelism": f"dp{world}",
                    "l2_policy": "inputs larger than L2: 92 MB of hidden states in, 61 MB of waveform out and ~2 GB of "
-                                "intermediate activations per step (> 126 MB L2)"},
+                                f"intermediate activations per step (> {L2_NOTE})"},
         "rtf": round((ms / 1e3) / (world * samples / 24000.0), 8),
         "e2e": {"value": round(world * samples / (ms_e2e / 1e3), 1), "unit": "audio-samples/s",
                 "h2d_bytes_per_step": int(x_host.numel() * 4), "d2h_bytes_per_step": int(wav_host.numel() * 4),
                 "ms_per_step": round(ms_e2e, 3)},
         "gpu_launches": launches, "clocks": clk.summary(),
-        "roofline": {"bound": "tensor", "kernel": "k_tc_gemm_p<EPI> (persistent tcgen05 3xTF32 conv-as-GEMM, two TMEM accumulators; 47 of the call's 70 launches, 94 % of its time)",
+        "roofline": {"bound": "tensor", "kernel": "k_tc_gemm<EPI> (persistent wgmma 3xTF32 conv-as-GEMM; 47 of the call's 70 launches)",
                      "achieved": round(ach, 1), "peak": round(tf32_peak, 1), "unit": "TFLOP/s", "frac": round(ach / tf32_peak, 4),
-                     "traffic": DEC_TRAFFIC_C4,
+                     "traffic": None,
                      "peak_source": "measured in this run: torch.matmul fp32 8192^3 with allow_tf32 (cuBLAS TF32), best of 5",
                      "note": "achieved = ALGORITHMIC fp32 flops (4.73 TFLOP at C4) / step time; the 3xTF32 split issues 3 tensor MACs "
                              "per algorithmic MAC, so the tensor pipes do 3x this figure",
                      "tensor_work_frac": round(3 * ach / tf32_peak, 4),
                      "hbm": {"algorithmic_bytes": int(DEC_ALGO_BYTES), "achieved_gbs": round(DEC_ALGO_BYTES / (ms / 1e3) / 1e9, 1),
-                             "dram_traffic_gbs": round(DEC_TRAFFIC_C4 / (ms / 1e3) / 1e9, 1),
-                             "traffic_note": "traffic = ncu dram bytes of one call (constant from profiles/r02_decoder_c4_dram.csv), "
-                                             "96x the algorithmic bytes: the 4x-wide ConvNeXt intermediates round-trip HBM",
                              "peak_gbs": hbm_peak, "peak_source": hbm_src},
                      "fma_twin_ms": None if fma_ms is None else round(fma_ms, 2)},
         "cpu_baseline": cpu,
@@ -531,7 +540,7 @@ def run_reference_decoder(args, rank: int):
 # ------------------------------------------------------------------ the reference's own stack on the same GPU
 def run_torch_cuda(args, rank: int):
     """`--impl torch-cuda` (BASELINE configs[1] "KV-cache kernel vs torch.sdpa"): HF LlamaModel in fp32 with SDPA attention and
-    its DynamicCache on the same B200, heads / temperature / penalty / greedy arg-max as eager torch ops - the reference's
+    its DynamicCache on the same GPU, heads / temperature / penalty / greedy arg-max as eager torch ops - the reference's
     library path (gpt.py:394-596) without its Python generator overhead.  Same synthetic weights, prompt and token count."""
     if rank != 0:
         return None
@@ -585,15 +594,16 @@ def run_torch_cuda(args, rank: int):
     for _ in range(max(1, min(args.warmup, 2))):
         gen(min(n, 32))
     torch.cuda.synchronize()
-    steps = max(1, min(args.steps, 3))
+    steps = args.steps
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(steps):
-        gen(n)
+        hist = gen(n)
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / steps
     value = B * n / (ms / 1e3)
+    dump_outputs(args.dump_outputs, {"ids": hist.transpose(1, 2)})  # [B, tokens, 4]
     return {"impl": "torch-cuda", "metric": "speech-tokens/sec (GPT decode loop, 4-codebook tokens; RTF = wall / audio seconds @ 24 kHz)",
             "value": round(value, 2), "unit": "speech-tokens/s", "n_gpus": 1, "steps": steps, "warmup": args.warmup,
             "ms_per_step": round(ms, 3), "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
@@ -655,13 +665,13 @@ def run_c3(args, rank: int, world: int, local_rank: int):
     for _ in range(max(1, min(args.warmup, 2))):
         pipeline()
     barrier()
-    steps = max(1, min(args.steps, 3))
+    steps = args.steps
     l0 = lib.ctb_launch_count()
     with ClockSampler(local_rank) as clk:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(steps):
-            pipeline()
+            code_ids = pipeline()
         e1.record()
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / steps
@@ -672,6 +682,7 @@ def run_c3(args, rank: int, world: int, local_rank: int):
     launches = int(lib.ctb_launch_count() - l0) // steps
     if rank != 0:
         return None
+    dump_outputs(args.dump_outputs, {"ids": torch.stack(code_ids)})  # code pass: [B, tokens, 4]
     value = world * B * tokens / (ms / 1e3)
     peak, peak_src = measured_peaks()
     code_bytes = algorithmic_bytes_per_step(B, sum(lengths) / B + tokens / 2) * tokens
@@ -690,7 +701,7 @@ def run_c3(args, rank: int, world: int, local_rank: int):
         "e2e": {"value": round(value, 2), "unit": "speech-tokens/s", "h2d_bytes_per_step": int(ids.numel() * 8 + mask.numel()),
                 "d2h_bytes_per_step": int(B * tokens * 16), "ms_per_step": round(ms, 3)},
         "gpu_launches": launches, "clocks": clk.summary(),
-        "roofline": {"bound": "hbm", "kernel": "whole pipeline (tcgen05 decode back end at B = 32, both passes)", "achieved":
+        "roofline": {"bound": "hbm", "kernel": "whole pipeline (wgmma decode back end at B = 32, both passes)", "achieved":
                      round((code_bytes + text_bytes) / (ms / 1e3) / 1e9, 1), "peak": peak, "unit": "GB/s",
                      "frac": round((code_bytes + text_bytes) / (ms / 1e3) / 1e9 / peak, 4), "traffic": None, "peak_source": peak_src},
         "cpu_baseline": None,
@@ -805,7 +816,11 @@ def main():
     ap.add_argument("--config", default="c2", choices=["c2", "c3"], help="c2: BASELINE configs[1] (default); c3: configs[2]")
     ap.add_argument("--path", default="gpt", choices=["gpt", "decoder"], help="decoder: hot path 2 at BASELINE configs[3]")
     ap.add_argument("--no-sweep", action="store_true", help="skip the short batch-8/32 and decoder side measurements")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else max(args.warmup, 1)
 
     rank = int(os.environ.get("RANK", "0"))

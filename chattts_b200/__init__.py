@@ -1,4 +1,4 @@
-"""chattts_b200 - B200-native (sm_100a) hot paths of ChatTTS behind the reference's API.
+"""chattts_b200 - H100-native (sm_90a) hot paths of ChatTTS behind the reference's API.
 
     from chattts_b200 import Chat          # same surface as ChatTTS.Chat (core.py)
 

@@ -132,4 +132,4 @@ def require_cuda():
     import torch
 
     if not torch.cuda.is_available():
-        raise CtbError("chattts_b200 needs a CUDA device (sm_100a); there is no CPU path")
+        raise CtbError("chattts_b200 needs a CUDA device (sm_90a); there is no CPU path")

@@ -1,4 +1,4 @@
-"""``Chat`` - the public API of the reference (ChatTTS/core.py) re-hosted on the B200 hot paths.
+"""``Chat`` - the public API of the reference (ChatTTS/core.py) re-hosted on the H100 hot paths.
 
 Same surface: ``Chat.load / infer / interrupt / unload / has_loaded / sample_random_speaker``,
 ``Chat.RefineTextParams`` / ``Chat.InferCodeParams`` (core.py:137-273).  The two hot paths are

@@ -84,7 +84,7 @@ struct ctb_decoder {
   size_t max_rows;  // max_batch * 2 * max_tokens frames
   size_t cap_rows;  // frames the activation buffers currently hold
   float *bufA, *bufB, *bufH, *mel_tm, *staged_in;
-  // tcgen05 path: tf32-rounded hi / lo copies of both blobs (same offsets as the fp32 blobs)
+  // tensor-core path: tf32-rounded hi / lo copies of both blobs (same offsets as the fp32 blobs)
   float *dW_hi, *dW_lo, *vW_hi, *vW_lo;
   bool use_tc;
 };

@@ -8,14 +8,14 @@
 //    slots filled by 1-D TMA bulk copies (cp.async.bulk + mbarrier complete_tx).  The warp's tasks for the whole step
 //    (QKV pair, K/V chunk, O row, gate/up pairs, down slices, head pairs; all layers) form one static sequence;
 //    after consuming task n the warp's lane 0 issues the copy of task n + FL_SLOTS into the slot it just freed.
-//    Weights (and the K/V of earlier tokens) never depend on this step's activations, so 148 x 192 KiB are always
+//    Weights (and the K/V of earlier tokens) never depend on this step's activations, so every SM's 192 KiB are always
 //    in flight across phase and layer boundaries and HBM streams while a CTA waits for its inputs.
 //
 //  * No grid barriers.  Activations cross CTAs as 8-byte {value, tag} words ("LL" protocol): the producer stores
 //    value and tag with ONE 64-bit store, the consumer polls the data words themselves until the tag of this
 //    (step, layer, phase) appears.  One L2 write + one L2 read per dependent edge - no release fence, no arrival
 //    counter, no separate data load after an acquire.  Broadcast vectors are written to R replicas so that the
-//    148 readers of a vector do not queue on the same L2 slices.
+//    grid's readers of a vector do not queue on the same L2 slices.
 //
 // Arithmetic order per row is independent of the batch; results differ from k_step only by fp32 reassociation in
 // the RMSNorm sum (per-lane strided instead of per-warp-row).
@@ -268,7 +268,7 @@ __device__ __forceinline__ bool fl_issue(const FlowP& p, const FlowGeo* gs, cons
         // Two-level stream: the SAME task of the next layer (of layer 0 of the next step after the last one) is pulled
         // HBM -> L2 now, so that its shared-memory copy, posted a layer later, is an L2 hit.  A global load issued after
         // a bulk copy only returns after it: a copy that completes in ~0.3 us instead of a DRAM latency holds the polls
-        // behind it that much less.  One layer of weights (37.75 MB) fits the 126 MB L2 next to the exchange arena.
+        // behind it that much less.  One layer of weights (37.75 MB) fits the H100's 50 MB L2 next to the exchange arena.
         const float* nsrc = it.l + 1 < p.L ? src + p.layer_stride : src - (int64_t)(p.L - 1) * p.layer_stride;
 #pragma unroll
         for (int k = 0; k < 4; ++k)
@@ -290,11 +290,10 @@ __device__ __forceinline__ bool fl_issue(const FlowP& p, const FlowGeo* gs, cons
 }
 
 // Per-warp ring state.  The consuming warp refills a slot itself, right after the stores of the phase that emptied it.
-// Two alternatives were built and measured on B200 (tools/flow_check.py, B = 1, 256 tokens):
-//   * lazy refills inside the poll loops (one per failed poll): 20-40 % slower (longer poll period);
+// Two alternatives were built and found slower (tools/flow_check.py, B = 1, 256 tokens):
+//   * lazy refills inside the poll loops (one per failed poll): a longer poll period;
 //   * a loader warpgroup (4 warps posting every copy of the CTA, consumers only publish a counter, registers moved
-//     with setmaxnreg): 360-380 us/step against 323 - the X edge grew from ~0.8 to ~2.5 us while the copies were posted
-//     concurrently with the polls.
+//     with setmaxnreg): the X edge grew while the copies were posted concurrently with the polls.
 struct FlowW {
   float* base;      // this warp's slots (generic pointer)
   uint32_t ring;    // same, shared-space address
@@ -1105,7 +1104,7 @@ __global__ void __launch_bounds__(FL_THREADS, 1) k_flow(const __grid_constant__ 
           }
         }
         // The splits of a (row, head) meet at the split-0 unit, which publishes the merged 64 outputs: the O-proj phase of
-        // all 148 CTAs then stages 768 words per row instead of every CTA reading (and merging) every partial.
+        // all CTAs then stages 768 words per row instead of every CTA reading (and merging) every partial.
         const int ns_u = min(g.u_nchunk, g.S);
         if (tid < 64) {
           unsigned long long* P = par + FL_A_P + ((size_t)(b * FL_HEADS + h) * FL_SMAX) * FL_PW;  // replica 0 only
@@ -1268,7 +1267,7 @@ __global__ void __launch_bounds__(FL_THREADS, 1) k_flow(const __grid_constant__ 
           if (b < p.B) {  // one poll loop per batch row keeps the 64-bit words of only one row live
             const unsigned long long* ap = myr + FL_A_ACT + (size_t)b * p.I + warp * kslice;
             unsigned long long w[12];
-            // 148 x 8 warps reading 3 KiB each is 3.5 MB through L2 per round: spin on the first two words of every lane
+            // 132 x 8 warps reading 3 KiB each is 3.2 MB through L2 per round: spin on the first two words of every lane
             // and read the rest once they are in; every word is still validated by its own tag.  (Arrival counters
             // bumped with red.add by the producers were tried instead of the sentinel words: no faster, 356 vs 352 us.)
             wd.spins = 0;

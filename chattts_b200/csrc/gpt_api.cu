@@ -28,7 +28,7 @@ int set_err(int code, const char* fmt, ...) {
   return code;
 }
 
-int g_num_sms = 148;
+int g_num_sms = 132;  // set from the device in ctb_gpt_create
 
 
 static int bt_for(int B) {
@@ -77,13 +77,13 @@ struct ctb_gpt {
   int *pf_npre, *pf_nvalid;
   size_t pf_rows;                  // capacity (B * T0) of the pf_* activation buffers
   bool mega_ok;      // one-kernel decode step (mega.cuh), built for B <= 8
-  int mega_max_batch; // batches that use it (default 4: measured faster up to there; CTB_MEGA_MAX_BATCH overrides)
+  int mega_max_batch; // batches that use it (default 4; CTB_MEGA_MAX_BATCH overrides)
   unsigned* bar;     // its grid-barrier counter
   unsigned long long* trace;  // CTB_MEGA_TRACE=1: per-phase timestamps of the last step
-  bool flow_ok;      // dataflow decode step (flow.cuh), B <= 4: default back end for those batches
+  bool flow_ok;      // dataflow decode step (flow.cuh), built for B <= 4
   int flow_R;        // replicas of the broadcast exchange regions (CTB_FLOW_R)
   int flow_l2_ahead;  // weight tasks prefetched one layer ahead into L2 (CTB_FLOW_L2_AHEAD)
-  int flow_max_batch; // batches that use it (CTB_FLOW_MAX_BATCH, default 4)
+  int flow_max_batch; // batches that use it (CTB_FLOW_MAX_BATCH, default 1)
   unsigned long long* flow_arena;
   unsigned* flow_epoch;
   int steps_enqueued;  // loop iterations enqueued since ctb_gpt_begin (host-side bound for ctb_gpt_decode)
@@ -288,11 +288,13 @@ extern "C" int ctb_gpt_create(const ctb_gpt_config* c, const float* weights_dev,
     TRY(dalloc(&h->flow_epoch, 4));
     const unsigned e0 = FL_EPOCH_STEP;
     cudaMemcpy(h->flow_epoch, &e0, sizeof(e0), cudaMemcpyHostToDevice);
-    // measured on B200 (tools/flow_check.py): one copy of the exchange words is fastest (replicas multiply the 8-byte
-    // stores; the read hot-spot they were meant to relieve is the smaller effect), and the kernel beats k_step at every batch it is built for (B <= 4)
+    // one copy of the exchange words by default (replicas multiply the 8-byte stores; CTB_FLOW_R selects more for
+    // tools/flow_check.py to compare)
     h->flow_R = getenv("CTB_FLOW_R") ? std::max(1, std::min(FL_RMAX, atoi(getenv("CTB_FLOW_R")))) : 1;
     h->flow_l2_ahead = getenv("CTB_FLOW_L2_AHEAD") ? atoi(getenv("CTB_FLOW_L2_AHEAD")) : 0;
-    h->flow_max_batch = getenv("CTB_FLOW_MAX_BATCH") ? std::max(0, std::min(FL_BMAX, atoi(getenv("CTB_FLOW_MAX_BATCH")))) : FL_BMAX;
+    // H100, 512-token passes: k_flow<1> 239 ms vs k_step<1> 309 ms, but at B = 2 / 3 / 4 k_step is faster (332 / 379 / 395 ms
+    // vs 342 / 530 / 550 ms), so the dataflow step serves B = 1 by default
+    h->flow_max_batch = getenv("CTB_FLOW_MAX_BATCH") ? std::max(0, std::min(FL_BMAX, atoi(getenv("CTB_FLOW_MAX_BATCH")))) : 1;
   }
 #undef TRY
   h->use_graph = getenv("CTB_NO_GRAPH") == nullptr;
@@ -301,10 +303,12 @@ extern "C" int ctb_gpt_create(const ctb_gpt_config* c, const float* weights_dev,
                (c->hidden_size / 2 + g_num_sms - 1) / g_num_sms <= MG_DOWN_PAIRS;
   h->mega_max_batch = getenv("CTB_MEGA_MAX_BATCH") ? std::min(8, atoi(getenv("CTB_MEGA_MAX_BATCH"))) : 4;
   // tensor-core decode GEMMs (tc_decode.cuh): CTB_GPT_TC=1 forces them for every batch, CTB_GPT_FMA=1 disables
-  // them; by default they serve batches > 16 rows, where the fp32 FMA path turns compute-bound.
+  // them; by default they serve batches of 9 rows and more, where the FMA kernels' batch tile grows to 16 rows
+  // (H100, 512-token passes: 726 / 786 ms vs 881 / 962 ms at B = 10 / 16; at B = 8 the FMA kernels take 481 ms).
+  constexpr int kTcMinBatch = 9;
   h->tc_ready = getenv("CTB_GPT_FMA") == nullptr && c->max_batch <= 32 &&
-                (getenv("CTB_GPT_TC") != nullptr || c->max_batch > 16);
-  h->tc_min_batch = getenv("CTB_GPT_TC") != nullptr ? 1 : 17;
+                (getenv("CTB_GPT_TC") != nullptr || c->max_batch >= kTcMinBatch);
+  h->tc_min_batch = getenv("CTB_GPT_TC") != nullptr ? 1 : kTcMinBatch;
   if (h->tc_ready && (rc = tc_setup(h)) != CTB_OK) { ctb_gpt_destroy(h); return rc; }
   *out = h;
   return CTB_OK;
@@ -334,8 +338,18 @@ static int launch_gemv_t(const GemvP& p, int ntiles, cudaStream_t s) {
   unsigned cluster = 1;
   if (EPI == EPI_DOWN) {
     cluster = DOWN_SPLIT;
-    // clusters of 4 can only occupy ~132 of the 148 SMs at once (GPC granularity): one wave of 33 clusters, not 37
-    const int max_groups = (g_num_sms * 132 / 148) / DOWN_SPLIT;
+    // clusters of 4 cannot use every SM at once (GPC granularity): size one wave by what the device reports
+    static int max_groups = 0;
+    if (!max_groups) {
+      cudaLaunchConfig_t qc{};
+      qc.gridDim = dim3(DOWN_SPLIT * (g_num_sms / DOWN_SPLIT)); qc.blockDim = dim3(GEMV_WARPS * 32); qc.dynamicSmemBytes = smem;
+      cudaLaunchAttribute qa[1];
+      qa[0].id = cudaLaunchAttributeClusterDimension;
+      qa[0].val.clusterDim.x = DOWN_SPLIT; qa[0].val.clusterDim.y = 1; qa[0].val.clusterDim.z = 1;
+      qc.attrs = qa; qc.numAttrs = 1;
+      CTB_CUDA(cudaOccupancyMaxActiveClusters(&max_groups, k_gemv<BT, EPI>, &qc));
+      if (max_groups < 1) return set_err(CTB_ERR_STATE, "DOWN kernel: no cluster of %d CTAs fits the device", DOWN_SPLIT);
+    }
     const int groups = std::max(1, std::min(max_groups, (p.ntasks + GEMV_WARPS - 1) / GEMV_WARPS));
     if ((p.ntasks + groups * GEMV_WARPS - 1) / (groups * GEMV_WARPS) > DOWN_MAX_TASKS)
       return set_err(CTB_ERR_STATE, "DOWN kernel: too few SMs (%d) for %d tasks", g_num_sms, p.ntasks);
@@ -902,7 +916,7 @@ extern "C" int ctb_gpt_begin(ctb_gpt* h, int32_t B, int32_t T0, const float* emb
   // prefill: the prompt is walked column by column through the decode kernels (left padding
   // keeps every row's last prompt token in the last column, like the reference's batches)
   if (h->pf_enabled && T0 >= 8 && T0 <= 1024) {
-    // whole prompt as token-parallel tcgen05 GEMMs (prefill.cuh)
+    // whole prompt as token-parallel wgmma GEMMs (prefill.cuh)
     if ((rc = prefill_batched(h, s))) return rc;
   } else {
     // short prompts: walk the columns through the decode kernels (left padding keeps every row's last prompt

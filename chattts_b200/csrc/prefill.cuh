@@ -1,5 +1,5 @@
 // Batched prefill (SURVEY.md 8f N1; reference gpt.py:396-427 at i == 0): the whole left-padded prompt batch
-// [B, T0, 768] goes through the 20 layers as token-parallel GEMMs on tcgen05 (k_tc_gemm, 3xTF32 =
+// [B, T0, 768] goes through the 20 layers as token-parallel GEMMs on wgmma (k_tc_gemm, 3xTF32 =
 // fp32-equivalent) instead of one decode step per prompt column.  Each batch row is one "utterance" of T0 frames
 // for the GEMM tiler; pad columns are computed but never written to the KV cache nor attended to.
 //
@@ -91,7 +91,7 @@ __global__ void k_prefill_rope_kv(const PrefillP p) {
 // Causal attention over the row's valid prompt tokens, query-parallel: grid (ceil(T0 / 8), Hq, B), 8 warps per CTA,
 // ONE WARP PER QUERY (hd == 64).  Pass 1: lane-per-key scores into the warp's shared-memory row (same fma order per score
 // as the decode kernels), warp max; pass 2: exponentials + sum; pass 3: P.V with lane = two output dims, keys in order.
-// (Round 1 walked the queries of a (row, head) serially in one 128-thread CTA: 12 CTAs on 148 SMs and O(T^2) per CTA -
+// (Round 1 walked the queries of a (row, head) serially in one 128-thread CTA: 12 CTAs on 132 SMs and O(T^2) per CTA -
 // fine for 16-token prompts, hopeless for speaker-prompt prefixes of hundreds of tokens.)
 constexpr int PF_ATT_WARPS = 8;
 __global__ void __launch_bounds__(PF_ATT_WARPS * 32) k_prefill_attn(const PrefillP p) {

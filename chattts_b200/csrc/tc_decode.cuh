@@ -1,10 +1,10 @@
-// Decode-step GEMMs on tcgen05 tensor cores (swap-AB, 3xTF32, split-K over a thread-block cluster).
+// Decode-step GEMMs on wgmma tensor cores (swap-AB, 3xTF32, split-K over a thread-block cluster).
 //
 //   Y[b, r] = sum_k W[r, k] * x[b, k]        W: [rows, K] fp32 streamed from HBM exactly once by TMA
 //
-//   * swap-AB: the 128 weight rows of a tile are the UMMA M dimension, the (padded) batch is N = NPAD.
+//   * swap-AB: the 128 weight rows of a tile are the MMA M dimension (two m64 wgmmas), the (padded) batch is N = NPAD.
 //   * fp32-equivalent accuracy for the bit-exact-ids contract: W = W_hi + W_lo is split in shared memory by
-//     the worker warps (cvt.rna.tf32; weights cannot be pre-split without doubling HBM traffic), the
+//     the worker warpgroup (cvt.rna.tf32; weights cannot be pre-split without doubling HBM traffic), the
 //     activations arrive pre-split (x_hi, x_lo written by the producing kernel's epilogue).  Two MMAs per
 //     k-step:  W_hi x [x_hi ; x_lo] (N = 2*NPAD, one pass over the W_hi tile) and W_lo x x_hi (N = NPAD).
 //   * split-K: the CS CTAs of a cluster own consecutive K slices of the same 128 rows, so 6..48 row tiles
@@ -23,8 +23,8 @@ namespace ctb {
 
 enum DecEpi { DE_QKV = 0, DE_OPROJ = 1, DE_GATEUP = 2, DE_DOWN = 3, DE_HEADS = 4 };
 
-constexpr int TD_STAGES = 3;  // 3 x 36-40 KiB: two CTAs (this kernel + its PDL successor) fit one SM
-constexpr int TD_THREADS = 192;
+constexpr int TD_STAGES = 3;  // 3 x 36-48 KiB: two CTAs (this kernel + its PDL successor) fit one SM
+constexpr int TD_THREADS = 160;  // warps 0-3: one warpgroup (rms, W split, wgmma, epilogue); warp 4: TMA
 constexpr int TD_A_BYTES = 128 * 32 * 4;  // 16 KiB weight tile (128 rows x 32 k)
 
 template <int NPAD>
@@ -56,12 +56,9 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
   extern __shared__ uint8_t td_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(td_smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + TD_STAGES * Cfg::STAGE_BYTES);
-  uint64_t* full = bars;
-  uint64_t* split = bars + TD_STAGES;
-  uint64_t* empty = bars + 2 * TD_STAGES;
-  uint64_t* accum_full = bars + 3 * TD_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * TD_STAGES + 1);
-  float* s_rinv = reinterpret_cast<float*>(bars + 3 * TD_STAGES + 2);  // [NPAD]
+  uint64_t* full = bars;                  // [stages]  TMA bytes landed
+  uint64_t* empty = bars + TD_STAGES;     // [stages]  the stage's MMAs retired
+  float* s_rinv = reinterpret_cast<float*>(bars + 2 * TD_STAGES);  // [NPAD]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rank = (CS > 1) ? (int)cluster_ctarank() : 0;
@@ -69,7 +66,6 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
   const int r_tile = tile * 128;
   const int kbase = rank * p.kslice;
   const int nk = p.kslice / 32;
-  constexpr uint32_t TMEM_COLS = (2 * NPAD <= 32) ? 32 : 64;
 
   if (threadIdx.x == 128) {  // TMA warp: hide the descriptor fetch latency
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
@@ -77,18 +73,10 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_xlo) : "memory");
   }
   if (threadIdx.x == 0) {
-    for (int s = 0; s < TD_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&split[s], 128); mbar_init(&empty[s], 1); }
-    mbar_init(accum_full, 1);
+    for (int s = 0; s < TD_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 128); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 5) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 4) {
     // ===================== TMA producer
@@ -114,28 +102,6 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
         tma_load_2d(st + 2 * TD_A_BYTES, &map_xhi, &full[s], kbase + t * 32, 0);
         tma_load_2d(st + 2 * TD_A_BYTES + Cfg::X_BYTES, &map_xlo, &full[s], kbase + t * 32, 0);
       }
-    }
-  } else if (warp == 5) {
-    // ===================== MMA issuer
-    const uint32_t idesc_wide = umma_idesc_tf32(128, 2 * NPAD), idesc_narrow = umma_idesc_tf32(128, NPAD);
-    for (int t = 0; t < nk; ++t) {
-      const int s = t % TD_STAGES, it = t / TD_STAGES;
-      mbar_wait(&split[s], it & 1);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t st = smem_u32(smem + s * Cfg::STAGE_BYTES);
-        const uint32_t w_hi = st, w_lo = st + TD_A_BYTES, x_hl = st + 2 * TD_A_BYTES;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const uint32_t ko = k * 32;
-          // cols [0,NPAD) += W_hi x_hi ; cols [NPAD,2NPAD) += W_hi x_lo   (x_hi | x_lo tiles are contiguous)
-          umma_tf32(tmem_base, umma_desc_sw128(w_hi + ko), umma_desc_sw128(x_hl + ko), idesc_wide, (t | k) ? 1u : 0u);
-          umma_tf32(tmem_base, umma_desc_sw128(w_lo + ko), umma_desc_sw128(x_hl + ko), idesc_narrow, 1u);
-        }
-        umma_commit(&empty[s]);
-        if (t == nk - 1) umma_commit(accum_full);
-      }
-      __syncwarp();
     }
   } else {
     // ===================== workers
@@ -174,6 +140,13 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
         }
       }
     }
+    // accumulators of weight rows [64 hf, 64 hf + 64): columns [0, NPAD) x_hi, [NPAD, 2 NPAD) x_lo
+    float acc[2][NPAD];
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+      for (int i = 0; i < NPAD; ++i) acc[hf][i] = 0.f;
+    int prev = 0;
     for (int t = 0; t < nk; ++t) {
       const int s = t % TD_STAGES, it = t / TD_STAGES;
       mbar_wait(&full[s], it & 1);
@@ -188,46 +161,48 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
         l.x = to_tf32(v.x - h.x); l.y = to_tf32(v.y - h.y); l.z = to_tf32(v.z - h.z); l.w = to_tf32(v.w - h.w);
         a[i] = h; lo[i] = l;
       }
-      fence_async_smem();
-      mbar_arrive(&split[s]);
-    }
-    // ---- accumulator -> this CTA's partial tile in shared memory [128 rows][NPAD]
-    mbar_wait(accum_full, 0);
-    tc_fence_after();
-    float* part = reinterpret_cast<float*>(smem);  // stage 0 is free: every MMA has retired
-    {
-      uint32_t r[2 * NPAD];
-      const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16);
-      if (NPAD == 16) {
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,"
-            "%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-              "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-              "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-              "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-            : "r"(taddr));
-      } else {
+      fence_async_smem();  // generic-proxy writes -> visible to the tensor core (async proxy)
+      warpgroup_bar(2);
+      const uint32_t st = smem_u32(smem + s * Cfg::STAGE_BYTES);
+      const uint32_t w_hi = st, w_lo = st + TD_A_BYTES, x_hl = st + 2 * TD_A_BYTES;
+      wgmma_fence();
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          uint32_t* q = r + 32 * half;
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,"
-              "%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-              : "=r"(q[0]), "=r"(q[1]), "=r"(q[2]), "=r"(q[3]), "=r"(q[4]), "=r"(q[5]), "=r"(q[6]), "=r"(q[7]), "=r"(q[8]),
-                "=r"(q[9]), "=r"(q[10]), "=r"(q[11]), "=r"(q[12]), "=r"(q[13]), "=r"(q[14]), "=r"(q[15]), "=r"(q[16]),
-                "=r"(q[17]), "=r"(q[18]), "=r"(q[19]), "=r"(q[20]), "=r"(q[21]), "=r"(q[22]), "=r"(q[23]), "=r"(q[24]),
-                "=r"(q[25]), "=r"(q[26]), "=r"(q[27]), "=r"(q[28]), "=r"(q[29]), "=r"(q[30]), "=r"(q[31])
-              : "r"(taddr + 32 * half));
+      for (int k = 0; k < 4; ++k) {
+        const uint32_t ko = k * 32;
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+          const uint32_t ro = hf * (TD_A_BYTES / 2);  // 64 rows x 128 B
+          // cols [0,NPAD) += W_hi x_hi ; cols [NPAD,2NPAD) += W_hi x_lo   (x_hi | x_lo tiles are contiguous)
+          // cols [0,NPAD) += W_lo x_hi
+          if constexpr (NPAD == 16) {
+            wgmma_tf32_n32(acc[hf], wgmma_desc_sw128(w_hi + ro + ko), wgmma_desc_sw128(x_hl + ko), (t | k) ? 1u : 0u);
+            wgmma_tf32_n16(acc[hf], wgmma_desc_sw128(w_lo + ro + ko), wgmma_desc_sw128(x_hl + ko), 1u);
+          } else {
+            wgmma_tf32_n64(acc[hf], wgmma_desc_sw128(w_hi + ro + ko), wgmma_desc_sw128(x_hl + ko), (t | k) ? 1u : 0u);
+            wgmma_tf32_n32(acc[hf], wgmma_desc_sw128(w_lo + ro + ko), wgmma_desc_sw128(x_hl + ko), 1u);
+          }
         }
       }
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      const int row = warp * 32 + lane;
-#pragma unroll
-      for (int b = 0; b < NPAD; ++b)
-        part[row * NPAD + b] = __uint_as_float(r[b]) + __uint_as_float(r[NPAD + b]);  // x_hi and x_lo halves
+      wgmma_commit();
+      if (t > 0) {  // the previous stage's MMAs have retired: hand it back to the producer
+        wgmma_wait<1>();
+        mbar_arrive(&empty[prev]);
+      }
+      prev = s;
     }
-    tc_fence_before();
+    wgmma_wait<0>();
+    wgmma_fence_operands(acc[0]);
+    wgmma_fence_operands(acc[1]);
+    // ---- accumulator -> this CTA's partial tile in shared memory [128 rows][NPAD]
+    float* part = reinterpret_cast<float*>(smem);  // stage 0 is free: every MMA has retired
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+      for (int i = 0; i < NPAD / 2; ++i) {  // register layout: see wgmma_tf32_n*
+        const int row = hf * 64 + warp * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+        const int b = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+        part[row * NPAD + b] = acc[hf][i] + acc[hf][i + NPAD / 2];  // x_hi and x_lo halves
+      }
   }
 
   // ===================== split-K merge through DSMEM + fused epilogue (worker warps)
@@ -298,11 +273,7 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
       }
     }
   }
-  if (CS > 1) cluster_sync_all(); else __syncthreads();  // partial tiles stay alive until every rank has read them
-  if (warp == 5) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
-  }
+  if (CS > 1) cluster_sync_all();  // partial tiles stay alive until every rank has read them
 }
 
 // ---- one-time construction of the tensor-core weight copy (device side, from the fp32 blob)

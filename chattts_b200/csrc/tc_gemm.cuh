@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / TMA GEMM with fp32-equivalent accuracy (3xTF32) for the dense contractions of
+// wgmma / TMA GEMM with fp32-equivalent accuracy (3xTF32) for the dense contractions of
 // hot path 2 (and prefill):   C[m, n] = epi( sum_kk A[m, kk] * W[n, kk] )
 //
 //   * A: time-major activations [B][F][lda] fp32, read by a 3-D TMA tensor map (c, f, b).  A Conv1d tap
@@ -6,12 +6,14 @@
 //     padding, per utterance - no im2col, no boundary code.
 //   * W: [N][K] fp32, pre-split on the host into tf32-rounded `hi` and `lo = tf32(w - hi)` copies (weights
 //     are constants), two 2-D TMA maps.
-//   * 3xTF32:  A*W ~= A_hi*W_hi + A_hi*W_lo + A_lo*W_hi, accumulated in fp32 in TMEM.  A is split in
-//     shared memory by the 4 worker warps (cvt.rna.tf32), which later run the epilogue.
-//   * warp roles: 0-3 workers (split A, epilogue: tcgen05.ld -> bias/GELU/... -> global), 4 = TMA producer,
-//     5 = MMA issuer (one elected lane issues tcgen05.mma.cta_group::1.kind::tf32, M=128, N=128, K=8).
+//   * 3xTF32:  A*W ~= A_hi*W_hi + A_hi*W_lo + A_lo*W_hi, accumulated in fp32 registers.  A is split in shared
+//     memory by the warpgroup that consumes it (cvt.rna.tf32).
+//   * warp roles: warpgroups 0-1 consume (each splits and multiplies 64 of the tile's 128 rows with
+//     wgmma.m64n128k8.tf32, then runs the epilogue from its registers), warp 8 = TMA producer.
 //   * tile 128 (frames of one utterance) x 128 (channels) x 32 (k) per stage, 3 stages of 64 KiB:
-//     [A | A_lo | W_hi | W_lo], 128-byte swizzle (TMA and UMMA descriptors agree).
+//     [A | A_lo | W_hi | W_lo], 128-byte swizzle (TMA and wgmma descriptors agree).
+//   * persistent: a CTA walks tiles (n fastest, so concurrent CTAs share A rows in L2); the producer runs ahead into
+//     the next tile's stages while the consumers run the epilogue of the current one.
 #pragma once
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -25,7 +27,8 @@ constexpr int TC_BM = 128, TC_BN = 128, TC_BK = 32, TC_STAGES = 3;
 constexpr int TC_TILE_BYTES = TC_BM * TC_BK * 4;          // 16 KiB
 constexpr int TC_STAGE_BYTES = 4 * TC_TILE_BYTES;         // A, A_lo, W_hi, W_lo
 constexpr int TC_SMEM_BYTES = TC_STAGES * TC_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-constexpr int TC_THREADS = 192;
+constexpr int TC_CONSUMERS = 256;                         // two warpgroups
+constexpr int TC_THREADS = TC_CONSUMERS + 32;             // + the TMA warp
 
 struct TcGemmP {
   int N, K;                   // K = taps * Cin, multiple of 32
@@ -36,52 +39,35 @@ struct TcGemmP {
 };
 
 
-// Epilogue of one 32-column block of one output row: r = the row's accumulators (tcgen05.ld 32x32b.x32), m = global row.
+// Epilogue of two adjacent output columns (n even) of one output row m.
 template <int EPI>
-__device__ __forceinline__ void tc_epi_store(const TcGemmP& p, const uint32_t (&r)[32], size_t m, int nbase) {
-#pragma unroll
-  for (int q = 0; q < 8; ++q) {
-    const int n = nbase + q * 4;
-    if (n >= p.N) continue;
-    float v[4] = {__uint_as_float(r[q * 4]), __uint_as_float(r[q * 4 + 1]), __uint_as_float(r[q * 4 + 2]),
-                  __uint_as_float(r[q * 4 + 3])};
-    if (EPI == GE_BIAS || EPI == GE_GELU || EPI == GE_SCALE_RES || EPI == GE_SPEC) {
-      const float4 bb = __ldg(reinterpret_cast<const float4*>(p.bias + n));
-      v[0] += bb.x; v[1] += bb.y; v[2] += bb.z; v[3] += bb.w;
-    }
-    if (EPI == GE_GELU) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) v[j] = gelu_erf(v[j]);
-    } else if (EPI == GE_SCALE_RES) {
-      const float4 g = __ldg(reinterpret_cast<const float4*>(p.gamma + n));
-      const float4 rr = *reinterpret_cast<const float4*>(p.res + m * p.ldres + n);
-      v[0] = __fadd_rn(__fmul_rn(v[0], g.x), rr.x); v[1] = __fadd_rn(__fmul_rn(v[1], g.y), rr.y);
-      v[2] = __fadd_rn(__fmul_rn(v[2], g.z), rr.z); v[3] = __fadd_rn(__fmul_rn(v[3], g.w), rr.w);
-    } else if (EPI == GE_COEF) {
-      const float4 g = __ldg(reinterpret_cast<const float4*>(p.gamma + n));
-      v[0] *= g.x; v[1] *= g.y; v[2] *= g.z; v[3] *= g.w;
-    } else if (EPI == GE_SPEC) {
-#pragma unroll
-      for (int j = 0; j < 4; j += 2) {
-        const float mag = fminf(expf(v[j]), 100.0f);
-        float sn, cs;
-        sincosf(v[j + 1], &sn, &cs);
-        v[j] = mag * cs; v[j + 1] = mag * sn;
-      }
-    }
-    *reinterpret_cast<float4*>(p.C + m * p.ldc + n) = make_float4(v[0], v[1], v[2], v[3]);
+__device__ __forceinline__ void tc_epi_store2(const TcGemmP& p, float v0, float v1, size_t m, int n) {
+  if (EPI == GE_BIAS || EPI == GE_GELU || EPI == GE_SCALE_RES || EPI == GE_SPEC) {
+    const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+    v0 += bb.x; v1 += bb.y;
   }
+  if (EPI == GE_GELU) {
+    v0 = gelu_erf(v0); v1 = gelu_erf(v1);
+  } else if (EPI == GE_SCALE_RES) {
+    const float2 g = __ldg(reinterpret_cast<const float2*>(p.gamma + n));
+    const float2 rr = *reinterpret_cast<const float2*>(p.res + m * p.ldres + n);
+    v0 = __fadd_rn(__fmul_rn(v0, g.x), rr.x); v1 = __fadd_rn(__fmul_rn(v1, g.y), rr.y);
+  } else if (EPI == GE_COEF) {
+    const float2 g = __ldg(reinterpret_cast<const float2*>(p.gamma + n));
+    v0 *= g.x; v1 *= g.y;
+  } else if (EPI == GE_SPEC) {  // columns (2j, 2j+1) = (log-magnitude, phase) of one bin
+    const float mag = fminf(expf(v0), 100.0f);
+    float sn, cs;
+    sincosf(v1, &sn, &cs);
+    v0 = mag * cs; v1 = mag * sn;
+  }
+  *reinterpret_cast<float2*>(p.C + m * p.ldc + n) = make_float2(v0, v1);
 }
 
-#define TC_TMEM_LD32(r, taddr)                                                                                              \
-  asm volatile(                                                                                                             \
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,"      \
-      "%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"                                                            \
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),          \
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),              \
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),             \
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])                            \
-      : "r"(taddr))
+__device__ __forceinline__ void mbar_wait_or_trap(uint64_t* bar, uint32_t parity) {
+  for (uint32_t spin = 0; !mbar_try_wait(bar, parity); ++spin)
+    if (spin > (1u << 28)) __trap();   // a protocol bug must end the kernel, not hang the GPU
+}
 
 template <int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
@@ -91,148 +77,7 @@ k_tc_gemm(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + TC_STAGES * TC_STAGE_BYTES);
   uint64_t* full = bars;                  // [stages]  TMA bytes landed
-  uint64_t* split = bars + TC_STAGES;     // [stages]  A split into hi / lo by the workers
-  uint64_t* empty = bars + 2 * TC_STAGES; // [stages]  MMAs of the stage retired
-  uint64_t* accum_full = bars + 3 * TC_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * TC_STAGES + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tiles_per_utt = (p.F + TC_BM - 1) / TC_BM;
-  const int b = blockIdx.y / tiles_per_utt, f0 = (blockIdx.y % tiles_per_utt) * TC_BM;
-  const int n0 = blockIdx.x * TC_BN;
-  const int nk = p.K / TC_BK;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < TC_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&split[s], 128); mbar_init(&empty[s], 1); }
-    mbar_init(accum_full, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 5) {  // TMEM: 128 fp32 accumulator columns
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TC_BN));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 4) {
-    // ===================== TMA producer
-    if (lane == 0) {
-      for (int t = 0; t < nk; ++t) {
-        const int s = t % TC_STAGES, it = t / TC_STAGES;
-        if (it > 0) mbar_wait(&empty[s], (it - 1) & 1);
-        uint8_t* st = smem + s * TC_STAGE_BYTES;
-        const int k0 = t * TC_BK;
-        const int tap = k0 / p.Cin, c0 = k0 - tap * p.Cin;
-        mbar_expect_tx(&full[s], 3 * TC_TILE_BYTES);
-        tma_load_3d(st, &map_a, &full[s], c0, f0 + (tap - p.pad) * p.dil, b);
-        tma_load_2d(st + 2 * TC_TILE_BYTES, &map_whi, &full[s], k0, n0);
-        tma_load_2d(st + 3 * TC_TILE_BYTES, &map_wlo, &full[s], k0, n0);
-      }
-    }
-  } else if (warp == 5) {
-    // ===================== MMA issuer
-    const uint32_t idesc = umma_idesc_tf32(TC_BM, TC_BN);
-    for (int t = 0; t < nk; ++t) {
-      const int s = t % TC_STAGES, it = t / TC_STAGES;
-      mbar_wait(&split[s], it & 1);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t st = smem_u32(smem + s * TC_STAGE_BYTES);
-        const uint32_t a_hi = st, a_lo = st + TC_TILE_BYTES, w_hi = st + 2 * TC_TILE_BYTES, w_lo = st + 3 * TC_TILE_BYTES;
-#pragma unroll
-        for (int k = 0; k < TC_BK / 8; ++k) {
-          const uint32_t ko = k * 32;  // 8 tf32 = 32 bytes inside the 128-byte swizzle row
-          umma_tf32(tmem_base, umma_desc_sw128(a_hi + ko), umma_desc_sw128(w_hi + ko), idesc, (t | k) ? 1u : 0u);
-          umma_tf32(tmem_base, umma_desc_sw128(a_hi + ko), umma_desc_sw128(w_lo + ko), idesc, 1u);
-          umma_tf32(tmem_base, umma_desc_sw128(a_lo + ko), umma_desc_sw128(w_hi + ko), idesc, 1u);
-        }
-        umma_commit(&empty[s]);
-        if (t == nk - 1) umma_commit(accum_full);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ===================== workers: split A, then epilogue
-    for (int t = 0; t < nk; ++t) {
-      const int s = t % TC_STAGES, it = t / TC_STAGES;
-      mbar_wait(&full[s], it & 1);
-      float4* a = reinterpret_cast<float4*>(smem + s * TC_STAGE_BYTES);
-      float4* lo = reinterpret_cast<float4*>(smem + s * TC_STAGE_BYTES + TC_TILE_BYTES);
-#pragma unroll
-      for (int j = 0; j < TC_TILE_BYTES / 16 / 128; ++j) {
-        const int i = threadIdx.x + 128 * j;  // elementwise: the swizzle pattern is the same in both tiles
-        const float4 v = a[i];
-        float4 h, l;
-        h.x = to_tf32(v.x); h.y = to_tf32(v.y); h.z = to_tf32(v.z); h.w = to_tf32(v.w);
-        l.x = to_tf32(v.x - h.x); l.y = to_tf32(v.y - h.y); l.z = to_tf32(v.z - h.z); l.w = to_tf32(v.w - h.w);
-        a[i] = h; lo[i] = l;
-      }
-      fence_async_smem();  // generic-proxy writes -> visible to the tensor core (async proxy)
-      mbar_arrive(&split[s]);
-    }
-    mbar_wait(accum_full, 0);
-    tc_fence_after();
-    const int row = warp * 32 + lane;  // TMEM lane == tile row; warp w may touch lanes [32w, 32w+32)
-    const int f = f0 + row;
-    const size_t m = (size_t)b * p.F + f;
-#pragma unroll 1
-    for (int cb = 0; cb < TC_BN / 32; ++cb) {
-      uint32_t r[32];
-      const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + cb * 32;
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,"
-          "%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-          : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-            "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-            "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-            "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-          : "r"(taddr));
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (f < p.F) tc_epi_store<EPI>(p, r, m, n0 + cb * 32);
-    }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TC_BN));
-  }
-}
-
-
-// ---------------------------------------------------------------- persistent variant (default)
-// Same arithmetic and tile shape as k_tc_gemm, but one CTA per SM walks tiles (n fastest, so concurrent CTAs share A rows
-// in L2) with TWO TMEM accumulators: warps 6-9 run the epilogue of tile i while warps 0-5 already feed tile i+1's
-// mainloop.  k_tc_gemm paid, per 128x128 tile, TMEM alloc + barrier init + a serial epilogue (bias / erf-GELU / stores of
-// 64 KB) behind a mainloop that is only 8 k-steps long for the ConvNeXt pw1 GEMMs (K = 256) - ncu at BASELINE configs[3]:
-// pw1 23.2 ms vs pw2 15.8 ms for the same flops (profiles/r02_decoder_c4_dram_summary.txt).  C4: 43.3 -> 33.8 ms.
-// Tried on top and rejected (measured): loading W as fp32 and splitting it hi / lo in the worker warps like A (no weight
-// copies in HBM, 32 instead of 48 KB per k-step from L2) - 41.9 ms.  The k-step is shared-memory-bandwidth bound: TMA
-// writes + split reads / writes + the operand reads of 12 MMAs were 192 KB per k-step and became 224 KB, against
-// ~158 KB that 128 B/clk deliver in the 0.65 us the MMAs take.  Less shared-memory traffic per MMA (operands pre-split by
-// their producer, or A from TMEM) is what would lift this kernel further.
-constexpr int TCP_THREADS = 320;
-
-__device__ __forceinline__ void mbar_wait_or_trap(uint64_t* bar, uint32_t parity) {
-  for (uint32_t spin = 0; !mbar_try_wait(bar, parity); ++spin)
-    if (spin > (1u << 28)) __trap();   // a protocol bug must end the kernel, not hang the GPU
-}
-
-template <int EPI>
-__global__ void __launch_bounds__(TCP_THREADS, 1)
-k_tc_gemm_p(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_whi,
-            const __grid_constant__ CUtensorMap map_wlo, const TcGemmP p) {
-  extern __shared__ uint8_t tc_smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + TC_STAGES * TC_STAGE_BYTES);
-  uint64_t* full = bars;                          // [stages]  TMA bytes landed
-  uint64_t* split = bars + TC_STAGES;             // [stages]  A split into hi / lo
-  uint64_t* empty = bars + 2 * TC_STAGES;         // [stages]  MMAs of the stage retired
-  uint64_t* accum_full = bars + 3 * TC_STAGES;    // [2]       all MMAs of a tile retired
-  uint64_t* accum_empty = bars + 3 * TC_STAGES + 2;  // [2]    epilogue has read the accumulator
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * TC_STAGES + 4);
+  uint64_t* empty = bars + TC_STAGES;     // [stages]  both warpgroups' MMAs of the stage retired
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_per_utt = (p.F + TC_BM - 1) / TC_BM;
@@ -241,20 +86,12 @@ k_tc_gemm_p(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
   const int nk = p.K / TC_BK;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < TC_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&split[s], 128); mbar_init(&empty[s], 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&accum_full[a], 1); mbar_init(&accum_empty[a], 128); }
+    for (int s = 0; s < TC_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], TC_CONSUMERS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 5) {  // TMEM: two 128-column fp32 accumulators
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(2 * TC_BN));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 4) {
+  if (warp == TC_CONSUMERS / 32) {
     // ===================== TMA producer
     if (lane == 0) {
       int g = 0;
@@ -274,88 +111,71 @@ k_tc_gemm_p(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
         }
       }
     }
-  } else if (warp == 5) {
-    // ===================== MMA issuer
-    const uint32_t idesc = umma_idesc_tf32(TC_BM, TC_BN);
-    int g = 0, i = 0;
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++i) {
-      const int acc = i & 1, use = i >> 1;
-      if (use > 0) mbar_wait_or_trap(&accum_empty[acc], (use - 1) & 1);   // the epilogue of tile i-2 has drained this accumulator
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + acc * TC_BN;
-      for (int t = 0; t < nk; ++t, ++g) {
-        const int s = g % TC_STAGES, it = g / TC_STAGES;
-        mbar_wait_or_trap(&split[s], it & 1);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t st = smem_u32(smem + s * TC_STAGE_BYTES);
-          const uint32_t a_hi = st, a_lo = st + TC_TILE_BYTES, w_hi = st + 2 * TC_TILE_BYTES, w_lo = st + 3 * TC_TILE_BYTES;
-#pragma unroll
-          for (int k = 0; k < TC_BK / 8; ++k) {
-            const uint32_t ko = k * 32;
-            umma_tf32(tmem_d, umma_desc_sw128(a_hi + ko), umma_desc_sw128(w_hi + ko), idesc, (t | k) ? 1u : 0u);
-            umma_tf32(tmem_d, umma_desc_sw128(a_hi + ko), umma_desc_sw128(w_lo + ko), idesc, 1u);
-            umma_tf32(tmem_d, umma_desc_sw128(a_lo + ko), umma_desc_sw128(w_hi + ko), idesc, 1u);
-          }
-          umma_commit(&empty[s]);
-          if (t == nk - 1) umma_commit(&accum_full[acc]);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp < 4) {
-    // ===================== workers: split A into tf32 hi / lo
-    int g = 0;
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
-      for (int t = 0; t < nk; ++t, ++g) {
-        const int s = g % TC_STAGES, it = g / TC_STAGES;
-        mbar_wait_or_trap(&full[s], it & 1);
-        float4* a = reinterpret_cast<float4*>(smem + s * TC_STAGE_BYTES);
-        float4* lo = reinterpret_cast<float4*>(smem + s * TC_STAGE_BYTES + TC_TILE_BYTES);
-#pragma unroll
-        for (int j = 0; j < TC_TILE_BYTES / 16 / 128; ++j) {
-          const int e = threadIdx.x + 128 * j;
-          const float4 v = a[e];
-          float4 h, l;
-          h.x = to_tf32(v.x); h.y = to_tf32(v.y); h.z = to_tf32(v.z); h.w = to_tf32(v.w);
-          l.x = to_tf32(v.x - h.x); l.y = to_tf32(v.y - h.y); l.z = to_tf32(v.z - h.z); l.w = to_tf32(v.w - h.w);
-          a[e] = h; lo[e] = l;
-        }
-        fence_async_smem();
-        mbar_arrive(&split[s]);
-      }
-    }
-  } else {
-    // ===================== epilogue warps 6..9: TMEM lane quarter = warp % 4
-    const int quarter = warp & 3;
-    int i = 0;
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++i) {
-      const int nt = tile % n_tiles, mt = tile / n_tiles;
-      const int b = mt / tiles_per_utt, f0 = (mt % tiles_per_utt) * TC_BM, n0 = nt * TC_BN;
-      const int acc = i & 1, use = i >> 1;
-      mbar_wait_or_trap(&accum_full[acc], use & 1);
-      tc_fence_after();
-      const int f = f0 + quarter * 32 + lane;
-      const size_t m = (size_t)b * p.F + f;
-#pragma unroll 1
-      for (int cb = 0; cb < TC_BN / 32; ++cb) {
-        uint32_t r[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * TC_BN + cb * 32;
-        TC_TMEM_LD32(r, taddr);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (cb == TC_BN / 32 - 1) {   // every column of this accumulator is in registers: hand it back before the stores
-          tc_fence_before();
-          mbar_arrive(&accum_empty[acc]);
-        }
-        if (f < p.F) tc_epi_store<EPI>(p, r, m, n0 + cb * 32);
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(2 * TC_BN));
+
+  // ===================== consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64)
+  const int wg = warp >> 2, tid = threadIdx.x & 127;
+  const uint32_t half_off = wg * (TC_TILE_BYTES / 2);   // 64 rows x 128 B: whole 1024-byte swizzle atoms
+  int g = 0;
+  for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
+    const int nt = tile % n_tiles, mt = tile / n_tiles;
+    const int b = mt / tiles_per_utt, f0 = (mt % tiles_per_utt) * TC_BM, n0 = nt * TC_BN;
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    int prev = 0;
+    for (int t = 0; t < nk; ++t, ++g) {
+      const int s = g % TC_STAGES, it = g / TC_STAGES;
+      mbar_wait_or_trap(&full[s], it & 1);
+      uint8_t* st = smem + s * TC_STAGE_BYTES;
+      float4* a = reinterpret_cast<float4*>(st + half_off);
+      float4* lo = reinterpret_cast<float4*>(st + TC_TILE_BYTES + half_off);
+#pragma unroll
+      for (int j = 0; j < TC_TILE_BYTES / 2 / 16 / 128; ++j) {
+        const int e = tid + 128 * j;  // elementwise: the swizzle pattern is the same in both tiles
+        const float4 v = a[e];
+        float4 h, l;
+        h.x = to_tf32(v.x); h.y = to_tf32(v.y); h.z = to_tf32(v.z); h.w = to_tf32(v.w);
+        l.x = to_tf32(v.x - h.x); l.y = to_tf32(v.y - h.y); l.z = to_tf32(v.z - h.z); l.w = to_tf32(v.w - h.w);
+        a[e] = h; lo[e] = l;
+      }
+      fence_async_smem();  // generic-proxy writes -> visible to the tensor core (async proxy)
+      warpgroup_bar(2 + wg);
+      const uint32_t su = smem_u32(st);
+      const uint32_t a_hi = su + half_off, a_lo = su + TC_TILE_BYTES + half_off;
+      const uint32_t w_hi = su + 2 * TC_TILE_BYTES, w_lo = su + 3 * TC_TILE_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TC_BK / 8; ++k) {
+        const uint32_t ko = k * 32;  // 8 tf32 = 32 bytes inside the 128-byte swizzle row
+        wgmma_tf32_n128(acc, wgmma_desc_sw128(a_hi + ko), wgmma_desc_sw128(w_hi + ko), (t | k) ? 1u : 0u);
+        wgmma_tf32_n128(acc, wgmma_desc_sw128(a_hi + ko), wgmma_desc_sw128(w_lo + ko), 1u);
+        wgmma_tf32_n128(acc, wgmma_desc_sw128(a_lo + ko), wgmma_desc_sw128(w_hi + ko), 1u);
+      }
+      wgmma_commit();
+      if (t > 0) {  // the previous stage's MMAs have retired: hand it back to the producer
+        wgmma_wait<1>();
+        mbar_arrive(&empty[prev]);
+      }
+      prev = s;
+    }
+    wgmma_wait<0>();
+    wgmma_fence_operands(acc);
+    mbar_arrive(&empty[prev]);
+    // epilogue straight from the accumulator registers (layout: see wgmma_tf32_n*)
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int f = f0 + r0 + 8 * h;
+      if (f >= p.F) continue;
+      const size_t m = (size_t)b * p.F + f;
+#pragma unroll
+      for (int j = 0; j < TC_BN / 8; ++j) {
+        const int n = n0 + 8 * j + 2 * (lane & 3);
+        if (n < p.N) tc_epi_store2<EPI>(p, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], m, n);
+      }
+    }
   }
 }
 
@@ -384,9 +204,9 @@ template <int EPI>
 inline int tc_gemm_launch(cudaStream_t s, const float* A, int lda, int B, int F, int N, int K, int taps, int Cin, int dil,
                           int pad, const float* W_hi, const float* W_lo, const float* bias, const float* gamma,
                           const float* res, int ldres, float* C, int ldc) {
-  const bool persistent = getenv("CTB_TC_NONPERSISTENT") == nullptr;   // the one-tile-per-CTA twin stays for cross-checks
-  { int arc = persistent ? ensure_smem_attr((const void*)k_tc_gemm_p<EPI>, TC_SMEM_BYTES)
-                         : ensure_smem_attr((const void*)k_tc_gemm<EPI>, TC_SMEM_BYTES); if (arc) return arc; }
+  // CTB_TC_NONPERSISTENT=1: one tile per CTA, the schedule the persistent one is cross-checked against
+  const bool persistent = getenv("CTB_TC_NONPERSISTENT") == nullptr;
+  { int arc = ensure_smem_attr((const void*)k_tc_gemm<EPI>, TC_SMEM_BYTES); if (arc) return arc; }
   CUtensorMap ma, mh, ml;
   const cuuint64_t adims[3] = {(cuuint64_t)lda, (cuuint64_t)F, (cuuint64_t)B};
   const cuuint64_t astr[2] = {(cuuint64_t)lda * 4, (cuuint64_t)F * lda * 4};
@@ -401,15 +221,10 @@ inline int tc_gemm_launch(cudaStream_t s, const float* A, int lda, int B, int F,
   TcGemmP p{};
   p.N = N; p.K = K; p.taps = taps; p.Cin = Cin; p.dil = dil; p.pad = pad; p.F = F; p.B = B;
   p.bias = bias; p.gamma = gamma; p.res = res; p.ldres = ldres; p.C = C; p.ldc = ldc;
-  if (persistent) {
-    static int sms = 0;
-    if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
-    const int total = ((N + TC_BN - 1) / TC_BN) * B * ((F + TC_BM - 1) / TC_BM);
-    k_tc_gemm_p<EPI><<<std::min(total, sms), TCP_THREADS, TC_SMEM_BYTES, s>>>(ma, mh, ml, p);
-  } else {
-    dim3 grid((N + TC_BN - 1) / TC_BN, B * ((F + TC_BM - 1) / TC_BM));
-    k_tc_gemm<EPI><<<grid, TC_THREADS, TC_SMEM_BYTES, s>>>(ma, mh, ml, p);
-  }
+  static int sms = 0;
+  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
+  const int total = ((N + TC_BN - 1) / TC_BN) * B * ((F + TC_BM - 1) / TC_BM);
+  k_tc_gemm<EPI><<<persistent ? std::min(total, sms) : total, TC_THREADS, TC_SMEM_BYTES, s>>>(ma, mh, ml, p);
   CTB_LAUNCH_CHECK();
   return CTB_OK;
 }

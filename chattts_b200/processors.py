@@ -117,7 +117,7 @@ def build_sampler_config(logits_processors: Sequence[object], temperature: Seque
             cfg.greedy = 2 if getattr(proc, "exclude_eos", False) else 1
         else:
             raise TypeError(
-                f"unsupported logits processor {type(proc).__name__}: the B200 sampler implements the reference's "
+                f"unsupported logits processor {type(proc).__name__}: the GPU sampler implements the reference's "
                 "repetition-penalty / top-p / top-k filters only (no host fallback)")
         if kind <= stage:
             raise ValueError("logits processors must be ordered penalty -> top-p -> top-k (reference core.py:649)")

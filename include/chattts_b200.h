@@ -1,5 +1,5 @@
 /*
- * chattts_b200 - C ABI of the B200-native (sm_100a) ChatTTS hot paths.
+ * chattts_b200 - C ABI of the H100-native (sm_90a) ChatTTS hot paths.
  *
  * The reference (2noise/ChatTTS) has no FFI boundary: its seams are Python objects
  * (SURVEY.md 8b).  This header is the boundary a maintainer binds from Python with

@@ -118,6 +118,125 @@ def gen_dvae_encode():
     print("dvae encode", tuple(ids.shape), "frames", mel.shape[1], "min margin", float(margin.min()))
 
 
+ENCODE_CASES = ((1.3, 0), (2.0, 1))     # (seconds, seed) of synth_speech_like
+ENCODE_CHANNELS = 96                     # encoder-output channels stored per case (a fixed, seeded sample of 1024)
+
+
+def encode_channel_sample() -> torch.Tensor:
+    return torch.randperm(1024, generator=torch.Generator().manual_seed(1024))[:ENCODE_CHANNELS].sort().values
+
+
+def gen_reference_checks():
+    """What tests/test_oracle_vs_reference.py compares the oracle against: the reference's GPT.generate (audio and text),
+    Embed, DVAE decode branch and encode-side modules, on seeded inputs."""
+    from chattts_b200.synth import synth_speech_like
+    from oracle.ref_models import build_reference_dvae_encoder
+
+    out = {}
+    gs, es = synth_gpt_state(0), synth_embed_state(1)
+    gpt, embed = build_reference_gpt(gs, es)
+    for tag, lengths, seed in (("audio_b1", [16], 1234), ("audio_b3", [5, 12, 9], 42)):
+        ids, mask, tmask = synth_prompt_batch(lengths, seed=1)
+        ref = reference_generate(gpt, embed, ids, mask, tmask, temperature=[0.3] * 4, eos_token=625,
+                                 max_new_token=12, min_new_token=12, manual_seed=seed)
+        out[tag + "_ids"] = torch.stack(list(ref.ids)).numpy()
+        out[tag + "_hiddens"] = torch.stack(list(ref.hiddens)).numpy()
+    ids, mask, tmask = synth_prompt_batch([7, 4], seed=3)
+    ref = reference_generate(gpt, embed, ids, mask, tmask, temperature=[0.7], eos_token=21001, max_new_token=6,
+                             repetition_penalty=1.0, num_code=21178, infer_text=True, return_hidden=False, manual_seed=7)
+    out["text_n"] = np.array([len(t) for t in ref.ids])
+    out["text_ids"] = np.full((2, 6), -1, np.int64)
+    for b, t in enumerate(ref.ids):
+        out["text_ids"][b, : len(t)] = t.reshape(len(t), -1)[:, 0].numpy()
+    ids, mask, tmask = synth_prompt_batch([6, 3], seed=5)
+    tmask[0, -2:] = False  # mixed text / code positions (audio prompt splice, tokenizer.py:115-124)
+    ids[0, -2:] = torch.randint(0, 626, (2, 4), generator=torch.Generator().manual_seed(5))
+    with torch.no_grad():
+        out.update(embed_ids=ids.numpy(), embed_tmask=tmask.numpy(), embed_out=embed(ids, tmask).numpy())
+
+    cfg = Config()
+    st = synth_dvae_state(2, cfg.decoder, cfg.decoder.idim)
+    x = torch.randn(2, 768, 20, generator=torch.Generator().manual_seed(20))
+    with torch.no_grad():
+        out.update(dvae_x=x.numpy(), dvae_mel=build_reference_dvae(st, cfg.decoder, cfg.decoder.idim)(x.clone(), "decode").numpy())
+
+    st = synth_dvae_state(3, cfg.dvae.decoder, cfg.dvae.decoder.idim, cfg.dvae.vq, encoder=cfg.dvae.encoder)
+    ref = build_reference_dvae_encoder(st, cfg.dvae.decoder, cfg.dvae.encoder, cfg.dvae.decoder.idim)
+    chans = encode_channel_sample()
+    for i, (seconds, seed) in enumerate(ENCODE_CASES):
+        wav = synth_speech_like(seconds, seed)
+        with torch.inference_mode():
+            mel = ref.preprocessor_mel(wav.clone())
+            x = ref.encoder(ref.downsample_conv(mel / ref.coef.view(100, 1)).unsqueeze(0))
+        out[f"encode{i}_mel"] = mel.numpy()
+        out[f"encode{i}_x_shape"] = np.array(x.shape)
+        out[f"encode{i}_x"] = x[:, chans].numpy()
+    np.savez_compressed(os.path.join(OUT, "reference_checks.npz"), **out)
+    print("reference checks", {k: v.shape for k, v in out.items()})
+
+
+def gen_host_checks():
+    """What the host-logic tests compare against: the reference's Normalizer, Speaker and Tokenizer outputs, and its
+    spk_stat asset (tests/golden/host_reference.json, tests/golden/speaker_apply.npz)."""
+    import json
+    import re
+    import tempfile
+
+    from oracle.ref_import import REFERENCE_ROOT, load_reference
+
+    import sys
+
+    sys.path.insert(0, os.path.dirname(OUT))  # the inputs are defined by the tests that use these outputs
+    import test_norm_audio as tn
+    import test_speaker as ts
+    import test_tokenizer as tt
+
+    load_reference()
+    from ChatTTS.model.speaker import Speaker as RefSpeaker
+    from ChatTTS.model.tokenizer import Tokenizer as RefTokenizer
+    from ChatTTS.norm import Normalizer as RefNormalizer
+
+    out = {}
+    cfg_src = open(os.path.join(REFERENCE_ROOT, "ChatTTS", "config", "config.py"), encoding="utf-8").read()
+    out["spk_stat"] = re.search(r'spk_stat: str = \(\s*"([^"]+)"', cfg_src).group(1)
+
+    fd, path = tempfile.mkstemp(suffix=".json")
+    with os.fdopen(fd, "w", encoding="utf-8") as f:
+        json.dump(tn.HOMO, f, ensure_ascii=False)
+    norm = RefNormalizer(path)
+    os.unlink(path)
+    assert norm.register("en", lambda s: s.upper())
+    out["normalizer"] = [[text, nm, homo, lang, norm(text, nm, homo, lang)]
+                         for text in tn.CASES for nm in (True, False) for homo in (True, False) for lang in (None, "zh", "en")]
+
+    ref = object.__new__(RefSpeaker)
+    emb, vec, ids = ts.apply_inputs()
+    applied = ref.apply(emb.clone(), vec, ids, 21143, torch.device("cpu"))
+    np.savez_compressed(os.path.join(OUT, "speaker_apply.npz"), applied=applied.numpy())
+    deco = []
+    for spk_emb, smp in ((None, None), ("x", None), ("x", "sample text")):
+        t = ["  hi [Stts] there[spk_emb] ", "[empty_spk]b"]
+        deco.append([spk_emb, smp, ref.decorate_code_prompts(t, "[speed_5]", smp, spk_emb), t])
+    out["decorate_code"] = deco
+    out["decorate_text"] = ref.decorate_text_prompts(["a", "b"], "[oral_2]")
+
+    with tempfile.TemporaryDirectory() as d:
+        import pathlib
+
+        tok = RefTokenizer(tt._write_vocab(pathlib.Path(d)))
+        if not hasattr(tok._tokenizer, "encode_plus"):       # API drift: transformers >= 5 removed encode_plus
+            tok._tokenizer.encode_plus = tok._tokenizer.__call__
+        out["tokenizer_attrs"] = [tok.len, tok.spk_emb_ids, tok.break_0_ids, tok.eos_token]
+        enc = []
+        for prompt in (None, tt.PROMPT):
+            enc.append([[str(x.dtype), x.tolist()] for x in tok.encode(list(tt.TEXTS), 4, prompt=None if prompt is None else prompt.clone())])
+        out["tokenizer_encode"] = enc
+        out["tokenizer_decode"] = tok.decode(tt.DECODE_SEQ)
+    with open(os.path.join(OUT, "host_reference.json"), "w", encoding="utf-8") as f:
+        json.dump(out, f, ensure_ascii=False, indent=0)
+    print("host checks", len(out["normalizer"]), "normalizer cases")
+
+
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     torch.set_num_threads(8)
@@ -125,3 +244,5 @@ if __name__ == "__main__":
     gen_sampler()
     gen_dvae()
     gen_dvae_encode()
+    gen_reference_checks()
+    gen_host_checks()

@@ -1,4 +1,4 @@
-"""CPU checks of the C-ABI boundary: the library builds for sm_100a, loads, and exports every
+"""CPU checks of the C-ABI boundary: the library builds for sm_90a, loads, and exports every
 symbol include/chattts_b200.h declares (no compute calls - there is no GPU here)."""
 import ctypes
 import os

@@ -161,7 +161,7 @@ def test_c4_full_size_batch64_rows_vs_oracle():
 
 
 def test_tensor_core_path_matches_fma_path():
-    """The tcgen05 3xTF32 GEMMs (default) against the plain fp32 FMA GEMMs (CTB_DECODER_FMA=1) on the same
+    """The wgmma 3xTF32 GEMMs (default) against the plain fp32 FMA GEMMs (CTB_DECODER_FMA=1) on the same
     handle configuration: fp32-equivalent accuracy is the contract of the hi/lo split."""
     import os
 
@@ -205,8 +205,8 @@ def test_windowed_decode_equals_slices_of_the_full_decode(use_decoder):
 
 
 def test_persistent_gemm_equals_the_one_tile_per_cta_twin_bit_for_bit():
-    """k_tc_gemm_p (persistent CTAs, two TMEM accumulators, weights split hi/lo on the fly) runs the same MMAs in the same
-    order as k_tc_gemm (CTB_TC_NONPERSISTENT=1: one tile per CTA, pre-split weight copies): identical mel and waveform."""
+    """k_tc_gemm with persistent CTAs (one per SM, walking tiles) runs the same MMAs in the same order as with one tile per
+    CTA (CTB_TC_NONPERSISTENT=1): identical mel and waveform."""
     import os
 
     from chattts_b200.decoder import DVAE, Vocos

@@ -1,5 +1,8 @@
-"""Host pre/post-processing (SURVEY.md 8f N4): chattts_b200.norm.Normalizer against the reference's own Normalizer where
-/root/reference is present, and against expectations generated from it (committed below) everywhere else."""
+"""Host pre/post-processing (SURVEY.md 8f N4): chattts_b200.norm.Normalizer against the reference's own Normalizer, through
+its outputs on every case and flag combination (tests/golden/host_reference.json, written by oracle/make_golden.py)."""
+import json
+import os
+
 import numpy as np
 import pytest
 
@@ -18,39 +21,18 @@ CASES = [
     "nested [a[b]c] text",
     "数字123和符号@#都会被删除",
 ]
-# produced by the reference's Normalizer (ChatTTS/norm.py) with the homophone map above, default flags, in the build container
-EXPECTED = None
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "host_reference.json")
 
 
-def _ref():
-    from oracle.ref_import import load_reference, reference_available
-
-    if not reference_available():
-        pytest.skip("/root/reference not present on this box")
-    load_reference()
-    import json
-    import os
-    import tempfile
-
-    from ChatTTS.norm import Normalizer as RefNormalizer
-
-    fd, path = tempfile.mkstemp(suffix=".json")
-    with os.fdopen(fd, "w", encoding="utf-8") as f:
-        json.dump(HOMO, f, ensure_ascii=False)
-    return RefNormalizer(path)
-
-
-@pytest.mark.reference
 def test_normalizer_matches_reference_on_every_case_and_flag_combination():
-    ref = _ref()
+    expected = json.load(open(GOLD, encoding="utf-8"))["normalizer"]
     ours = Normalizer(homophones=HOMO)
-    up = lambda s: s.upper()
-    assert ref.register("en", up) and ours.register("en", up)
-    for text in CASES:
-        for norm in (True, False):
-            for homo in (True, False):
-                for lang in (None, "zh", "en"):
-                    assert ours(text, norm, homo, lang) == ref(text, norm, homo, lang), (text, norm, homo, lang)
+    assert ours.register("en", lambda s: s.upper())
+    cases = [(text, norm, homo, lang) for text in CASES for norm in (True, False) for homo in (True, False)
+             for lang in (None, "zh", "en")]
+    assert [e[:4] for e in expected] == [list(c) for c in cases]
+    for (text, norm, homo, lang), e in zip(cases, expected):
+        assert ours(text, norm, homo, lang) == e[4], (text, norm, homo, lang)
 
 
 def test_normalizer_golden_strings():

@@ -1,4 +1,8 @@
-"""Pin oracle/gpt_oracle.py against the reference's own code (build container only)."""
+"""Pin oracle/gpt_oracle.py and oracle/dvae_oracle.py against the reference's own code, through what the reference computed
+on seeded inputs (tests/golden/reference_checks.npz, written by oracle/make_golden.py gen_reference_checks)."""
+import os
+
+import numpy as np
 import pytest
 import torch
 
@@ -6,55 +10,41 @@ from chattts_b200.prompts import synth_prompt_batch
 from chattts_b200.synth import synth_embed_state, synth_gpt_state
 from oracle.gpt_oracle import GPTOracle, SamplerParams
 
-pytestmark = [pytest.mark.reference]
+GOLD = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_checks.npz"))
 
 
 @pytest.fixture(scope="module")
-def models():
-    from oracle.ref_models import build_reference_gpt
-
-    gs, es = synth_gpt_state(0), synth_embed_state(1)
-    gpt, embed = build_reference_gpt(gs, es)
-    return gpt, embed, GPTOracle(gs, es)
+def orc():
+    return GPTOracle(synth_gpt_state(0), synth_embed_state(1))
 
 
 @pytest.mark.parametrize("lengths,seed", [([16], 1234), ([5, 12, 9], 42)])
-def test_audio_generate_ids_and_hiddens(models, lengths, seed):
-    from oracle.ref_models import reference_generate
-
-    gpt, embed, orc = models
+def test_audio_generate_ids_and_hiddens(orc, lengths, seed):
+    tag = f"audio_b{len(lengths)}"
     ids, mask, tmask = synth_prompt_batch(lengths, seed=1)
-    ref = reference_generate(gpt, embed, ids, mask, tmask, temperature=[0.3] * 4, eos_token=625,
-                             max_new_token=12, min_new_token=12, manual_seed=seed)
     out = orc.generate(orc.embed_prompt(ids, tmask), ids, torch.tensor([0.3] * 4), 625, attention_mask=mask,
                        max_new_token=12, min_new_token=12, sampler=SamplerParams(), return_hidden=True,
                        manual_seed=seed)
     for b in range(len(lengths)):
-        assert torch.equal(ref.ids[b], out.ids[b]), (b, ref.ids[b], out.ids[b])
-        assert (ref.hiddens[b] - out.hiddens[b]).abs().max() < 2e-5
+        ref_ids, ref_h = GOLD[tag + "_ids"][b], GOLD[tag + "_hiddens"][b]
+        assert np.array_equal(ref_ids, out.ids[b].numpy()), (b, ref_ids, out.ids[b])
+        assert np.abs(ref_h - out.hiddens[b].numpy()).max() < 2e-5
 
 
-def test_text_generate_ids(models):
-    from oracle.ref_models import reference_generate
-
-    gpt, embed, orc = models
+def test_text_generate_ids(orc):
     ids, mask, tmask = synth_prompt_batch([7, 4], seed=3)
-    ref = reference_generate(gpt, embed, ids, mask, tmask, temperature=[0.7], eos_token=21001, max_new_token=6,
-                             repetition_penalty=1.0, num_code=21178, infer_text=True, return_hidden=False,
-                             manual_seed=7)
     out = orc.generate(orc.embed_prompt(ids, tmask), ids, torch.tensor([0.7]), 21001, attention_mask=mask,
                        max_new_token=6, sampler=SamplerParams(repetition_penalty=1.0, penalty_max_ids=21178),
                        infer_text=True, manual_seed=7)
     for b in range(2):
-        assert torch.equal(ref.ids[b], out.ids[b])
+        n = int(GOLD["text_n"][b])
+        assert np.array_equal(out.ids[b].reshape(-1).numpy(), GOLD["text_ids"][b, :n])
 
 
-def test_embed_prompt_matches(models):
-    gpt, embed, orc = models
-    ids, mask, tmask = synth_prompt_batch([6, 3], seed=5)
-    tmask[0, -2:] = False  # mixed text / code positions (audio prompt splice, tokenizer.py:115-124)
-    ids[0, -2:] = torch.randint(0, 626, (2, 4))
-    assert torch.equal(embed(ids, tmask), orc.embed_prompt(ids, tmask))
+def test_embed_prompt_matches(orc):
+    ids, tmask = torch.from_numpy(GOLD["embed_ids"]), torch.from_numpy(GOLD["embed_tmask"])
+    assert not bool(tmask[0, -2:].any()) and bool(tmask[0, :-2].all())  # mixed text / code positions
+    assert np.array_equal(orc.embed_prompt(ids, tmask).numpy(), GOLD["embed_out"])
 
 
 def test_dvae_decoder_branch_matches_reference():
@@ -62,39 +52,34 @@ def test_dvae_decoder_branch_matches_reference():
     from chattts_b200.config import Config
     from chattts_b200.synth import synth_dvae_state
     from oracle.dvae_oracle import dvae_decode
-    from oracle.ref_models import build_reference_dvae
 
     cfg = Config()
     st = synth_dvae_state(2, cfg.decoder, cfg.decoder.idim)
-    ref = build_reference_dvae(st, cfg.decoder, cfg.decoder.idim)
-    x = torch.randn(2, 768, 20)
-    with torch.no_grad():
-        want = ref(x.clone(), "decode")
-    got = dvae_decode(x, st)
+    want = torch.from_numpy(GOLD["dvae_mel"])
+    got = dvae_decode(torch.from_numpy(GOLD["dvae_x"]), st)
     assert want.shape == got.shape == (2, 100, 40)
     assert (want - got).abs().max() < 1e-5 * max(1.0, float(want.abs().max()))
 
 
 def test_dvae_encode_branch_matches_reference_up_to_the_quantizer():
     """Encode branch (dvae.py:265-274) piece by piece against the reference's own modules: MelSpectrogramFeatures
-    (torchaudio), downsample_conv, encoder stack.  The FSQ quantiser itself is third-party and absent (parity unpinned)."""
+    (torchaudio), downsample_conv, encoder stack (a fixed sample of its output channels is stored).  The FSQ quantiser
+    itself is third-party and absent (parity unpinned)."""
     from chattts_b200.config import Config
     from chattts_b200.synth import synth_dvae_state, synth_speech_like
     from oracle.dvae_oracle import dvae_encode, mel_features
-    from oracle.ref_models import build_reference_dvae_encoder
+    from oracle.make_golden import ENCODE_CASES, encode_channel_sample
 
     cfg = Config()
     st = synth_dvae_state(3, cfg.dvae.decoder, cfg.dvae.decoder.idim, cfg.dvae.vq, encoder=cfg.dvae.encoder)
-    ref = build_reference_dvae_encoder(st, cfg.dvae.decoder, cfg.dvae.encoder, cfg.dvae.decoder.idim)
-    for seconds, seed in ((1.3, 0), (2.0, 1)):
+    chans = encode_channel_sample()
+    for i, (seconds, seed) in enumerate(ENCODE_CASES):
         wav = synth_speech_like(seconds, seed)
-        with torch.inference_mode():
-            mel_ref = ref.preprocessor_mel(wav.clone())
-            x_ref = ref.encoder(ref.downsample_conv(mel_ref / ref.coef.view(100, 1)).unsqueeze(0))
+        mel_ref, x_ref = torch.from_numpy(GOLD[f"encode{i}_mel"]), torch.from_numpy(GOLD[f"encode{i}_x"])
         mel = mel_features(wav)
         assert mel.shape == mel_ref.shape == (100, wav.numel() // 256 + 1)
         assert (mel - mel_ref).abs().max() < 2e-4          # same stft; the filterbank matmul runs in another order
         ids, margin, _, x = dvae_encode(wav, st, return_parts=True)
-        assert x.shape == x_ref.shape == (1, 1024, (wav.numel() // 256 + 1) // 2)
-        assert (x - x_ref).abs().max() < 1e-4 * max(1.0, float(x_ref.abs().max()))
+        assert tuple(x.shape) == tuple(GOLD[f"encode{i}_x_shape"]) == (1, 1024, (wav.numel() // 256 + 1) // 2)
+        assert (x[:, chans] - x_ref).abs().max() < 1e-4 * max(1.0, float(x_ref.abs().max()))
         assert ids.shape == (1, 4, x.shape[2]) and int(ids.min()) >= 0 and int(ids.max()) < 625

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Development check of the dataflow decode step (csrc/flow.cuh) on a B200: ids/hiddens against the older one-kernel
+"""Development check of the dataflow decode step (csrc/flow.cuh) on the GPU: ids/hiddens against the older one-kernel
 step (CTB_NO_FLOW=1) for B = 1..4, per-step time for a sweep of replica counts, per-phase trace of CTA 0.
 
     python tools/flow_check.py [--steps 96] [--tokens 512]
