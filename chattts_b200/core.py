@@ -201,6 +201,74 @@ class Chat:
             return stripped
         return next(res_gen)
 
+    def infer_continuous(self, texts, params_infer_code=None, use_decoder=True, slots=None, stream=False, lang=None,
+                         skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
+                         params_refine_text=None):
+        """Synthesise many texts with continuous batching (``GPT.generate_continuous``): each text is one request,
+        ``params_infer_code`` is one ``InferCodeParams`` for all texts or a list with one per text (speaker, seed,
+        temperature, top-P/K, penalty, token limits).  Generator of ``(index, wav)`` in completion order; ``wav`` is
+        what ``infer([texts[index]], split_text=False, skip_refine_text=True)`` returns for that text with its params.
+        Normalisation and the optional text refinement run as in ``infer``."""
+        if stream:
+            raise ValueError("infer_continuous: stream=True is not supported; each waveform is yielded when complete")
+        if isinstance(texts, str):
+            texts = [texts]
+        texts = list(texts)
+        if isinstance(params_infer_code, (list, tuple)):
+            if len(params_infer_code) != len(texts):
+                raise ValueError("params_infer_code: one InferCodeParams per text")
+            params = list(params_infer_code)
+        else:
+            params = [params_infer_code or Chat.InferCodeParams()] * len(texts)
+        return self._infer_continuous(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
+                                      do_homophone_replacement, params_refine_text or Chat.RefineTextParams())
+
+    def _infer_continuous(self, texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
+                          do_homophone_replacement, params_refine_text):
+        assert self.has_loaded(use_decoder=use_decoder)
+        self.context.set(False)
+        if not texts:
+            return
+        texts = [self.normalizer(t, do_text_normalization, do_homophone_replacement, lang) for t in texts]
+        if not skip_refine_text:
+            tokens = []
+            for lo in range(0, len(texts), self.gpt.max_batch):
+                refined = self._refine_text(texts[lo: lo + self.gpt.max_batch], self.device, params_refine_text)
+                tokens += [i[i.less(self.tokenizer.break_0_ids)] for i in refined.ids]
+                refined.destroy()
+            texts = self.tokenizer.decode(tokens)
+        requests = [self._code_request(t, p) for t, p in zip(texts, params)]
+        thr = np.float32(1e-5)
+        with torch.no_grad():
+            for i, out in self.gpt.generate_continuous(requests, slots=slots, return_hidden=use_decoder,
+                                                       context=self.context):
+                res = out.hiddens if use_decoder else out.ids
+                wav = self._decode_to_wavs(res, use_decoder)[0] if int(res[0].shape[0]) > 0 else np.zeros(0, np.float32)
+                out.destroy()
+                yield i, wav[np.abs(wav) > thr]  # quirk Q20, as infer() returns it
+
+    def _code_request(self, text, params):
+        """The request ``_infer_code([text], ...)`` would decode as a batch of one."""
+        from .engine import Request
+
+        temperature = params.temperature if isinstance(params.temperature, list) else [params.temperature] * self.config.gpt.num_vq
+        input_ids, attention_mask, text_mask = self.tokenizer.encode(
+            self.speaker.decorate_code_prompts([text], params.prompt, params.txt_smp, params.spk_emb),
+            self.config.gpt.num_vq,
+            prompt=(self.speaker.decode_prompt(params.spk_smp) if params.spk_smp is not None else None),
+            device=self.device_gpt)
+        num_code = self.config.gpt.num_audio_tokens - 1
+        warpers, processors = gen_logits(num_code=num_code, top_P=params.top_P, top_K=params.top_K,
+                                         repetition_penalty=params.repetition_penalty)
+        emb = self.embed(input_ids, text_mask)
+        if params.spk_emb is not None:
+            self.speaker.apply(emb, params.spk_emb, input_ids, self.tokenizer.spk_emb_ids, self.gpt.device_gpt)
+        valid = attention_mask[0].to(torch.bool).cpu()
+        return Request(emb=emb[0][valid.to(emb.device)], temperature=temperature, eos_token=num_code,
+                       max_new_token=params.max_new_token, min_new_token=params.min_new_token,
+                       logits_processors=(*processors, *warpers), manual_seed=params.manual_seed,
+                       ensure_non_empty=params.ensure_non_empty)
+
     def interrupt(self):
         self.context.set(True)
 

@@ -93,6 +93,13 @@ struct ctb_gpt {
   CUtensorMap m_hcode, m_htext;
   CUtensorMap m_x[2][2], m_attn[2][2], m_h[2][2];            // [npad16|32][hi|lo]
   bool use_graph;
+  // ---- slot engine (ctb_gpt_engine_*): B = S slots, max_new = the per-slot capacity of ids_out / hiddens_out
+  int engine;                 // 1 between ctb_gpt_engine_begin and the next ctb_gpt_begin
+  int phase;                  // rows the heads / sampler / finalize serve: RS_RUNNING (decode) or RS_PENDING (admission)
+  RowState* rows;             // [Bpad] per-slot loop state
+  ctb_sampler_config* cfgs;   // [max_batch] per-slot sampling parameters
+  float* eng_noise;           // [max_batch * num_vq, num_audio] per-slot Exp(1) rows
+  int* eng_slot;              // [max_batch] slot of each prompt of the admission being prefilled
 };
 
 extern "C" int ctb_abi_version(void) { return CTB_ABI_VERSION; }
@@ -321,7 +328,8 @@ extern "C" int ctb_gpt_destroy(ctb_gpt* h) {
   void* ptrs[] = {h->x, h->qbuf, h->attn, h->mlp, h->logits, h->kv, h->part, h->block_table, h->seq_len,
                   h->pos, h->counter, h->end_idx, h->idx, h->active, h->finish, h->st, h->tc_wqkv, h->tc_wgu,
                   h->tc_heads_code, h->tc_heads_text, h->x_hi, h->x_lo, h->attn_hi, h->attn_lo, h->h_hi, h->h_lo, h->bar, h->trace, h->flow_arena, h->flow_epoch, h->gw_hi, h->gw_lo, h->pf_resid, h->pf_xn, h->pf_qkv, h->pf_q,
-                  h->pf_attn, h->pf_gu, h->pf_h, h->pf_ones, h->pf_zeros, h->pf_npre, h->pf_nvalid};
+                  h->pf_attn, h->pf_gu, h->pf_h, h->pf_ones, h->pf_zeros, h->pf_npre, h->pf_nvalid,
+                  h->rows, h->cfgs, h->eng_noise, h->eng_slot};
   delete[] h->m_wqkv; delete[] h->m_wo; delete[] h->m_wgu; delete[] h->m_wd;
   for (void* p : ptrs) if (p) cudaFree(p);
   delete h;
@@ -409,12 +417,16 @@ static int launch_down_small(int bt, const GemvP& p, cudaStream_t s) {
   }
 }
 
-static int launch_sample(const SampleP& sp, cudaStream_t s) {
+template <bool ENGINE>
+static int launch_sample_t(const SampleP& sp, cudaStream_t s) {
   const size_t smem = (size_t)sp.V * sizeof(float) + 2 * 1024 * sizeof(uint32_t);
-  { int rc = ensure_smem_attr((const void*)k_sample, (int)smem); if (rc) return rc; }
-  CTB_CUDA(launch_pdl(k_sample, dim3(sp.rows), dim3(SAMPLE_THREADS), smem, s, sp));
+  { int rc = ensure_smem_attr((const void*)k_sample<ENGINE>, (int)smem); if (rc) return rc; }
+  CTB_CUDA(launch_pdl(k_sample<ENGINE>, dim3(sp.rows), dim3(SAMPLE_THREADS), smem, s, sp));
   CTB_LAUNCH_CHECK();
   return CTB_OK;
+}
+static int launch_sample(const SampleP& sp, cudaStream_t s) {
+  return sp.rstate != nullptr ? launch_sample_t<true>(sp, s) : launch_sample_t<false>(sp, s);
 }
 
 struct StepCtx {
@@ -460,8 +472,9 @@ static int launch_layer_kernel(ctb_gpt* h, const StepCtx& x, int l, int kind, cu
     case 1: {
       AttnP a = x.a;
       a.kv = kvl;
-      // context after this call <= T0 + max_new: only launch splits that can be populated
-      const int max_ctx = std::min(c.max_context, h->T0 + h->max_new);
+      // context after this call <= T0 + max_new: only launch splits that can be populated (a slot engine's rows may
+      // reach max_context)
+      const int max_ctx = h->engine ? c.max_context : std::min(c.max_context, h->T0 + h->max_new);
       // enough CTAs to fill the chip twice; a CTA walks chunks c, c + grid.x, ... with a running softmax,
       // so large batches need no cross-CTA merge at all
       const int want = (2 * g_num_sms + c.num_heads * h->B - 1) / (c.num_heads * h->B);
@@ -499,6 +512,7 @@ static int launch_heads(ctb_gpt* h, const StepCtx& x, cudaStream_t s) {
   hp.K = c.hidden_size; hp.nrows = rpi * V; hp.ntasks = (hp.nrows + 1) / 2; hp.xin = h->x;
   hp.normw = h->W + h->lay.final_norm; hp.out = h->logits; hp.rows_per_item = rpi; hp.V = V;
   hp.hidden_out = h->hiddens_out; hp.hidden_stride = h->max_new * c.hidden_size;
+  hp.rows = h->engine ? h->rows : nullptr; hp.want = h->phase;
   return launch_gemv<EPI_HEADS>(x.bt, hp, x.ntiles, s);
 }
 
@@ -510,6 +524,7 @@ static int launch_sampler(ctb_gpt* h, const StepCtx& x, cudaStream_t s) {
   sp.V = h->infer_text ? c.num_text_tokens : c.num_audio_tokens;
   sp.rows_per_item = rpi; sp.cfg = h->sampler; sp.q_noise = h->q_noise; sp.gen_ids = h->ids_out;
   sp.gen_stride = h->max_new; sp.gen_inner = c.num_vq; sp.out_idx = h->idx;
+  if (h->engine) { sp.rstate = h->rows; sp.cfgs = h->cfgs; sp.want = h->phase; sp.q_noise = h->eng_noise; }
   return launch_sample(sp, s);
 }
 
@@ -569,6 +584,7 @@ static int launch_heads_tc(ctb_gpt* h, cudaStream_t s) {
   p.K = c.hidden_size; p.kslice = p.K / CS_HEADS; p.nrows = rpi * V; p.xraw = h->x;
   p.logits = h->logits; p.rows_per_item = rpi; p.V = V; p.hidden_out = h->hiddens_out;
   p.hidden_stride = h->max_new * c.hidden_size; p.final_norm_w = h->W + h->lay.final_norm;
+  p.rows = h->engine ? h->rows : nullptr; p.want = h->phase;
   return launch_tc<DE_HEADS, CS_HEADS>(npad, h->infer_text ? h->m_htext : h->m_hcode, h->m_x[n][0], h->m_x[n][1], p, s);
 }
 
@@ -663,12 +679,29 @@ static int launch_step_flow(ctb_gpt* h, int col, bool sample, cudaStream_t s, in
   }
 }
 
-static bool use_flow(const ctb_gpt* h) { return h->flow_ok && !h->use_tc && h->B <= h->flow_max_batch; }
+// the one-kernel steps (k_flow, k_step) keep the batch's loop counters in LoopState: never used by a slot engine
+static bool use_flow(const ctb_gpt* h) { return h->flow_ok && !h->engine && !h->use_tc && h->B <= h->flow_max_batch; }
 // decode steps of audio generation at B <= 2 sample inside k_flow and run many steps per launch
 static bool flow_ink(const ctb_gpt* h) {
   static const bool off = getenv("CTB_FLOW_NO_INK") != nullptr;
   return !off && use_flow(h) && !h->infer_text && h->B <= 2 && h->cfg.num_audio_tokens <= FL_VPAD &&
          h->B * h->cfg.num_vq <= FL_SROWS && h->cfg.num_vq <= 8;
+}
+
+static int launch_finalize(ctb_gpt* h, cudaStream_t s) {
+  const ctb_gpt_config& c = h->cfg;
+  FinalP fp{};
+  fp.st = h->st; fp.B = h->B; fp.rows_per_item = h->infer_text ? 1 : c.num_vq; fp.num_vq = c.num_vq;
+  fp.max_new = h->max_new; fp.eos = h->sampler.eos_token; fp.idx = h->idx; fp.ids_out = h->ids_out;
+  fp.finish = h->finish; fp.end_idx = h->end_idx;
+  if (h->engine) {
+    fp.rows = h->rows; fp.want = h->phase;
+    CTB_CUDA(launch_pdl(k_finalize_rows, dim3(1), dim3(256), 0, s, fp));
+  } else {
+    CTB_CUDA(launch_pdl(k_finalize, dim3(1), dim3(256), 0, s, fp));
+  }
+  CTB_LAUNCH_CHECK();
+  return CTB_OK;
 }
 
 // One loop iteration.  col >= 0: prefill column `col` of the prompt; col < 0: decode step.
@@ -679,7 +712,7 @@ static int enqueue_step(ctb_gpt* h, int col, bool sample, cudaStream_t s) {
   const int decode = col < 0;
   int rc;
 
-  if (use_flow(h) || (h->mega_ok && !h->use_tc && h->B <= h->mega_max_batch)) {
+  if (use_flow(h) || (h->mega_ok && !h->engine && !h->use_tc && h->B <= h->mega_max_batch)) {
     // small batches: the whole step (input -> 20 layers -> heads) is one persistent cooperative kernel
     if ((rc = use_flow(h) ? launch_step_flow(h, col, sample, s) : launch_step_mega(h, col, sample, s))) return rc;
     if (!sample) return CTB_OK;
@@ -702,6 +735,7 @@ static int enqueue_step(ctb_gpt* h, int col, bool sample, cudaStream_t s) {
   ip.infer_text = h->infer_text;
   ip.x = h->x; ip.seq_len = h->seq_len; ip.pos = h->pos; ip.active = h->active;
   ip.x_hi = h->use_tc ? h->x_hi : nullptr; ip.x_lo = h->use_tc ? h->x_lo : nullptr;
+  ip.rows = h->engine ? h->rows : nullptr;
   CTB_CUDA(launch_pdl(k_input, dim3(h->B), dim3(256), 0, s, ip));
   CTB_LAUNCH_CHECK();
 
@@ -713,14 +747,7 @@ static int enqueue_step(ctb_gpt* h, int col, bool sample, cudaStream_t s) {
   if (!sample) return CTB_OK;
   if ((rc = h->use_tc ? launch_heads_tc(h, s) : launch_heads(h, x, s))) return rc;
   if ((rc = launch_sampler(h, x, s))) return rc;
-
-  FinalP fp{};
-  fp.st = h->st; fp.B = h->B; fp.rows_per_item = h->infer_text ? 1 : c.num_vq; fp.num_vq = c.num_vq;
-  fp.max_new = h->max_new; fp.eos = h->sampler.eos_token; fp.idx = h->idx; fp.ids_out = h->ids_out;
-  fp.finish = h->finish; fp.end_idx = h->end_idx;
-  CTB_CUDA(launch_pdl(k_finalize, dim3(1), dim3(256), 0, s, fp));
-  CTB_LAUNCH_CHECK();
-  return CTB_OK;
+  return launch_finalize(h, s);
 }
 
 // Measurement hook (bench.py roofline): launch ONE kernel kind for every layer (20 launches over
@@ -791,18 +818,21 @@ static int prefill_reserve(ctb_gpt* h, size_t rows) {
   return CTB_OK;
 }
 
-static int prefill_batched(ctb_gpt* h, cudaStream_t s) {
+// B left-padded prompts [B, T0] -> decode rows slot[b] (slot == nullptr: rows 0..B-1), then the first token of every
+// row in state h->phase (all h->B rows of a static batch; the admitted slots of a slot engine)
+static int prefill_batched(ctb_gpt* h, int B, int T0, const float* emb, const uint8_t* mask, const int* slot,
+                           cudaStream_t s) {
   const ctb_gpt_config& c = h->cfg;
   const ctb_gpt_layout& L = h->lay;
-  const int B = h->B, T0 = h->T0, M = B * T0;
+  const int M = B * T0;
   const int d = c.hidden_size, I = c.intermediate_size, nqkv = (c.num_heads + 2 * c.num_kv_heads) * c.head_dim;
   int rc;
   if ((rc = prefill_reserve(h, (size_t)M))) return rc;
-  CTB_CUDA(cudaMemcpyAsync(h->pf_resid, h->emb, (size_t)M * d * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  k_prefill_positions<<<B, 32, 0, s>>>(h->mask, h->pf_npre, h->pf_nvalid, T0);
+  CTB_CUDA(cudaMemcpyAsync(h->pf_resid, emb, (size_t)M * d * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  k_prefill_positions<<<B, 32, 0, s>>>(mask, h->pf_npre, h->pf_nvalid, T0);
   CTB_LAUNCH_CHECK();
   PrefillP pp{};
-  pp.B = B; pp.T0 = T0; pp.Hq = c.num_heads; pp.Hkv = c.num_kv_heads; pp.hd = c.head_dim; pp.d = d; pp.mask = h->mask;
+  pp.B = B; pp.T0 = T0; pp.Hq = c.num_heads; pp.Hkv = c.num_kv_heads; pp.hd = c.head_dim; pp.d = d; pp.mask = mask; pp.slot = slot;
   pp.npre = h->pf_npre; pp.nvalid = h->pf_nvalid; pp.qkv = h->pf_qkv; pp.q = h->pf_q; pp.block_table = h->block_table;
   pp.pages_per_row = h->pages_per_row; pp.rope_cos = h->W + L.rope_cos; pp.rope_sin = h->W + L.rope_sin;
   pp.permute_qk = h->use_tc ? 1 : 0; pp.attn = h->pf_attn; pp.scaling = 1.0f / sqrtf((float)c.head_dim);
@@ -833,18 +863,13 @@ static int prefill_batched(ctb_gpt* h, cudaStream_t s) {
                                            h->pf_zeros, h->pf_ones, h->pf_resid, d, h->pf_resid, d))) return rc;
   }
   k_prefill_finish<<<B, 256, 0, s>>>(h->pf_resid, h->x, h->use_tc ? h->x_hi : nullptr, h->use_tc ? h->x_lo : nullptr,
-                                     h->pf_nvalid, h->seq_len, h->pos, h->active, T0, d);
+                                     h->pf_nvalid, h->seq_len, h->pos, h->active, T0, d, slot);
   CTB_LAUNCH_CHECK();
   // first token: heads -> sampler -> finalize (the i == 0 iteration of gpt.py:394)
   const StepCtx x = make_ctx(h, 0);
   if ((rc = h->use_tc ? launch_heads_tc(h, s) : launch_heads(h, x, s))) return rc;
   if ((rc = launch_sampler(h, x, s))) return rc;
-  FinalP fp{};
-  fp.st = h->st; fp.B = B; fp.rows_per_item = h->infer_text ? 1 : c.num_vq; fp.num_vq = c.num_vq; fp.max_new = h->max_new;
-  fp.eos = h->sampler.eos_token; fp.idx = h->idx; fp.ids_out = h->ids_out; fp.finish = h->finish; fp.end_idx = h->end_idx;
-  CTB_CUDA(launch_pdl(k_finalize, dim3(1), dim3(256), 0, s, fp));
-  CTB_LAUNCH_CHECK();
-  return CTB_OK;
+  return launch_finalize(h, s);
 }
 
 // Pages for B rows of up to `tokens` tokens each: grow the pool if needed (page = 16 tokens x K|V x heads x 64 floats per
@@ -889,6 +914,7 @@ extern "C" int ctb_gpt_begin(ctb_gpt* h, int32_t B, int32_t T0, const float* emb
   if (sampler->min_tokens_to_keep < 1) return set_err(CTB_ERR_ARG, "min_tokens_to_keep must be >= 1");
   cudaStream_t s = (cudaStream_t)stream;
   h->B = B; h->T0 = T0; h->max_new = max_new_token; h->infer_text = infer_text ? 1 : 0;
+  h->engine = 0; h->phase = RS_RUNNING;
   h->use_tc = h->tc_ready && B >= h->tc_min_batch;
   h->sampler = *sampler; h->q_noise = q_noise_dev; h->emb = emb_dev; h->mask = mask_dev;
   h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev;
@@ -917,7 +943,7 @@ extern "C" int ctb_gpt_begin(ctb_gpt* h, int32_t B, int32_t T0, const float* emb
   // keeps every row's last prompt token in the last column, like the reference's batches)
   if (h->pf_enabled && T0 >= 8 && T0 <= 1024) {
     // whole prompt as token-parallel wgmma GEMMs (prefill.cuh)
-    if ((rc = prefill_batched(h, s))) return rc;
+    if ((rc = prefill_batched(h, B, T0, emb_dev, mask_dev, nullptr, s))) return rc;
   } else {
     // short prompts: walk the columns through the decode kernels (left padding keeps every row's last prompt
     // token in the last column, like the reference's batches)
@@ -934,7 +960,8 @@ extern "C" int ctb_gpt_decode(ctb_gpt* h, int32_t n_steps, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;
   int rc;
   // ids_out / hiddens_out hold max_new steps and the KV pages max_context tokens: never enqueue past either
-  n_steps = std::min(n_steps, h->max_new - h->steps_enqueued);
+  // (a slot engine's rows stop at their own max_new, checked against both at admission)
+  if (!h->engine) n_steps = std::min(n_steps, h->max_new - h->steps_enqueued);
   if (n_steps <= 0) return CTB_OK;
   h->steps_enqueued += n_steps;
   if (flow_ink(h)) {
@@ -968,6 +995,119 @@ extern "C" int ctb_gpt_decode(ctb_gpt* h, int32_t n_steps, void* stream) {
       return rc;
     }
   }
+  return CTB_OK;
+}
+
+// ------------------------------------------------------------------ slot engine (continuous batching)
+extern "C" int ctb_gpt_engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t* ids_out_dev,
+                                    float* hiddens_out_dev, void* stream) {
+  if (!h || !ids_out_dev) return set_err(CTB_ERR_ARG, "null argument");
+  const ctb_gpt_config& c = h->cfg;
+  if (S < 2 || S > c.max_batch) return set_err(CTB_ERR_ARG, "S=%d outside [2,%d]", S, c.max_batch);
+  if (max_new_cap < 1 || max_new_cap >= c.max_context)
+    return set_err(CTB_ERR_ARG, "max_new_cap=%d outside [1,%d)", max_new_cap, c.max_context);
+  cudaStream_t s = (cudaStream_t)stream;
+  int rc;
+  if (!h->rows) {
+    if ((rc = dalloc(&h->rows, (size_t)h->bpad_max))) return rc;
+    if ((rc = dalloc(&h->cfgs, (size_t)c.max_batch))) return rc;
+    if ((rc = dalloc(&h->eng_noise, (size_t)c.max_batch * c.num_vq * c.num_audio_tokens))) return rc;
+    if ((rc = dalloc(&h->eng_slot, (size_t)c.max_batch))) return rc;
+  }
+  // S rows of audio codes, each slot owning a fixed page range of max_context tokens; PDL chain (S <= 8) or wgmma
+  // step (S >= 9) - the one-kernel steps are never selected (use_flow, enqueue_step)
+  h->engine = 1; h->phase = RS_RUNNING;
+  h->B = S; h->T0 = 0; h->max_new = max_new_cap; h->infer_text = 0;
+  h->use_tc = h->tc_ready && S >= h->tc_min_batch;
+  h->q_noise = h->eng_noise; h->emb = nullptr; h->mask = nullptr;
+  h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev;
+  if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
+  if ((rc = kv_reserve(h, S, c.max_context, s))) return rc;
+  static const LoopState idle_state = {0, 1, 0, 0, 0};  // no running slot: decode steps are no-ops
+  CTB_CUDA(cudaMemcpyAsync(h->st, &idle_state, sizeof(LoopState), cudaMemcpyHostToDevice, s));
+  CTB_CUDA(cudaMemsetAsync(h->rows, 0, sizeof(RowState) * h->bpad_max, s));  // every slot RS_IDLE
+  CTB_CUDA(cudaMemsetAsync(h->seq_len, 0, sizeof(int) * h->bpad_max, s));
+  CTB_CUDA(cudaMemsetAsync(h->pos, 0, sizeof(int) * h->bpad_max, s));
+  CTB_CUDA(cudaMemsetAsync(h->active, 0, h->bpad_max, s));
+  CTB_CUDA(cudaMemsetAsync(h->finish, 0, h->bpad_max, s));
+  CTB_CUDA(cudaMemsetAsync(h->end_idx, 0, sizeof(int) * h->bpad_max, s));
+  CTB_CUDA(cudaMemsetAsync(h->counter, 0, sizeof(int) * c.max_batch * c.num_heads, s));
+  CTB_CUDA(cudaMemsetAsync(h->x, 0, sizeof(float) * h->bpad_max * c.hidden_size, s));
+  if (h->use_tc) {
+    const size_t d = c.hidden_size, I = c.intermediate_size;
+    float* z768[] = {h->x_hi, h->x_lo, h->attn_hi, h->attn_lo};
+    for (float* zp : z768) CTB_CUDA(cudaMemsetAsync(zp, 0, 32 * d * sizeof(float), s));
+    CTB_CUDA(cudaMemsetAsync(h->h_hi, 0, 32 * I * sizeof(float), s));
+    CTB_CUDA(cudaMemsetAsync(h->h_lo, 0, 32 * I * sizeof(float), s));
+  }
+  CTB_CUDA(cudaStreamSynchronize(s));  // idle_state is read by the copy engine
+  h->started = 1;
+  h->steps_enqueued = 0;
+  return CTB_OK;
+}
+
+extern "C" int ctb_gpt_engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0, const float* emb_dev,
+                                    const uint8_t* mask_dev, const ctb_sampler_config* samplers,
+                                    const float* q_noise_dev, const int32_t* max_new, void* stream) {
+  if (!h || !slots || !emb_dev || !mask_dev || !samplers || !max_new) return set_err(CTB_ERR_ARG, "null argument");
+  if (!h->engine) return set_err(CTB_ERR_STATE, "ctb_gpt_engine_begin has not been called");
+  const ctb_gpt_config& c = h->cfg;
+  const int S = h->B;
+  if (n < 1 || n > S) return set_err(CTB_ERR_ARG, "n=%d outside [1,%d]", n, S);
+  if (T0 < 8 || T0 > 1024) return set_err(CTB_ERR_ARG, "T0=%d outside [8,1024]: left-pad shorter prompts to 8", T0);
+  cudaStream_t s = (cudaStream_t)stream;
+  std::vector<RowState> rows((size_t)h->bpad_max);
+  CTB_CUDA(cudaMemcpyAsync(rows.data(), h->rows, sizeof(RowState) * rows.size(), cudaMemcpyDeviceToHost, s));
+  CTB_CUDA(cudaStreamSynchronize(s));
+  std::vector<char> taken((size_t)S, 0);
+  for (int i = 0; i < n; ++i) {
+    const int b = slots[i];
+    const ctb_sampler_config& sc = samplers[i];
+    if (b < 0 || b >= S || taken[b]) return set_err(CTB_ERR_ARG, "slot %d out of range or repeated", b);
+    taken[b] = 1;
+    if (rows[b].state == RS_RUNNING || rows[b].state == RS_PENDING)
+      return set_err(CTB_ERR_STATE, "slot %d is still generating", b);
+    if (max_new[i] < 1 || max_new[i] > h->max_new || T0 + max_new[i] > c.max_context)
+      return set_err(CTB_ERR_ARG, "slot %d: max_new=%d (capacity %d) with T0=%d exceeds max_context=%d", b, max_new[i],
+                     h->max_new, T0, c.max_context);
+    if (sc.past_window > 31 || sc.past_window < 0) return set_err(CTB_ERR_ARG, "past_window out of range");
+    if (sc.min_tokens_to_keep < 1) return set_err(CTB_ERR_ARG, "min_tokens_to_keep must be >= 1");
+    RowState& r = rows[b];
+    r.n_gen = 0; r.step = 0; r.state = RS_PENDING; r.max_new = max_new[i]; r.has_noise = q_noise_dev != nullptr;
+    r.eos = sc.eos_token;
+  }
+  // host arrays are copied before this call returns (synchronised below), so the caller may free them at once
+  CTB_CUDA(cudaMemcpyAsync(h->rows, rows.data(), sizeof(RowState) * rows.size(), cudaMemcpyHostToDevice, s));
+  CTB_CUDA(cudaMemcpyAsync(h->eng_slot, slots, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
+  const size_t nrow = (size_t)c.num_vq * c.num_audio_tokens;
+  for (int i = 0; i < n; ++i) {
+    const int b = slots[i];
+    CTB_CUDA(cudaMemcpyAsync(h->cfgs + b, samplers + i, sizeof(ctb_sampler_config), cudaMemcpyHostToDevice, s));
+    if (q_noise_dev)
+      CTB_CUDA(cudaMemcpyAsync(h->eng_noise + b * nrow, q_noise_dev + i * nrow, nrow * sizeof(float),
+                               cudaMemcpyDeviceToDevice, s));
+    CTB_CUDA(cudaMemsetAsync(h->finish + b, 0, 1, s));
+    CTB_CUDA(cudaMemsetAsync(h->end_idx + b, 0, sizeof(int), s));
+  }
+  CTB_CUDA(cudaStreamSynchronize(s));
+  // prompts -> their slots' pages, then heads / sampler / finalize for the RS_PENDING rows only
+  h->phase = RS_PENDING;
+  const int rc = prefill_batched(h, n, T0, emb_dev, mask_dev, h->eng_slot, s);
+  h->phase = RS_RUNNING;
+  return rc;
+}
+
+extern "C" int ctb_gpt_engine_status(ctb_gpt* h, ctb_gpt_status* out, int32_t* state_host, int32_t* end_idx_host,
+                                     uint8_t* finish_host, void* stream) {
+  if (!h || !out) return set_err(CTB_ERR_ARG, "null argument");
+  if (!h->engine) return set_err(CTB_ERR_STATE, "ctb_gpt_engine_begin has not been called");
+  cudaStream_t s = (cudaStream_t)stream;
+  std::vector<RowState> rows((size_t)h->B);
+  CTB_CUDA(cudaMemcpyAsync(rows.data(), h->rows, sizeof(RowState) * h->B, cudaMemcpyDeviceToHost, s));
+  int rc = ctb_gpt_status_query(h, out, end_idx_host, finish_host, stream);  // synchronises `stream`
+  if (rc) return rc;
+  if (state_host)
+    for (int b = 0; b < h->B; ++b) state_host[b] = rows[b].state;
   return CTB_OK;
 }
 

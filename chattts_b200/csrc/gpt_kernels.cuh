@@ -20,6 +20,19 @@ struct LoopState {
   int err;             // != 0: a device-side watchdog fired (flow.cuh); reported by ctb_gpt_status_query
 };
 
+// Slot engine (ctb_gpt_engine_*): every batch row is a slot holding one request at its own point of generation, so
+// the loop counters live per row.  The static path passes rows == nullptr and keeps using LoopState's counters.
+enum RowStateKind { RS_IDLE = 0, RS_RUNNING = 1, RS_FINISHED = 2, RS_PENDING = 3 /* prefilled, first token not yet sampled */ };
+struct RowState {
+  int n_gen;      // tokens this row has appended to ids_out
+  int step;       // loop iterations this row has run (its own gpt.py `i`)
+  int state;      // RowStateKind
+  int max_new;    // the row finishes after this many tokens
+  int has_noise;  // 1: Exp(1) rows in the engine's noise buffer (seeded request); 0: device Philox
+  int eos;
+  int pad[2];
+};
+
 constexpr int KC = 768;        // K chunk staged in shared memory (= hidden size of the model)
 constexpr int GEMV_WARPS = 8;  // warps per CTA, one 2-row task per warp
 constexpr int ATT_CHUNK = 128;      // keys per k_attn chunk: 8 warps x 16 keys, all K/V rows of a chunk in flight at once
@@ -55,6 +68,8 @@ struct GemvP {
   int V;
   float* hidden_out;     // [B, max_new, d] or nullptr
   int hidden_stride;     // max_new * d
+  const RowState* rows;  // slot engine: only rows in state `want` get logits / hidden states; nullptr: every row
+  int want;
 };
 
 // KV pool layout of one layer: [page][2 (K,V)][Hkv][16 tokens][hd]
@@ -165,10 +180,20 @@ __global__ void __launch_bounds__(GEMV_WARPS * 32) k_gemv(const GemvP p) {
     __syncthreads();
     if (EPI == EPI_HEADS && p.hidden_out != nullptr && blockIdx.x == 0) {
       // last_hidden_state of this step (gpt.py:430-436), written once per batch tile
-      const int step = ldg_cg(&p.st->n_gen);
-      for (int i = tid; i < nb * KC; i += GEMV_WARPS * 32) {
-        const int b = i / KC, k = i % KC;
-        p.hidden_out[(size_t)(bbase + b) * p.hidden_stride + (size_t)step * KC + k] = xs[i];
+      if (p.rows == nullptr) {
+        const int step = ldg_cg(&p.st->n_gen);
+        for (int i = tid; i < nb * KC; i += GEMV_WARPS * 32) {
+          const int b = i / KC, k = i % KC;
+          p.hidden_out[(size_t)(bbase + b) * p.hidden_stride + (size_t)step * KC + k] = xs[i];
+        }
+      } else {
+        for (int b = 0; b < nb; ++b) {
+          const RowState* r = p.rows + bbase + b;
+          if (ldg_cg(&r->state) != p.want) continue;
+          const int step = ldg_cg(&r->n_gen);
+          for (int k = tid; k < KC; k += GEMV_WARPS * 32)
+            p.hidden_out[(size_t)(bbase + b) * p.hidden_stride + (size_t)step * KC + k] = xs[b * KC + k];
+        }
       }
     }
   }
@@ -249,6 +274,7 @@ __global__ void __launch_bounds__(GEMV_WARPS * 32) k_gemv(const GemvP p) {
       const float sg = __fdiv_rn(v0, __fadd_rn(1.0f, expf(-v0)));
       p.out[(size_t)b * p.I + task] = __fmul_rn(sg, v1);
     } else {  // EPI_HEADS: logits rows ordered (b, q) like gpt.py:459-464
+      if (p.rows != nullptr && ldg_cg(&p.rows[b].state) != p.want) continue;
       const int q0 = r0 / p.V, c0 = r0 % p.V;
       p.out[((size_t)b * p.rows_per_item + q0) * p.V + c0] = v0;
       if (r1_valid) {
@@ -453,6 +479,7 @@ struct InputP {
   int* seq_len;           // [Bpad]
   int* pos;               // [Bpad]
   uint8_t* active;        // [Bpad]
+  const RowState* rows;   // slot engine: decode only running rows, each at its own n_gen; nullptr: static batch
 };
 
 #ifdef CTB_GPT_KERNELS_IMPL
@@ -469,7 +496,18 @@ __global__ void k_input(const InputP p) {
     for (int k = threadIdx.x; k < p.d; k += blockDim.x) x[k] = act ? e[k] : 0.f;
   } else {
     act = true;
-    const int32_t* id = p.ids_out + ((size_t)b * p.max_new + (ldg_cg(&p.st->n_gen) - 1)) * p.num_vq;
+    int n_gen;
+    if (p.rows != nullptr) {
+      // idle / finished slots append no KV and keep their position: only the active flag is written
+      if (ldg_cg(&p.rows[b].state) != RS_RUNNING) {
+        if (threadIdx.x == 0) p.active[b] = 0;
+        return;
+      }
+      n_gen = ldg_cg(&p.rows[b].n_gen);
+    } else {
+      n_gen = ldg_cg(&p.st->n_gen);
+    }
+    const int32_t* id = p.ids_out + ((size_t)b * p.max_new + (n_gen - 1)) * p.num_vq;
     if (p.infer_text) {
       const float* e = p.emb_text + (size_t)ldg_cg(&id[0]) * p.d;
       for (int k = threadIdx.x; k < p.d; k += blockDim.x) x[k] = e[k];
@@ -673,9 +711,16 @@ struct SampleP {
   int gen_stride, gen_inner;
   int n_gen_fixed, step_fixed;  // used when st == nullptr (stand-alone ctb_sample)
   int32_t* out_idx;      // [rows]
+  // slot engine (k_sample<true>): counters, noise flag and state per item from `rstate`, the sampling parameters of
+  // item b from cfgs[b] (device memory, so a captured decode graph serves every admitted request); only items in
+  // state `want` are sampled
+  const RowState* rstate;
+  const ctb_sampler_config* cfgs;
+  int want;
 };
 
 constexpr int SAMPLE_THREADS = 1024;
+template <bool ENGINE>
 __global__ void k_sample(const SampleP p);
 
 struct FinalP {
@@ -684,7 +729,10 @@ struct FinalP {
   const int32_t* idx;    // [B*rpi]
   int32_t* ids_out;      // [B, max_new, num_vq]
   uint8_t* finish; int32_t* end_idx;
+  RowState* rows;        // k_finalize_rows only
+  int want;
 };
 __global__ void k_finalize(const FinalP p);
+__global__ void k_finalize_rows(const FinalP p);
 
 }  // namespace ctb

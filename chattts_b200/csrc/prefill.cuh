@@ -52,6 +52,7 @@ struct PrefillP {
   int permute_qk;           // tensor-core decode path keeps q/k rows pair-interleaved (tc_decode.cuh)
   float* attn;              // [B*T0, Hq*hd]
   float scaling;
+  const int* slot;          // [B] decode row (block-table row) of prompt b; nullptr: row b
 };
 
 // RoPE + KV append for every valid prompt token; grid (T0, B), 256 threads over (which, head, j)
@@ -61,7 +62,7 @@ __global__ void k_prefill_rope_kv(const PrefillP p) {
   const int pos = p.npre[(size_t)b * p.T0 + c];
   const int half = p.hd / 2, nq = p.Hq * p.hd, nkv = p.Hkv * p.hd;
   const float* src = p.qkv + ((size_t)b * p.T0 + c) * (nq + 2 * nkv);
-  const int page = p.block_table[b * p.pages_per_row + pos / kPageTokens];
+  const int page = p.block_table[(p.slot ? p.slot[b] : b) * p.pages_per_row + pos / kPageTokens];
   const int npairs = (p.Hq + 2 * p.Hkv) * half;
   for (int i = threadIdx.x; i < npairs; i += blockDim.x) {
     const int which = i < p.Hq * half ? 0 : (i < (p.Hq + p.Hkv) * half ? 1 : 2);
@@ -103,8 +104,8 @@ __global__ void __launch_bounds__(PF_ATT_WARPS * 32) k_prefill_attn(const Prefil
   extern __shared__ float pa_smem[];
   float* s_p = pa_smem + (size_t)warp * p.T0;      // [T0] scores / probabilities of this warp's query
   const int hk = h / (p.Hq / p.Hkv);
-  const int* bt = p.block_table + b * p.pages_per_row;
-  const int c0 = p.T0 - n;                         // first valid column (left padding)
+  const int* bt = p.block_table + (p.slot ? p.slot[b] : b) * p.pages_per_row;
+  const int c0 = p.T0 - n;                        // first valid column (left padding)
   const size_t qrow = ((size_t)b * p.T0 + c0 + t) * p.Hq * HD + h * HD;
   float4 q[HD / 4];
 #pragma unroll
@@ -156,26 +157,27 @@ __global__ void k_prefill_positions(const uint8_t* __restrict__ mask, int* __res
   }
 }
 
-// hand the last prompt column's residual to the decode-loop state
+// hand the last prompt column's residual to the decode-loop state of decode row slot[b] (slot == nullptr: row b)
 __global__ void k_prefill_finish(const float* __restrict__ resid, float* __restrict__ x, float* __restrict__ x_hi,
                                  float* __restrict__ x_lo, const int* __restrict__ nvalid, int* __restrict__ seq_len,
-                                 int* __restrict__ pos, uint8_t* __restrict__ active, int T0, int d) {
-  const int b = blockIdx.x;
+                                 int* __restrict__ pos, uint8_t* __restrict__ active, int T0, int d,
+                                 const int* __restrict__ slot) {
+  const int b = blockIdx.x, sb = slot ? slot[b] : b;
   const float* r = resid + ((size_t)b * T0 + T0 - 1) * d;
   for (int k = threadIdx.x; k < d; k += blockDim.x) {
     const float v = r[k];
-    x[(size_t)b * d + k] = v;
+    x[(size_t)sb * d + k] = v;
     if (x_hi != nullptr) {
       uint32_t hb, lb;
       asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(v));
       asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(v - __uint_as_float(hb)));
-      x_hi[(size_t)b * d + k] = __uint_as_float(hb);
-      x_lo[(size_t)b * d + k] = __uint_as_float(lb);
+      x_hi[(size_t)sb * d + k] = __uint_as_float(hb);
+      x_lo[(size_t)sb * d + k] = __uint_as_float(lb);
     }
   }
   if (threadIdx.x == 0) {
     const int n = nvalid[b];
-    seq_len[b] = n; pos[b] = n - 1; active[b] = 1;
+    seq_len[sb] = n; pos[sb] = n - 1; active[sb] = 1;
   }
 }
 

@@ -44,10 +44,22 @@ __device__ __forceinline__ float block_max_f(float v, float* s_red) {
 
 }  // namespace
 
+template <bool ENGINE>
 __global__ void __launch_bounds__(SAMPLE_THREADS) k_sample(const SampleP p) {
   pdl_trigger();
   pdl_wait();
   if (p.check_finished && ldg_cg(&p.st->all_finished)) return;
+  const int row = blockIdx.x, V = p.V, rpi = p.rows_per_item;
+  const int item = row / rpi, qi = row % rpi;
+  __shared__ ctb_sampler_config s_cfg;
+  if (ENGINE) {
+    if (ldg_cg(&p.rstate[item].state) != p.want) return;  // CTA-uniform
+    static_assert(sizeof(ctb_sampler_config) % 4 == 0, "config is copied as words");
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(p.cfgs + item);
+    for (int i = threadIdx.x; i < (int)(sizeof(ctb_sampler_config) / 4); i += SAMPLE_THREADS)
+      reinterpret_cast<uint32_t*>(&s_cfg)[i] = __ldg(src + i);
+    __syncthreads();
+  }
   extern __shared__ __align__(16) unsigned char smem_raw[];
   float* s_x = reinterpret_cast<float*>(smem_raw);                 // [V] processed logits
   uint32_t* s_key = reinterpret_cast<uint32_t*>(s_x + p.V);        // [2][1024] sort path only
@@ -58,16 +70,16 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) k_sample(const SampleP p) {
   __shared__ uint32_t s_thr;
 
   const int tid = threadIdx.x;
-  const int row = blockIdx.x, V = p.V, rpi = p.rows_per_item;
-  const int item = row / rpi, qi = row % rpi;
-  const int n_gen = p.st ? ldg_cg(&p.st->n_gen) : p.n_gen_fixed;
-  const int step = p.st ? ldg_cg(&p.st->step) : p.step_fixed;
-  const ctb_sampler_config& c = p.cfg;
+  const int n_gen = ENGINE ? ldg_cg(&p.rstate[item].n_gen) : (p.st ? ldg_cg(&p.st->n_gen) : p.n_gen_fixed);
+  const int step = ENGINE ? ldg_cg(&p.rstate[item].step) : (p.st ? ldg_cg(&p.st->step) : p.step_fixed);
+  const ctb_sampler_config& c = ENGINE ? s_cfg : p.cfg;
   const float* lg = p.logits + (size_t)row * V;
+  // a slot's request is sampled as if it were decoded alone (B = 1): its logits row index is the codebook index
+  const int prow = ENGINE ? qi : row;
 
   // ---- S2 window of the last <= past_window generated ids of this (item, codebook) row
   int nwin = 0;
-  const bool pen = c.penalty_on && row < c.penalty_max_ids;
+  const bool pen = c.penalty_on && prow < c.penalty_max_ids;
   if (pen) {
     nwin = min(n_gen, c.past_window);
     if (tid < nwin) s_win[tid] = ldg_cg(&p.gen_ids[((size_t)item * p.gen_stride + (n_gen - nwin + tid)) * p.gen_inner + qi]);
@@ -224,12 +236,13 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) k_sample(const SampleP p) {
   den2 = block_sum_d(den2, s_redd);
   const float den2f = (float)den2;
 
+  const bool noise = ENGINE ? ldg_cg(&p.rstate[item].has_noise) != 0 : p.q_noise != nullptr;
   float best = -1.f;
   int besti = 0x7fffffff;
   for (int v = tid; v < V; v += SAMPLE_THREADS) {
     const float pr = __fdiv_rn(expf(s_x[v] - mx2), den2f);
-    const float qn = p.q_noise ? p.q_noise[(size_t)row * V + v]
-                               : philox_exp1(c.philox_seed, (uint32_t)row, (uint32_t)v, (uint32_t)step);
+    const float qn = noise ? p.q_noise[(size_t)row * V + v]
+                           : philox_exp1(c.philox_seed, (uint32_t)prow, (uint32_t)v, (uint32_t)step);
     const float r = __fdiv_rn(pr, qn);
     if (r > best) { best = r; besti = v; }  // ascending v within a thread: first max wins
   }
@@ -285,5 +298,45 @@ __global__ void k_finalize(const FinalP p) {
     p.st->step = step0 + 1;
   }
 }
+
+// Slot-engine counterpart of k_finalize: every row in state `want` (RS_RUNNING in a decode step, RS_PENDING after an
+// admission's prefill) writes its token at its own n_gen and advances its own counters; a row ends at EOS or at its
+// own max_new.  A B = 1 request that samples EOS first ends empty (end_idx 0, finish 1): the reference's first-step
+// return (gpt.py:527) seen from a batch of one.  all_finished = no running row.
+__global__ void k_finalize_rows(const FinalP p) {
+  pdl_trigger();
+  pdl_wait();
+  const bool decode = p.want == RS_RUNNING;
+  if (decode && ldg_cg(&p.st->all_finished)) return;
+  __shared__ int s_running;
+  if (threadIdx.x == 0) s_running = 0;
+  __syncthreads();
+  for (int b = threadIdx.x; b < p.B; b += blockDim.x) {
+    RowState* r = p.rows + b;
+    int state = ldg_cg(&r->state);
+    if (state == p.want) {
+      const int n = ldg_cg(&r->n_gen), eos_tok = ldg_cg(&r->eos);
+      bool eos = false;
+      for (int q = 0; q < p.rows_per_item; ++q) eos |= (ldg_cg(&p.idx[b * p.rows_per_item + q]) == eos_tok);
+      p.finish[b] = eos ? 1 : 0;
+      int32_t* dst = p.ids_out + ((size_t)b * p.max_new + n) * p.num_vq;
+      for (int q = 0; q < p.num_vq; ++q) dst[q] = ldg_cg(&p.idx[b * p.rows_per_item + (p.rows_per_item == 1 ? 0 : q)]);
+      if (!eos) p.end_idx[b] = ldg_cg(&p.end_idx[b]) + 1;
+      r->n_gen = n + 1;
+      r->step = ldg_cg(&r->step) + 1;
+      state = (eos || n + 1 >= ldg_cg(&r->max_new)) ? RS_FINISHED : RS_RUNNING;
+      r->state = state;
+    }
+    if (state == RS_RUNNING) atomicOr(&s_running, 1);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    p.st->all_finished = s_running ? 0 : 1;
+    if (decode) p.st->step = ldg_cg(&p.st->step) + 1;
+  }
+}
+
+template __global__ void k_sample<false>(const SampleP p);
+template __global__ void k_sample<true>(const SampleP p);
 
 }  // namespace ctb

@@ -45,6 +45,7 @@ struct TcDecP {
   float* h_hi; float* h_lo; int I;                                    // GATEUP
   float* logits; int rows_per_item, V;                                // HEADS
   float* hidden_out; int hidden_stride; const float* final_norm_w; const LoopState* st;
+  const RowState* rows; int want;  // HEADS in slot-engine mode: only rows in state `want` (nullptr: every row)
 };
 
 template <int EPI, int NPAD, int CS>
@@ -132,11 +133,21 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
       if (EPI == DE_HEADS && p.hidden_out != nullptr && blockIdx.x == 0) {
         // last_hidden_state (gpt.py:430-436): w * (x * rinv), written once
         asm volatile("bar.sync 1, 128;" ::: "memory");
-        const int step = ldg_cg(&p.st->n_gen);
-        for (int i = threadIdx.x; i < p.B * p.K; i += 128) {
-          const int b = i / p.K, k = i % p.K;
-          p.hidden_out[(size_t)b * p.hidden_stride + (size_t)step * p.K + k] =
-              __fmul_rn(__ldg(p.final_norm_w + k), __fmul_rn(ldg_cg(p.xraw + i), s_rinv[b]));
+        if (p.rows == nullptr) {
+          const int step = ldg_cg(&p.st->n_gen);
+          for (int i = threadIdx.x; i < p.B * p.K; i += 128) {
+            const int b = i / p.K, k = i % p.K;
+            p.hidden_out[(size_t)b * p.hidden_stride + (size_t)step * p.K + k] =
+                __fmul_rn(__ldg(p.final_norm_w + k), __fmul_rn(ldg_cg(p.xraw + i), s_rinv[b]));
+          }
+        } else {
+          for (int b = 0; b < p.B; ++b) {
+            if (ldg_cg(&p.rows[b].state) != p.want) continue;
+            const int step = ldg_cg(&p.rows[b].n_gen);
+            for (int k = threadIdx.x; k < p.K; k += 128)
+              p.hidden_out[(size_t)b * p.hidden_stride + (size_t)step * p.K + k] =
+                  __fmul_rn(__ldg(p.final_norm_w + k), __fmul_rn(ldg_cg(p.xraw + (size_t)b * p.K + k), s_rinv[b]));
+          }
         }
       }
     }
@@ -264,6 +275,7 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
         p.h_hi[(size_t)b * p.I + R / 2] = hh;
         p.h_lo[(size_t)b * p.I + R / 2] = to_tf32(hv - hh);
       } else {  // DE_HEADS
+        if (p.rows != nullptr && ldg_cg(&p.rows[b].state) != p.want) continue;
         const int q0 = R / p.V, c0 = R % p.V;
         p.logits[((size_t)b * p.rows_per_item + q0) * p.V + c0] = __fmul_rn(v0, rinv);
         if (R + 1 < p.nrows) {

@@ -1,0 +1,213 @@
+"""Continuous batching of audio-code generation: a slot engine on one GPT handle.
+
+The handle's decode rows become ``S`` slots (``ctb_gpt_engine_*`` in include/chattts_b200.h).  Each request - one
+utterance: a prompt embedding with its own sampling parameters, seed and token limits - enters a free slot between
+decode chunks, and its slot is reused as soon as it finishes.  A request's token ids are bit for bit what
+``GPT.generate`` returns for it alone (B = 1, same ``manual_seed``), whatever else is in flight.
+
+The scheduling policy (``schedule``) is plain Python over a small device interface, so it can be driven by a stub.
+"""
+from __future__ import annotations
+
+import ctypes as C
+from collections import deque
+from dataclasses import dataclass
+from typing import Iterator, List, Optional, Sequence, Tuple
+
+import torch
+
+from . import _lib
+from .processors import build_sampler_config, exp_noise
+
+#: shortest prompt the token-parallel prefill takes; shorter prompts are left padded with masked columns
+MIN_PROMPT_COLS = 8
+
+
+@dataclass(eq=False)
+class Request:
+    """One utterance for ``GPT.generate_continuous``.
+
+    ``emb``: [T, d] prompt embedding (every position valid, as a batch of one has no padding) or [1, T, d].
+    The other fields mean what the ``GPT.generate`` arguments of the same name mean."""
+
+    emb: torch.Tensor
+    temperature: Sequence[float]
+    eos_token: int
+    max_new_token: int = 2048
+    min_new_token: int = 0
+    logits_processors: tuple = ()
+    manual_seed: Optional[int] = None
+    ensure_non_empty: bool = True
+
+    def __post_init__(self):
+        if self.emb.dim() == 3:
+            if self.emb.shape[0] != 1:
+                raise ValueError("Request.emb holds one prompt: [T, d] or [1, T, d]")
+            self.emb = self.emb[0]
+        if self.emb.dim() != 2 or self.emb.shape[0] < 1:
+            raise ValueError("Request.emb must be [T, d] with T >= 1")
+        if self.max_new_token < 1:
+            raise ValueError("max_new_token must be >= 1")
+
+
+@dataclass
+class SlotStatus:
+    state: List[int]
+    end_idx: List[int]
+    finish: List[int]
+    steps_done: int = 0
+
+
+@dataclass
+class ScheduleStats:
+    """What one ``schedule`` run did: admissions, (device) decode steps and harvested tokens."""
+
+    admissions: int = 0
+    admitted: int = 0
+    requeued: int = 0
+    decode_steps: int = 0
+    tokens: int = 0
+    interrupted: bool = False
+
+
+def schedule(requests: Sequence[Request], dev, chunk: int, context=None,
+             stats: Optional[ScheduleStats] = None) -> Iterator[Tuple[int, Optional[int], int]]:
+    """Drive ``dev`` (``slots``, ``admit([(slot, request_index)])``, ``decode(n)``, ``status() -> SlotStatus``) until
+    every request has finished; yields ``(request_index, slot, n_tokens)`` as each one completes - the caller harvests
+    the slot's first ``n_tokens`` outputs before resuming the generator - or ``(request_index, None, 0)`` for a seeded
+    request whose first token is EOS (it ends empty, gpt.py:527).  An unseeded one with ``ensure_non_empty`` is queued
+    again instead.
+
+    Waiting requests enter free slots in order, lowest slot first, at every poll (every ``chunk`` decode steps).  On a
+    ``context`` interrupt the running requests are yielded with what they have so far and the waiting ones are dropped.
+    """
+    stats = stats if stats is not None else ScheduleStats()
+    waiting = deque(range(len(requests)))
+    owner: List[Optional[int]] = [None] * dev.slots
+    while True:
+        free = [s for s in range(dev.slots) if owner[s] is None]
+        batch = []
+        while free and waiting:
+            s, i = free.pop(0), waiting.popleft()
+            owner[s] = i
+            batch.append((s, i))
+        if batch:
+            dev.admit(batch)
+            stats.admissions += 1
+            stats.admitted += len(batch)
+        st = dev.status()
+        stats.decode_steps = st.steps_done
+        freed = False
+        for s in range(dev.slots):
+            i = owner[s]
+            if i is None or st.state[s] != _lib.SLOT_FINISHED:
+                continue
+            owner[s] = None
+            freed = True
+            if st.end_idx[s] == 0 and st.finish[s]:
+                r = requests[i]
+                if r.manual_seed is None and r.ensure_non_empty:
+                    waiting.appendleft(i)  # regenerate (gpt.py:527-570); a fresh Philox seed is drawn at admission
+                    stats.requeued += 1
+                    continue
+                yield i, None, 0
+                continue
+            stats.tokens += st.end_idx[s]
+            yield i, s, st.end_idx[s]
+        if freed and waiting:
+            continue  # refill the freed slots before the next chunk
+        running = [s for s in range(dev.slots) if owner[s] is not None]
+        if not running:
+            return
+        if context is not None and context.get():
+            stats.interrupted = True
+            for s in running:
+                stats.tokens += st.end_idx[s]
+                yield owner[s], s, st.end_idx[s]
+            return
+        dev.decode(chunk)
+
+
+class EngineDevice:
+    """The device layer of ``schedule`` on a GPT handle (ctb_gpt_engine_begin / _admit / _status, ctb_gpt_decode)."""
+
+    def __init__(self, gpt, requests: Sequence[Request], slots: int, max_new_cap: int, return_hidden: bool = True):
+        self.gpt, self.requests, self.slots = gpt, requests, slots
+        self.lib = _lib.load()
+        dev = gpt.device_gpt
+        self.dev = dev
+        self.stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        self.ids_out = torch.zeros(slots, max_new_cap, gpt.num_vq, dtype=torch.int32, device=dev)
+        self.hid_out = (torch.zeros(slots, max_new_cap, gpt.config.hidden_size, dtype=torch.float32, device=dev)
+                        if return_hidden else None)
+        _lib.check(self.lib.ctb_gpt_engine_begin(
+            gpt._handle, slots, max_new_cap, C.c_void_p(self.ids_out.data_ptr()),
+            C.c_void_p(self.hid_out.data_ptr()) if self.hid_out is not None else None, self.stream))
+        self._state = (C.c_int32 * slots)()
+        self._end = torch.zeros(slots, dtype=torch.int32)
+        self._fin = torch.zeros(slots, dtype=torch.uint8)
+
+    def admit(self, batch: List[Tuple[int, int]]) -> None:
+        # one prefill per kind: seeded requests bring their Exp(1) rows, unseeded ones sample with device Philox
+        for seeded in (True, False):
+            group = [(s, i) for s, i in batch if (self.requests[i].manual_seed is not None) == seeded]
+            if not group:
+                continue
+            # the prompts share one padded width; a request whose max_new no longer fits its slot's max_context
+            # next to that width is admitted on its own
+            T0 = max(MIN_PROMPT_COLS, max(int(self.requests[i].emb.shape[0]) for _, i in group))
+            alone = [(s, i) for s, i in group if T0 + self.requests[i].max_new_token > self.gpt.max_context]
+            rest = [p for p in group if p not in alone]
+            for part in ([rest] if rest else []) + [[p] for p in alone]:
+                self._admit(part, seeded)
+
+    def _admit(self, group, seeded: bool) -> None:
+        gpt, n = self.gpt, len(group)
+        reqs = [self.requests[i] for _, i in group]
+        T0 = max(MIN_PROMPT_COLS, max(int(r.emb.shape[0]) for r in reqs))
+        d = gpt.config.hidden_size
+        emb = torch.zeros(n, T0, d, dtype=torch.float32, device=self.dev)
+        mask = torch.zeros(n, T0, dtype=torch.uint8, device=self.dev)
+        for k, r in enumerate(reqs):  # left padding: the prompt is a suffix of its row
+            T = int(r.emb.shape[0])
+            emb[k, T0 - T:] = r.emb.to(self.dev, torch.float32)
+            mask[k, T0 - T:] = 1
+        cfgs = (_lib.SamplerConfig * n)()
+        for k, r in enumerate(reqs):
+            temps = [float(t) for t in torch.as_tensor(r.temperature).flatten().tolist()]
+            philox = 0 if seeded else int(torch.randint(0, 2 ** 62, (1,)).item())
+            cfgs[k] = build_sampler_config(r.logits_processors, temps, int(r.eos_token), r.min_new_token, philox)
+        noise = None
+        if seeded:  # the rows GPT.generate draws for a batch of one with this seed
+            noise = torch.cat([exp_noise(gpt.num_vq, gpt.num_audio_tokens, r.manual_seed) for r in reqs]).to(self.dev)
+        slots = (C.c_int32 * n)(*[s for s, _ in group])
+        max_new = (C.c_int32 * n)(*[r.max_new_token for r in reqs])
+        _lib.check(self.lib.ctb_gpt_engine_admit(
+            gpt._handle, n, slots, T0, C.c_void_p(emb.data_ptr()), C.c_void_p(mask.data_ptr()), cfgs,
+            C.c_void_p(noise.data_ptr()) if noise is not None else None, max_new, self.stream))
+
+    def decode(self, n: int) -> None:
+        _lib.check(self.lib.ctb_gpt_decode(self.gpt._handle, n, self.stream))
+
+    def status(self) -> SlotStatus:
+        st = _lib.GptStatus()
+        _lib.check(self.lib.ctb_gpt_engine_status(self.gpt._handle, C.byref(st), self._state,
+                                                  C.c_void_p(self._end.data_ptr()), C.c_void_p(self._fin.data_ptr()),
+                                                  self.stream))
+        return SlotStatus(list(self._state), self._end.tolist(), self._fin.tolist(), int(st.steps_done))
+
+    def harvest(self, slot: int, n: int):
+        """GenerationOutputs of the request in ``slot``: its first ``n`` ids and hidden states (copies)."""
+        from .gpt import GPT
+
+        ids = self.ids_out[slot, :n].to(torch.int64)
+        hid = [self.hid_out[slot, :n].clone()] if self.hid_out is not None else []
+        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid)
+
+    def empty(self):
+        from .gpt import GPT
+
+        ids = torch.zeros(0, self.gpt.num_vq, dtype=torch.int64, device=self.dev)
+        hid = ([torch.zeros(0, self.gpt.config.hidden_size, dtype=torch.float32, device=self.dev)]
+               if self.hid_out is not None else [])
+        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid)

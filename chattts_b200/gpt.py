@@ -223,6 +223,54 @@ class GPT:
         if n > 0:
             _lib.check(lib.ctb_gpt_decode(self._handle, n, stream_ptr))
 
+    # ------------------------------------------------------------------ continuous batching
+    @torch.no_grad()
+    def generate_continuous(self, requests, slots: Optional[int] = None, return_hidden=True, infer_text=False,
+                            stream=False, return_attn=False, context=None, chunk: Optional[int] = None):
+        """Generate audio codes for many utterances on a slot engine (chattts_b200.engine): up to ``slots`` requests
+        (default: ``max_batch``, at most the number of requests) decode together, and a waiting request takes the
+        place of a finished one at the next poll (every ``chunk`` steps, default CTB_DECODE_CHUNK or 32).
+
+        Generator of ``(request_index, GenerationOutputs)`` in completion order.  Each request's ids equal, bit for
+        bit, ``generate`` on that request alone with the same arguments and ``manual_seed``.  A seeded request that
+        samples EOS first yields empty outputs (``generate`` yields nothing then); an unseeded one with
+        ``ensure_non_empty`` runs again.  The handle serves one generator at a time; ``generate`` may be called again
+        once it is exhausted."""
+        from .engine import MIN_PROMPT_COLS, EngineDevice, Request, ScheduleStats, schedule
+
+        if infer_text:
+            raise ValueError("generate_continuous: audio codes only (infer_text=True stays on generate)")
+        if stream:
+            raise ValueError("generate_continuous: stream=True is not supported; results are yielded per request")
+        if return_attn:
+            raise ValueError("generate_continuous: return_attn is not supported")
+        if not self._handle:
+            raise _lib.CtbError("GPT weights not loaded")
+        requests = list(requests)
+        if not requests:
+            return
+        if not all(isinstance(r, Request) for r in requests):
+            raise TypeError("requests must be chattts_b200.engine.Request objects")
+
+        S = min(self.max_batch, len(requests)) if slots is None else int(slots)
+        S = max(S, 2)
+        if S > self.max_batch:
+            raise ValueError(f"slots={S} exceed this handle's max_batch={self.max_batch}")
+        for r in requests:
+            T0 = max(MIN_PROMPT_COLS, int(r.emb.shape[0]))
+            if T0 > 1024 or T0 + r.max_new_token > self.max_context:
+                raise ValueError(f"prompt {int(r.emb.shape[0])} + max_new_token {r.max_new_token} exceed this handle "
+                                 f"(max_context={self.max_context}; prompts up to 1024 tokens)")
+        chunk = int(os.environ.get("CTB_DECODE_CHUNK", "32")) if chunk is None else int(chunk)
+        context = context if context is not None else GPT.Context()
+        with torch.cuda.device(self.device_gpt):
+            dev = EngineDevice(self, requests, S, max(r.max_new_token for r in requests), return_hidden)
+            self.last_schedule_stats = stats = ScheduleStats()  # admissions, decode steps (tools/bench_continuous.py)
+            for i, slot, n in schedule(requests, dev, chunk, context, stats):
+                yield i, (dev.empty() if slot is None else dev.harvest(slot, n))
+            if stats.interrupted:
+                self.logger.warning("generation is interrupted")
+
     # ------------------------------------------------------------------ the loop
     @torch.no_grad()
     def generate(self, emb: torch.Tensor, inputs_ids: torch.Tensor, temperature: torch.Tensor,

@@ -138,6 +138,45 @@ typedef struct ctb_gpt_status {
 int ctb_gpt_status_query(ctb_gpt* h, ctb_gpt_status* out, int32_t* end_idx_host, uint8_t* finish_host,
                          void* stream);
 
+/* ---- slot engine: continuous batching of audio-code generation (no reference counterpart; the reference serves
+ * this with the vLLM fork behind Chat.load(use_vllm=True)).  The handle's rows become S independent slots; each holds
+ * one request (one utterance) at its own point of generation, with its own sampling parameters, noise and max_new,
+ * and produces exactly what ctb_gpt_begin / ctb_gpt_decode produce for that request alone (B = 1).  Requests enter
+ * free slots between ctb_gpt_decode calls; ctb_gpt_decode is used unchanged (steps advance every running slot; with
+ * no running slot they are no-ops).  ctb_gpt_begin returns the handle to static batches. */
+
+#define CTB_SLOT_IDLE 0
+#define CTB_SLOT_RUNNING 1
+#define CTB_SLOT_FINISHED 2
+
+/* Turn the handle into S slots (2 <= S <= max_batch), all idle.  Every slot owns a fixed KV page range of
+ * max_context tokens (S x max_context tokens in all).
+ *   ids_out_dev      [S, max_new_cap, num_vq] int32   slot b's tokens: ids_out_dev[b, 0 : end_idx[b]]
+ *   hiddens_out_dev  [S, max_new_cap, d] fp32 or NULL  its last hidden states, same rows */
+int ctb_gpt_engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t* ids_out_dev, float* hiddens_out_dev,
+                         void* stream);
+
+/* Admit n requests into the idle or finished slots slots[0..n) (host array): prefill their prompts (token-parallel,
+ * left padded, 8 <= T0 <= 1024: pad shorter prompts with masked columns) into those slots and sample each one's first
+ * token; no other slot's state, outputs or KV pages are touched.
+ *   emb_dev [n, T0, d] fp32, mask_dev [n, T0] uint8 (valid tokens a suffix of each row, as for ctb_gpt_begin)
+ *   samplers[n] (host)   sampling parameters of each request (audio codes; penalty_max_ids applies to its own rows
+ *                        0..num_vq-1, as in a batch of one)
+ *   q_noise_dev          [n, num_vq, num_audio] fp32 Exp(1) rows of each request's seeded generator, or NULL: device
+ *                        Philox from samplers[i].philox_seed
+ *   max_new[n] (host)    tokens each request may generate (<= max_new_cap, T0 + max_new <= max_context)
+ * Enqueued on `stream`; the host arrays may be released on return. */
+int ctb_gpt_engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0, const float* emb_dev,
+                         const uint8_t* mask_dev, const ctb_sampler_config* samplers, const float* q_noise_dev,
+                         const int32_t* max_new, void* stream);
+
+/* Synchronises `stream`, then reports per-slot results (each array [S], any may be NULL): state_host CTB_SLOT_*,
+ * end_idx_host tokens of the slot's request, finish_host 1 if it ended at EOS.  A finished slot with end_idx 0 and
+ * finish 1 sampled EOS as its first token (gpt.py:527: the request ends empty).  out->steps_done counts decode steps
+ * with at least one running slot; out->all_finished = no running slot. */
+int ctb_gpt_engine_status(ctb_gpt* h, ctb_gpt_status* out, int32_t* state_host, int32_t* end_idx_host,
+                          uint8_t* finish_host, void* stream);
+
 /* Measurement hook for bench.py's roofline: launches ONE kernel kind once per layer on the
  * state left by the last generate call (kind 0 qkv, 1 attention, 2 o-proj, 3 gate/up, 4 down;
  * 5 = heads, 6 = sampler, 7 = one decode step as ONE kernel launch (k_flow / k_step), 8 = 16 decode steps in one
