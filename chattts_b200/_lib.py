@@ -63,7 +63,7 @@ EXPORTS = (
     "ctb_gpt_destroy", "ctb_gpt_begin", "ctb_gpt_decode", "ctb_gpt_status_query", "ctb_gpt_profile_kernel", "ctb_gpt_debug_trace", "ctb_gpt_embed_prompt", "ctb_sample",
     "ctb_gpt_engine_begin", "ctb_gpt_engine_admit", "ctb_gpt_engine_status",
     "ctb_dvae_blob_floats", "ctb_vocos_blob_floats", "ctb_decoder_create", "ctb_decoder_destroy",
-    "ctb_dvae_decode", "ctb_vocos_decode",
+    "ctb_dvae_decode", "ctb_vocos_decode", "ctb_decode_rows",
     "ctb_dvae_encoder_blob_floats", "ctb_dvae_encoder_create", "ctb_dvae_encoder_destroy", "ctb_dvae_encode",
 )
 
@@ -120,6 +120,7 @@ def load(build_if_missing: bool = True):
         lib.ctb_decoder_destroy.argtypes = [vp]
         lib.ctb_dvae_decode.argtypes = [vp, vp, i32, i32, i32, vp, vp]
         lib.ctb_vocos_decode.argtypes = [vp, vp, i32, i32, vp, vp]
+        lib.ctb_decode_rows.argtypes = [vp, i32, i32, C.POINTER(vp), C.POINTER(i32), vp, i64, vp]
         lib.ctb_dvae_encoder_blob_floats.argtypes = [C.POINTER(ConvStackConfig)]
         lib.ctb_dvae_encoder_blob_floats.restype = i64
         lib.ctb_dvae_encoder_create.argtypes = [C.POINTER(ConvStackConfig), vp, i64, C.POINTER(vp)]

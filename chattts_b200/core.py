@@ -19,7 +19,7 @@ import numpy as np
 import torch
 
 from .config import Config
-from .decoder import decode_to_wavs_window, DVAE, Vocos, decode_to_wavs
+from .decoder import decode_to_wavs_window, DVAE, Vocos, decode_to_wavs, stream_window
 from .embed import Embed
 from .gpt import GPT
 from .norm import Normalizer
@@ -210,25 +210,45 @@ class Chat:
         what ``infer([texts[index]], split_text=False, skip_refine_text=True)`` returns for that text with its params.
         Normalisation and the optional text refinement run as in ``infer``."""
         if stream:
-            raise ValueError("infer_continuous: stream=True is not supported; each waveform is yielded when complete")
+            raise ValueError("infer_continuous: stream=True is not supported; each waveform is yielded when complete "
+                             "(infer_continuous_stream streams)")
+        texts, params = self._continuous_params(texts, params_infer_code)
+        return self._infer_continuous(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
+                                      do_homophone_replacement, params_refine_text or Chat.RefineTextParams())
+
+    def infer_continuous_stream(self, texts, params_infer_code=None, use_decoder=True, slots=None, lang=None,
+                                skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
+                                params_refine_text=None):
+        """Streaming synthesis of many texts with continuous batching (``GPT.generate_continuous_stream``).
+        Generator of ``(index, chunk, last)``, ``chunk`` a ``[1, n]`` float32 array; for each text the chunks are
+        those ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=True)`` yields with that
+        text's params (its own ``stream_batch``, ``stream_speed`` and ``pass_first_n_batches``), and ``last`` marks
+        its final chunk.  A seeded text whose first code is EOS yields one empty final chunk.  All windows due at one
+        engine poll are decoded in one ragged call (``TokenDecoder.decode_rows``), straight from the engine's
+        buffers.  Arguments as for ``infer_continuous``."""
+        texts, params = self._continuous_params(texts, params_infer_code)
+        return self._infer_continuous_stream(texts, params, use_decoder, slots, lang, skip_refine_text,
+                                             do_text_normalization, do_homophone_replacement,
+                                             params_refine_text or Chat.RefineTextParams())
+
+    @staticmethod
+    def _continuous_params(texts, params_infer_code):
         if isinstance(texts, str):
             texts = [texts]
         texts = list(texts)
         if isinstance(params_infer_code, (list, tuple)):
             if len(params_infer_code) != len(texts):
                 raise ValueError("params_infer_code: one InferCodeParams per text")
-            params = list(params_infer_code)
-        else:
-            params = [params_infer_code or Chat.InferCodeParams()] * len(texts)
-        return self._infer_continuous(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
-                                      do_homophone_replacement, params_refine_text or Chat.RefineTextParams())
+            return texts, list(params_infer_code)
+        return texts, [params_infer_code or Chat.InferCodeParams()] * len(texts)
 
-    def _infer_continuous(self, texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
-                          do_homophone_replacement, params_refine_text):
+    def _continuous_requests(self, texts, params, use_decoder, lang, skip_refine_text, do_text_normalization,
+                             do_homophone_replacement, params_refine_text):
+        """Normalisation, optional refinement and one engine request per text (as ``_infer`` prepares them)."""
         assert self.has_loaded(use_decoder=use_decoder)
         self.context.set(False)
         if not texts:
-            return
+            return []
         texts = [self.normalizer(t, do_text_normalization, do_homophone_replacement, lang) for t in texts]
         if not skip_refine_text:
             tokens = []
@@ -237,7 +257,24 @@ class Chat:
                 tokens += [i[i.less(self.tokenizer.break_0_ids)] for i in refined.ids]
                 refined.destroy()
             texts = self.tokenizer.decode(tokens)
-        requests = [self._code_request(t, p) for t, p in zip(texts, params)]
+        return [self._code_request(t, p) for t, p in zip(texts, params)]
+
+    def _infer_continuous_stream(self, texts, params, use_decoder, slots, lang, skip_refine_text,
+                                 do_text_normalization, do_homophone_replacement, params_refine_text):
+        requests = self._continuous_requests(texts, params, use_decoder, lang, skip_refine_text, do_text_normalization,
+                                             do_homophone_replacement, params_refine_text)
+        if not requests:
+            return
+        windows = [StreamWindows(p.stream_speed, p.pass_first_n_batches) for p in params]
+        yield from stream_continuous(self.gpt, self.decoder if use_decoder else self.dvae, requests, windows,
+                                     use_decoder, slots, self.context)
+
+    def _infer_continuous(self, texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
+                          do_homophone_replacement, params_refine_text):
+        requests = self._continuous_requests(texts, params, use_decoder, lang, skip_refine_text, do_text_normalization,
+                                             do_homophone_replacement, params_refine_text)
+        if not requests:
+            return
         thr = np.float32(1e-5)
         with torch.no_grad():
             for i, out in self.gpt.generate_continuous(requests, slots=slots, return_hidden=use_decoder,
@@ -267,7 +304,7 @@ class Chat:
         return Request(emb=emb[0][valid.to(emb.device)], temperature=temperature, eos_token=num_code,
                        max_new_token=params.max_new_token, min_new_token=params.min_new_token,
                        logits_processors=(*processors, *warpers), manual_seed=params.manual_seed,
-                       ensure_non_empty=params.ensure_non_empty)
+                       ensure_non_empty=params.ensure_non_empty, stream_batch=params.stream_batch)
 
     def interrupt(self):
         self.context.set(True)
@@ -393,3 +430,80 @@ class Chat:
             attention_mask=attention_mask, max_new_token=params.max_new_token, min_new_token=params.min_new_token,
             logits_processors=(*processors, *warpers), infer_text=True, stream=False, show_tqdm=params.show_tqdm,
             ensure_non_empty=params.ensure_non_empty, manual_seed=params.manual_seed, context=self.context))
+
+
+class StreamWindows:
+    """The streaming hand-off of ``Chat._infer`` (reference core.py:455-503) for one request decoded alone: turns its
+    cumulative GPT yields into the sample windows ``infer([text], stream=True, split_text=False)`` yields.  The first
+    ``pass_first_n_batches`` yields are skipped (and do not advance the position); every other yield, the final one
+    included, takes the next ``stream_speed`` samples, clamped to the 512 n - 256 samples of its n tokens; the final
+    yield is then followed by the rest of the sequence, whose all-silent samples are dropped."""
+
+    def __init__(self, stream_speed: int, pass_first_n_batches: int):
+        self.speed, self.skip = int(stream_speed), int(pass_first_n_batches)
+        self.length = self.count = 0
+
+    def windows(self, n_tokens: int, last: bool):
+        """``[(a, b, flush)]``: the sample windows of one GPT yield of `n_tokens` tokens (b <= a: an empty chunk)."""
+        if n_tokens == 0:  # a seeded request that ended empty: one empty closing chunk
+            return [(0, 0, True)] if last else []
+        total = 512 * n_tokens - 256
+        out = []
+        self.count += 1
+        if self.count > self.skip:
+            a, b = self.length, min(self.length + self.speed, total)
+            self.length = b
+            out.append((a, b, False))
+        if last:
+            out.append((self.length, total, True))
+        return out
+
+
+def stream_continuous(gpt: GPT, model: DVAE, requests, windows: List[StreamWindows], use_decoder: bool, slots=None,
+                      context=None, ragged: bool = True, stats: Optional[Dict[str, float]] = None):
+    """Streamed audio of many requests on the slot engine: generator of ``(request_index, chunk [1, n] float32, last)``.
+
+    At every engine poll the windows of every GPT yield due then (``GPT._stream_polls``) are decoded together: each
+    window's token range (``decoder.stream_window``) is read straight from the engine's hidden states (``model`` =
+    the DVAE decoder) or codes (``model`` = the code DVAE, ``use_decoder=False``) in one ``decode_rows`` call, and the
+    window is cut out of its row.  ``ragged=False`` decodes the windows one ``decode_to_wavs_window`` call each
+    instead (the straightforward form tools/bench_continuous.py compares against).  ``stats['path2_s']`` (optional)
+    accumulates the host time spent decoding and copying the audio."""
+    import time
+
+    thr = np.float32(1e-5)
+    for dev, batch in gpt._stream_polls(requests, slots, use_decoder, context):
+        t_start = time.perf_counter()
+        buf = dev.hid_out if use_decoder else dev.ids_out
+        jobs = []  # (request, slot, n_tokens, a, b, flush, last)
+        for i, s, n, last in batch:
+            ws = windows[i].windows(n, last)
+            jobs += [(i, s, n, a, b, flush, last and k == len(ws) - 1) for k, (a, b, flush) in enumerate(ws)]
+        due = [k for k, j in enumerate(jobs) if j[4] > j[3]]
+        chunks: Dict[int, np.ndarray] = {}
+        if due and ragged:
+            rows, cuts = [], []
+            for k in due:
+                _, s, n, a, b = jobs[k][:5]
+                a, b, t0, t1 = stream_window(n, a, b)
+                rows.append(buf[s, t0:t1])
+                cuts.append((a - 512 * t0, b - 512 * t0))
+            wavs = model.engine.decode_rows(rows, 1 if use_decoder else 2)
+            flat = torch.cat([w[c0:c1] for w, (c0, c1) in zip(wavs, cuts)]).cpu().numpy()
+            off = 0
+            for k, (c0, c1) in zip(due, cuts):
+                chunks[k] = flat[None, off: off + c1 - c0]
+                off += c1 - c0
+        elif due:
+            for k in due:
+                _, s, n, a, b = jobs[k][:5]
+                chunks[k] = decode_to_wavs_window([buf[s, :n]], use_decoder, model, model, a, b)
+        out = []
+        for k, (i, _, _, _, _, flush, last) in enumerate(jobs):
+            chunk = chunks.get(k, np.zeros((1, 0), dtype=np.float32))
+            if flush:
+                chunk = chunk[:, np.abs(chunk[0]) > thr]
+            out.append((i, chunk, last))
+        if stats is not None:
+            stats["path2_s"] = stats.get("path2_s", 0.0) + time.perf_counter() - t_start
+        yield from out

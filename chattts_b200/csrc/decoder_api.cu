@@ -1,5 +1,7 @@
 // extern "C" entry points for hot path 2 (token -> waveform); see include/chattts_b200.h.
 #define CTB_DECODER_KERNELS_IMPL
+#include <vector>
+
 #include "tc_gemm.cuh"
 
 using namespace ctb;
@@ -84,6 +86,8 @@ struct ctb_decoder {
   size_t max_rows;  // max_batch * 2 * max_tokens frames
   size_t cap_rows;  // frames the activation buffers currently hold
   float *bufA, *bufB, *bufH, *mel_tm, *staged_in;
+  void* rows_meta;      // ctb_decode_rows: [B] row pointers + [B] frame counts, grown with B
+  int rows_meta_cap;
   // tensor-core path: tf32-rounded hi / lo copies of both blobs (same offsets as the fp32 blobs)
   float *dW_hi, *dW_lo, *vW_hi, *vW_lo;
   bool use_tc;
@@ -94,7 +98,8 @@ extern "C" int64_t ctb_vocos_blob_floats(const ctb_vocos_config* c) { return c ?
 
 extern "C" int ctb_decoder_destroy(ctb_decoder* h) {
   if (!h) return CTB_OK;
-  void* ptrs[] = {h->bufA, h->bufB, h->bufH, h->mel_tm, h->staged_in, h->dW_hi, h->dW_lo, h->vW_hi, h->vW_lo};
+  void* ptrs[] = {h->bufA, h->bufB, h->bufH, h->mel_tm, h->staged_in, h->dW_hi, h->dW_lo, h->vW_hi, h->vW_lo,
+                  h->rows_meta};
   for (void* p : ptrs) if (p) cudaFree(p);
   delete h;
   return CTB_OK;
@@ -183,50 +188,69 @@ struct GemmCtx {  // which blob a weight pointer lives in, for the hi / lo looku
   const float* W; const float* hi; const float* lo; bool tc;
 };
 
+// fr (device [M / F], or null): ragged mode, the utterances have fr[b] <= F frames each and every layer writes zeros
+// in the rows past them (see k_tc_gemm)
 template <int EPI>
 static int gemm(cudaStream_t s, const GemmCtx& gc, const float* A, int lda, int M, int N, int K, int taps, int Cin,
                 int dil, int pad, int F, const float* W, const float* bias, const float* gamma, const float* res,
-                int ldres, float* C, int ldc) {
-  if (gc.tc && K % TC_BK == 0 && Cin % TC_BK == 0 && M % F == 0)
+                int ldres, float* C, int ldc, const int* fr = nullptr) {
+  if (gc.tc && K % TC_BK == 0 && Cin % TC_BK == 0 && M % F == 0) {
+    if (fr)
+      return tc_gemm_launch<EPI, true>(s, A, lda, M / F, F, N, K, taps, Cin, dil, pad, gc.hi + (W - gc.W),
+                                       gc.lo + (W - gc.W), bias, gamma, res, ldres, C, ldc, fr);
     return tc_gemm_launch<EPI>(s, A, lda, M / F, F, N, K, taps, Cin, dil, pad, gc.hi + (W - gc.W), gc.lo + (W - gc.W), bias,
                                gamma, res, ldres, C, ldc);
+  }
   GemmP p{};
   p.A = A; p.lda = lda; p.M = M; p.N = N; p.K = K; p.taps = taps; p.Cin = Cin; p.dil = dil; p.pad = pad; p.F = F;
-  p.W = W; p.bias = bias; p.gamma = gamma; p.res = res; p.ldres = ldres; p.C = C; p.ldc = ldc;
+  p.W = W; p.bias = bias; p.gamma = gamma; p.res = res; p.ldres = ldres; p.C = C; p.ldc = ldc; p.fr = fr;
   dim3 grid((N + GBN - 1) / GBN, (M + GBM - 1) / GBM);
-  k_sgemm_nt<EPI><<<grid, 256, 0, s>>>(p);
+  if (fr)
+    k_sgemm_nt<EPI, true><<<grid, 256, 0, s>>>(p);
+  else
+    k_sgemm_nt<EPI><<<grid, 256, 0, s>>>(p);
   CTB_LAUNCH_CHECK();
   return CTB_OK;
 }
 
-static int dwln(cudaStream_t s, const float* x, float* out, int M, int F, int C, int taps, int dil, const float* w,
-                const float* b, const float* lnw, const float* lnb) {
-  DwLnP p{x, out, M, F, C, taps, dil, w, b, lnw, lnb, 1e-6f};
-  const int blocks = (M + 7) / 8;
-  switch (C / 128) {
-    case 1: k_dwconv_ln<1><<<blocks, 256, 0, s>>>(p); break;
-    case 2: k_dwconv_ln<2><<<blocks, 256, 0, s>>>(p); break;
-    case 3: k_dwconv_ln<3><<<blocks, 256, 0, s>>>(p); break;
-    default: k_dwconv_ln<4><<<blocks, 256, 0, s>>>(p); break;
+template <bool RAGGED>
+static void dwln_launch(cudaStream_t s, const DwLnP& p, int blocks) {
+  switch (p.C / 128) {
+    case 1: k_dwconv_ln<1, RAGGED><<<blocks, 256, 0, s>>>(p); break;
+    case 2: k_dwconv_ln<2, RAGGED><<<blocks, 256, 0, s>>>(p); break;
+    case 3: k_dwconv_ln<3, RAGGED><<<blocks, 256, 0, s>>>(p); break;
+    default: k_dwconv_ln<4, RAGGED><<<blocks, 256, 0, s>>>(p); break;
   }
+}
+
+static int dwln(cudaStream_t s, const float* x, float* out, int M, int F, int C, int taps, int dil, const float* w,
+                const float* b, const float* lnw, const float* lnb, const int* fr = nullptr) {
+  DwLnP p{x, out, M, F, C, taps, dil, w, b, lnw, lnb, 1e-6f, fr};
+  const int blocks = (M + 7) / 8;
+  if (fr)
+    dwln_launch<true>(s, p, blocks);
+  else
+    dwln_launch<false>(s, p, blocks);
   CTB_LAUNCH_CHECK();
   return CTB_OK;
 }
 
 // x (time-major [M, C]) -> x through one ConvNeXt block; tmp = [M, C], hbuf = [M, inter]
 static int convnext(cudaStream_t s, const GemmCtx& gc, const float* W, const BlockOff& b, float* x, float* tmp, float* hbuf, int M,
-                    int F, int C, int inter, int dil) {
+                    int F, int C, int inter, int dil, const int* fr = nullptr) {
   int rc;
-  if ((rc = dwln(s, x, tmp, M, F, C, 7, dil, W + b.dw_w, W + b.dw_b, W + b.ln_w, W + b.ln_b))) return rc;
+  if ((rc = dwln(s, x, tmp, M, F, C, 7, dil, W + b.dw_w, W + b.dw_b, W + b.ln_w, W + b.ln_b, fr))) return rc;
   if ((rc = gemm<GE_GELU>(s, gc, tmp, C, M, inter, C, 1, C, 1, 0, F, W + b.pw1_w, W + b.pw1_b, nullptr, nullptr, 0, hbuf,
-                          inter))) return rc;
+                          inter, fr))) return rc;
   return gemm<GE_SCALE_RES>(s, gc, hbuf, inter, M, C, inter, 1, inter, 1, 0, F, W + b.pw2_w, W + b.pw2_b, W + b.gamma, x,
-                            C, x, C);
+                            C, x, C, fr);
 }
 
 // in_layout: 0 = channels-first [B, C, T] fp32 (DVAE.__call__ layout), 1 = token-major [B, T, C] fp32
-// (the decode loop's hidden states; frame doubling is then a re-interpretation), 2 = codes [B, G*R, T] int32
-static int dvae_run(ctb_decoder* h, const void* in, int layout, int B, int T, float* mel_cf, cudaStream_t s) {
+// (the decode loop's hidden states; frame doubling is then a re-interpretation), 2 = codes [B, G*R, T] int32.
+// fr: ragged mode (ctb_decode_rows), layout 1 with rows past each utterance's fr[b] frames zero.
+static int dvae_run(ctb_decoder* h, const void* in, int layout, int B, int T, float* mel_cf, cudaStream_t s,
+                    const int* fr = nullptr) {
   const ctb_convstack_config& c = h->dc;
   const DvaeOff& L = h->dl;
   const float* W = h->dW;
@@ -255,16 +279,17 @@ static int dvae_run(ctb_decoder* h, const void* in, int layout, int B, int T, fl
   }
   // conv_in: Conv1d(idim -> bn, k3, p1) + GELU + Conv1d(bn -> hidden, k3, p1)   (dvae.py:144-148)
   if ((rc = gemm<GE_GELU>(s, gc, x0, c.idim, M, c.bn_dim, 3 * c.idim, 3, c.idim, 1, 1, F, W + L.in0_w, W + L.in0_b,
-                          nullptr, nullptr, 0, h->bufB, c.bn_dim))) return rc;
+                          nullptr, nullptr, 0, h->bufB, c.bn_dim, fr))) return rc;
   if ((rc = gemm<GE_BIAS>(s, gc, h->bufB, c.bn_dim, M, c.hidden, 3 * c.bn_dim, 3, c.bn_dim, 1, 1, F, W + L.in2_w,
-                          W + L.in2_b, nullptr, nullptr, 0, h->bufA, c.hidden))) return rc;
+                          W + L.in2_b, nullptr, nullptr, 0, h->bufA, c.hidden, fr))) return rc;
   for (int i = 0; i < c.n_layer; ++i)
-    if ((rc = convnext(s, gc, W, L.blk[i], h->bufA, h->bufB, h->bufH, M, F, c.hidden, 4 * c.hidden, c.dilation))) return rc;
+    if ((rc = convnext(s, gc, W, L.blk[i], h->bufA, h->bufB, h->bufH, M, F, c.hidden, 4 * c.hidden, c.dilation, fr)))
+      return rc;
   // conv_out 1x1 (no bias), out_conv k3 (no bias) * coef        (dvae.py:159,236,289-297)
   if ((rc = gemm<GE_NONE>(s, gc, h->bufA, c.hidden, M, c.odim, c.hidden, 1, c.hidden, 1, 0, F, W + L.conv_out_w, nullptr,
-                          nullptr, nullptr, 0, h->bufB, c.odim))) return rc;
+                          nullptr, nullptr, 0, h->bufB, c.odim, fr))) return rc;
   if ((rc = gemm<GE_COEF>(s, gc, h->bufB, c.out_dim, M, MEL_PAD, 3 * c.out_dim, 3, c.out_dim, 1, 1, F, W + L.out_conv_w,
-                          nullptr, W + L.coef, nullptr, 0, h->mel_tm, MEL_PAD))) return rc;
+                          nullptr, W + L.coef, nullptr, 0, h->mel_tm, MEL_PAD, fr))) return rc;
   if (mel_cf) {
     dim3 g((F + 31) / 32, (MEL + 31) / 32, B);
     k_tm_to_cf<<<g, dim3(32, 8), 0, s>>>(h->mel_tm, mel_cf, B, MEL, F, MEL_PAD);
@@ -273,7 +298,9 @@ static int dvae_run(ctb_decoder* h, const void* in, int layout, int B, int T, fl
   return CTB_OK;
 }
 
-static int vocos_run(ctb_decoder* h, const float* mel_cf, int B, int F, float* wav, cudaStream_t s) {
+// fr: ragged mode (ctb_decode_rows); wav is then [B, wav_ld] and row b receives hop * (fr[b] - 1) samples
+static int vocos_run(ctb_decoder* h, const float* mel_cf, int B, int F, float* wav, cudaStream_t s,
+                     const int* fr = nullptr, int64_t wav_ld = 0) {
   const ctb_vocos_config& c = h->vc;
   const VocosOff& L = h->vl;
   const float* W = h->vW;
@@ -287,19 +314,23 @@ static int vocos_run(ctb_decoder* h, const float* mel_cf, int B, int F, float* w
   }
   // backbone: Conv1d(100 -> dim, k7, p3) -> LN -> ConvNeXt x num_layers -> LN
   if ((rc = gemm<GE_BIAS>(s, gc, h->mel_tm, MEL_PAD, M, c.dim, 7 * MEL_PAD, 7, MEL_PAD, 1, 3, F, W + L.embed_w,
-                          W + L.embed_b, nullptr, nullptr, 0, h->bufB, c.dim))) return rc;
-  if ((rc = dwln(s, h->bufB, h->bufA, M, F, c.dim, 0, 1, nullptr, nullptr, W + L.norm_w, W + L.norm_b))) return rc;
+                          W + L.embed_b, nullptr, nullptr, 0, h->bufB, c.dim, fr))) return rc;
+  if ((rc = dwln(s, h->bufB, h->bufA, M, F, c.dim, 0, 1, nullptr, nullptr, W + L.norm_w, W + L.norm_b, fr))) return rc;
   for (int i = 0; i < c.num_layers; ++i)
-    if ((rc = convnext(s, gc, W, L.blk[i], h->bufA, h->bufB, h->bufH, M, F, c.dim, c.intermediate_dim, 1))) return rc;
-  if ((rc = dwln(s, h->bufA, h->bufB, M, F, c.dim, 0, 1, nullptr, nullptr, W + L.fin_w, W + L.fin_b))) return rc;
+    if ((rc = convnext(s, gc, W, L.blk[i], h->bufA, h->bufB, h->bufH, M, F, c.dim, c.intermediate_dim, 1, fr))) return rc;
+  if ((rc = dwln(s, h->bufA, h->bufB, M, F, c.dim, 0, 1, nullptr, nullptr, W + L.fin_w, W + L.fin_b, fr))) return rc;
   // ISTFTHead: Linear(dim -> n_fft + 2) -> (mag, phase) -> complex spectrum (interleaved re/im)
   if ((rc = gemm<GE_SPEC>(s, gc, h->bufB, c.dim, M, SK, c.dim, 1, c.dim, 1, 0, F, W + L.head_w, W + L.head_b, nullptr,
-                          nullptr, 0, h->bufA, SK))) return rc;
+                          nullptr, 0, h->bufA, SK, fr))) return rc;
   // inverse real DFT * window as a GEMM against the constant basis, then overlap-add / envelope
   if ((rc = gemm<GE_NONE>(s, gc, h->bufA, SK, M, c.n_fft, SK, 1, SK, 1, 0, F, W + L.basis, nullptr, nullptr, nullptr, 0,
-                          h->bufH, c.n_fft))) return rc;
+                          h->bufH, c.n_fft, fr))) return rc;
   const size_t total = (size_t)B * c.hop_length * (F - 1);
-  k_overlap_add<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(h->bufH, W + L.window, wav, B, F, c.n_fft, c.hop_length);
+  if (fr)
+    k_overlap_add<true><<<(unsigned)((total + 255) / 256), 256, 0, s>>>(h->bufH, W + L.window, wav, B, F, c.n_fft,
+                                                                        c.hop_length, fr, wav_ld);
+  else
+    k_overlap_add<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(h->bufH, W + L.window, wav, B, F, c.n_fft, c.hop_length);
   CTB_LAUNCH_CHECK();
   return CTB_OK;
 }
@@ -325,6 +356,60 @@ extern "C" int ctb_vocos_decode(ctb_decoder* h, const float* mel_dev, int32_t B,
     return set_err(CTB_ERR_STATE, "no mel of this shape was left in the handle by ctb_dvae_decode");
   { int rc = dec_reserve(h, (size_t)B * F, (cudaStream_t)stream); if (rc) return rc; }
   return vocos_run(h, mel_dev, B, F, wav_dev, (cudaStream_t)stream);
+}
+
+extern "C" int ctb_decode_rows(ctb_decoder* h, int32_t kind, int32_t B, const void* const* rows_dev,
+                               const int32_t* n_tokens, float* wav_dev, int64_t wav_ld, void* stream) {
+  if (!h || !rows_dev || !n_tokens || !wav_dev) return set_err(CTB_ERR_ARG, "null argument");
+  if (!h->dW || !h->vW) return set_err(CTB_ERR_STATE, "ctb_decode_rows needs a handle with DVAE and Vocos weights");
+  if (kind != 1 && kind != 2) return set_err(CTB_ERR_ARG, "bad kind %d (1: hidden states, 2: codes)", kind);
+  if (B < 1) return set_err(CTB_ERR_ARG, "B=%d", B);
+  const ctb_convstack_config& c = h->dc;
+  if (kind == 2 && (c.vq_dim <= 0 || c.vq_groups != 2))
+    return set_err(CTB_ERR_ARG, "codes need a decoder with a VQ layer of 2 groups (use_decoder=False model)");
+  int W = 0;
+  for (int k = 0; k < B; ++k) {
+    if (n_tokens[k] < 1) return set_err(CTB_ERR_ARG, "row %d has %d tokens", k, n_tokens[k]);
+    if (!rows_dev[k] || (kind == 1 && (reinterpret_cast<uintptr_t>(rows_dev[k]) & 15)))
+      return set_err(CTB_ERR_ARG, "row %d: null or (hidden states) not 16-byte aligned", k);
+    W = std::max(W, (int)n_tokens[k]);
+  }
+  const int hop = h->vc.hop_length;
+  if (wav_ld < (int64_t)hop * (2 * W - 1)) return set_err(CTB_ERR_ARG, "wav_ld %lld < %d", (long long)wav_ld, hop * (2 * W - 1));
+  if ((size_t)B * 2 * W > h->max_rows)
+    return set_err(CTB_ERR_ARG, "B=%d rows x %d tokens exceed this handle's %zu frames", B, W, h->max_rows);
+  cudaStream_t s = (cudaStream_t)stream;
+  { int rc = dec_reserve(h, (size_t)B * 2 * W, s); if (rc) return rc; }
+  // one upload of the row table: [B] pointers then [B] frame counts (2 n_k).  From pageable memory the copy is staged
+  // before cudaMemcpyAsync returns, so the caller's arrays may go away; stream order protects the device table.
+  if (B > h->rows_meta_cap) {
+    CTB_CUDA(cudaStreamSynchronize(s));
+    if (h->rows_meta) { cudaFree(h->rows_meta); h->rows_meta = nullptr; h->rows_meta_cap = 0; }
+    CTB_CUDA(cudaMalloc(&h->rows_meta, (size_t)B * (sizeof(void*) + sizeof(int))));
+    h->rows_meta_cap = B;
+  }
+  std::vector<uint8_t> meta((size_t)B * (sizeof(void*) + sizeof(int)));
+  memcpy(meta.data(), rows_dev, (size_t)B * sizeof(void*));
+  int* fr_host = reinterpret_cast<int*>(meta.data() + (size_t)B * sizeof(void*));
+  for (int k = 0; k < B; ++k) fr_host[k] = 2 * n_tokens[k];
+  CTB_CUDA(cudaMemcpyAsync(h->rows_meta, meta.data(), meta.size(), cudaMemcpyHostToDevice, s));
+  const void* const* rows_d = static_cast<const void* const*>(h->rows_meta);
+  const int* fr = reinterpret_cast<const int*>(static_cast<uint8_t*>(h->rows_meta) + (size_t)B * sizeof(void*));
+  if (kind == 1) {
+    k_gather_hidden_rows<<<dim3(2 * W, B), 128, 0, s>>>(reinterpret_cast<const float* const*>(rows_d), fr, h->staged_in, W,
+                                                        c.idim);
+  } else {
+    GfsqRowsP g{};
+    g.rows = reinterpret_cast<const int32_t* const*>(rows_d); g.fr = fr; g.out = h->staged_in; g.W = W;
+    g.G = c.vq_groups; g.R = c.vq_residual; g.levels = c.vq_levels & 0xff; g.nlev = 4; g.per_group = c.vq_dim / c.vq_groups;
+    g.scale_base = (float)(((c.vq_levels >> 8) & 0xff) ? ((c.vq_levels >> 8) & 0xff) : (g.levels - 1));
+    g.w = h->dW + h->dl.vq_w; g.b = h->dW + h->dl.vq_b;
+    k_gfsq_dequant_rows<<<dim3(2 * W, B), 128, 0, s>>>(g);
+  }
+  CTB_LAUNCH_CHECK();
+  int rc;
+  if ((rc = dvae_run(h, h->staged_in, 1, B, W, nullptr, s, fr))) return rc;
+  return vocos_run(h, nullptr, B, 2 * W, wav_dev, s, fr, wav_ld);
 }
 
 // ------------------------------------------------------------------ DVAE encode branch (speaker enrolment)

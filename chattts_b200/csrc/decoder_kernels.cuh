@@ -25,6 +25,7 @@ struct GemmP {
   const float* gamma;        // GE_SCALE_RES: layer scale; GE_COEF: per-channel coefficient
   const float* res; int ldres;
   float* C; int ldc;
+  const int* fr;             // ragged mode: frames of each utterance (F = the widest); rows f >= fr[b] are written as 0
 };
 
 constexpr int GBM = 128, GBN = 128, GBK = 16;
@@ -33,7 +34,7 @@ __device__ __forceinline__ float gelu_erf(float x) {  // nn.GELU() default (exac
   return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f));
 }
 
-template <int EPI>
+template <int EPI, bool RAGGED = false>
 __global__ void __launch_bounds__(256) k_sgemm_nt(const GemmP p) {
   __shared__ __align__(16) float As[2][GBK][GBM];
   __shared__ __align__(16) float Bs[2][GBK][GBN];
@@ -118,10 +119,16 @@ __global__ void __launch_bounds__(256) k_sgemm_nt(const GemmP p) {
   for (int i = 0; i < 8; ++i) {
     const int m = m0 + ty * 4 + (i & 3) + (i >> 2) * 64;
     if (m >= p.M) continue;
+    bool pad_row = false;
+    if (RAGGED) { const int b = m / p.F; pad_row = m - b * p.F >= p.fr[b]; }
 #pragma unroll
     for (int jb = 0; jb < 2; ++jb) {
       const int n = n0 + tx * 4 + jb * 64;
       if (n >= p.N) continue;  // N is a multiple of 4 for every layer here
+      if (RAGGED && pad_row) {
+        *reinterpret_cast<float4*>(p.C + (size_t)m * p.ldc + n) = make_float4(0.f, 0.f, 0.f, 0.f);
+        continue;
+      }
       float v[4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) v[j] = acc[i][jb * 4 + j];
@@ -166,13 +173,22 @@ struct DwLnP {
   const float* b;     // [C]
   const float* lnw; const float* lnb;
   float eps;
+  const int* fr;      // ragged mode: frames of each utterance; rows f >= fr[b] are written as 0
 };
 
-template <int NV>
+// RAGGED: the taps stop at the utterance's own last frame, exactly as for F = fr[b] (no fmaf with a padding zero)
+template <int NV, bool RAGGED = false>
 __global__ void __launch_bounds__(256) k_dwconv_ln(const DwLnP p) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= p.M) return;
   const int m = warp, b = m / p.F, f = m - b * p.F;
+  const int Fb = RAGGED ? p.fr[b] : p.F;
+  if (RAGGED && f >= Fb) {
+#pragma unroll
+    for (int i = 0; i < NV; ++i)
+      *reinterpret_cast<float4*>(p.out + (size_t)m * p.C + (i * 32 + lane) * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+    return;
+  }
   float4 v[NV];
   if (p.taps == 0) {
 #pragma unroll
@@ -184,7 +200,7 @@ __global__ void __launch_bounds__(256) k_dwconv_ln(const DwLnP p) {
     const int half = p.taps / 2;
     for (int t = 0; t < p.taps; ++t) {
       const int ff = f + (t - half) * p.dil;
-      if (ff < 0 || ff >= p.F) continue;
+      if (ff < 0 || ff >= Fb) continue;
       const float* xr = p.x + ((size_t)b * p.F + ff) * p.C;
 #pragma unroll
       for (int i = 0; i < NV; ++i) {
@@ -304,14 +320,20 @@ __global__ void k_gfsq_dequant(const GfsqP p) {
 // torch.istft tail: overlap-add of windowed frames, divide by the window-square envelope, trim
 // n_fft/2 on both sides (center=True).  frames [B, F, n_fft] (already multiplied by the window
 // through the DFT basis) -> wav [B, hop * (F - 1)].
+// RAGGED: utterance b has fr[b] <= F frames (its envelope, trim and length follow them); wav is [B, wav_ld] and
+// row b receives hop * (fr[b] - 1) samples.
+template <bool RAGGED = false>
 __global__ void k_overlap_add(const float* __restrict__ frames, const float* __restrict__ window,
-                              float* __restrict__ wav, int B, int F, int n_fft, int hop) {
+                              float* __restrict__ wav, int B, int F, int n_fft, int hop, const int* __restrict__ fr = nullptr,
+                              int64_t wav_ld = 0) {
   const int L = hop * (F - 1);
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)B * L) return;
   const int b = (int)(i / L), j = (int)(i - (size_t)b * L);
+  const int Fb = RAGGED ? fr[b] : F;
+  if (RAGGED && j >= hop * (Fb - 1)) return;
   const int pidx = j + n_fft / 2;
-  const int f_hi = min(F - 1, pidx / hop);
+  const int f_hi = min(Fb - 1, pidx / hop);
   const int f_lo = pidx >= n_fft ? (pidx - n_fft) / hop + 1 : 0;
   float s = 0.f, env = 0.f;
   for (int f = f_lo; f <= f_hi; ++f) {
@@ -320,7 +342,59 @@ __global__ void k_overlap_add(const float* __restrict__ frames, const float* __r
     s += frames[((size_t)b * F + f) * n_fft + n];
     env = fmaf(w, w, env);
   }
-  wav[i] = s / env;
+  if (RAGGED)
+    wav[(size_t)b * wav_ld + j] = s / env;
+  else
+    wav[i] = s / env;
+}
+
+// Ragged-mode inputs, staged time-major [B, 2W, idim] with rows f >= 2 n_b zero (W = the widest row's tokens).
+// Hidden rows: token-major [n_b, 2 idim] fp32, whose frame doubling is a re-interpretation as [2 n_b, idim].
+__global__ void k_gather_hidden_rows(const float* const* __restrict__ rows, const int* __restrict__ fr,
+                                     float* __restrict__ out, int W, int idim) {
+  const int b = blockIdx.y, f = blockIdx.x;
+  float4* o = reinterpret_cast<float4*>(out + ((size_t)b * 2 * W + f) * idim);
+  const bool in = f < fr[b];
+  const float4* src = in ? reinterpret_cast<const float4*>(rows[b] + (size_t)f * idim) : nullptr;
+  for (int c = threadIdx.x; c < idim / 4; c += blockDim.x) o[c] = in ? src[c] : make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+// GFSQ._embed of k_gfsq_dequant for ragged token-major codes: row b is [n_b, G*R] int32; frame (t, g) of row b goes to
+// staged row b * 2W + t * G + g.  The arithmetic is k_gfsq_dequant's, term for term (that kernel is left as it is).
+struct GfsqRowsP {
+  const int32_t* const* rows; const int* fr; float* out;
+  int W, G, R, levels, nlev, per_group;
+  float scale_base;
+  const float* w; const float* b;
+};
+__global__ void k_gfsq_dequant_rows(const GfsqRowsP p) {
+  const int frame = blockIdx.x;  // t * G + g of row blockIdx.y
+  const int b = blockIdx.y, g = frame % p.G, t = frame / p.G;
+  float* out = p.out + ((size_t)b * 2 * p.W + frame) * p.per_group;
+  if (frame >= p.fr[b]) {
+    for (int c = threadIdx.x; c < p.per_group; c += blockDim.x) out[c] = 0.f;
+    return;
+  }
+  float z[8];
+  for (int k = 0; k < p.nlev; ++k) z[k] = 0.f;
+  float sc = 1.f;
+  const float half = (float)(p.levels / 2);
+  const int32_t* ids = p.rows[b] + (size_t)t * p.G * p.R + g * p.R;
+  for (int r = 0; r < p.R; ++r) {
+    int id = ids[r];
+    for (int k = 0; k < p.nlev; ++k) {
+      const int li = id % p.levels;
+      id /= p.levels;
+      z[k] += (((float)li - half) / half) * sc;
+    }
+    sc /= p.scale_base;
+  }
+  for (int c = threadIdx.x; c < p.per_group; c += blockDim.x) {
+    const float* w = p.w + ((size_t)g * p.per_group + c) * p.nlev;
+    float a = 0.f;
+    for (int k = 0; k < p.nlev; ++k) a = fmaf(z[k], w[k], a);
+    out[c] = a + p.b[g * p.per_group + c];
+  }
 }
 
 // ---------------------------------------------------------------- DVAE encode branch (dvae.py:175-206,265-274,102-128)

@@ -36,6 +36,7 @@ struct TcGemmP {
   const float* bias; const float* gamma;
   const float* res; int ldres;
   float* C; int ldc;
+  const int* fr;              // ragged mode: frames of each utterance (F = the widest); rows f >= fr[b] are written as 0
 };
 
 
@@ -69,7 +70,10 @@ __device__ __forceinline__ void mbar_wait_or_trap(uint64_t* bar, uint32_t parity
     if (spin > (1u << 28)) __trap();   // a protocol bug must end the kernel, not hang the GPU
 }
 
-template <int EPI>
+// RAGGED: the utterances have fr[b] <= F frames each.  Rows past an utterance's end are written as exact zeros, so a
+// later tapped layer reads there what TMA's out-of-bounds fill gives an utterance decoded alone, and every output row
+// of the utterance is bit-identical to that decode (same tile origin, same operands, same k order).
+template <int EPI, bool RAGGED = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_tc_gemm(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_whi,
           const __grid_constant__ CUtensorMap map_wlo, const TcGemmP p) {
@@ -170,6 +174,14 @@ k_tc_gemm(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUt
       const int f = f0 + r0 + 8 * h;
       if (f >= p.F) continue;
       const size_t m = (size_t)b * p.F + f;
+      if (RAGGED && f >= p.fr[b]) {
+#pragma unroll
+        for (int j = 0; j < TC_BN / 8; ++j) {
+          const int n = n0 + 8 * j + 2 * (lane & 3);
+          if (n < p.N) *reinterpret_cast<float2*>(p.C + m * p.ldc + n) = make_float2(0.f, 0.f);
+        }
+        continue;
+      }
 #pragma unroll
       for (int j = 0; j < TC_BN / 8; ++j) {
         const int n = n0 + 8 * j + 2 * (lane & 3);
@@ -199,14 +211,15 @@ inline int tc_make_map(CUtensorMap* m, const float* base, int rank, const cuuint
   return CTB_OK;
 }
 
-// C[B*F rows, N] = epi(A (x) W^T): A time-major [B][F][lda], W given as tf32 hi / lo copies [N][K]
-template <int EPI>
+// C[B*F rows, N] = epi(A (x) W^T): A time-major [B][F][lda], W given as tf32 hi / lo copies [N][K].
+// fr (device [B], ragged mode): frames of each utterance, see k_tc_gemm.
+template <int EPI, bool RAGGED = false>
 inline int tc_gemm_launch(cudaStream_t s, const float* A, int lda, int B, int F, int N, int K, int taps, int Cin, int dil,
                           int pad, const float* W_hi, const float* W_lo, const float* bias, const float* gamma,
-                          const float* res, int ldres, float* C, int ldc) {
+                          const float* res, int ldres, float* C, int ldc, const int* fr = nullptr) {
   // CTB_TC_NONPERSISTENT=1: one tile per CTA, the schedule the persistent one is cross-checked against
   const bool persistent = getenv("CTB_TC_NONPERSISTENT") == nullptr;
-  { int arc = ensure_smem_attr((const void*)k_tc_gemm<EPI>, TC_SMEM_BYTES); if (arc) return arc; }
+  { int arc = ensure_smem_attr((const void*)k_tc_gemm<EPI, RAGGED>, TC_SMEM_BYTES); if (arc) return arc; }
   CUtensorMap ma, mh, ml;
   const cuuint64_t adims[3] = {(cuuint64_t)lda, (cuuint64_t)F, (cuuint64_t)B};
   const cuuint64_t astr[2] = {(cuuint64_t)lda * 4, (cuuint64_t)F * lda * 4};
@@ -220,11 +233,11 @@ inline int tc_gemm_launch(cudaStream_t s, const float* A, int lda, int B, int F,
   if ((rc = tc_make_map(&ml, W_lo, 2, wdims, wstr, wbox))) return rc;
   TcGemmP p{};
   p.N = N; p.K = K; p.taps = taps; p.Cin = Cin; p.dil = dil; p.pad = pad; p.F = F; p.B = B;
-  p.bias = bias; p.gamma = gamma; p.res = res; p.ldres = ldres; p.C = C; p.ldc = ldc;
+  p.bias = bias; p.gamma = gamma; p.res = res; p.ldres = ldres; p.C = C; p.ldc = ldc; p.fr = fr;
   static int sms = 0;
   if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
   const int total = ((N + TC_BN - 1) / TC_BN) * B * ((F + TC_BM - 1) / TC_BM);
-  k_tc_gemm<EPI><<<persistent ? std::min(total, sms) : total, TC_THREADS, TC_SMEM_BYTES, s>>>(ma, mh, ml, p);
+  k_tc_gemm<EPI, RAGGED><<<persistent ? std::min(total, sms) : total, TC_THREADS, TC_SMEM_BYTES, s>>>(ma, mh, ml, p);
   CTB_LAUNCH_CHECK();
   return CTB_OK;
 }

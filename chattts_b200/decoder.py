@@ -204,6 +204,43 @@ class TokenDecoder:
         self.dvae_decode(inp, layout, want_mel=False)
         return self.vocos_decode(None)
 
+    def decode_rows(self, rows: Sequence[torch.Tensor], kind: int) -> List[torch.Tensor]:
+        """Independent token sequences -> waveforms through ``ctb_decode_rows``; row k comes out bit-identical to
+        ``tokens_to_wav`` of that row alone.  kind 1: rows of [n_k, 2*idim] fp32 hidden states; kind 2: rows of
+        [n_k, num_vq] int32 codes, both token-major on the device (slices of the GPT engine's output buffers work as
+        they are).  Returns one [hop * (2 n_k - 1)] tensor per row (views into one buffer per call).  A batch larger
+        than the handle's max_batch * 2 * max_tokens frames is split into several calls."""
+        if kind not in (1, 2):
+            raise ValueError("kind: 1 = hidden states, 2 = codes")
+        dtype = torch.float32 if kind == 1 else torch.int32
+        rows = [r if r.dtype == dtype and r.is_contiguous() and r.device == self.device
+                else r.to(self.device, dtype).contiguous() for r in rows]
+        if any(r.dim() != 2 or r.shape[0] < 1 for r in rows):
+            raise ValueError("decode_rows: every row must be [n, C] with n >= 1")
+        lib = _lib.load()
+        hop, cap = self.vocos_cfg.hop_length, self.max_batch * 2 * self.max_tokens
+        out: List[torch.Tensor] = []
+        lo = 0
+        while lo < len(rows):
+            hi, W = lo, 0
+            while hi < len(rows) and (hi - lo + 1) * 2 * max(W, int(rows[hi].shape[0])) <= cap:
+                W = max(W, int(rows[hi].shape[0]))
+                hi += 1
+            if hi == lo:
+                raise ValueError(f"a row of {int(rows[lo].shape[0])} tokens exceeds this handle "
+                                 f"(max_tokens={self.max_tokens})")
+            part = rows[lo:hi]
+            ld = hop * (2 * W - 1)
+            wav = torch.empty(len(part), ld, dtype=torch.float32, device=self.device)
+            ptrs = (C.c_void_p * len(part))(*[r.data_ptr() for r in part])
+            ns = (C.c_int32 * len(part))(*[int(r.shape[0]) for r in part])
+            with torch.cuda.device(self.device):
+                _lib.check(lib.ctb_decode_rows(self._handle, kind, len(part), ptrs, ns, C.c_void_p(wav.data_ptr()), ld,
+                                               self._stream()))
+            out += [wav[k, : hop * (2 * int(r.shape[0]) - 1)] for k, r in enumerate(part)]
+            lo = hi
+        return out
+
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -455,6 +492,19 @@ def decode_to_wavs(result_list: Sequence[torch.Tensor], use_decoder: bool, decod
 STREAM_HALO_TOKENS = 56
 
 
+def stream_window(n_tokens: int, a: int, b: int, halo: int = STREAM_HALO_TOKENS):
+    """``(a, b, t0, t1)``: samples [a, b) of the decode of an `n_tokens` sequence, clamped to its 512 n - 256 samples,
+    and the tokens [t0, t1) they depend on (`halo` each side, clamped to the sequence, where the clamp reproduces the
+    true boundary).  Samples [a, b) are samples [a - 512 t0, b - 512 t0) of the decode of tokens [t0, t1) alone."""
+    total = 512 * n_tokens - 256
+    a, b = max(0, a), min(b, total)
+    t0 = max(0, a // 512 - halo)
+    t1 = min(n_tokens, (b + 511) // 512 + halo + 1)
+    if t1 - t0 < 2:  # a one-token window has a single frame pair: widen (the iSTFT needs >= 2 frames)
+        t0, t1 = max(0, t1 - 2), max(t1, min(n_tokens, t0 + 2))
+    return a, b, t0, t1
+
+
 def _pad_batch(result_list: Sequence[torch.Tensor], use_decoder: bool, dev, t0: int, t1: int):
     """Columns [t0, t1) of the zero-padded batch `decode_to_wavs` builds (quirk Q23 padding included)."""
     n = len(result_list)
@@ -487,12 +537,7 @@ def decode_to_wavs_window(result_list: Sequence[torch.Tensor], use_decoder: bool
     model = decoder if use_decoder else dvae
     eng = model.engine
     max_len = max(int(r.size(0)) for r in result_list)
-    total = 512 * max_len - 256
-    a, b = max(0, a), min(b, total)
-    t0 = max(0, a // 512 - halo)
-    t1 = min(max_len, (b + 511) // 512 + halo + 1)
-    if t1 - t0 < 2:  # a one-token window has a single frame pair: widen (the iSTFT needs >= 2 frames)
-        t0, t1 = max(0, t1 - 2), max(t1, min(max_len, t0 + 2))
+    a, b, t0, t1 = stream_window(max_len, a, b, halo)
     batch, layout = _pad_batch(result_list, use_decoder, eng.device, t0, t1)
     wav = eng.tokens_to_wav(batch, layout)
     return wav[:, a - 512 * t0: b - 512 * t0].cpu().numpy()

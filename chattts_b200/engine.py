@@ -6,6 +6,8 @@ decode chunks, and its slot is reused as soon as it finishes.  A request's token
 ``GPT.generate`` returns for it alone (B = 1, same ``manual_seed``), whatever else is in flight.
 
 The scheduling policy (``schedule``) is plain Python over a small device interface, so it can be driven by a stub.
+``stream_schedule`` runs the same policy and reconstructs, per request, the cumulative yields of
+``GPT.generate(stream=True)`` from the slots' token counts at each poll.
 """
 from __future__ import annotations
 
@@ -38,6 +40,7 @@ class Request:
     logits_processors: tuple = ()
     manual_seed: Optional[int] = None
     ensure_non_empty: bool = True
+    stream_batch: int = 24
 
     def __post_init__(self):
         if self.emb.dim() == 3:
@@ -48,6 +51,8 @@ class Request:
             raise ValueError("Request.emb must be [T, d] with T >= 1")
         if self.max_new_token < 1:
             raise ValueError("max_new_token must be >= 1")
+        if self.stream_batch < 1:
+            raise ValueError("stream_batch must be >= 1")
 
 
 @dataclass
@@ -70,17 +75,11 @@ class ScheduleStats:
     interrupted: bool = False
 
 
-def schedule(requests: Sequence[Request], dev, chunk: int, context=None,
-             stats: Optional[ScheduleStats] = None) -> Iterator[Tuple[int, Optional[int], int]]:
-    """Drive ``dev`` (``slots``, ``admit([(slot, request_index)])``, ``decode(n)``, ``status() -> SlotStatus``) until
-    every request has finished; yields ``(request_index, slot, n_tokens)`` as each one completes - the caller harvests
-    the slot's first ``n_tokens`` outputs before resuming the generator - or ``(request_index, None, 0)`` for a seeded
-    request whose first token is EOS (it ends empty, gpt.py:527).  An unseeded one with ``ensure_non_empty`` is queued
-    again instead.
-
-    Waiting requests enter free slots in order, lowest slot first, at every poll (every ``chunk`` decode steps).  On a
-    ``context`` interrupt the running requests are yielded with what they have so far and the waiting ones are dropped.
-    """
+def _poll_cycles(requests: Sequence[Request], dev, chunk: int, context=None,
+                 stats: Optional[ScheduleStats] = None) -> Iterator[Tuple[SlotStatus, List[Optional[int]], list]]:
+    """The scheduling policy of ``schedule``: yields once per poll ``(status, owner, ended)`` - the slots' status, the
+    request each slot held when it was read, and the requests that ended at this poll as ``(request_index, slot or
+    None, n_tokens, eos)``.  The slots of the ended requests are refilled only after the generator is resumed."""
     stats = stats if stats is not None else ScheduleStats()
     waiting = deque(range(len(requests)))
     owner: List[Optional[int]] = [None] * dev.slots
@@ -97,6 +96,8 @@ def schedule(requests: Sequence[Request], dev, chunk: int, context=None,
             stats.admitted += len(batch)
         st = dev.status()
         stats.decode_steps = st.steps_done
+        polled = list(owner)
+        ended = []
         freed = False
         for s in range(dev.slots):
             i = owner[s]
@@ -110,22 +111,74 @@ def schedule(requests: Sequence[Request], dev, chunk: int, context=None,
                     waiting.appendleft(i)  # regenerate (gpt.py:527-570); a fresh Philox seed is drawn at admission
                     stats.requeued += 1
                     continue
-                yield i, None, 0
+                ended.append((i, None, 0, True))
                 continue
             stats.tokens += st.end_idx[s]
-            yield i, s, st.end_idx[s]
+            ended.append((i, s, st.end_idx[s], bool(st.finish[s])))
         if freed and waiting:
+            yield st, polled, ended
             continue  # refill the freed slots before the next chunk
         running = [s for s in range(dev.slots) if owner[s] is not None]
-        if not running:
-            return
-        if context is not None and context.get():
+        interrupted = bool(running) and context is not None and context.get()
+        if interrupted:
             stats.interrupted = True
             for s in running:
                 stats.tokens += st.end_idx[s]
-                yield owner[s], s, st.end_idx[s]
+                ended.append((owner[s], s, st.end_idx[s], False))
+        yield st, polled, ended
+        if not running or interrupted:
             return
         dev.decode(chunk)
+
+
+def schedule(requests: Sequence[Request], dev, chunk: int, context=None,
+             stats: Optional[ScheduleStats] = None) -> Iterator[Tuple[int, Optional[int], int]]:
+    """Drive ``dev`` (``slots``, ``admit([(slot, request_index)])``, ``decode(n)``, ``status() -> SlotStatus``) until
+    every request has finished; yields ``(request_index, slot, n_tokens)`` as each one completes - the caller harvests
+    the slot's first ``n_tokens`` outputs before resuming the generator - or ``(request_index, None, 0)`` for a seeded
+    request whose first token is EOS (it ends empty, gpt.py:527).  An unseeded one with ``ensure_non_empty`` is queued
+    again instead.
+
+    Waiting requests enter free slots in order, lowest slot first, at every poll (every ``chunk`` decode steps).  On a
+    ``context`` interrupt the running requests are yielded with what they have so far and the waiting ones are dropped.
+    """
+    for _, _, ended in _poll_cycles(requests, dev, chunk, context, stats):
+        for i, s, n, _ in ended:
+            yield i, s, n
+
+
+def stream_schedule(requests: Sequence[Request], dev, chunk: int, context=None,
+                    stats: Optional[ScheduleStats] = None) -> Iterator[List[Tuple[int, Optional[int], int, bool]]]:
+    """``schedule``'s policy, yielding once per poll the list of ``(request_index, slot, n_tokens, last)``: for each
+    request, the yields ``GPT.generate(stream=True, stream_batch=r.stream_batch)`` makes for it alone, in its order,
+    as cumulative token counts (the slot's first ``n_tokens`` outputs; slot None: a seeded request that ended empty).
+
+    The static loop (gpt.py here, generate) yields at every multiple of ``stream_batch`` (from step 2 on) that the row
+    reaches unfinished, yields a boundary a second time when EOS follows it on the very next step, and ends with the
+    final yield; a row that stops at ``max_new_token`` is not finished there, so it gets no second yield.  Tokens only
+    ever append to a slot, so each poll rebuilds every boundary a slot crossed since the last one from its token count:
+    the yields do not depend on ``chunk``.  The slots' outputs stay in place until the generator is resumed."""
+    sent = [0] * len(requests)  # last boundary yielded per request
+    for st, owner, ended in _poll_cycles(requests, dev, chunk, context, stats):
+        out = []
+        for s, i in enumerate(owner):
+            if i is None:
+                continue
+            sb = requests[i].stream_batch
+            nxt = sent[i] + sb
+            if nxt < 2:  # step 1 (the prefill's token) is never a boundary
+                nxt += sb
+            # running: end_idx steps so far, all unfinished; EOS at step end_idx + 1; max_new: end_idx = max_new
+            while nxt <= st.end_idx[s]:
+                out.append((i, s, nxt, False))
+                sent[i] = nxt
+                nxt += sb
+        for i, s, n, eos in ended:
+            if s is not None and eos and n > 0 and n % requests[i].stream_batch == 0:
+                out.append((i, s, n, False))  # the boundary before the finishing step, again (gpt.py:381-384)
+            out.append((i, s, n, True))
+        if out:
+            yield out
 
 
 class EngineDevice:
@@ -196,12 +249,14 @@ class EngineDevice:
                                                   self.stream))
         return SlotStatus(list(self._state), self._end.tolist(), self._fin.tolist(), int(st.steps_done))
 
-    def harvest(self, slot: int, n: int):
-        """GenerationOutputs of the request in ``slot``: its first ``n`` ids and hidden states (copies)."""
+    def harvest(self, slot: int, n: int, copy: bool = True):
+        """GenerationOutputs of the request in ``slot``: its first ``n`` ids (int64 copies) and hidden states (copies,
+        or with ``copy=False`` views into the engine buffer, valid until the engine decodes or admits again)."""
         from .gpt import GPT
 
         ids = self.ids_out[slot, :n].to(torch.int64)
-        hid = [self.hid_out[slot, :n].clone()] if self.hid_out is not None else []
+        hid = ([self.hid_out[slot, :n].clone() if copy else self.hid_out[slot, :n]] if self.hid_out is not None
+               else [])
         return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid)
 
     def empty(self):

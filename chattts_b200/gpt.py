@@ -236,22 +236,73 @@ class GPT:
         samples EOS first yields empty outputs (``generate`` yields nothing then); an unseeded one with
         ``ensure_non_empty`` runs again.  The handle serves one generator at a time; ``generate`` may be called again
         once it is exhausted."""
-        from .engine import MIN_PROMPT_COLS, EngineDevice, Request, ScheduleStats, schedule
+        from .engine import EngineDevice, ScheduleStats, schedule
+
+        if stream:
+            raise ValueError("generate_continuous: stream=True is not supported; results are yielded per request "
+                             "(generate_continuous_stream streams)")
+        requests, S, chunk, context = self._engine_args("generate_continuous", requests, slots, infer_text, return_attn,
+                                                        context, chunk, 32)
+        if not requests:
+            return
+        with torch.cuda.device(self.device_gpt):
+            dev = EngineDevice(self, requests, S, max(r.max_new_token for r in requests), return_hidden)
+            self.last_schedule_stats = stats = ScheduleStats()  # admissions, decode steps (tools/bench_continuous.py)
+            for i, slot, n in schedule(requests, dev, chunk, context, stats):
+                yield i, (dev.empty() if slot is None else dev.harvest(slot, n))
+            if stats.interrupted:
+                self.logger.warning("generation is interrupted")
+
+    @torch.no_grad()
+    def generate_continuous_stream(self, requests, slots: Optional[int] = None, return_hidden=True, context=None,
+                                   chunk: Optional[int] = None, infer_text=False, return_attn=False):
+        """Streaming form of ``generate_continuous``: generator of ``(request_index, GenerationOutputs, last)``.
+
+        For each request the yields are exactly those ``generate(stream=True, stream_batch=r.stream_batch)`` makes for
+        it alone, in the same order: cumulative outputs every ``stream_batch`` steps while unfinished, the repeated
+        boundary when EOS follows it on the next step, then the final yield, which alone has ``last=True``.  Yields of
+        different requests interleave in poll order.  The engine polls every ``chunk`` steps (default:
+        CTB_DECODE_CHUNK, or the smallest ``stream_batch`` among the requests); the yields do not depend on it.
+        A seeded request that samples EOS first yields one empty final output.
+
+        ``ids`` are copies.  ``hiddens`` are views into the engine's buffer, like the narrowed views ``generate``
+        hands out: they stay valid until this generator is resumed (copy them to keep them)."""
+        for dev, batch in self._stream_polls(requests, slots, return_hidden, context, chunk, infer_text, return_attn):
+            for i, slot, n, last in batch:
+                yield i, (dev.empty() if slot is None else dev.harvest(slot, n, copy=False)), last
+
+    def _stream_polls(self, requests, slots=None, return_hidden=True, context=None, chunk=None, infer_text=False,
+                      return_attn=False):
+        """``(EngineDevice, [(request_index, slot, n_tokens, last)])`` once per poll (engine.stream_schedule): every
+        yield due at that poll, while the engine's buffers hold all of them."""
+        from .engine import EngineDevice, ScheduleStats, stream_schedule
+
+        requests, S, chunk, context = self._engine_args("generate_continuous_stream", requests, slots, infer_text,
+                                                        return_attn, context, chunk, None)
+        if not requests:
+            return
+        with torch.cuda.device(self.device_gpt):
+            dev = EngineDevice(self, requests, S, max(r.max_new_token for r in requests), return_hidden)
+            self.last_schedule_stats = stats = ScheduleStats()
+            for batch in stream_schedule(requests, dev, chunk, context, stats):
+                yield dev, batch
+            if stats.interrupted:
+                self.logger.warning("generation is interrupted")
+
+    def _engine_args(self, name, requests, slots, infer_text, return_attn, context, chunk, default_chunk):
+        """Checks shared by the slot-engine generators -> (requests, slots, chunk, context).  The poll interval is
+        `chunk`, else CTB_DECODE_CHUNK, else `default_chunk` (None: the smallest ``stream_batch``)."""
+        from .engine import MIN_PROMPT_COLS, Request
 
         if infer_text:
-            raise ValueError("generate_continuous: audio codes only (infer_text=True stays on generate)")
-        if stream:
-            raise ValueError("generate_continuous: stream=True is not supported; results are yielded per request")
+            raise ValueError(f"{name}: audio codes only (infer_text=True stays on generate)")
         if return_attn:
-            raise ValueError("generate_continuous: return_attn is not supported")
+            raise ValueError(f"{name}: return_attn is not supported")
         if not self._handle:
             raise _lib.CtbError("GPT weights not loaded")
         requests = list(requests)
-        if not requests:
-            return
         if not all(isinstance(r, Request) for r in requests):
             raise TypeError("requests must be chattts_b200.engine.Request objects")
-
         S = min(self.max_batch, len(requests)) if slots is None else int(slots)
         S = max(S, 2)
         if S > self.max_batch:
@@ -261,15 +312,11 @@ class GPT:
             if T0 > 1024 or T0 + r.max_new_token > self.max_context:
                 raise ValueError(f"prompt {int(r.emb.shape[0])} + max_new_token {r.max_new_token} exceed this handle "
                                  f"(max_context={self.max_context}; prompts up to 1024 tokens)")
-        chunk = int(os.environ.get("CTB_DECODE_CHUNK", "32")) if chunk is None else int(chunk)
-        context = context if context is not None else GPT.Context()
-        with torch.cuda.device(self.device_gpt):
-            dev = EngineDevice(self, requests, S, max(r.max_new_token for r in requests), return_hidden)
-            self.last_schedule_stats = stats = ScheduleStats()  # admissions, decode steps (tools/bench_continuous.py)
-            for i, slot, n in schedule(requests, dev, chunk, context, stats):
-                yield i, (dev.empty() if slot is None else dev.harvest(slot, n))
-            if stats.interrupted:
-                self.logger.warning("generation is interrupted")
+        if default_chunk is None:
+            default_chunk = min((r.stream_batch for r in requests), default=24)
+        env = os.environ.get("CTB_DECODE_CHUNK")
+        chunk = (int(env) if env else default_chunk) if chunk is None else int(chunk)
+        return requests, S, chunk, (context if context is not None else GPT.Context())
 
     # ------------------------------------------------------------------ the loop
     @torch.no_grad()

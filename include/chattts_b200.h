@@ -239,6 +239,16 @@ int ctb_dvae_decode(ctb_decoder* h, const void* in_dev, int32_t in_layout, int32
 /* Vocos.decode (core.py:505-510): mel [B,100,F] channels-first (NULL: the mel left in the handle by
  * the last ctb_dvae_decode) -> wav [B, hop*(F-1)] fp32 */
 int ctb_vocos_decode(ctb_decoder* h, const float* mel_dev, int32_t B, int32_t F, float* wav_dev, void* stream);
+/* Ragged batch of independent token sequences -> waveforms.  Row k is decoded exactly as ctb_dvae_decode +
+ * ctb_vocos_decode decode it alone (B = 1, T = n_tokens[k]): bit-identical, on either back end (CTB_DECODER_FMA).
+ *   kind 1: rows_dev[k] -> [n_k, 2*idim] fp32 token-major hidden states (e.g. a slice of the engine's hiddens_out),
+ *           16-byte aligned
+ *   kind 2: rows_dev[k] -> [n_k, num_vq] int32 token-major codes (e.g. a slice of the engine's ids_out)
+ *   rows_dev, n_tokens: host arrays of B entries, n_k >= 1; they may be released on return
+ *   wav_dev [B, wav_ld] fp32: row k receives hop*(2 n_k - 1) samples; the rest of the row is not written.
+ * CTB_ERR_ARG when B * 2 * max(n_k) exceeds the handle's max_batch * 2 * max_tokens frames.  Needs both weight sets. */
+int ctb_decode_rows(ctb_decoder* h, int32_t kind, int32_t B, const void* const* rows_dev, const int32_t* n_tokens,
+                    float* wav_dev, int64_t wav_ld, void* stream);
 
 /* ---- waveform -> codes: replaces DVAE.forward(mode="encode") (ChatTTS/model/dvae.py:265-274), i.e. ------
  * MelSpectrogramFeatures (dvae.py:175-206; n_fft 1024, hop 256, 100 mel bins, center/reflect, power 1, log(clip 1e-5))

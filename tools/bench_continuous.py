@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Continuous-batching benchmark: the slot engine against static batches, one JSON line.
 
-    python tools/bench_continuous.py [--requests N] [--slots S] [--steps K] [--warmup W] [--dump-outputs DIR]
+    python tools/bench_continuous.py [--requests N] [--slots S] [--steps K] [--warmup W] [--dump-outputs DIR] [--stream]
 
 N requests (default 128), each one utterance with its own seeded prompt (8..128 tokens) and forced length (64..1024
 tokens, min_new = max_new: synthetic weights have no meaningful EOS), run through the slot engine with S slots
@@ -9,6 +9,16 @@ tokens, min_new = max_new: synthetic weights have no meaningful EOS), run throug
 run to their longest row (``GPT.generate``).  Reports useful speech-tokens/s of both arms (the tokens the requests
 asked for), mean slot occupancy, the card and its power limit.  ``--steps`` = timed repeats of each arm, alternating.
 ``--dump-outputs DIR`` writes both arms' ids (concatenated in request order) and the lengths as DIR/<name>.npy.
+
+``--stream`` then prints a second JSON line: the same requests streamed as audio (hidden path, DVAE decoder and Vocos
+from synthetic weights, InferCodeParams' default stream_batch / stream_speed / pass_first_n_batches), timed
+alternately in three arms: (a) the streaming engine with one ragged ``decode_rows`` call per poll, (b) the same engine
+with one ``decode_to_wavs_window`` call per window, (c) the non-streaming engine without path 2.  Per arm: wall time,
+useful speech-tokens/s, seconds of audio delivered per wall second, time to first chunk from admission and from start
+(p50 / p95 / max), playback underruns (chunks that arrive after the request's earlier chunks have finished playing,
+counted from its first chunk) and the share of wall time in path 2.  (a) and (b) must yield the same chunks; with
+``--dump-outputs`` the chunks of (a) are written as stream_chunks.npy (concatenated in yield order),
+stream_chunk_index.npy and stream_chunk_lengths.npy.
 """
 from __future__ import annotations
 
@@ -143,6 +153,136 @@ def run_continuous(args, local_rank: int = 0):
     }
 
 
+def run_stream(args, local_rank: int = 0):
+    """Streamed audio on the slot engine, three arms timed alternately in this process (see the module docstring)."""
+    import numpy as np
+
+    from chattts_b200.config import Config
+    from chattts_b200.core import Chat, StreamWindows, stream_continuous
+    from chattts_b200.decoder import DVAE, Vocos
+    from chattts_b200.embed import Embed
+    from chattts_b200.engine import EngineDevice, Request
+    from chattts_b200.gpt import GPT
+    from chattts_b200.processors import gen_logits
+    from chattts_b200.prompts import synth_prompt_batch
+    from chattts_b200.synth import synth_dvae_state, synth_embed_state, synth_gpt_state, synth_vocos_state
+
+    dev = torch.device("cuda", local_rank)
+    torch.cuda.set_device(dev)
+    n, S, cfg = args.requests, args.slots, Config()
+    plen, tok = continuous_workload(n, seed=7)
+    embed = Embed(768, 626, 21178, 4).load_state_dict(synth_embed_state(1)).to(dev)
+    gpt = GPT(cfg.gpt, embed, device=dev, device_gpt=dev, max_batch=S, max_context=max(plen) + max(tok))
+    gpt.load_state(synth_gpt_state(0))
+    voc = Vocos(cfg.vocos, dev, max_batch=S, max_tokens=256).load_state_dict(synth_vocos_state(5))
+    dec = DVAE(cfg.decoder, dim=cfg.decoder.idim, device=dev, vocos=voc, max_batch=S, max_tokens=256)
+    dec.load_state_dict(synth_dvae_state(2, cfg.decoder, cfg.decoder.idim))
+    p = Chat.InferCodeParams()
+    warp, proc = gen_logits(num_code=625, top_P=0.7, top_K=20, repetition_penalty=1.05)
+    procs, temp = (*proc, *warp), [0.3] * 4
+    embs = []
+    for i, L in enumerate(plen):
+        ids, _, tmask = synth_prompt_batch([L], seed=1000 + i)
+        embs.append(embed(ids, tmask)[0])
+
+    def requests(lengths):
+        return [Request(emb=embs[i], temperature=temp, eos_token=625, max_new_token=lengths[i],
+                        min_new_token=lengths[i], logits_processors=procs, manual_seed=5000 + i,
+                        stream_batch=p.stream_batch) for i in range(len(lengths))]
+
+    admitted = {}
+    admit = EngineDevice.admit
+
+    def timed_admit(self, batch):  # admission time of each request, for the time to first chunk
+        t = time.perf_counter()
+        for _, i in batch:
+            admitted.setdefault(i, t)
+        admit(self, batch)
+
+    EngineDevice.admit = timed_admit
+
+    def stream_arm(lengths, ragged):
+        admitted.clear()
+        stats, chunks, arrive = {}, [], []
+        windows = [StreamWindows(p.stream_speed, p.pass_first_n_batches) for _ in lengths]
+        t0 = time.perf_counter()
+        for i, chunk, _ in stream_continuous(gpt, dec, requests(lengths), windows, True, slots=S, ragged=ragged,
+                                             stats=stats):
+            chunks.append((i, chunk))
+            arrive.append(time.perf_counter())
+        wall = time.perf_counter() - t0
+        return dict(wall=wall, t0=t0, chunks=chunks, arrive=arrive, admitted=dict(admitted),
+                    path2=stats.get("path2_s", 0.0))
+
+    def plain_arm(lengths):
+        t0 = time.perf_counter()
+        for _ in gpt.generate_continuous(requests(lengths), slots=S, return_hidden=True):
+            pass
+        torch.cuda.synchronize()
+        return dict(wall=time.perf_counter() - t0)
+
+    short = [min(t, 96) for t in tok[: 2 * S]]
+    for _ in range(max(1, min(args.warmup, 2))):
+        stream_arm(short, True)
+        stream_arm(short, False)
+        plain_arm(short)
+    runs = {"a": [], "b": [], "c": []}
+    for _ in range(args.steps):
+        runs["a"].append(stream_arm(tok, True))
+        runs["b"].append(stream_arm(tok, False))
+        runs["c"].append(plain_arm(tok))
+    ca, cb = runs["a"][-1]["chunks"], runs["b"][-1]["chunks"]
+    per = lambda ch: {i: [c for j, c in ch if j == i] for i in range(n)}  # noqa: E731
+    pa, pb = per(ca), per(cb)
+    assert all(len(pa[i]) == len(pb[i]) and all(np.array_equal(x, y) for x, y in zip(pa[i], pb[i])) for i in range(n)), \
+        "arms (a) and (b) yield different chunks"
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {
+            "stream_chunks": np.concatenate([c[0] for _, c in ca]) if ca else np.zeros(0, np.float32),
+            "stream_chunk_index": np.array([i for i, _ in ca], dtype=np.int64),
+            "stream_chunk_lengths": np.array([c.shape[1] for _, c in ca], dtype=np.int64)})
+    sr = 24000.0
+    med = lambda v: sorted(v)[len(v) // 2]  # noqa: E731
+    pct = lambda v, q: float(np.percentile(np.asarray(v), q)) if v else None  # noqa: E731
+    useful = sum(tok)
+
+    def summary(r):
+        first, under = {}, 0
+        played = {}
+        for (i, c), t in zip(r["chunks"], r["arrive"]):
+            if c.shape[1] == 0:
+                continue
+            if i not in first:
+                first[i], played[i] = t, 0.0
+            elif t > first[i] + played[i]:
+                under += 1
+            played[i] += c.shape[1] / sr
+        ttfc_adm = [first[i] - r["admitted"][i] for i in first]
+        ttfc_start = [first[i] - r["t0"] for i in first]
+        audio = sum(c.shape[1] for _, c in r["chunks"]) / sr
+        q = lambda v: {"p50": round(pct(v, 50), 4), "p95": round(pct(v, 95), 4), "max": round(max(v), 4)}  # noqa: E731
+        return {"seconds": round(r["wall"], 3), "tokens_per_s": round(useful / r["wall"], 1),
+                "audio_s_per_wall_s": round(audio / r["wall"], 2), "chunks": len(r["chunks"]),
+                "ttfc_from_admission_s": q(ttfc_adm), "ttfc_from_start_s": q(ttfc_start), "underruns": under,
+                "path2_share": round(r["path2"] / r["wall"], 4)}
+
+    out = {"metric": "continuous_stream", "card": None, "power_limit": None, "requests": n, "slots": S,
+           "stream_batch": p.stream_batch, "stream_speed": p.stream_speed,
+           "pass_first_n_batches": p.pass_first_n_batches, "useful_tokens": useful, "repeats": args.steps}
+    for arm in ("a", "b"):
+        rs = runs[arm]
+        pick = sorted(rs, key=lambda r: r["wall"])[len(rs) // 2]  # the median run
+        out[arm] = summary(pick)
+        out[arm]["seconds_all"] = [round(r["wall"], 3) for r in rs]
+    tc = med([r["wall"] for r in runs["c"]])
+    out["c"] = {"seconds": round(tc, 3), "tokens_per_s": round(useful / tc, 1),
+                "seconds_all": [round(r["wall"], 3) for r in runs["c"]]}
+    out["a_over_b_speedup"] = round(out["b"]["seconds"] / out["a"]["seconds"], 3)
+    out["card"], out["power_limit"] = gpu_card(local_rank)
+    EngineDevice.admit = admit
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--requests", type=int, default=128)
@@ -150,10 +290,14 @@ def main():
     ap.add_argument("--steps", type=int, default=3, help="timed repeats of each arm")
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--dump-outputs", default=None, metavar="DIR")
+    ap.add_argument("--stream", action="store_true", help="also measure streamed audio (a second JSON line)")
     args = ap.parse_args()
     if args.steps < 1:
         ap.error("--steps must be >= 1")
-    print(json.dumps(run_continuous(args, int(os.environ.get("LOCAL_RANK", "0")))), flush=True)
+    rank = int(os.environ.get("LOCAL_RANK", "0"))
+    print(json.dumps(run_continuous(args, rank)), flush=True)
+    if args.stream:
+        print(json.dumps(run_stream(args, rank)), flush=True)
 
 
 if __name__ == "__main__":
