@@ -203,33 +203,62 @@ class Chat:
 
     def infer_continuous(self, texts, params_infer_code=None, use_decoder=True, slots=None, stream=False, lang=None,
                          skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
-                         params_refine_text=None):
+                         params_refine_text=None, refine_on_engine=False):
         """Synthesise many texts with continuous batching (``GPT.generate_continuous``): each text is one request,
         ``params_infer_code`` is one ``InferCodeParams`` for all texts or a list with one per text (speaker, seed,
         temperature, top-P/K, penalty, token limits).  Generator of ``(index, wav)`` in completion order; ``wav`` is
         what ``infer([texts[index]], split_text=False, skip_refine_text=True)`` returns for that text with its params.
-        Normalisation and the optional text refinement run as in ``infer``."""
+        Normalisation and the optional text refinement run as in ``infer``; ``params_refine_text`` is one
+        ``RefineTextParams`` or one per text.
+
+        With ``skip_refine_text=False`` the texts are refined first, in static batches of up to ``max_batch`` texts,
+        and no speech code starts before every text is refined.  ``refine_on_engine=True`` refines each text as a
+        request of its own on the slot engine instead, and its speech codes follow as soon as its refinement ends:
+        ``wav`` is then what ``infer([texts[index]], split_text=False, skip_refine_text=False)`` returns with that
+        text's params.  A seeded refinement depends on the batch it is drawn in, so the two modes give different
+        seeded results; the batched one stays the default."""
         if stream:
             raise ValueError("infer_continuous: stream=True is not supported; each waveform is yielded when complete "
                              "(infer_continuous_stream streams)")
         texts, params = self._continuous_params(texts, params_infer_code)
         return self._infer_continuous(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
-                                      do_homophone_replacement, params_refine_text or Chat.RefineTextParams())
+                                      do_homophone_replacement, self._refine_params(texts, params_refine_text),
+                                      refine_on_engine)
 
     def infer_continuous_stream(self, texts, params_infer_code=None, use_decoder=True, slots=None, lang=None,
                                 skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
-                                params_refine_text=None):
+                                params_refine_text=None, refine_on_engine=False):
         """Streaming synthesis of many texts with continuous batching (``GPT.generate_continuous_stream``).
         Generator of ``(index, chunk, last)``, ``chunk`` a ``[1, n]`` float32 array; for each text the chunks are
         those ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=True)`` yields with that
         text's params (its own ``stream_batch``, ``stream_speed`` and ``pass_first_n_batches``), and ``last`` marks
         its final chunk.  A seeded text whose first code is EOS yields one empty final chunk.  All windows due at one
         engine poll are decoded in one ragged call (``TokenDecoder.decode_rows``), straight from the engine's
-        buffers.  Arguments as for ``infer_continuous``."""
+        buffers.  Arguments as for ``infer_continuous``; with ``refine_on_engine=True`` the chunks are those of
+        ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=False)``."""
         texts, params = self._continuous_params(texts, params_infer_code)
         return self._infer_continuous_stream(texts, params, use_decoder, slots, lang, skip_refine_text,
                                              do_text_normalization, do_homophone_replacement,
-                                             params_refine_text or Chat.RefineTextParams())
+                                             self._refine_params(texts, params_refine_text), refine_on_engine)
+
+    def refine_continuous(self, texts, params_refine_text=None, slots=None, lang=None, do_text_normalization=True,
+                          do_homophone_replacement=True):
+        """Refine many texts on the slot engine, each as a request of its own: generator of ``(index, refined_text)``
+        in completion order.  ``refined_text`` is what ``infer([texts[index]], refine_text_only=True,
+        split_text=False, params_refine_text=...)[0]`` returns for that text; ``params_refine_text`` is one
+        ``RefineTextParams`` or one per text."""
+        if isinstance(texts, str):
+            texts = [texts]
+        texts = list(texts)
+        refine = self._refine_params(texts, params_refine_text)
+        assert self.has_loaded()
+        self.context.set(False)
+        if not texts:
+            return
+        texts = [self.normalizer(t, do_text_normalization, do_homophone_replacement, lang) for t in texts]
+        requests = [self._refine_request(t, r) for t, r in zip(texts, refine)]
+        for i, out in self.gpt.generate_continuous(requests, slots=slots, return_hidden=False, context=self.context):
+            yield i, self._refined_text(out)
 
     @staticmethod
     def _continuous_params(texts, params_infer_code):
@@ -242,47 +271,75 @@ class Chat:
             return texts, list(params_infer_code)
         return texts, [params_infer_code or Chat.InferCodeParams()] * len(texts)
 
+    @staticmethod
+    def _refine_params(texts, params_refine_text):
+        if isinstance(params_refine_text, (list, tuple)):
+            if len(params_refine_text) != len(texts):
+                raise ValueError("params_refine_text: one RefineTextParams per text")
+            return list(params_refine_text)
+        return [params_refine_text or Chat.RefineTextParams()] * len(texts)
+
     def _continuous_requests(self, texts, params, use_decoder, lang, skip_refine_text, do_text_normalization,
-                             do_homophone_replacement, params_refine_text):
-        """Normalisation, optional refinement and one engine request per text (as ``_infer`` prepares them)."""
+                             do_homophone_replacement, refine, refine_on_engine=False):
+        """Normalisation, optional refinement and one engine request per text (as ``_infer`` prepares them) ->
+        (requests, max_new_cap).  With ``refine_on_engine`` (and refinement on) each request refines its text and
+        names the text's speech-code request as its follow-up."""
         assert self.has_loaded(use_decoder=use_decoder)
         self.context.set(False)
         if not texts:
-            return []
+            return [], 0
         texts = [self.normalizer(t, do_text_normalization, do_homophone_replacement, lang) for t in texts]
+        cap = max(p.max_new_token for p in params)
+        if not skip_refine_text and refine_on_engine:
+            requests = []
+            for t, p, r in zip(texts, params, refine):
+                req = self._refine_request(t, r)
+                req.then = lambda out, p=p: self._code_request(self._refined_text(out), p)
+                req.stream_batch = p.stream_batch  # the engine polls at the smallest stream_batch of its requests
+                requests.append(req)
+            return requests, max(cap, max(r.max_new_token for r in requests))
         if not skip_refine_text:
+            if any(r is not refine[0] for r in refine):
+                raise ValueError("one RefineTextParams per text needs refine_on_engine=True (batched refinement "
+                                 "draws every text of a batch with one set of parameters)")
             tokens = []
             for lo in range(0, len(texts), self.gpt.max_batch):
-                refined = self._refine_text(texts[lo: lo + self.gpt.max_batch], self.device, params_refine_text)
+                refined = self._refine_text(texts[lo: lo + self.gpt.max_batch], self.device, refine[0])
                 tokens += [i[i.less(self.tokenizer.break_0_ids)] for i in refined.ids]
                 refined.destroy()
             texts = self.tokenizer.decode(tokens)
-        return [self._code_request(t, p) for t, p in zip(texts, params)]
+        return [self._code_request(t, p) for t, p in zip(texts, params)], cap
 
     def _infer_continuous_stream(self, texts, params, use_decoder, slots, lang, skip_refine_text,
-                                 do_text_normalization, do_homophone_replacement, params_refine_text):
-        requests = self._continuous_requests(texts, params, use_decoder, lang, skip_refine_text, do_text_normalization,
-                                             do_homophone_replacement, params_refine_text)
+                                 do_text_normalization, do_homophone_replacement, refine, refine_on_engine=False):
+        requests, cap = self._continuous_requests(texts, params, use_decoder, lang, skip_refine_text,
+                                                  do_text_normalization, do_homophone_replacement, refine,
+                                                  refine_on_engine)
         if not requests:
             return
         windows = [StreamWindows(p.stream_speed, p.pass_first_n_batches) for p in params]
         yield from stream_continuous(self.gpt, self.decoder if use_decoder else self.dvae, requests, windows,
-                                     use_decoder, slots, self.context)
+                                     use_decoder, slots, self.context, max_new_cap=cap)
 
     def _infer_continuous(self, texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
-                          do_homophone_replacement, params_refine_text):
-        requests = self._continuous_requests(texts, params, use_decoder, lang, skip_refine_text, do_text_normalization,
-                                             do_homophone_replacement, params_refine_text)
+                          do_homophone_replacement, refine, refine_on_engine=False):
+        requests, cap = self._continuous_requests(texts, params, use_decoder, lang, skip_refine_text,
+                                                  do_text_normalization, do_homophone_replacement, refine,
+                                                  refine_on_engine)
         if not requests:
             return
         thr = np.float32(1e-5)
         with torch.no_grad():
             for i, out in self.gpt.generate_continuous(requests, slots=slots, return_hidden=use_decoder,
-                                                       context=self.context):
+                                                       context=self.context, max_new_cap=cap):
+                k = _text_index(self.gpt, requests, i)
+                if k is None:  # a refinement stage: its follow-up carries the text on
+                    out.destroy()
+                    continue
                 res = out.hiddens if use_decoder else out.ids
                 wav = self._decode_to_wavs(res, use_decoder)[0] if int(res[0].shape[0]) > 0 else np.zeros(0, np.float32)
                 out.destroy()
-                yield i, wav[np.abs(wav) > thr]  # quirk Q20, as infer() returns it
+                yield k, wav[np.abs(wav) > thr]  # quirk Q20, as infer() returns it
 
     def _code_request(self, text, params):
         """The request ``_infer_code([text], ...)`` would decode as a batch of one."""
@@ -305,6 +362,26 @@ class Chat:
                        max_new_token=params.max_new_token, min_new_token=params.min_new_token,
                        logits_processors=(*processors, *warpers), manual_seed=params.manual_seed,
                        ensure_non_empty=params.ensure_non_empty, stream_batch=params.stream_batch)
+
+    def _refine_request(self, text, params):
+        """The text request ``_refine_text([text], ...)`` would generate as a batch of one."""
+        from .engine import Request
+
+        input_ids, attention_mask, text_mask = self.tokenizer.encode(
+            self.speaker.decorate_text_prompts([text], params.prompt), self.config.gpt.num_vq, device=self.device_gpt)
+        warpers, processors = gen_logits(num_code=self.tokenizer.len, top_P=params.top_P, top_K=params.top_K,
+                                         repetition_penalty=params.repetition_penalty)
+        emb = self.embed(input_ids, text_mask)
+        valid = attention_mask[0].to(torch.bool).cpu()
+        return Request(emb=emb[0][valid.to(emb.device)], temperature=[params.temperature],
+                       eos_token=self.tokenizer.eos_token, max_new_token=params.max_new_token,
+                       min_new_token=params.min_new_token, logits_processors=(*processors, *warpers),
+                       manual_seed=params.manual_seed, ensure_non_empty=params.ensure_non_empty, infer_text=True)
+
+    def _refined_text(self, out) -> str:
+        """The text ``_infer`` makes of one refined row: ids below ``break_0_ids``, decoded."""
+        ids = out.ids[0]
+        return self.tokenizer.decode([ids[ids.less(self.tokenizer.break_0_ids)]])[0]
 
     def interrupt(self):
         self.context.set(True)
@@ -459,9 +536,19 @@ class StreamWindows:
         return out
 
 
+def _text_index(gpt: GPT, requests, i: int) -> Optional[int]:
+    """Engine request index -> index of the text it speaks (a follow-up speaks its parent's text); None for a text
+    request (a refinement stage)."""
+    if i < len(requests):
+        return None if requests[i].infer_text else i
+    return {c: p for p, c in gpt.last_schedule_stats.children.items()}[i]
+
+
 def stream_continuous(gpt: GPT, model: DVAE, requests, windows: List[StreamWindows], use_decoder: bool, slots=None,
-                      context=None, ragged: bool = True, stats: Optional[Dict[str, float]] = None):
+                      context=None, ragged: bool = True, stats: Optional[Dict[str, float]] = None,
+                      max_new_cap: Optional[int] = None):
     """Streamed audio of many requests on the slot engine: generator of ``(request_index, chunk [1, n] float32, last)``.
+    Text requests stream nothing; a follow-up's chunks come under its parent's index, with its parent's windows.
 
     At every engine poll the windows of every GPT yield due then (``GPT._stream_polls``) are decoded together: each
     window's token range (``decoder.stream_window``) is read straight from the engine's hidden states (``model`` =
@@ -472,13 +559,16 @@ def stream_continuous(gpt: GPT, model: DVAE, requests, windows: List[StreamWindo
     import time
 
     thr = np.float32(1e-5)
-    for dev, batch in gpt._stream_polls(requests, slots, use_decoder, context):
+    for dev, batch in gpt._stream_polls(requests, slots, use_decoder, context, max_new_cap=max_new_cap):
         t_start = time.perf_counter()
         buf = dev.hid_out if use_decoder else dev.ids_out
-        jobs = []  # (request, slot, n_tokens, a, b, flush, last)
+        jobs = []  # (text, slot, n_tokens, a, b, flush, last)
         for i, s, n, last in batch:
-            ws = windows[i].windows(n, last)
-            jobs += [(i, s, n, a, b, flush, last and k == len(ws) - 1) for k, (a, b, flush) in enumerate(ws)]
+            t = _text_index(gpt, requests, i)
+            if t is None:
+                continue
+            ws = windows[t].windows(n, last)
+            jobs += [(t, s, n, a, b, flush, last and k == len(ws) - 1) for k, (a, b, flush) in enumerate(ws)]
         due = [k for k, j in enumerate(jobs) if j[4] > j[3]]
         chunks: Dict[int, np.ndarray] = {}
         if due and ragged:

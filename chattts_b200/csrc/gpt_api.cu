@@ -98,9 +98,21 @@ struct ctb_gpt {
   int phase;                  // rows the heads / sampler / finalize serve: RS_RUNNING (decode) or RS_PENDING (admission)
   RowState* rows;             // [Bpad] per-slot loop state
   ctb_sampler_config* cfgs;   // [max_batch] per-slot sampling parameters
-  float* eng_noise;           // [max_batch * num_vq, num_audio] per-slot Exp(1) rows
+  float* eng_noise;           // [max_batch, noise_stride(h)] per-slot Exp(1) rows ([num_vq, num_audio] or [1, num_text])
   int* eng_slot;              // [max_batch] slot of each prompt of the admission being prefilled
+  float* eng_text_logits;     // [max_batch, num_text] text-head logits of text slots (h->logits holds the code rows)
+  int32_t* eng_text_idx;      // [max_batch] the text sampler's ids
+  // 1 while a text slot may be pending or running (set by ctb_gpt_engine_admit_text, cleared by the status read that
+  // finds none): steps carry the text head / sampler launches only then, from their own captured graph
+  int eng_text;
+  cudaGraphExec_t graph_exec_text;
+  uint64_t graph_kernels_text;
 };
+
+// floats of one slot's noise in the engine's buffer: room for a code request's or a text request's rows
+static size_t noise_stride(const ctb_gpt* h) {
+  return std::max((size_t)h->cfg.num_vq * h->cfg.num_audio_tokens, (size_t)h->cfg.num_text_tokens);
+}
 
 extern "C" int ctb_abi_version(void) { return CTB_ABI_VERSION; }
 extern "C" const char* ctb_last_error(void) { return g_err; }
@@ -324,12 +336,13 @@ extern "C" int ctb_gpt_create(const ctb_gpt_config* c, const float* weights_dev,
 extern "C" int ctb_gpt_destroy(ctb_gpt* h) {
   if (!h) return CTB_OK;
   if (h->graph_exec) cudaGraphExecDestroy(h->graph_exec);
+  if (h->graph_exec_text) cudaGraphExecDestroy(h->graph_exec_text);
   if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
   void* ptrs[] = {h->x, h->qbuf, h->attn, h->mlp, h->logits, h->kv, h->part, h->block_table, h->seq_len,
                   h->pos, h->counter, h->end_idx, h->idx, h->active, h->finish, h->st, h->tc_wqkv, h->tc_wgu,
                   h->tc_heads_code, h->tc_heads_text, h->x_hi, h->x_lo, h->attn_hi, h->attn_lo, h->h_hi, h->h_lo, h->bar, h->trace, h->flow_arena, h->flow_epoch, h->gw_hi, h->gw_lo, h->pf_resid, h->pf_xn, h->pf_qkv, h->pf_q,
                   h->pf_attn, h->pf_gu, h->pf_h, h->pf_ones, h->pf_zeros, h->pf_npre, h->pf_nvalid,
-                  h->rows, h->cfgs, h->eng_noise, h->eng_slot};
+                  h->rows, h->cfgs, h->eng_noise, h->eng_slot, h->eng_text_logits, h->eng_text_idx};
   delete[] h->m_wqkv; delete[] h->m_wo; delete[] h->m_wgu; delete[] h->m_wd;
   for (void* p : ptrs) if (p) cudaFree(p);
   delete h;
@@ -513,6 +526,13 @@ static int launch_heads(ctb_gpt* h, const StepCtx& x, cudaStream_t s) {
   hp.normw = h->W + h->lay.final_norm; hp.out = h->logits; hp.rows_per_item = rpi; hp.V = V;
   hp.hidden_out = h->hiddens_out; hp.hidden_stride = h->max_new * c.hidden_size;
   hp.rows = h->engine ? h->rows : nullptr; hp.want = h->phase;
+  const int rc = launch_gemv<EPI_HEADS>(x.bt, hp, x.ntiles, s);
+  if (rc || !h->engine || !h->eng_text) return rc;
+  // slot engine: the code heads above served the code rows; the text head serves the text rows, into its own logits
+  // buffer and without hidden states (its CTAs leave at once when no text row is in state `phase`)
+  hp.W = h->W + h->lay.head_text; hp.nrows = c.num_text_tokens; hp.ntasks = (hp.nrows + 1) / 2;
+  hp.out = h->eng_text_logits; hp.rows_per_item = 1; hp.V = c.num_text_tokens; hp.hidden_out = nullptr;
+  hp.want = h->phase | WANT_TEXT;
   return launch_gemv<EPI_HEADS>(x.bt, hp, x.ntiles, s);
 }
 
@@ -524,7 +544,14 @@ static int launch_sampler(ctb_gpt* h, const StepCtx& x, cudaStream_t s) {
   sp.V = h->infer_text ? c.num_text_tokens : c.num_audio_tokens;
   sp.rows_per_item = rpi; sp.cfg = h->sampler; sp.q_noise = h->q_noise; sp.gen_ids = h->ids_out;
   sp.gen_stride = h->max_new; sp.gen_inner = c.num_vq; sp.out_idx = h->idx;
-  if (h->engine) { sp.rstate = h->rows; sp.cfgs = h->cfgs; sp.want = h->phase; sp.q_noise = h->eng_noise; }
+  if (!h->engine) return launch_sample(sp, s);
+  sp.rstate = h->rows; sp.cfgs = h->cfgs; sp.want = h->phase; sp.q_noise = h->eng_noise;
+  sp.noise_stride = (int)noise_stride(h);
+  const int rc = launch_sample(sp, s);
+  if (rc || !h->eng_text) return rc;
+  // text rows: one row per slot over the text head's logits, as a batch of one samples them
+  sp.logits = h->eng_text_logits; sp.rows = h->B; sp.V = c.num_text_tokens; sp.rows_per_item = 1;
+  sp.out_idx = h->eng_text_idx; sp.want = h->phase | WANT_TEXT;
   return launch_sample(sp, s);
 }
 
@@ -585,7 +612,12 @@ static int launch_heads_tc(ctb_gpt* h, cudaStream_t s) {
   p.logits = h->logits; p.rows_per_item = rpi; p.V = V; p.hidden_out = h->hiddens_out;
   p.hidden_stride = h->max_new * c.hidden_size; p.final_norm_w = h->W + h->lay.final_norm;
   p.rows = h->engine ? h->rows : nullptr; p.want = h->phase;
-  return launch_tc<DE_HEADS, CS_HEADS>(npad, h->infer_text ? h->m_htext : h->m_hcode, h->m_x[n][0], h->m_x[n][1], p, s);
+  const int rc = launch_tc<DE_HEADS, CS_HEADS>(npad, h->infer_text ? h->m_htext : h->m_hcode, h->m_x[n][0], h->m_x[n][1], p, s);
+  if (rc || !h->engine || !h->eng_text) return rc;
+  // slot engine: the text head over the text rows (see launch_heads)
+  p.nrows = c.num_text_tokens; p.logits = h->eng_text_logits; p.rows_per_item = 1; p.V = c.num_text_tokens;
+  p.hidden_out = nullptr; p.want = h->phase | WANT_TEXT;
+  return launch_tc<DE_HEADS, CS_HEADS>(npad, h->m_htext, h->m_x[n][0], h->m_x[n][1], p, s);
 }
 
 template <int BT>
@@ -695,7 +727,7 @@ static int launch_finalize(ctb_gpt* h, cudaStream_t s) {
   fp.max_new = h->max_new; fp.eos = h->sampler.eos_token; fp.idx = h->idx; fp.ids_out = h->ids_out;
   fp.finish = h->finish; fp.end_idx = h->end_idx;
   if (h->engine) {
-    fp.rows = h->rows; fp.want = h->phase;
+    fp.rows = h->rows; fp.want = h->phase; fp.idx_text = h->eng_text_idx;
     CTB_CUDA(launch_pdl(k_finalize_rows, dim3(1), dim3(256), 0, s, fp));
   } else {
     CTB_CUDA(launch_pdl(k_finalize, dim3(1), dim3(256), 0, s, fp));
@@ -919,6 +951,7 @@ extern "C" int ctb_gpt_begin(ctb_gpt* h, int32_t B, int32_t T0, const float* emb
   h->sampler = *sampler; h->q_noise = q_noise_dev; h->emb = emb_dev; h->mask = mask_dev;
   h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev;
   if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
+  if (h->graph_exec_text) { cudaGraphExecDestroy(h->graph_exec_text); h->graph_exec_text = nullptr; }
   { int rc0 = kv_reserve(h, B, T0 + max_new_token, s); if (rc0) return rc0; }
   CTB_CUDA(cudaMemsetAsync(h->st, 0, sizeof(LoopState), s));
   CTB_CUDA(cudaMemsetAsync(h->seq_len, 0, sizeof(int) * h->bpad_max, s));
@@ -971,7 +1004,10 @@ extern "C" int ctb_gpt_decode(ctb_gpt* h, int32_t n_steps, void* stream) {
       if ((rc = launch_step_flow(h, -1, true, s, std::min(per_launch, n_steps - done)))) return rc;
     return CTB_OK;
   }
-  if (h->use_graph && !h->graph_exec) {
+  // a slot engine with text slots replays the graph that carries the text head and sampler
+  cudaGraphExec_t& graph_exec = (h->engine && h->eng_text) ? h->graph_exec_text : h->graph_exec;
+  uint64_t& graph_kernels = (h->engine && h->eng_text) ? h->graph_kernels_text : h->graph_kernels;
+  if (h->use_graph && !graph_exec) {
     // capture on a private stream (the caller's may be the legacy default stream, which cannot
     // be captured); the instantiated graph is then launched on the caller's stream
     cudaGraph_t graph;
@@ -979,18 +1015,18 @@ extern "C" int ctb_gpt_decode(ctb_gpt* h, int32_t n_steps, void* stream) {
     CTB_CUDA(cudaStreamBeginCapture(h->cap_stream, cudaStreamCaptureModeThreadLocal));
     const uint64_t before = g_launches.load();
     rc = enqueue_step(h, -1, true, h->cap_stream);
-    h->graph_kernels = g_launches.load() - before;
+    graph_kernels = g_launches.load() - before;
     g_launches.store(before);  // captured, not launched
     cudaError_t e = cudaStreamEndCapture(h->cap_stream, &graph);
     if (rc) return rc;
     if (e != cudaSuccess) return set_err(CTB_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
-    CTB_CUDA(cudaGraphInstantiate(&h->graph_exec, graph, 0));
+    CTB_CUDA(cudaGraphInstantiate(&graph_exec, graph, 0));
     cudaGraphDestroy(graph);
   }
   for (int i = 0; i < n_steps; ++i) {
-    if (h->graph_exec) {
-      CTB_CUDA(cudaGraphLaunch(h->graph_exec, s));
-      g_launches.fetch_add(h->graph_kernels, std::memory_order_relaxed);
+    if (graph_exec) {
+      CTB_CUDA(cudaGraphLaunch(graph_exec, s));
+      g_launches.fetch_add(graph_kernels, std::memory_order_relaxed);
     } else if ((rc = enqueue_step(h, -1, true, s))) {
       return rc;
     }
@@ -1011,17 +1047,20 @@ extern "C" int ctb_gpt_engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, 
   if (!h->rows) {
     if ((rc = dalloc(&h->rows, (size_t)h->bpad_max))) return rc;
     if ((rc = dalloc(&h->cfgs, (size_t)c.max_batch))) return rc;
-    if ((rc = dalloc(&h->eng_noise, (size_t)c.max_batch * c.num_vq * c.num_audio_tokens))) return rc;
+    if ((rc = dalloc(&h->eng_noise, (size_t)c.max_batch * noise_stride(h)))) return rc;
     if ((rc = dalloc(&h->eng_slot, (size_t)c.max_batch))) return rc;
+    if ((rc = dalloc(&h->eng_text_logits, (size_t)c.max_batch * c.num_text_tokens))) return rc;
+    if ((rc = dalloc(&h->eng_text_idx, (size_t)c.max_batch))) return rc;
   }
-  // S rows of audio codes, each slot owning a fixed page range of max_context tokens; PDL chain (S <= 8) or wgmma
+  // S rows of audio codes or text, each slot owning a fixed page range of max_context tokens; PDL chain (S <= 8) or wgmma
   // step (S >= 9) - the one-kernel steps are never selected (use_flow, enqueue_step)
   h->engine = 1; h->phase = RS_RUNNING;
   h->B = S; h->T0 = 0; h->max_new = max_new_cap; h->infer_text = 0;
   h->use_tc = h->tc_ready && S >= h->tc_min_batch;
   h->q_noise = h->eng_noise; h->emb = nullptr; h->mask = nullptr;
-  h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev;
+  h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev; h->eng_text = 0;
   if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
+  if (h->graph_exec_text) { cudaGraphExecDestroy(h->graph_exec_text); h->graph_exec_text = nullptr; }
   if ((rc = kv_reserve(h, S, c.max_context, s))) return rc;
   static const LoopState idle_state = {0, 1, 0, 0, 0};  // no running slot: decode steps are no-ops
   CTB_CUDA(cudaMemcpyAsync(h->st, &idle_state, sizeof(LoopState), cudaMemcpyHostToDevice, s));
@@ -1046,9 +1085,9 @@ extern "C" int ctb_gpt_engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, 
   return CTB_OK;
 }
 
-extern "C" int ctb_gpt_engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0, const float* emb_dev,
-                                    const uint8_t* mask_dev, const ctb_sampler_config* samplers,
-                                    const float* q_noise_dev, const int32_t* max_new, void* stream) {
+static int engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0, const float* emb_dev,
+                        const uint8_t* mask_dev, const ctb_sampler_config* samplers, const float* q_noise_dev,
+                        const int32_t* max_new, int text, void* stream) {
   if (!h || !slots || !emb_dev || !mask_dev || !samplers || !max_new) return set_err(CTB_ERR_ARG, "null argument");
   if (!h->engine) return set_err(CTB_ERR_STATE, "ctb_gpt_engine_begin has not been called");
   const ctb_gpt_config& c = h->cfg;
@@ -1074,27 +1113,40 @@ extern "C" int ctb_gpt_engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots,
     if (sc.min_tokens_to_keep < 1) return set_err(CTB_ERR_ARG, "min_tokens_to_keep must be >= 1");
     RowState& r = rows[b];
     r.n_gen = 0; r.step = 0; r.state = RS_PENDING; r.max_new = max_new[i]; r.has_noise = q_noise_dev != nullptr;
-    r.eos = sc.eos_token;
+    r.eos = sc.eos_token; r.text = text;
   }
   // host arrays are copied before this call returns (synchronised below), so the caller may free them at once
   CTB_CUDA(cudaMemcpyAsync(h->rows, rows.data(), sizeof(RowState) * rows.size(), cudaMemcpyHostToDevice, s));
   CTB_CUDA(cudaMemcpyAsync(h->eng_slot, slots, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
-  const size_t nrow = (size_t)c.num_vq * c.num_audio_tokens;
+  const size_t nrow = text ? (size_t)c.num_text_tokens : (size_t)c.num_vq * c.num_audio_tokens;
   for (int i = 0; i < n; ++i) {
     const int b = slots[i];
     CTB_CUDA(cudaMemcpyAsync(h->cfgs + b, samplers + i, sizeof(ctb_sampler_config), cudaMemcpyHostToDevice, s));
     if (q_noise_dev)
-      CTB_CUDA(cudaMemcpyAsync(h->eng_noise + b * nrow, q_noise_dev + i * nrow, nrow * sizeof(float),
+      CTB_CUDA(cudaMemcpyAsync(h->eng_noise + b * noise_stride(h), q_noise_dev + i * nrow, nrow * sizeof(float),
                                cudaMemcpyDeviceToDevice, s));
     CTB_CUDA(cudaMemsetAsync(h->finish + b, 0, 1, s));
     CTB_CUDA(cudaMemsetAsync(h->end_idx + b, 0, sizeof(int), s));
   }
   CTB_CUDA(cudaStreamSynchronize(s));
   // prompts -> their slots' pages, then heads / sampler / finalize for the RS_PENDING rows only
+  if (text) h->eng_text = 1;
   h->phase = RS_PENDING;
   const int rc = prefill_batched(h, n, T0, emb_dev, mask_dev, h->eng_slot, s);
   h->phase = RS_RUNNING;
   return rc;
+}
+
+extern "C" int ctb_gpt_engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0, const float* emb_dev,
+                                    const uint8_t* mask_dev, const ctb_sampler_config* samplers,
+                                    const float* q_noise_dev, const int32_t* max_new, void* stream) {
+  return engine_admit(h, n, slots, T0, emb_dev, mask_dev, samplers, q_noise_dev, max_new, 0, stream);
+}
+
+extern "C" int ctb_gpt_engine_admit_text(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0, const float* emb_dev,
+                                         const uint8_t* mask_dev, const ctb_sampler_config* samplers,
+                                         const float* q_noise_dev, const int32_t* max_new, void* stream) {
+  return engine_admit(h, n, slots, T0, emb_dev, mask_dev, samplers, q_noise_dev, max_new, 1, stream);
 }
 
 extern "C" int ctb_gpt_engine_status(ctb_gpt* h, ctb_gpt_status* out, int32_t* state_host, int32_t* end_idx_host,
@@ -1108,6 +1160,11 @@ extern "C" int ctb_gpt_engine_status(ctb_gpt* h, ctb_gpt_status* out, int32_t* s
   if (rc) return rc;
   if (state_host)
     for (int b = 0; b < h->B; ++b) state_host[b] = rows[b].state;
+  if (h->eng_text) {  // the stream is synchronised: the rows are current
+    h->eng_text = 0;
+    for (int b = 0; b < h->B; ++b)
+      if (rows[b].text && (rows[b].state == RS_RUNNING || rows[b].state == RS_PENDING)) h->eng_text = 1;
+  }
   return CTB_OK;
 }
 

@@ -30,8 +30,22 @@ struct RowState {
   int max_new;    // the row finishes after this many tokens
   int has_noise;  // 1: Exp(1) rows in the engine's noise buffer (seeded request); 0: device Philox
   int eos;
-  int pad[2];
+  int text;       // 1: text tokens (emb_text input, text head, one sampled row); 0: audio codes
+  int pad;
 };
+
+// The heads and the sampler of a slot engine run once for code rows and once for text rows: their `want` is a
+// RowStateKind, plus WANT_TEXT when the launch serves text rows.  k_finalize_rows serves both kinds in one launch.
+constexpr int WANT_TEXT = 8;
+__device__ __forceinline__ bool row_wanted(const RowState* r, int want) {
+  return ldg_cg(&r->state) == (want & ~WANT_TEXT) && (ldg_cg(&r->text) != 0) == ((want & WANT_TEXT) != 0);
+}
+// CTA-uniform: does any of the B rows match `want`?  (every warp reads the <= 32 row states itself)
+__device__ __forceinline__ bool any_row_wanted(const RowState* rows, int B, int want) {
+  bool any = false;
+  for (int b = threadIdx.x & 31; b < B; b += 32) any |= row_wanted(rows + b, want);
+  return __any_sync(0xffffffffu, any);
+}
 
 constexpr int KC = 768;        // K chunk staged in shared memory (= hidden size of the model)
 constexpr int GEMV_WARPS = 8;  // warps per CTA, one 2-row task per warp
@@ -68,7 +82,7 @@ struct GemvP {
   int V;
   float* hidden_out;     // [B, max_new, d] or nullptr
   int hidden_stride;     // max_new * d
-  const RowState* rows;  // slot engine: only rows in state `want` get logits / hidden states; nullptr: every row
+  const RowState* rows;  // slot engine: only rows matching `want` (row_wanted) get logits / hidden states; nullptr: every row
   int want;
 };
 
@@ -146,13 +160,19 @@ __global__ void __launch_bounds__(GEMV_WARPS * 32) k_gemv(const GemvP p) {
     for (int i = 0; i < 6; ++i) { w0[i] = ldg_stream(w0p + i * 32); w1[i] = ldg_stream(w1p + i * 32); }
   };
 
-  // the first task's weights do not depend on earlier kernels: request them before the PDL wait
+  // the first task's weights do not depend on earlier kernels: request them before the PDL wait.  A slot engine's
+  // text head streams nothing until the row states show a text row to serve.
+  const bool text_rows = EPI == EPI_HEADS && p.rows != nullptr && (p.want & WANT_TEXT);
   float4 w0[6], w1[6];
-  if (task0 < p.ntasks) load_w(task0, w0, w1);
+  if (task0 < p.ntasks && !text_rows) load_w(task0, w0, w1);
   pdl_wait();  // everything below reads activations / loop state written by earlier kernels
   if (p.check_finished && ldg_cg(&p.st->all_finished)) {
     if (EPI == EPI_DOWN) { cluster_sync_all(); cluster_sync_all(); }
     return;
+  }
+  if (text_rows) {
+    if (!any_row_wanted(p.rows, p.B, p.want)) return;
+    if (task0 < p.ntasks) load_w(task0, w0, w1);
   }
 
   // ---- stage the batch tile's activations (K chunk kc) once per CTA
@@ -189,7 +209,7 @@ __global__ void __launch_bounds__(GEMV_WARPS * 32) k_gemv(const GemvP p) {
       } else {
         for (int b = 0; b < nb; ++b) {
           const RowState* r = p.rows + bbase + b;
-          if (ldg_cg(&r->state) != p.want) continue;
+          if (!row_wanted(r, p.want)) continue;
           const int step = ldg_cg(&r->n_gen);
           for (int k = tid; k < KC; k += GEMV_WARPS * 32)
             p.hidden_out[(size_t)(bbase + b) * p.hidden_stride + (size_t)step * KC + k] = xs[b * KC + k];
@@ -274,7 +294,7 @@ __global__ void __launch_bounds__(GEMV_WARPS * 32) k_gemv(const GemvP p) {
       const float sg = __fdiv_rn(v0, __fadd_rn(1.0f, expf(-v0)));
       p.out[(size_t)b * p.I + task] = __fmul_rn(sg, v1);
     } else {  // EPI_HEADS: logits rows ordered (b, q) like gpt.py:459-464
-      if (p.rows != nullptr && ldg_cg(&p.rows[b].state) != p.want) continue;
+      if (p.rows != nullptr && !row_wanted(p.rows + b, p.want)) continue;
       const int q0 = r0 / p.V, c0 = r0 % p.V;
       p.out[((size_t)b * p.rows_per_item + q0) * p.V + c0] = v0;
       if (r1_valid) {
@@ -496,7 +516,7 @@ __global__ void k_input(const InputP p) {
     for (int k = threadIdx.x; k < p.d; k += blockDim.x) x[k] = act ? e[k] : 0.f;
   } else {
     act = true;
-    int n_gen;
+    int n_gen, text = p.infer_text;
     if (p.rows != nullptr) {
       // idle / finished slots append no KV and keep their position: only the active flag is written
       if (ldg_cg(&p.rows[b].state) != RS_RUNNING) {
@@ -504,11 +524,12 @@ __global__ void k_input(const InputP p) {
         return;
       }
       n_gen = ldg_cg(&p.rows[b].n_gen);
+      text = ldg_cg(&p.rows[b].text);
     } else {
       n_gen = ldg_cg(&p.st->n_gen);
     }
     const int32_t* id = p.ids_out + ((size_t)b * p.max_new + (n_gen - 1)) * p.num_vq;
-    if (p.infer_text) {
+    if (text) {
       const float* e = p.emb_text + (size_t)ldg_cg(&id[0]) * p.d;
       for (int k = threadIdx.x; k < p.d; k += blockDim.x) x[k] = e[k];
     } else {
@@ -712,11 +733,12 @@ struct SampleP {
   int n_gen_fixed, step_fixed;  // used when st == nullptr (stand-alone ctb_sample)
   int32_t* out_idx;      // [rows]
   // slot engine (k_sample<true>): counters, noise flag and state per item from `rstate`, the sampling parameters of
-  // item b from cfgs[b] (device memory, so a captured decode graph serves every admitted request); only items in
-  // state `want` are sampled
+  // item b from cfgs[b] (device memory, so a captured decode graph serves every admitted request); only items
+  // matching `want` (row_wanted) are sampled.  Item b's noise rows start at q_noise + b * noise_stride.
   const RowState* rstate;
   const ctb_sampler_config* cfgs;
   int want;
+  int noise_stride;
 };
 
 constexpr int SAMPLE_THREADS = 1024;
@@ -731,6 +753,7 @@ struct FinalP {
   uint8_t* finish; int32_t* end_idx;
   RowState* rows;        // k_finalize_rows only
   int want;
+  const int32_t* idx_text;  // k_finalize_rows: [B] the text sampler's ids (text rows)
 };
 __global__ void k_finalize(const FinalP p);
 __global__ void k_finalize_rows(const FinalP p);

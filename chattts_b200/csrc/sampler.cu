@@ -53,7 +53,7 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) k_sample(const SampleP p) {
   const int item = row / rpi, qi = row % rpi;
   __shared__ ctb_sampler_config s_cfg;
   if (ENGINE) {
-    if (ldg_cg(&p.rstate[item].state) != p.want) return;  // CTA-uniform
+    if (!row_wanted(p.rstate + item, p.want)) return;  // CTA-uniform
     static_assert(sizeof(ctb_sampler_config) % 4 == 0, "config is copied as words");
     const uint32_t* src = reinterpret_cast<const uint32_t*>(p.cfgs + item);
     for (int i = threadIdx.x; i < (int)(sizeof(ctb_sampler_config) / 4); i += SAMPLE_THREADS)
@@ -241,7 +241,8 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) k_sample(const SampleP p) {
   int besti = 0x7fffffff;
   for (int v = tid; v < V; v += SAMPLE_THREADS) {
     const float pr = __fdiv_rn(expf(s_x[v] - mx2), den2f);
-    const float qn = noise ? p.q_noise[(size_t)row * V + v]
+    const float qn = noise ? (ENGINE ? p.q_noise[(size_t)item * p.noise_stride + (size_t)qi * V + v]
+                                     : p.q_noise[(size_t)row * V + v])
                            : philox_exp1(c.philox_seed, (uint32_t)prow, (uint32_t)v, (uint32_t)step);
     const float r = __fdiv_rn(pr, qn);
     if (r > best) { best = r; besti = v; }  // ascending v within a thread: first max wins
@@ -317,10 +318,16 @@ __global__ void k_finalize_rows(const FinalP p) {
     if (state == p.want) {
       const int n = ldg_cg(&r->n_gen), eos_tok = ldg_cg(&r->eos);
       bool eos = false;
-      for (int q = 0; q < p.rows_per_item; ++q) eos |= (ldg_cg(&p.idx[b * p.rows_per_item + q]) == eos_tok);
-      p.finish[b] = eos ? 1 : 0;
       int32_t* dst = p.ids_out + ((size_t)b * p.max_new + n) * p.num_vq;
-      for (int q = 0; q < p.num_vq; ++q) dst[q] = ldg_cg(&p.idx[b * p.rows_per_item + (p.rows_per_item == 1 ? 0 : q)]);
+      if (ldg_cg(&r->text)) {  // one text id, written to every column (k_finalize with rows_per_item == 1)
+        const int32_t id = ldg_cg(&p.idx_text[b]);
+        eos = id == eos_tok;
+        for (int q = 0; q < p.num_vq; ++q) dst[q] = id;
+      } else {
+        for (int q = 0; q < p.rows_per_item; ++q) eos |= (ldg_cg(&p.idx[b * p.rows_per_item + q]) == eos_tok);
+        for (int q = 0; q < p.num_vq; ++q) dst[q] = ldg_cg(&p.idx[b * p.rows_per_item + (p.rows_per_item == 1 ? 0 : q)]);
+      }
+      p.finish[b] = eos ? 1 : 0;
       if (!eos) p.end_idx[b] = ldg_cg(&p.end_idx[b]) + 1;
       r->n_gen = n + 1;
       r->step = ldg_cg(&r->step) + 1;

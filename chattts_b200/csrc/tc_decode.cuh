@@ -45,7 +45,7 @@ struct TcDecP {
   float* h_hi; float* h_lo; int I;                                    // GATEUP
   float* logits; int rows_per_item, V;                                // HEADS
   float* hidden_out; int hidden_stride; const float* final_norm_w; const LoopState* st;
-  const RowState* rows; int want;  // HEADS in slot-engine mode: only rows in state `want` (nullptr: every row)
+  const RowState* rows; int want;  // HEADS in slot-engine mode: only rows matching `want` (nullptr: every row)
 };
 
 template <int EPI, int NPAD, int CS>
@@ -78,6 +78,12 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
+  if (EPI == DE_HEADS && p.rows != nullptr && (p.want & WANT_TEXT)) {
+    // a slot engine's text head: no weight request before the row states show a text row to serve (every CTA of
+    // the cluster reads the same states and leaves together, before any cluster barrier)
+    pdl_wait();
+    if (!any_row_wanted(p.rows, p.B, p.want)) return;
+  }
 
   if (warp == 4) {
     // ===================== TMA producer
@@ -142,7 +148,7 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
           }
         } else {
           for (int b = 0; b < p.B; ++b) {
-            if (ldg_cg(&p.rows[b].state) != p.want) continue;
+            if (!row_wanted(p.rows + b, p.want)) continue;
             const int step = ldg_cg(&p.rows[b].n_gen);
             for (int k = threadIdx.x; k < p.K; k += 128)
               p.hidden_out[(size_t)b * p.hidden_stride + (size_t)step * p.K + k] =
@@ -275,7 +281,7 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
         p.h_hi[(size_t)b * p.I + R / 2] = hh;
         p.h_lo[(size_t)b * p.I + R / 2] = to_tf32(hv - hh);
       } else {  // DE_HEADS
-        if (p.rows != nullptr && ldg_cg(&p.rows[b].state) != p.want) continue;
+        if (p.rows != nullptr && !row_wanted(p.rows + b, p.want)) continue;
         const int q0 = R / p.V, c0 = R % p.V;
         p.logits[((size_t)b * p.rows_per_item + q0) * p.V + c0] = __fmul_rn(v0, rinv);
         if (R + 1 < p.nrows) {

@@ -1,9 +1,11 @@
-"""Continuous batching of audio-code generation: a slot engine on one GPT handle.
+"""Continuous batching of audio-code and text generation: a slot engine on one GPT handle.
 
 The handle's decode rows become ``S`` slots (``ctb_gpt_engine_*`` in include/chattts_b200.h).  Each request - one
-utterance: a prompt embedding with its own sampling parameters, seed and token limits - enters a free slot between
-decode chunks, and its slot is reused as soon as it finishes.  A request's token ids are bit for bit what
-``GPT.generate`` returns for it alone (B = 1, same ``manual_seed``), whatever else is in flight.
+utterance: a prompt embedding with its own sampling parameters, seed and token limits, generating audio codes or
+(``infer_text``) text tokens - enters a free slot between decode chunks, and its slot is reused as soon as it finishes.
+A request's token ids are bit for bit what ``GPT.generate`` returns for it alone (B = 1, same ``manual_seed``, same
+``infer_text``), whatever else is in flight.  A request may name a follow-up (``then``), which is queued ahead of
+every waiting request when it ends: text refinement followed by the speech codes of the refined text.
 
 The scheduling policy (``schedule``) is plain Python over a small device interface, so it can be driven by a stub.
 ``stream_schedule`` runs the same policy and reconstructs, per request, the cumulative yields of
@@ -13,8 +15,8 @@ from __future__ import annotations
 
 import ctypes as C
 from collections import deque
-from dataclasses import dataclass
-from typing import Iterator, List, Optional, Sequence, Tuple
+from dataclasses import dataclass, field
+from typing import Callable, Dict, Iterator, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -30,7 +32,13 @@ class Request:
     """One utterance for ``GPT.generate_continuous``.
 
     ``emb``: [T, d] prompt embedding (every position valid, as a batch of one has no padding) or [1, T, d].
-    The other fields mean what the ``GPT.generate`` arguments of the same name mean."""
+    The other fields mean what the ``GPT.generate`` arguments of the same name mean; ``infer_text=True`` generates
+    text tokens (one temperature, ``eos_token`` the tokenizer's EOS) and its outputs are those of
+    ``GPT.generate(infer_text=True)`` for one row: 1-D int64 ids and no hidden states.
+
+    ``then``: called with the request's outputs when it ends at EOS or ``max_new_token`` (a seeded request that ended
+    empty included; not on an interrupt); the ``Request`` it returns, if any, is queued ahead of every waiting request
+    under the next unused request index."""
 
     emb: torch.Tensor
     temperature: Sequence[float]
@@ -41,6 +49,8 @@ class Request:
     manual_seed: Optional[int] = None
     ensure_non_empty: bool = True
     stream_batch: int = 24
+    infer_text: bool = False
+    then: Optional[Callable[[object], Optional["Request"]]] = None
 
     def __post_init__(self):
         if self.emb.dim() == 3:
@@ -53,6 +63,8 @@ class Request:
             raise ValueError("max_new_token must be >= 1")
         if self.stream_batch < 1:
             raise ValueError("stream_batch must be >= 1")
+        if self.infer_text and torch.as_tensor(self.temperature).numel() != 1:
+            raise ValueError("a text request takes one temperature")
 
 
 @dataclass
@@ -73,13 +85,35 @@ class ScheduleStats:
     decode_steps: int = 0
     tokens: int = 0
     interrupted: bool = False
+    children: Dict[int, int] = field(default_factory=dict)  # request index -> index of the follow-up it returned
 
 
-def _poll_cycles(requests: Sequence[Request], dev, chunk: int, context=None,
-                 stats: Optional[ScheduleStats] = None) -> Iterator[Tuple[SlotStatus, List[Optional[int]], list]]:
+def _follow_up(requests: List[Request], i: int, slot: Optional[int], n: int, dev, check, stats: ScheduleStats):
+    """Request ``i`` ended: its follow-up's index as a list (empty without one)."""
+    then = requests[i].then
+    if then is None:
+        return []
+    child = then(dev.empty(i) if slot is None else dev.harvest(slot, n))
+    if child is None:
+        return []
+    if not isinstance(child, Request):
+        raise TypeError("Request.then must return a Request or None")
+    if check is not None:
+        check(child)
+    requests.append(child)
+    stats.children[i] = len(requests) - 1
+    return [len(requests) - 1]
+
+
+def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: Optional[ScheduleStats] = None,
+                 check: Optional[Callable[[Request], None]] = None
+                 ) -> Iterator[Tuple[SlotStatus, List[Optional[int]], list]]:
     """The scheduling policy of ``schedule``: yields once per poll ``(status, owner, ended)`` - the slots' status, the
     request each slot held when it was read, and the requests that ended at this poll as ``(request_index, slot or
-    None, n_tokens, eos)``.  The slots of the ended requests are refilled only after the generator is resumed."""
+    None, n_tokens, eos)``.  The slots of the ended requests are refilled only after the generator is resumed.
+
+    A request's follow-up (``Request.then``, called here while the slot's outputs are valid and checked by ``check``)
+    is appended to ``requests`` and queued ahead of the waiting requests, so the refill after this poll admits it."""
     stats = stats if stats is not None else ScheduleStats()
     waiting = deque(range(len(requests)))
     owner: List[Optional[int]] = [None] * dev.slots
@@ -98,6 +132,7 @@ def _poll_cycles(requests: Sequence[Request], dev, chunk: int, context=None,
         stats.decode_steps = st.steps_done
         polled = list(owner)
         ended = []
+        follow: List[int] = []
         freed = False
         for s in range(dev.slots):
             i = owner[s]
@@ -112,9 +147,12 @@ def _poll_cycles(requests: Sequence[Request], dev, chunk: int, context=None,
                     stats.requeued += 1
                     continue
                 ended.append((i, None, 0, True))
+                follow += _follow_up(requests, i, None, 0, dev, check, stats)
                 continue
             stats.tokens += st.end_idx[s]
             ended.append((i, s, st.end_idx[s], bool(st.finish[s])))
+            follow += _follow_up(requests, i, s, st.end_idx[s], dev, check, stats)
+        waiting.extendleft(reversed(follow))  # ahead of the waiting requests, in slot order
         if freed and waiting:
             yield st, polled, ended
             continue  # refill the freed slots before the next chunk
@@ -131,8 +169,8 @@ def _poll_cycles(requests: Sequence[Request], dev, chunk: int, context=None,
         dev.decode(chunk)
 
 
-def schedule(requests: Sequence[Request], dev, chunk: int, context=None,
-             stats: Optional[ScheduleStats] = None) -> Iterator[Tuple[int, Optional[int], int]]:
+def schedule(requests: List[Request], dev, chunk: int, context=None, stats: Optional[ScheduleStats] = None,
+             check: Optional[Callable[[Request], None]] = None) -> Iterator[Tuple[int, Optional[int], int]]:
     """Drive ``dev`` (``slots``, ``admit([(slot, request_index)])``, ``decode(n)``, ``status() -> SlotStatus``) until
     every request has finished; yields ``(request_index, slot, n_tokens)`` as each one completes - the caller harvests
     the slot's first ``n_tokens`` outputs before resuming the generator - or ``(request_index, None, 0)`` for a seeded
@@ -141,14 +179,16 @@ def schedule(requests: Sequence[Request], dev, chunk: int, context=None,
 
     Waiting requests enter free slots in order, lowest slot first, at every poll (every ``chunk`` decode steps).  On a
     ``context`` interrupt the running requests are yielded with what they have so far and the waiting ones are dropped.
+    Follow-ups (``Request.then``) need ``dev.harvest(slot, n)`` and ``dev.empty(request_index)``; see ``_poll_cycles``.
     """
-    for _, _, ended in _poll_cycles(requests, dev, chunk, context, stats):
+    for _, _, ended in _poll_cycles(requests, dev, chunk, context, stats, check):
         for i, s, n, _ in ended:
             yield i, s, n
 
 
-def stream_schedule(requests: Sequence[Request], dev, chunk: int, context=None,
-                    stats: Optional[ScheduleStats] = None) -> Iterator[List[Tuple[int, Optional[int], int, bool]]]:
+def stream_schedule(requests: List[Request], dev, chunk: int, context=None, stats: Optional[ScheduleStats] = None,
+                    check: Optional[Callable[[Request], None]] = None
+                    ) -> Iterator[List[Tuple[int, Optional[int], int, bool]]]:
     """``schedule``'s policy, yielding once per poll the list of ``(request_index, slot, n_tokens, last)``: for each
     request, the yields ``GPT.generate(stream=True, stream_batch=r.stream_batch)`` makes for it alone, in its order,
     as cumulative token counts (the slot's first ``n_tokens`` outputs; slot None: a seeded request that ended empty).
@@ -158,14 +198,14 @@ def stream_schedule(requests: Sequence[Request], dev, chunk: int, context=None,
     final yield; a row that stops at ``max_new_token`` is not finished there, so it gets no second yield.  Tokens only
     ever append to a slot, so each poll rebuilds every boundary a slot crossed since the last one from its token count:
     the yields do not depend on ``chunk``.  The slots' outputs stay in place until the generator is resumed."""
-    sent = [0] * len(requests)  # last boundary yielded per request
-    for st, owner, ended in _poll_cycles(requests, dev, chunk, context, stats):
+    sent: Dict[int, int] = {}  # last boundary yielded per request
+    for st, owner, ended in _poll_cycles(requests, dev, chunk, context, stats, check):
         out = []
         for s, i in enumerate(owner):
             if i is None:
                 continue
             sb = requests[i].stream_batch
-            nxt = sent[i] + sb
+            nxt = sent.get(i, 0) + sb
             if nxt < 2:  # step 1 (the prefill's token) is never a boundary
                 nxt += sb
             # running: end_idx steps so far, all unfinished; EOS at step end_idx + 1; max_new: end_idx = max_new
@@ -199,11 +239,14 @@ class EngineDevice:
         self._state = (C.c_int32 * slots)()
         self._end = torch.zeros(slots, dtype=torch.int32)
         self._fin = torch.zeros(slots, dtype=torch.uint8)
+        self._text = [False] * slots  # mode of the request each slot was last given
 
     def admit(self, batch: List[Tuple[int, int]]) -> None:
-        # one prefill per kind: seeded requests bring their Exp(1) rows, unseeded ones sample with device Philox
-        for seeded in (True, False):
-            group = [(s, i) for s, i in batch if (self.requests[i].manual_seed is not None) == seeded]
+        # one prefill per kind: seeded requests bring their Exp(1) rows, unseeded ones sample with device Philox; code
+        # and text requests are admitted by separate calls
+        for seeded, text in ((True, False), (True, True), (False, False), (False, True)):
+            group = [(s, i) for s, i in batch if (self.requests[i].manual_seed is not None) == seeded
+                     and bool(self.requests[i].infer_text) == text]
             if not group:
                 continue
             # the prompts share one padded width; a request whose max_new no longer fits its slot's max_context
@@ -212,9 +255,9 @@ class EngineDevice:
             alone = [(s, i) for s, i in group if T0 + self.requests[i].max_new_token > self.gpt.max_context]
             rest = [p for p in group if p not in alone]
             for part in ([rest] if rest else []) + [[p] for p in alone]:
-                self._admit(part, seeded)
+                self._admit(part, seeded, text)
 
-    def _admit(self, group, seeded: bool) -> None:
+    def _admit(self, group, seeded: bool, text: bool) -> None:
         gpt, n = self.gpt, len(group)
         reqs = [self.requests[i] for _, i in group]
         T0 = max(MIN_PROMPT_COLS, max(int(r.emb.shape[0]) for r in reqs))
@@ -232,10 +275,14 @@ class EngineDevice:
             cfgs[k] = build_sampler_config(r.logits_processors, temps, int(r.eos_token), r.min_new_token, philox)
         noise = None
         if seeded:  # the rows GPT.generate draws for a batch of one with this seed
-            noise = torch.cat([exp_noise(gpt.num_vq, gpt.num_audio_tokens, r.manual_seed) for r in reqs]).to(self.dev)
+            rows, cols = (1, gpt.num_text_tokens) if text else (gpt.num_vq, gpt.num_audio_tokens)
+            noise = torch.cat([exp_noise(rows, cols, r.manual_seed) for r in reqs]).to(self.dev)
         slots = (C.c_int32 * n)(*[s for s, _ in group])
         max_new = (C.c_int32 * n)(*[r.max_new_token for r in reqs])
-        _lib.check(self.lib.ctb_gpt_engine_admit(
+        for s, _ in group:
+            self._text[s] = text
+        admit = self.lib.ctb_gpt_engine_admit_text if text else self.lib.ctb_gpt_engine_admit
+        _lib.check(admit(
             gpt._handle, n, slots, T0, C.c_void_p(emb.data_ptr()), C.c_void_p(mask.data_ptr()), cfgs,
             C.c_void_p(noise.data_ptr()) if noise is not None else None, max_new, self.stream))
 
@@ -251,17 +298,25 @@ class EngineDevice:
 
     def harvest(self, slot: int, n: int, copy: bool = True):
         """GenerationOutputs of the request in ``slot``: its first ``n`` ids (int64 copies) and hidden states (copies,
-        or with ``copy=False`` views into the engine buffer, valid until the engine decodes or admits again)."""
+        or with ``copy=False`` views into the engine buffer, valid until the engine decodes or admits again).  A text
+        request's ids are 1-D and it has no hidden states, as ``GPT.generate(infer_text=True)`` returns them."""
         from .gpt import GPT
 
+        if self._text[slot]:
+            return GPT.GenerationOutputs(ids=[self.ids_out[slot, :n, 0].to(torch.int64)], attentions=[], hiddens=[])
         ids = self.ids_out[slot, :n].to(torch.int64)
         hid = ([self.hid_out[slot, :n].clone() if copy else self.hid_out[slot, :n]] if self.hid_out is not None
                else [])
         return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid)
 
-    def empty(self):
+    def empty(self, index: Optional[int] = None):
+        """The outputs of request ``index`` (default: a code request) when it ended empty (a seeded request whose
+        first token was EOS)."""
         from .gpt import GPT
 
+        if index is not None and self.requests[index].infer_text:
+            return GPT.GenerationOutputs(ids=[torch.zeros(0, dtype=torch.int64, device=self.dev)], attentions=[],
+                                         hiddens=[])
         ids = torch.zeros(0, self.gpt.num_vq, dtype=torch.int64, device=self.dev)
         hid = ([torch.zeros(0, self.gpt.config.hidden_size, dtype=torch.float32, device=self.dev)]
                if self.hid_out is not None else [])

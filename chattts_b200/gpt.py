@@ -226,36 +226,44 @@ class GPT:
     # ------------------------------------------------------------------ continuous batching
     @torch.no_grad()
     def generate_continuous(self, requests, slots: Optional[int] = None, return_hidden=True, infer_text=False,
-                            stream=False, return_attn=False, context=None, chunk: Optional[int] = None):
-        """Generate audio codes for many utterances on a slot engine (chattts_b200.engine): up to ``slots`` requests
-        (default: ``max_batch``, at most the number of requests) decode together, and a waiting request takes the
-        place of a finished one at the next poll (every ``chunk`` steps, default CTB_DECODE_CHUNK or 32).
+                            stream=False, return_attn=False, context=None, chunk: Optional[int] = None,
+                            max_new_cap: Optional[int] = None):
+        """Generate audio codes or text for many utterances on a slot engine (chattts_b200.engine): up to ``slots``
+        requests (default: ``max_batch``, at most the number of requests) decode together, and a waiting request takes
+        the place of a finished one at the next poll (every ``chunk`` steps, default CTB_DECODE_CHUNK or 32).  Each
+        ``Request`` chooses its mode (``Request.infer_text``); code and text requests share the engine.
 
         Generator of ``(request_index, GenerationOutputs)`` in completion order.  Each request's ids equal, bit for
         bit, ``generate`` on that request alone with the same arguments and ``manual_seed``.  A seeded request that
         samples EOS first yields empty outputs (``generate`` yields nothing then); an unseeded one with
         ``ensure_non_empty`` runs again.  The handle serves one generator at a time; ``generate`` may be called again
-        once it is exhausted."""
+        once it is exhausted.
+
+        Follow-ups (``Request.then``) are yielded under new indices, ``len(requests)`` on; ``last_schedule_stats
+        .children`` maps each request index to its follow-up's.  ``max_new_cap`` (default: the largest
+        ``max_new_token`` of ``requests``) bounds every request's ``max_new_token``, follow-ups included: the engine's
+        output buffers are sized by it."""
         from .engine import EngineDevice, ScheduleStats, schedule
 
         if stream:
             raise ValueError("generate_continuous: stream=True is not supported; results are yielded per request "
                              "(generate_continuous_stream streams)")
-        requests, S, chunk, context = self._engine_args("generate_continuous", requests, slots, infer_text, return_attn,
-                                                        context, chunk, 32)
+        requests, S, chunk, context, cap, check = self._engine_args(
+            "generate_continuous", requests, slots, infer_text, return_attn, context, chunk, 32, max_new_cap)
         if not requests:
             return
         with torch.cuda.device(self.device_gpt):
-            dev = EngineDevice(self, requests, S, max(r.max_new_token for r in requests), return_hidden)
+            dev = EngineDevice(self, requests, S, cap, return_hidden)
             self.last_schedule_stats = stats = ScheduleStats()  # admissions, decode steps (tools/bench_continuous.py)
-            for i, slot, n in schedule(requests, dev, chunk, context, stats):
-                yield i, (dev.empty() if slot is None else dev.harvest(slot, n))
+            for i, slot, n in schedule(requests, dev, chunk, context, stats, check):
+                yield i, (dev.empty(i) if slot is None else dev.harvest(slot, n))
             if stats.interrupted:
                 self.logger.warning("generation is interrupted")
 
     @torch.no_grad()
     def generate_continuous_stream(self, requests, slots: Optional[int] = None, return_hidden=True, context=None,
-                                   chunk: Optional[int] = None, infer_text=False, return_attn=False):
+                                   chunk: Optional[int] = None, infer_text=False, return_attn=False,
+                                   max_new_cap: Optional[int] = None):
         """Streaming form of ``generate_continuous``: generator of ``(request_index, GenerationOutputs, last)``.
 
         For each request the yields are exactly those ``generate(stream=True, stream_batch=r.stream_batch)`` makes for
@@ -263,39 +271,43 @@ class GPT:
         boundary when EOS follows it on the next step, then the final yield, which alone has ``last=True``.  Yields of
         different requests interleave in poll order.  The engine polls every ``chunk`` steps (default:
         CTB_DECODE_CHUNK, or the smallest ``stream_batch`` among the requests); the yields do not depend on it.
-        A seeded request that samples EOS first yields one empty final output.
+        A seeded request that samples EOS first yields one empty final output.  Text requests and follow-ups are
+        served as in ``generate_continuous``.
 
         ``ids`` are copies.  ``hiddens`` are views into the engine's buffer, like the narrowed views ``generate``
         hands out: they stay valid until this generator is resumed (copy them to keep them)."""
-        for dev, batch in self._stream_polls(requests, slots, return_hidden, context, chunk, infer_text, return_attn):
+        for dev, batch in self._stream_polls(requests, slots, return_hidden, context, chunk, infer_text, return_attn,
+                                             max_new_cap):
             for i, slot, n, last in batch:
-                yield i, (dev.empty() if slot is None else dev.harvest(slot, n, copy=False)), last
+                yield i, (dev.empty(i) if slot is None else dev.harvest(slot, n, copy=False)), last
 
     def _stream_polls(self, requests, slots=None, return_hidden=True, context=None, chunk=None, infer_text=False,
-                      return_attn=False):
+                      return_attn=False, max_new_cap=None):
         """``(EngineDevice, [(request_index, slot, n_tokens, last)])`` once per poll (engine.stream_schedule): every
         yield due at that poll, while the engine's buffers hold all of them."""
         from .engine import EngineDevice, ScheduleStats, stream_schedule
 
-        requests, S, chunk, context = self._engine_args("generate_continuous_stream", requests, slots, infer_text,
-                                                        return_attn, context, chunk, None)
+        requests, S, chunk, context, cap, check = self._engine_args(
+            "generate_continuous_stream", requests, slots, infer_text, return_attn, context, chunk, None, max_new_cap)
         if not requests:
             return
         with torch.cuda.device(self.device_gpt):
-            dev = EngineDevice(self, requests, S, max(r.max_new_token for r in requests), return_hidden)
+            dev = EngineDevice(self, requests, S, cap, return_hidden)
             self.last_schedule_stats = stats = ScheduleStats()
-            for batch in stream_schedule(requests, dev, chunk, context, stats):
+            for batch in stream_schedule(requests, dev, chunk, context, stats, check):
                 yield dev, batch
             if stats.interrupted:
                 self.logger.warning("generation is interrupted")
 
-    def _engine_args(self, name, requests, slots, infer_text, return_attn, context, chunk, default_chunk):
-        """Checks shared by the slot-engine generators -> (requests, slots, chunk, context).  The poll interval is
-        `chunk`, else CTB_DECODE_CHUNK, else `default_chunk` (None: the smallest ``stream_batch``)."""
+    def _engine_args(self, name, requests, slots, infer_text, return_attn, context, chunk, default_chunk,
+                     max_new_cap=None):
+        """Checks shared by the slot-engine generators -> (requests, slots, chunk, context, max_new_cap, check), where
+        ``check`` validates a follow-up request as the up-front ones are.  The poll interval is `chunk`, else
+        CTB_DECODE_CHUNK, else `default_chunk` (None: the smallest ``stream_batch``)."""
         from .engine import MIN_PROMPT_COLS, Request
 
         if infer_text:
-            raise ValueError(f"{name}: audio codes only (infer_text=True stays on generate)")
+            raise ValueError(f"{name}: the mode is chosen per request: set Request.infer_text for text generation")
         if return_attn:
             raise ValueError(f"{name}: return_attn is not supported")
         if not self._handle:
@@ -307,16 +319,27 @@ class GPT:
         S = max(S, 2)
         if S > self.max_batch:
             raise ValueError(f"slots={S} exceed this handle's max_batch={self.max_batch}")
-        for r in requests:
+        cap = max((r.max_new_token for r in requests), default=1) if max_new_cap is None else int(max_new_cap)
+        if cap < 1 or cap >= self.max_context:
+            raise ValueError(f"max_new_cap={cap} outside [1, max_context={self.max_context})")
+
+        def check(r):
+            if not isinstance(r, Request):
+                raise TypeError("requests must be chattts_b200.engine.Request objects")
             T0 = max(MIN_PROMPT_COLS, int(r.emb.shape[0]))
             if T0 > 1024 or T0 + r.max_new_token > self.max_context:
                 raise ValueError(f"prompt {int(r.emb.shape[0])} + max_new_token {r.max_new_token} exceed this handle "
                                  f"(max_context={self.max_context}; prompts up to 1024 tokens)")
+            if r.max_new_token > cap:
+                raise ValueError(f"max_new_token {r.max_new_token} exceeds max_new_cap={cap}")
+
+        for r in requests:
+            check(r)
         if default_chunk is None:
             default_chunk = min((r.stream_batch for r in requests), default=24)
         env = os.environ.get("CTB_DECODE_CHUNK")
         chunk = (int(env) if env else default_chunk) if chunk is None else int(chunk)
-        return requests, S, chunk, (context if context is not None else GPT.Context())
+        return requests, S, chunk, (context if context is not None else GPT.Context()), cap, check
 
     # ------------------------------------------------------------------ the loop
     @torch.no_grad()

@@ -170,6 +170,16 @@ int ctb_gpt_engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0
                          const uint8_t* mask_dev, const ctb_sampler_config* samplers, const float* q_noise_dev,
                          const int32_t* max_new, void* stream);
 
+/* ctb_gpt_engine_admit for text requests (GPT.generate(infer_text=True) for a batch of one): the slots take text
+ * tokens - emb_text input, the text head, one sampled row (temperature[0]; penalty_max_ids applies to row 0).  Text
+ * and code slots decode in the same ctb_gpt_decode steps.  Each token is written to all num_vq columns of
+ * ids_out_dev[b, n]; no hidden states are written for text slots.
+ *   q_noise_dev  [n, num_text] fp32 Exp(1) rows of each request's seeded generator, or NULL: device Philox
+ * Other arguments as for ctb_gpt_engine_admit. */
+int ctb_gpt_engine_admit_text(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0, const float* emb_dev,
+                              const uint8_t* mask_dev, const ctb_sampler_config* samplers, const float* q_noise_dev,
+                              const int32_t* max_new, void* stream);
+
 /* Synchronises `stream`, then reports per-slot results (each array [S], any may be NULL): state_host CTB_SLOT_*,
  * end_idx_host tokens of the slot's request, finish_host 1 if it ended at EOS.  A finished slot with end_idx 0 and
  * finish 1 sampled EOS as its first token (gpt.py:527: the request ends empty).  out->steps_done counts decode steps

@@ -2,6 +2,7 @@
 """Continuous-batching benchmark: the slot engine against static batches, one JSON line.
 
     python tools/bench_continuous.py [--requests N] [--slots S] [--steps K] [--warmup W] [--dump-outputs DIR] [--stream]
+                                     [--refine]
 
 N requests (default 128), each one utterance with its own seeded prompt (8..128 tokens) and forced length (64..1024
 tokens, min_new = max_new: synthetic weights have no meaningful EOS), run through the slot engine with S slots
@@ -9,6 +10,14 @@ tokens, min_new = max_new: synthetic weights have no meaningful EOS), run throug
 run to their longest row (``GPT.generate``).  Reports useful speech-tokens/s of both arms (the tokens the requests
 asked for), mean slot occupancy, the card and its power limit.  ``--steps`` = timed repeats of each arm, alternating.
 ``--dump-outputs DIR`` writes both arms' ids (concatenated in request order) and the lengths as DIR/<name>.npy.
+
+``--refine`` prints one more JSON line: each request is a text-refinement stage (16..160 forced text tokens) followed by
+its speech codes (the forced lengths above), through S slots, timed alternately in three arms: (a) both stages on the
+engine, the speech request admitted as the request's refinement ends (``Request.then``); (b) what
+``Chat.infer_continuous(skip_refine_text=False)`` does by default: static refinement in batches of S texts, then the
+speech codes on the engine; (c) the speech codes alone on the engine (the first line's workload).  Per arm: wall time,
+useful speech-tokens/s, decode steps, mean slot occupancy and the time from start to each request's first speech token
+(p50 / p95 / max; the token is sampled by the admission's prefill and counted at the status read that follows it).
 
 ``--stream`` then prints a second JSON line: the same requests streamed as audio (hidden path, DVAE decoder and Vocos
 from synthetic weights, InferCodeParams' default stream_batch / stream_speed / pass_first_n_batches), timed
@@ -283,6 +292,135 @@ def run_stream(args, local_rank: int = 0):
     return out
 
 
+def run_refine(args, local_rank: int = 0):
+    """Text refinement followed by speech codes, three arms timed alternately in this process (module docstring)."""
+    import numpy as np
+
+    from chattts_b200.config import Config
+    from chattts_b200.embed import Embed
+    from chattts_b200.engine import EngineDevice, Request
+    from chattts_b200.gpt import GPT
+    from chattts_b200.processors import gen_logits
+    from chattts_b200.prompts import synth_prompt_batch
+    from chattts_b200.synth import synth_embed_state, synth_gpt_state
+
+    dev = torch.device("cuda", local_rank)
+    torch.cuda.set_device(dev)
+    n, S = args.requests, args.slots
+    plen, tok = continuous_workload(n, seed=7)
+    tlen = torch.randint(16, 161, (n,), generator=torch.Generator().manual_seed(11)).tolist()
+    embed = Embed(768, 626, 21178, 4).load_state_dict(synth_embed_state(1)).to(dev)
+    gpt = GPT(Config().gpt, embed, device=dev, device_gpt=dev, max_batch=S, max_context=max(plen) + max(tok))
+    gpt.load_state(synth_gpt_state(0))
+    warp, proc = gen_logits(num_code=625, top_P=0.7, top_K=20, repetition_penalty=1.05)
+    cprocs, ctemp = (*proc, *warp), [0.3] * 4
+    warp, proc = gen_logits(num_code=21178, top_P=0.7, top_K=20, repetition_penalty=1.0)  # RefineTextParams()
+    tprocs = (*proc, *warp)
+    embs = []
+    for i, L in enumerate(plen):
+        ids, _, tmask = synth_prompt_batch([L], seed=1000 + i)
+        embs.append(embed(ids, tmask)[0])
+
+    # synthetic weights refine to no meaningful text, so each speech stage reuses its utterance's seeded prompt: the
+    # arms differ in scheduling only
+    def code_req(i, lengths):
+        return Request(emb=embs[i], temperature=ctemp, eos_token=625, max_new_token=lengths[i],
+                       min_new_token=lengths[i], logits_processors=cprocs, manual_seed=5000 + i)
+
+    def text_req(i, tl, lengths):
+        return Request(emb=embs[i], temperature=[0.7], eos_token=21001, max_new_token=tl[i], min_new_token=tl[i],
+                       logits_processors=tprocs, manual_seed=9000 + i, infer_text=True,
+                       then=lambda out, i=i: code_req(i, lengths))
+
+    first, pending = {}, []
+    admit, status = EngineDevice.admit, EngineDevice.status
+
+    def timed_admit(self, batch):  # speech requests admitted now have sampled their first token at the next status
+        pending.extend(self.requests[i].manual_seed - 5000 for _, i in batch if not self.requests[i].infer_text)
+        admit(self, batch)
+
+    def timed_status(self):
+        st = status(self)  # synchronises the stream: the admission's prefill and first token are done
+        t = time.perf_counter()
+        for k in pending:
+            first.setdefault(k, t)
+        pending.clear()
+        return st
+
+    EngineDevice.admit, EngineDevice.status = timed_admit, timed_status
+
+    def engine_run(reqs, cap):
+        for _ in gpt.generate_continuous(reqs, slots=S, return_hidden=False, max_new_cap=cap):
+            pass
+        torch.cuda.synchronize()
+        return gpt.last_schedule_stats
+
+    def arm_a(tl, lengths):  # refinement and speech on the engine
+        first.clear()
+        t0 = time.perf_counter()
+        st = engine_run([text_req(i, tl, lengths) for i in range(len(lengths))], max(max(lengths), max(tl)))
+        return dict(wall=time.perf_counter() - t0, t0=t0, first=dict(first), steps=st.decode_steps,
+                    row_tokens=sum(tl) + sum(lengths) - 2 * len(lengths))
+
+    def arm_b(tl, lengths):  # infer_continuous(skip_refine_text=False) today: static refinement, then the engine
+        first.clear()
+        t0 = time.perf_counter()
+        steps = 0
+        for lo in range(0, len(lengths), S):
+            idx = list(range(lo, min(lo + S, len(lengths))))
+            T0, mx = max(plen[i] for i in idx), max(tl[i] for i in idx)
+            emb = torch.zeros(len(idx), T0, 768, device=dev)
+            mask = torch.zeros(len(idx), T0, dtype=torch.bool)
+            for k, i in enumerate(idx):
+                emb[k, T0 - plen[i]:] = embs[i]
+                mask[k, T0 - plen[i]:] = True
+            list(gpt.generate(emb, torch.zeros(len(idx), T0, 4, dtype=torch.long), temperature=torch.tensor([0.7]),
+                              eos_token=21001, attention_mask=mask, max_new_token=mx, min_new_token=mx,
+                              logits_processors=tprocs, infer_text=True, show_tqdm=False, manual_seed=9000 + lo))
+            steps += mx
+        st = engine_run([code_req(i, lengths) for i in range(len(lengths))], max(lengths))
+        # the static batches' rows count the tokens their requests asked for, decode steps their longest rows
+        return dict(wall=time.perf_counter() - t0, t0=t0, first=dict(first), steps=steps + st.decode_steps,
+                    row_tokens=sum(tl) + sum(lengths) - 2 * len(lengths))
+
+    def arm_c(tl, lengths):  # the code-only engine workload of the first line
+        first.clear()
+        t0 = time.perf_counter()
+        st = engine_run([code_req(i, lengths) for i in range(len(lengths))], max(lengths))
+        return dict(wall=time.perf_counter() - t0, t0=t0, first=dict(first), steps=st.decode_steps,
+                    row_tokens=sum(lengths) - len(lengths))
+
+    arms = {"a": arm_a, "b": arm_b, "c": arm_c}
+    for _ in range(max(1, min(args.warmup, 2))):
+        for f in arms.values():
+            f([min(t, 32) for t in tlen[: 2 * S]], [min(t, 64) for t in tok[: 2 * S]])
+    runs = {k: [] for k in arms}
+    for _ in range(args.steps):
+        for k, f in arms.items():
+            runs[k].append(f(tlen, tok))
+    EngineDevice.admit, EngineDevice.status = admit, status
+    useful = sum(tok)
+
+    def summary(rs):
+        r = sorted(rs, key=lambda x: x["wall"])[len(rs) // 2]  # the median run
+        ft = [r["first"][i] - r["t0"] for i in range(n)]
+        out = {"seconds": round(r["wall"], 3), "seconds_all": [round(x["wall"], 3) for x in rs],
+               "tokens_per_s": round(useful / r["wall"], 1), "decode_steps": r["steps"],
+               "mean_slot_occupancy": round(r["row_tokens"] / (S * max(1, r["steps"])), 4),
+               "first_speech_token_s": {"p50": round(float(np.percentile(ft, 50)), 3),
+                                        "p95": round(float(np.percentile(ft, 95)), 3), "max": round(max(ft), 3)}}
+        return out
+
+    name, limit = gpu_card(local_rank)
+    out = {"metric": "continuous_refine", "card": name, "power_limit": limit, "requests": n, "slots": S,
+           "text_tokens": [min(tlen), max(tlen)], "forced_tokens": [min(tok), max(tok)], "useful_tokens": useful,
+           "repeats": args.steps}
+    for k in arms:
+        out[k] = summary(runs[k])
+    out["a_over_b_speedup"] = round(out["b"]["seconds"] / out["a"]["seconds"], 3)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--requests", type=int, default=128)
@@ -291,6 +429,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--dump-outputs", default=None, metavar="DIR")
     ap.add_argument("--stream", action="store_true", help="also measure streamed audio (a second JSON line)")
+    ap.add_argument("--refine", action="store_true", help="also measure refinement + speech (one more JSON line)")
     args = ap.parse_args()
     if args.steps < 1:
         ap.error("--steps must be >= 1")
@@ -298,6 +437,8 @@ def main():
     print(json.dumps(run_continuous(args, rank)), flush=True)
     if args.stream:
         print(json.dumps(run_stream(args, rank)), flush=True)
+    if args.refine:
+        print(json.dumps(run_refine(args, rank)), flush=True)
 
 
 if __name__ == "__main__":
