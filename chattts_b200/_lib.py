@@ -62,6 +62,7 @@ EXPORTS = (
     "ctb_abi_version", "ctb_last_error", "ctb_launch_count", "ctb_gpt_layout_query", "ctb_gpt_create",
     "ctb_gpt_destroy", "ctb_gpt_begin", "ctb_gpt_decode", "ctb_gpt_status_query", "ctb_gpt_profile_kernel", "ctb_gpt_debug_trace", "ctb_gpt_embed_prompt", "ctb_sample",
     "ctb_gpt_engine_begin", "ctb_gpt_engine_admit", "ctb_gpt_engine_admit_text", "ctb_gpt_engine_status",
+    "ctb_gpt_engine_cancel",
     "ctb_dvae_blob_floats", "ctb_vocos_blob_floats", "ctb_decoder_create", "ctb_decoder_destroy",
     "ctb_dvae_decode", "ctb_vocos_decode", "ctb_decode_rows",
     "ctb_dvae_encoder_blob_floats", "ctb_dvae_encoder_create", "ctb_dvae_encoder_destroy", "ctb_dvae_encode",
@@ -111,6 +112,7 @@ def load(build_if_missing: bool = True):
         lib.ctb_gpt_engine_admit.argtypes = [vp, i32, vp, i32, vp, vp, C.POINTER(SamplerConfig), vp, vp, vp]
         lib.ctb_gpt_engine_admit_text.argtypes = lib.ctb_gpt_engine_admit.argtypes
         lib.ctb_gpt_engine_status.argtypes = [vp, C.POINTER(GptStatus), vp, vp, vp, vp]
+        lib.ctb_gpt_engine_cancel.argtypes = [vp, i32, vp, vp]
         lib.ctb_sample.argtypes = [vp, i32, i32, i32, C.POINTER(SamplerConfig), vp, vp, i32, i32, i32, vp, vp]
         lib.ctb_dvae_blob_floats.argtypes = [C.POINTER(ConvStackConfig)]
         lib.ctb_dvae_blob_floats.restype = i64

@@ -21,6 +21,7 @@ import torch
 from .config import Config
 from .decoder import decode_to_wavs_window, DVAE, Vocos, decode_to_wavs, stream_window
 from .embed import Embed
+from .engine import Job, OpenEngine
 from .gpt import GPT
 from .norm import Normalizer
 from .processors import gen_logits
@@ -291,12 +292,7 @@ class Chat:
         texts = [self.normalizer(t, do_text_normalization, do_homophone_replacement, lang) for t in texts]
         cap = max(p.max_new_token for p in params)
         if not skip_refine_text and refine_on_engine:
-            requests = []
-            for t, p, r in zip(texts, params, refine):
-                req = self._refine_request(t, r)
-                req.then = lambda out, p=p: self._code_request(self._refined_text(out), p)
-                req.stream_batch = p.stream_batch  # the engine polls at the smallest stream_batch of its requests
-                requests.append(req)
+            requests = [self._chained_request(t, p, r) for t, p, r in zip(texts, params, refine)]
             return requests, max(cap, max(r.max_new_token for r in requests))
         if not skip_refine_text:
             if any(r is not refine[0] for r in refine):
@@ -378,10 +374,27 @@ class Chat:
                        min_new_token=params.min_new_token, logits_processors=(*processors, *warpers),
                        manual_seed=params.manual_seed, ensure_non_empty=params.ensure_non_empty, infer_text=True)
 
+    def _chained_request(self, text, params, refine):
+        """The text's refinement request, whose follow-up is the speech-code request of the refined text."""
+        req = self._refine_request(text, refine)
+        req.then = lambda out: self._code_request(self._refined_text(out), params)
+        req.stream_batch = params.stream_batch  # the engine polls at the smallest stream_batch of its requests
+        return req
+
     def _refined_text(self, out) -> str:
         """The text ``_infer`` makes of one refined row: ids below ``break_0_ids``, decoded."""
         ids = out.ids[0]
         return self.tokenizer.decode([ids[ids.less(self.tokenizer.break_0_ids)]])[0]
+
+    def open_engine(self, slots: Optional[int] = None, max_new_cap: int = 2048, use_decoder: bool = True):
+        """A long-lived slot engine (``GPT.open_engine``) that synthesises texts submitted from any thread while it
+        decodes: ``engine.submit(text, params_infer_code=None, stream=False, skip_refine_text=True, ...) -> Job``,
+        ``Job.cancel()`` for one text, ``close(cancel=False)`` or a ``with`` block to drain it (``close(cancel=True)``
+        is its interrupt; ``Chat.context`` is not read).  ``slots`` defaults to the handle's ``max_batch``; every
+        stage's ``max_new_token`` must be at most ``max_new_cap``.  See ``ChatEngine.submit``."""
+        assert self.has_loaded(use_decoder=use_decoder)
+        return self.gpt._open_slot_engine(ChatEngine, self.gpt.max_batch if slots is None else slots, max_new_cap,
+                                          use_decoder, None, self, use_decoder)
 
     def interrupt(self):
         self.context.set(True)
@@ -558,10 +571,8 @@ def stream_continuous(gpt: GPT, model: DVAE, requests, windows: List[StreamWindo
     accumulates the host time spent decoding and copying the audio."""
     import time
 
-    thr = np.float32(1e-5)
     for dev, batch in gpt._stream_polls(requests, slots, use_decoder, context, max_new_cap=max_new_cap):
         t_start = time.perf_counter()
-        buf = dev.hid_out if use_decoder else dev.ids_out
         jobs = []  # (text, slot, n_tokens, a, b, flush, last)
         for i, s, n, last in batch:
             t = _text_index(gpt, requests, i)
@@ -569,31 +580,98 @@ def stream_continuous(gpt: GPT, model: DVAE, requests, windows: List[StreamWindo
                 continue
             ws = windows[t].windows(n, last)
             jobs += [(t, s, n, a, b, flush, last and k == len(ws) - 1) for k, (a, b, flush) in enumerate(ws)]
-        due = [k for k, j in enumerate(jobs) if j[4] > j[3]]
-        chunks: Dict[int, np.ndarray] = {}
-        if due and ragged:
-            rows, cuts = [], []
-            for k in due:
-                _, s, n, a, b = jobs[k][:5]
-                a, b, t0, t1 = stream_window(n, a, b)
-                rows.append(buf[s, t0:t1])
-                cuts.append((a - 512 * t0, b - 512 * t0))
-            wavs = model.engine.decode_rows(rows, 1 if use_decoder else 2)
-            flat = torch.cat([w[c0:c1] for w, (c0, c1) in zip(wavs, cuts)]).cpu().numpy()
-            off = 0
-            for k, (c0, c1) in zip(due, cuts):
-                chunks[k] = flat[None, off: off + c1 - c0]
-                off += c1 - c0
-        elif due:
-            for k in due:
-                _, s, n, a, b = jobs[k][:5]
-                chunks[k] = decode_to_wavs_window([buf[s, :n]], use_decoder, model, model, a, b)
-        out = []
-        for k, (i, _, _, _, _, flush, last) in enumerate(jobs):
-            chunk = chunks.get(k, np.zeros((1, 0), dtype=np.float32))
-            if flush:
-                chunk = chunk[:, np.abs(chunk[0]) > thr]
-            out.append((i, chunk, last))
+        out = _decode_windows(dev, jobs, model, use_decoder, ragged)
         if stats is not None:
             stats["path2_s"] = stats.get("path2_s", 0.0) + time.perf_counter() - t_start
         yield from out
+
+
+def _decode_windows(dev, jobs, model: DVAE, use_decoder: bool, ragged: bool = True):
+    """One poll's path-2 work on the slot engine ``dev``: ``jobs`` are ``(key, slot, n_tokens, a, b, flush, last)``,
+    samples [a, b) of the decode of the slot's first ``n_tokens`` tokens (``flush``: drop its silent samples) ->
+    ``[(key, chunk [1, m] float32, last)]`` in the same order.  Every non-empty window goes into one ``decode_rows``
+    call (``ragged=False``: one ``decode_to_wavs_window`` call each)."""
+    thr = np.float32(1e-5)
+    buf = dev.hid_out if use_decoder else dev.ids_out
+    due = [k for k, j in enumerate(jobs) if j[4] > j[3]]
+    chunks: Dict[int, np.ndarray] = {}
+    if due and ragged:
+        rows, cuts = [], []
+        for k in due:
+            _, s, n, a, b = jobs[k][:5]
+            a, b, t0, t1 = stream_window(n, a, b)
+            rows.append(buf[s, t0:t1])
+            cuts.append((a - 512 * t0, b - 512 * t0))
+        wavs = model.engine.decode_rows(rows, 1 if use_decoder else 2)
+        flat = torch.cat([w[c0:c1] for w, (c0, c1) in zip(wavs, cuts)]).cpu().numpy()
+        off = 0
+        for k, (c0, c1) in zip(due, cuts):
+            chunks[k] = flat[None, off: off + c1 - c0]
+            off += c1 - c0
+    elif due:
+        for k in due:
+            _, s, n, a, b = jobs[k][:5]
+            chunks[k] = decode_to_wavs_window([buf[s, :n]], use_decoder, model, model, a, b)
+    out = []
+    for k, (i, _, _, _, _, flush, last) in enumerate(jobs):
+        chunk = chunks.get(k, np.zeros((1, 0), dtype=np.float32))
+        if flush:
+            chunk = chunk[:, np.abs(chunk[0]) > thr]
+        out.append((i, chunk, last))
+    return out
+
+
+class ChatEngine(OpenEngine):
+    """``Chat.open_engine``: an open slot engine whose jobs are texts (see there).  At each poll every window due for a
+    streaming job and the whole sequence of every non-streaming job that completed go into one ``decode_rows`` call."""
+
+    def __init__(self, make_device, chunk, check, device, on_close, chat: "Chat", use_decoder: bool,
+                 max_new_cap: Optional[int] = None):
+        self.chat, self.use_decoder = chat, use_decoder
+        self.model = chat.decoder if use_decoder else chat.dvae
+        super().__init__(make_device, chunk, check, device, on_close, max_new_cap)
+
+    def submit(self, text: str, params_infer_code=None, stream=False, skip_refine_text=True, params_refine_text=None,
+               lang=None, do_text_normalization=True, do_homophone_replacement=True) -> Job:
+        """Queue one text -> ``Job``: ``result()`` is the waveform ``infer_continuous`` yields for it, or with
+        ``stream=True`` the job iterates the ``(chunk, last)`` pairs ``infer_continuous_stream`` yields for it.
+        ``skip_refine_text=False`` refines the text on the engine first (``refine_on_engine=True``).  A cancelled
+        job's ``result()`` raises ``concurrent.futures.CancelledError`` and its stream ends."""
+        chat = self.chat
+        params = params_infer_code or Chat.InferCodeParams()
+        if not skip_refine_text and self.max_new_cap is not None and params.max_new_token > self.max_new_cap:
+            # the speech stage is made only when the refinement ends: check its limit here, in the caller's thread
+            raise ValueError(f"max_new_token {params.max_new_token} exceeds max_new_cap={self.max_new_cap}")
+        text = chat.normalizer(text, do_text_normalization, do_homophone_replacement, lang)
+        # the prompt is embedded here, on the caller's stream: ctb_gpt_embed_prompt is the one handle call that may run
+        # beside the worker (it only reads the weights); submit orders the engine's stream after the caller's
+        if skip_refine_text:
+            request = chat._code_request(text, params)
+        else:
+            request = chat._chained_request(text, params, params_refine_text or Chat.RefineTextParams())
+        windows = StreamWindows(params.stream_speed, params.pass_first_n_batches) if stream else None
+        return super().submit(request, stream, windows)
+
+    def _serve(self, dev, requests, batch, jobs) -> None:
+        wjobs = []  # (job, slot, n_tokens, a, b, flush, last), as stream_continuous builds them
+        for (i, s, n, last), (job, final) in zip(batch, jobs):
+            if i in self.stats.failed:
+                job._fail(self.stats.failed[i])
+            elif job.done():
+                continue
+            elif i in self.stats.cancelled:
+                job._stop()
+            elif requests[i].infer_text:  # a refinement stage: its follow-up carries the text on
+                continue
+            elif job.stream:
+                ws = job.state.windows(n, last)
+                wjobs += [(job, s, n, a, b, flush, last and k == len(ws) - 1) for k, (a, b, flush) in enumerate(ws)]
+            elif last:  # the whole sequence, silent samples dropped: what infer_continuous yields
+                wjobs.append((job, s, n, 0, 512 * n - 256, True, True))
+        for job, chunk, last in _decode_windows(dev, wjobs, self.model, self.use_decoder):
+            if job.stream:
+                job._put((chunk, last))
+                if last:
+                    job._finish(None)
+            else:
+                job._finish(chunk[0])

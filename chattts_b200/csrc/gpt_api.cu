@@ -1168,6 +1168,26 @@ extern "C" int ctb_gpt_engine_status(ctb_gpt* h, ctb_gpt_status* out, int32_t* s
   return CTB_OK;
 }
 
+extern "C" int ctb_gpt_engine_cancel(ctb_gpt* h, int32_t n, const int32_t* slots, void* stream) {
+  if (!h || !slots) return set_err(CTB_ERR_ARG, "null argument");
+  if (!h->engine) return set_err(CTB_ERR_STATE, "ctb_gpt_engine_begin has not been called");
+  const int S = h->B;
+  if (n < 1 || n > S) return set_err(CTB_ERR_ARG, "n=%d outside [1,%d]", n, S);
+  if (S > CANCEL_MAX_SLOTS) return set_err(CTB_ERR_ARG, "S=%d: cancellation serves up to %d slots", S, CANCEL_MAX_SLOTS);
+  CancelP p{};
+  p.st = h->st; p.rows = h->rows; p.finish = h->finish; p.B = S;
+  for (int i = 0; i < n; ++i) {
+    const int b = slots[i];
+    if (b < 0 || b >= S || (p.mask[b >> 5] >> (b & 31) & 1u))
+      return set_err(CTB_ERR_ARG, "slot %d out of range or repeated", b);
+    p.mask[b >> 5] |= 1u << (b & 31);
+  }
+  // h->eng_text stays as it is: the next ctb_gpt_engine_status recomputes it from the rows
+  k_cancel_rows<<<1, 256, 0, (cudaStream_t)stream>>>(p);
+  CTB_LAUNCH_CHECK();
+  return CTB_OK;
+}
+
 namespace ctb {
 // Embed.forward (embed.py:51-79): one CTA per prompt position
 __global__ void k_embed_prompt(const int64_t* __restrict__ ids, const uint8_t* __restrict__ text_mask,

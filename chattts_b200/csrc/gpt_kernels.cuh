@@ -758,4 +758,15 @@ struct FinalP {
 __global__ void k_finalize(const FinalP p);
 __global__ void k_finalize_rows(const FinalP p);
 
+// ctb_gpt_engine_cancel: the slots to stop travel by value as a bit set, so the launch needs no host-to-device copy
+constexpr int CANCEL_MAX_SLOTS = 1024;
+struct CancelP {
+  LoopState* st;
+  RowState* rows;
+  uint8_t* finish;
+  int B;
+  uint32_t mask[CANCEL_MAX_SLOTS / 32];  // bit b: stop slot b
+};
+__global__ void k_cancel_rows(const CancelP p);
+
 }  // namespace ctb

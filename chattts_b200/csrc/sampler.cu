@@ -343,6 +343,28 @@ __global__ void k_finalize_rows(const FinalP p) {
   }
 }
 
+// Slot-engine cancellation (ctb_gpt_engine_cancel), launched between decode steps outside the captured graphs: every
+// listed row that is running or pending ends as a row that stopped short of EOS (RS_FINISHED, finish 0) and keeps its
+// end_idx, so its outputs stay a valid prefix.  Other rows are untouched.  all_finished = no running row, as in
+// k_finalize_rows, so later decode steps with nothing running stay no-ops and do not advance st->step.
+__global__ void k_cancel_rows(const CancelP p) {
+  __shared__ int s_running;
+  if (threadIdx.x == 0) s_running = 0;
+  __syncthreads();
+  for (int b = threadIdx.x; b < p.B; b += blockDim.x) {
+    RowState* r = p.rows + b;
+    int state = ldg_cg(&r->state);
+    if (((p.mask[b >> 5] >> (b & 31)) & 1u) && (state == RS_RUNNING || state == RS_PENDING)) {
+      p.finish[b] = 0;
+      state = RS_FINISHED;
+      r->state = state;
+    }
+    if (state == RS_RUNNING) atomicOr(&s_running, 1);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) p.st->all_finished = s_running ? 0 : 1;
+}
+
 template __global__ void k_sample<false>(const SampleP p);
 template __global__ void k_sample<true>(const SampleP p);
 

@@ -14,9 +14,13 @@ The scheduling policy (``schedule``) is plain Python over a small device interfa
 from __future__ import annotations
 
 import ctypes as C
+import logging
+import queue
+import threading
 from collections import deque
+from concurrent.futures import Future
 from dataclasses import dataclass, field
-from typing import Callable, Dict, Iterator, List, Optional, Sequence, Tuple
+from typing import Callable, Dict, Iterator, List, Optional, Sequence, Set, Tuple
 
 import torch
 
@@ -86,38 +90,122 @@ class ScheduleStats:
     tokens: int = 0
     interrupted: bool = False
     children: Dict[int, int] = field(default_factory=dict)  # request index -> index of the follow-up it returned
+    cancelled: Set[int] = field(default_factory=set)  # request indices stopped by an ``Arrivals.cancel``
+    keys: Dict[int, object] = field(default_factory=dict)  # open source: index of a submitted request -> its key
+    failed: Dict[int, BaseException] = field(default_factory=dict)  # open source: request index -> its follow-up's error
 
 
-def _follow_up(requests: List[Request], i: int, slot: Optional[int], n: int, dev, check, stats: ScheduleStats):
-    """Request ``i`` ended: its follow-up's index as a list (empty without one)."""
+class Arrivals:
+    """The request source of an open engine: requests submitted and cancelled from any thread, taken by the scheduling
+    loop at each poll.  Each submission carries a key (an open engine's ``Job``; by default the request itself), so one
+    ``Request`` may be submitted several times under different keys; ``cancel(key)`` stops whichever stage of that
+    submission's follow-up chain is live."""
+
+    def __init__(self):
+        self._cv = threading.Condition()
+        self._new: List[Tuple[object, Request]] = []
+        self._cancel: List[object] = []
+        self.closed = False
+
+    def submit(self, r: Request, key=None) -> None:
+        with self._cv:
+            if self.closed:
+                raise RuntimeError("the engine is closed")
+            self._new.append((r if key is None else key, r))
+            self._cv.notify()
+
+    def cancel(self, key) -> None:
+        with self._cv:
+            self._cancel.append(key)
+            self._cv.notify()
+
+    def close(self) -> None:
+        with self._cv:
+            self.closed = True
+            self._cv.notify()
+
+    def take(self, block: bool) -> Tuple[List[Tuple[object, Request]], List[object], bool]:
+        """``([(key, request)] submitted, [key] cancelled, closed)`` since the last call; with ``block``, waits until
+        there is one of them."""
+        with self._cv:
+            while block and not self._new and not self._cancel and not self.closed:
+                self._cv.wait()
+            new, cancel, self._new, self._cancel = self._new, self._cancel, [], []
+            return new, cancel, self.closed
+
+
+def _follow_up(requests: List[Request], i: int, slot: Optional[int], n: int, dev, check, stats: ScheduleStats,
+               source: Optional[Arrivals] = None):
+    """Request ``i`` ended: its follow-up's index as a list (empty without one).  With an open ``source`` a follow-up
+    that fails (``then`` raises or ``check`` rejects it) is recorded in ``stats.failed`` instead of stopping the loop."""
     then = requests[i].then
     if then is None:
         return []
-    child = then(dev.empty(i) if slot is None else dev.harvest(slot, n))
-    if child is None:
+    try:
+        child = then(dev.empty(i) if slot is None else dev.harvest(slot, n))
+        if child is None:
+            return []
+        if not isinstance(child, Request):
+            raise TypeError("Request.then must return a Request or None")
+        if check is not None:
+            check(child)
+    except Exception as e:
+        if source is None:
+            raise
+        stats.failed[i] = e
         return []
-    if not isinstance(child, Request):
-        raise TypeError("Request.then must return a Request or None")
-    if check is not None:
-        check(child)
     requests.append(child)
     stats.children[i] = len(requests) - 1
     return [len(requests) - 1]
 
 
 def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: Optional[ScheduleStats] = None,
-                 check: Optional[Callable[[Request], None]] = None
+                 check: Optional[Callable[[Request], None]] = None, source: Optional[Arrivals] = None
                  ) -> Iterator[Tuple[SlotStatus, List[Optional[int]], list]]:
     """The scheduling policy of ``schedule``: yields once per poll ``(status, owner, ended)`` - the slots' status, the
     request each slot held when it was read, and the requests that ended at this poll as ``(request_index, slot or
     None, n_tokens, eos)``.  The slots of the ended requests are refilled only after the generator is resumed.
 
     A request's follow-up (``Request.then``, called here while the slot's outputs are valid and checked by ``check``)
-    is appended to ``requests`` and queued ahead of the waiting requests, so the refill after this poll admits it."""
+    is appended to ``requests`` and queued ahead of the waiting requests, so the refill after this poll admits it.
+
+    ``source`` (open engine): every poll first takes the requests submitted since the last one (appended to
+    ``requests`` and queued behind the waiting ones; ``stats.keys`` maps each one's index to its submission key) and
+    the cancellations.  A cancelled waiting request leaves the
+    queue and ends empty without touching a slot; a cancelled running request is stopped with ``dev.cancel`` right
+    after the status read, so it ends with the ``end_idx`` tokens that read reported (a request the same read shows
+    finished is finished); neither calls its ``then``, and cancelling a request whose follow-up was already made
+    cancels the follow-up.  Cancelled requests are listed in ``stats.cancelled``.  With nothing running and nothing
+    waiting the loop blocks in ``source.take`` instead of decoding, and it ends once the source is closed and drained."""
     stats = stats if stats is not None else ScheduleStats()
     waiting = deque(range(len(requests)))
     owner: List[Optional[int]] = [None] * dev.slots
+    live: Dict[object, int] = {}  # open source: submission key -> index of its live stage
+    root: Dict[int, object] = {}  # and back
+    doomed: Set[int] = set()  # running requests to stop after the next status read
     while True:
+        taken: list = []
+        if source is not None:
+            idle = not waiting and all(o is None for o in owner)
+            new, cancels, closed = source.take(block=idle)
+            for key, r in new:
+                requests.append(r)
+                i = len(requests) - 1
+                live[key], root[i], stats.keys[i] = i, key, key
+                waiting.append(i)
+            for key in cancels:
+                i = live.get(key)
+                if i is None:  # ended already
+                    continue
+                if i in waiting:
+                    waiting.remove(i)
+                    del live[root.pop(i)]
+                    stats.cancelled.add(i)
+                    taken.append((i, None, 0, False))
+                else:
+                    doomed.add(i)
+            if idle and closed and not new and not taken:
+                return
         free = [s for s in range(dev.slots) if owner[s] is None]
         batch = []
         while free and waiting:
@@ -131,15 +219,26 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
         st = dev.status()
         stats.decode_steps = st.steps_done
         polled = list(owner)
-        ended = []
+        ended = taken
         follow: List[int] = []
         freed = False
+        stop = [s for s in range(dev.slots) if owner[s] in doomed and st.state[s] != _lib.SLOT_FINISHED]
+        if stop:
+            dev.cancel(stop)
         for s in range(dev.slots):
             i = owner[s]
-            if i is None or st.state[s] != _lib.SLOT_FINISHED:
+            if i is None or (st.state[s] != _lib.SLOT_FINISHED and s not in stop):
                 continue
             owner[s] = None
             freed = True
+            was_doomed = i in doomed
+            doomed.discard(i)
+            if s in stop:  # no follow-up after a cancel
+                del live[root.pop(i)]
+                stats.cancelled.add(i)
+                stats.tokens += st.end_idx[s]
+                ended.append((i, s, st.end_idx[s], False))
+                continue
             if st.end_idx[s] == 0 and st.finish[s]:
                 r = requests[i]
                 if r.manual_seed is None and r.ensure_non_empty:
@@ -147,11 +246,22 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
                     stats.requeued += 1
                     continue
                 ended.append((i, None, 0, True))
-                follow += _follow_up(requests, i, None, 0, dev, check, stats)
-                continue
-            stats.tokens += st.end_idx[s]
-            ended.append((i, s, st.end_idx[s], bool(st.finish[s])))
-            follow += _follow_up(requests, i, s, st.end_idx[s], dev, check, stats)
+                kids = _follow_up(requests, i, None, 0, dev, check, stats, source)
+            else:
+                stats.tokens += st.end_idx[s]
+                ended.append((i, s, st.end_idx[s], bool(st.finish[s])))
+                kids = _follow_up(requests, i, s, st.end_idx[s], dev, check, stats, source)
+            if i in root:  # the submitted request's live stage moves on to its follow-up, or it is done
+                key = root.pop(i)
+                if kids and was_doomed:  # finished at the read that applies its cancel: the follow-up is cancelled
+                    stats.cancelled.add(kids[0])
+                    ended.append((kids[0], None, 0, False))
+                    kids = []
+                if kids:
+                    live[key], root[kids[0]] = kids[0], key
+                else:
+                    del live[key]
+            follow += kids
         waiting.extendleft(reversed(follow))  # ahead of the waiting requests, in slot order
         if freed and waiting:
             yield st, polled, ended
@@ -164,9 +274,10 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
                 stats.tokens += st.end_idx[s]
                 ended.append((owner[s], s, st.end_idx[s], False))
         yield st, polled, ended
-        if not running or interrupted:
+        if interrupted or (not running and source is None):
             return
-        dev.decode(chunk)
+        if running:
+            dev.decode(chunk)
 
 
 def schedule(requests: List[Request], dev, chunk: int, context=None, stats: Optional[ScheduleStats] = None,
@@ -187,7 +298,7 @@ def schedule(requests: List[Request], dev, chunk: int, context=None, stats: Opti
 
 
 def stream_schedule(requests: List[Request], dev, chunk: int, context=None, stats: Optional[ScheduleStats] = None,
-                    check: Optional[Callable[[Request], None]] = None
+                    check: Optional[Callable[[Request], None]] = None, source: Optional[Arrivals] = None
                     ) -> Iterator[List[Tuple[int, Optional[int], int, bool]]]:
     """``schedule``'s policy, yielding once per poll the list of ``(request_index, slot, n_tokens, last)``: for each
     request, the yields ``GPT.generate(stream=True, stream_batch=r.stream_batch)`` makes for it alone, in its order,
@@ -197,9 +308,12 @@ def stream_schedule(requests: List[Request], dev, chunk: int, context=None, stat
     reaches unfinished, yields a boundary a second time when EOS follows it on the very next step, and ends with the
     final yield; a row that stops at ``max_new_token`` is not finished there, so it gets no second yield.  Tokens only
     ever append to a slot, so each poll rebuilds every boundary a slot crossed since the last one from its token count:
-    the yields do not depend on ``chunk``.  The slots' outputs stay in place until the generator is resumed."""
+    the yields do not depend on ``chunk``.  The slots' outputs stay in place until the generator is resumed.
+
+    With an open ``source`` (see ``_poll_cycles``) a cancelled request gets a final yield of what it has, and
+    ``stats.cancelled`` tells it apart."""
     sent: Dict[int, int] = {}  # last boundary yielded per request
-    for st, owner, ended in _poll_cycles(requests, dev, chunk, context, stats, check):
+    for st, owner, ended in _poll_cycles(requests, dev, chunk, context, stats, check, source):
         out = []
         for s, i in enumerate(owner):
             if i is None:
@@ -217,6 +331,7 @@ def stream_schedule(requests: List[Request], dev, chunk: int, context=None, stat
             if s is not None and eos and n > 0 and n % requests[i].stream_batch == 0:
                 out.append((i, s, n, False))  # the boundary before the finishing step, again (gpt.py:381-384)
             out.append((i, s, n, True))
+            sent.pop(i, None)
         if out:
             yield out
 
@@ -289,6 +404,11 @@ class EngineDevice:
     def decode(self, n: int) -> None:
         _lib.check(self.lib.ctb_gpt_decode(self.gpt._handle, n, self.stream))
 
+    def cancel(self, slots: List[int]) -> None:
+        """Stop the requests in ``slots`` (ctb_gpt_engine_cancel): each keeps the tokens it has."""
+        _lib.check(self.lib.ctb_gpt_engine_cancel(self.gpt._handle, len(slots), (C.c_int32 * len(slots))(*slots),
+                                                  self.stream))
+
     def status(self) -> SlotStatus:
         st = _lib.GptStatus()
         _lib.check(self.lib.ctb_gpt_engine_status(self.gpt._handle, C.byref(st), self._state,
@@ -321,3 +441,265 @@ class EngineDevice:
         hid = ([torch.zeros(0, self.gpt.config.hidden_size, dtype=torch.float32, device=self.dev)]
                if self.hid_out is not None else [])
         return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid)
+
+
+_END = object()  # closes a streaming job's iterator
+_log = logging.getLogger(__name__)
+
+
+class _RequestTable:
+    """An open engine's requests by index (the ``requests`` of ``_poll_cycles``): indices are never reused, and an entry
+    is dropped once its request has been served, so a long-lived engine holds only the requests still in it."""
+
+    def __init__(self):
+        self._items: Dict[int, Request] = {}
+        self._next = 0
+
+    def append(self, r: Request) -> None:
+        self._items[self._next] = r
+        self._next += 1
+
+    def __len__(self) -> int:  # the next index
+        return self._next
+
+    def __getitem__(self, i: int) -> Request:
+        return self._items[i]
+
+    def __delitem__(self, i: int) -> None:
+        del self._items[i]
+
+    def held(self) -> int:
+        return len(self._items)
+
+
+class Job:
+    """A request submitted to an open engine (``GPT.open_engine``, ``Chat.open_engine``).
+
+    ``result(timeout)`` waits for it to end; ``cancel()`` stops it at the engine's next poll; a streaming job
+    (``submit(..., stream=True)``) is also an iterator of its yields, which simply ends when the job is cancelled.
+    Results and yields are handed over on the caller's current CUDA stream: whatever the engine copied for them is
+    complete before the caller's later work on that stream reads it."""
+
+    def __init__(self, engine: "OpenEngine", stream: bool):
+        self._engine, self.stream = engine, stream
+        self._future: Future = Future()
+        self._items: Optional[queue.Queue] = queue.Queue() if stream else None
+        self._cancelled = False
+        self.state = None
+
+    def cancel(self) -> None:
+        self._engine._source.cancel(self)
+
+    def result(self, timeout: Optional[float] = None):
+        return self._engine._receive(*self._future.result(timeout))
+
+    def done(self) -> bool:
+        return self._future.done()
+
+    def cancelled(self) -> bool:
+        return self._cancelled or self._future.cancelled()
+
+    def __iter__(self):
+        if self._items is None:
+            raise TypeError("only a job submitted with stream=True is iterable")
+        while True:
+            item = self._items.get()
+            if item is _END:
+                return
+            if isinstance(item, BaseException):
+                raise item
+            yield self._engine._receive(*item)
+
+    # worker side
+    def _put(self, value, event=None) -> None:
+        self._items.put((value, event))
+
+    def _finish(self, value, event=None) -> None:
+        if self._items is not None:
+            self._items.put(_END)
+        self._future.set_result((value, event))
+
+    def _stop(self) -> None:
+        """Cancelled: a streaming job's iterator ends and ``result()`` raises ``CancelledError``."""
+        self._cancelled = True
+        if self._items is not None:
+            self._items.put(_END)
+        self._future.cancel()
+
+    def _fail(self, e: BaseException) -> None:
+        if self._items is not None:
+            self._items.put(e)
+        if not self._future.done():
+            self._future.set_exception(e)
+
+
+class OpenEngine:
+    """A slot engine that takes requests while it decodes (``schedule``'s policy with an ``Arrivals`` source).
+
+    One worker thread owns the device: it makes the device layer with ``make_device(requests)`` and issues every
+    admission, decode, status read, cancellation and harvest copy on the engine's CUDA stream.  ``submit`` and
+    ``Job.cancel`` only queue under a lock, from any thread.  ``check`` validates a request in the caller's thread at
+    ``submit`` (and each follow-up in the worker, where a failure fails that job only).  An error in the worker fails
+    every pending job with it, stops the engine and is raised again by ``close``.  Subclasses turn each poll's yields
+    into job results (``_serve``)."""
+
+    def __init__(self, make_device: Callable[[List[Request]], object], chunk: int,
+                 check: Optional[Callable[[Request], None]] = None, device=None,
+                 on_close: Optional[Callable[[], None]] = None, max_new_cap: Optional[int] = None):
+        self._make_device, self.chunk, self._check, self._on_close = make_device, int(chunk), check, on_close
+        self.device, self.max_new_cap = device, max_new_cap
+        cuda = device is not None and torch.device(device).type == "cuda"
+        self._stream = torch.cuda.Stream(device) if cuda else None
+        self._source = Arrivals()
+        self._lock = threading.Lock()
+        self._pending: Set[Job] = set()  # submitted jobs, until each one ends
+        self._job_at: Dict[int, Job] = {}  # request index (a stage) -> its job, while the stage is live
+        self._error: Optional[BaseException] = None
+        self._stopped = False
+        self.stats = ScheduleStats()
+        self._requests = _RequestTable()
+        self._thread = threading.Thread(target=self._run, name="ctb-open-engine", daemon=True)
+        self._thread.start()
+
+    # ---------------------------------------------------------------- callers
+    def submit(self, request: Request, stream: bool = False, state=None) -> Job:
+        """Queue ``request``; ``state`` is kept on the job for ``_serve`` (``Job.state``)."""
+        if not isinstance(request, Request):
+            raise TypeError("requests must be chattts_b200.engine.Request objects")
+        if self._check is not None:
+            self._check(request)
+        job = Job(self, stream)
+        job.state = state
+        with self._lock:
+            if self._stopped:
+                raise RuntimeError("the engine is closed") from self._error
+            if self._stream is not None:  # the prompt was made on the caller's stream
+                self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            self._pending.add(job)
+            self._source.submit(request, job)
+        return job
+
+    def close(self, cancel: bool = False) -> None:
+        """Wait for every submitted job (``cancel=True``: cancel them all first), then join the worker.  Raises the
+        worker's error, if it had one."""
+        if cancel:
+            with self._lock:
+                for job in list(self._pending):
+                    self._source.cancel(job)
+        self._source.close()
+        self._thread.join()
+        if self._on_close is not None:
+            self._on_close()
+            self._on_close = None
+        if self._error is not None:
+            raise self._error
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, exc_type, exc, tb):
+        if exc_type is None:
+            self.close()
+            return
+        try:  # the block's own exception is the one to propagate; a worker error is only logged beside it
+            self.close(cancel=True)
+        except Exception:
+            _log.exception("the open engine had failed as well")
+
+    def _receive(self, value, event):
+        """A job's result or yield in the caller's thread (``event``: recorded by ``_serve`` after its copies)."""
+        return value
+
+    # ---------------------------------------------------------------- worker
+    def _run(self) -> None:
+        requests = self._requests
+        try:
+            if self._stream is not None:
+                with torch.cuda.device(self.device), torch.cuda.stream(self._stream), torch.no_grad():
+                    self._loop(requests)
+            else:
+                self._loop(requests)
+        except BaseException as e:
+            self._error = e
+        finally:
+            with self._lock:
+                self._stopped = True
+                self._source.close()
+                jobs = list(self._pending)
+                self._pending.clear()
+            for job in jobs:
+                if not job.done():
+                    job._fail(self._error or RuntimeError("the engine stopped"))
+
+    def _loop(self, requests: _RequestTable) -> None:
+        dev = self._make_device(requests)
+        for batch in stream_schedule(requests, dev, self.chunk, None, self.stats, self._check, self._source):
+            jobs = []
+            for i, s, n, last in batch:
+                job = self._job_at.get(i)
+                if job is None:  # a submitted request's first yield
+                    job = self._job_at[i] = self.stats.keys.pop(i)
+                child = self.stats.children.get(i) if last else None
+                if child is not None:
+                    self._job_at[child] = job
+                jobs.append((job, child is None))
+            self._serve(dev, requests, batch, jobs)
+            for (i, _, _, last), (job, final) in zip(batch, jobs):
+                if last:  # every stage's outputs are handed out once its final yield is served: release it
+                    del self._job_at[i], requests[i]
+                    self.stats.children.pop(i, None)
+                    self.stats.cancelled.discard(i)
+                    self.stats.failed.pop(i, None)
+                    if final:
+                        with self._lock:
+                            self._pending.discard(job)
+
+    def _serve(self, dev, requests, batch, jobs) -> None:
+        """Hand one poll's yields ``batch`` (``stream_schedule``) to their ``jobs``: ``(job, final)`` per yield,
+        ``final`` False on the last yield of a stage that has a follow-up.  The slots' outputs are valid here."""
+        raise NotImplementedError
+
+
+class GptEngine(OpenEngine):
+    """``GPT.open_engine``: a job's result is its ``GenerationOutputs``, the outputs ``GPT.generate`` gives the request
+    alone; a streaming job yields ``(GenerationOutputs, last)``, the yields of ``GPT.generate_continuous_stream`` for
+    it (for a request with a follow-up: every stage's, ``last`` only on the final one)."""
+
+    def _receive(self, value, event):
+        # the harvest copies were made on the engine's stream: order the caller's stream after them, and tell the
+        # caching allocator that the caller's stream uses the tensors
+        if event is not None:
+            out = value[0] if isinstance(value, tuple) else value
+            cur = torch.cuda.current_stream(self.device)
+            cur.wait_event(event)
+            for t in [*out.ids, *out.hiddens]:
+                t.record_stream(cur)
+        return value
+
+    def _serve(self, dev, requests, batch, jobs) -> None:
+        done = []
+        for (i, s, n, last), (job, final) in zip(batch, jobs):
+            if i in self.stats.failed:
+                job._fail(self.stats.failed[i])
+                continue
+            if job.done():
+                continue
+            cancelled = i in self.stats.cancelled
+            if not (job.stream or (last and final) or cancelled):
+                continue
+            out = dev.empty(i) if s is None else dev.harvest(s, n)
+            out.cancelled = cancelled
+            done.append((job, out, last and final, cancelled))
+        event = None
+        if done and self._stream is not None:
+            event = torch.cuda.Event()
+            event.record(self._stream)
+        for job, out, last, cancelled in done:
+            if cancelled:
+                job._cancelled = True
+                job._finish(out, event)
+                continue
+            if job.stream:
+                job._put((out, last), event)
+            if last:
+                job._finish(out, event)

@@ -58,6 +58,7 @@ class GPT:
         ids: List[torch.Tensor]
         attentions: List[Optional[Tuple[torch.FloatTensor, ...]]]
         hiddens: List[torch.Tensor]
+        cancelled: bool = False  # an open engine's job that was cancelled: the outputs are the prefix it had
 
         def destroy(self):
             _del_all(self.ids)
@@ -84,6 +85,7 @@ class GPT:
         self._handle = C.c_void_p()
         self._weights: Optional[torch.Tensor] = None
         self._stream_keepalive = []
+        self._open = None  # the open engine (open_engine) that owns the handle until it is closed
 
     # ------------------------------------------------------------------ loading
     def load_pretrained(self, gpt_folder: str, embed_file_path: str, experimental=False):
@@ -299,6 +301,39 @@ class GPT:
             if stats.interrupted:
                 self.logger.warning("generation is interrupted")
 
+    def open_engine(self, slots: int, max_new_cap: int, return_hidden=True, chunk: Optional[int] = None):
+        """A slot engine that takes requests while it decodes: ``submit(request, stream=False) -> engine.Job`` from
+        any thread, ``Job.cancel()`` for one request, ``close(cancel=False)`` (or a ``with`` block) to drain it.
+
+        A job's ``result()`` is the request's ``GenerationOutputs``, bit for bit what ``generate_continuous`` yields
+        for it; a cancelled job's result is the prefix it had at the poll that stopped it, with ``cancelled=True``.  A
+        streaming job iterates ``(GenerationOutputs, last)``, the yields ``generate_continuous_stream`` makes for it
+        (copies), and simply ends when cancelled.  ``submit`` checks the request against this handle and
+        ``max_new_cap`` in the caller's thread.  One worker thread owns the handle and its stream; while the engine
+        is open ``generate``, ``generate_continuous*`` and another ``open_engine`` raise.  The poll interval is
+        ``chunk`` steps (default CTB_DECODE_CHUNK, else 24)."""
+        from .engine import GptEngine
+
+        return self._open_slot_engine(GptEngine, slots, max_new_cap, return_hidden, chunk)
+
+    def _open_slot_engine(self, cls, slots, max_new_cap, return_hidden, chunk, *args):
+        """An ``engine.OpenEngine`` subclass ``cls`` that owns this handle until it is closed."""
+        from .engine import EngineDevice
+
+        _, S, chunk, _, cap, check = self._engine_args("open_engine", [], slots, False, False, None, chunk, None,
+                                                       max_new_cap)
+        engine = cls(lambda requests: EngineDevice(self, requests, S, cap, return_hidden), chunk, check,
+                     self.device_gpt, self._close_engine, *args, max_new_cap=cap)
+        self._open = engine
+        return engine
+
+    def _close_engine(self):
+        self._open = None
+
+    def _check_free(self, name):
+        if self._open is not None:
+            raise RuntimeError(f"{name}: an open engine owns this handle; close it first")
+
     def _engine_args(self, name, requests, slots, infer_text, return_attn, context, chunk, default_chunk,
                      max_new_cap=None):
         """Checks shared by the slot-engine generators -> (requests, slots, chunk, context, max_new_cap, check), where
@@ -306,6 +341,7 @@ class GPT:
         CTB_DECODE_CHUNK, else `default_chunk` (None: the smallest ``stream_batch``)."""
         from .engine import MIN_PROMPT_COLS, Request
 
+        self._check_free(name)
         if infer_text:
             raise ValueError(f"{name}: the mode is chosen per request: set Request.infer_text for text generation")
         if return_attn:
@@ -351,6 +387,7 @@ class GPT:
                  ensure_non_empty=True, stream_batch=24, manual_seed: Optional[int] = None,
                  context=Context()):
         """Generator with the reference's contract (gpt.py:315-618)."""
+        self._check_free("generate")
         if return_attn:
             raise NotImplementedError("return_attn: attention maps never leave the fused attention kernel")
         if not self._handle:

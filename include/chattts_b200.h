@@ -187,6 +187,18 @@ int ctb_gpt_engine_admit_text(ctb_gpt* h, int32_t n, const int32_t* slots, int32
 int ctb_gpt_engine_status(ctb_gpt* h, ctb_gpt_status* out, int32_t* state_host, int32_t* end_idx_host,
                           uint8_t* finish_host, void* stream);
 
+/* Stop the requests in `slots` (host array of n distinct slot indices, 1 <= n <= S): a server whose client went away
+ * frees the slot for the next request at once instead of decoding to EOS or max_new.  Enqueued on `stream`, no
+ * synchronisation; the host array may be released on return.
+ * A listed slot that is running or pending becomes CTB_SLOT_FINISHED with finish 0; its ids_out / hiddens_out rows
+ * 0 .. end_idx-1 stay valid.  Idle and already finished slots are left as they are (not an error): the host cannot
+ * know that a row did not finish on the device since its last status read.  Afterwards all_finished = no running
+ * slot, so later ctb_gpt_decode steps with nothing running stay no-ops and do not count in steps_done.  A cancelled
+ * slot takes a new request through ctb_gpt_engine_admit / _admit_text.
+ * Errors: CTB_ERR_STATE outside engine mode; CTB_ERR_ARG for a null argument, n outside [1, S], a slot out of range
+ * or repeated, or an engine of more than 1024 slots. */
+int ctb_gpt_engine_cancel(ctb_gpt* h, int32_t n, const int32_t* slots, void* stream);
+
 /* Measurement hook for bench.py's roofline: launches ONE kernel kind once per layer on the
  * state left by the last generate call (kind 0 qkv, 1 attention, 2 o-proj, 3 gate/up, 4 down;
  * 5 = heads, 6 = sampler, 7 = one decode step as ONE kernel launch (k_flow / k_step), 8 = 16 decode steps in one
@@ -199,7 +211,10 @@ int ctb_gpt_debug_trace(ctb_gpt* h, unsigned long long* host_out, int n);
 
 /* Prompt embedding mix: replaces Embed.forward (ChatTTS/model/embed.py:51-79).
  *   ids_dev [B, T, num_vq] int64 (tokenizer output), text_mask_dev [B, T] uint8, tables inside the packed blob of `h`;
- *   out_dev [B, T, d] fp32: text positions get emb_text[ids[...,0]], the others sum_q emb_code[q][ids[...,q]]. */
+ *   out_dev [B, T, d] fp32: text positions get emb_text[ids[...,0]], the others sum_q emb_code[q][ids[...,q]].
+ * Reads only the handle's weights and configuration, so unlike the other calls on a handle it may run in one thread
+ * while another thread drives the handle (a server embeds new prompts while its slot engine decodes); it must keep
+ * writing nothing the handle owns. */
 int ctb_gpt_embed_prompt(ctb_gpt* h, const int64_t* ids_dev, const uint8_t* text_mask_dev, int32_t B, int32_t T,
                          float* out_dev, void* stream);
 

@@ -2,7 +2,7 @@
 """Continuous-batching benchmark: the slot engine against static batches, one JSON line.
 
     python tools/bench_continuous.py [--requests N] [--slots S] [--steps K] [--warmup W] [--dump-outputs DIR] [--stream]
-                                     [--refine]
+                                     [--refine] [--online RATE[,RATE...] [--cancel FRACTION]]
 
 N requests (default 128), each one utterance with its own seeded prompt (8..128 tokens) and forced length (64..1024
 tokens, min_new = max_new: synthetic weights have no meaningful EOS), run through the slot engine with S slots
@@ -28,6 +28,14 @@ useful speech-tokens/s, seconds of audio delivered per wall second, time to firs
 counted from its first chunk) and the share of wall time in path 2.  (a) and (b) must yield the same chunks; with
 ``--dump-outputs`` the chunks of (a) are written as stream_chunks.npy (concatenated in yield order),
 stream_chunk_index.npy and stream_chunk_lengths.npy.
+
+``--online 12,24`` prints one more line per rate: the same requests streamed (hidden path, 32 slots, InferCodeParams'
+defaults) but arriving over time, seeded Poisson arrivals at that many requests/s; (a) the open engine, each request
+submitted at its arrival, against (b) consecutive ``stream_continuous`` calls, each starting every request that arrived
+while the previous one ran.  Per arm: time from arrival to first and to last chunk (p50 / p95 / max), useful tokens/s
+over the span from the first arrival to the last chunk, decode steps, mean slot occupancy and underruns.  ``--cancel F``
+adds a line with a seeded fraction F of the requests cancelled 0..1 s after their first chunk (open engine, highest
+rate), against the same arrivals without cancellation: decode steps and span.
 """
 from __future__ import annotations
 
@@ -421,6 +429,170 @@ def run_refine(args, local_rank: int = 0):
     return out
 
 
+def run_online(args, local_rank: int = 0):
+    """Requests arriving over time (seeded Poisson arrivals at each rate of ``--online``), streamed as audio: (a) the
+    open engine (``GPT.open_engine`` / ``ChatEngine``: every request submitted at its arrival) against (b) what a
+    server can do without it: the requests that arrived while one ``stream_continuous`` call ran start together in the
+    next call.  Arms alternate, ``--steps`` repeats each; the median run by span is reported.  One JSON line per rate,
+    and with ``--cancel F`` one more: arm (a) at the highest rate with a seeded fraction F of the requests cancelled
+    at a seeded time (0..1 s) after their first chunk, against the same arrivals without cancellation."""
+    import threading
+    import types
+
+    import numpy as np
+
+    from chattts_b200.config import Config
+    from chattts_b200.core import Chat, ChatEngine, StreamWindows, stream_continuous
+    from chattts_b200.decoder import DVAE, Vocos
+    from chattts_b200.embed import Embed
+    from chattts_b200.engine import OpenEngine, Request
+    from chattts_b200.gpt import GPT
+    from chattts_b200.processors import gen_logits
+    from chattts_b200.prompts import synth_prompt_batch
+    from chattts_b200.synth import synth_dvae_state, synth_embed_state, synth_gpt_state, synth_vocos_state
+
+    dev = torch.device("cuda", local_rank)
+    torch.cuda.set_device(dev)
+    n, S, cfg = args.requests, args.slots, Config()
+    plen, tok = continuous_workload(n, seed=7)
+    cap = max(tok)
+    embed = Embed(768, 626, 21178, 4).load_state_dict(synth_embed_state(1)).to(dev)
+    gpt = GPT(cfg.gpt, embed, device=dev, device_gpt=dev, max_batch=S, max_context=max(plen) + max(tok))
+    gpt.load_state(synth_gpt_state(0))
+    voc = Vocos(cfg.vocos, dev, max_batch=S, max_tokens=256).load_state_dict(synth_vocos_state(5))
+    dec = DVAE(cfg.decoder, dim=cfg.decoder.idim, device=dev, vocos=voc, max_batch=S, max_tokens=256)
+    dec.load_state_dict(synth_dvae_state(2, cfg.decoder, cfg.decoder.idim))
+    models = types.SimpleNamespace(decoder=dec, dvae=dec)  # what ChatEngine reads of a Chat
+    p = Chat.InferCodeParams()
+    warp, proc = gen_logits(num_code=625, top_P=0.7, top_K=20, repetition_penalty=1.05)
+    procs, temp = (*proc, *warp), [0.3] * 4
+    embs = []
+    for i, L in enumerate(plen):
+        ids, _, tmask = synth_prompt_batch([L], seed=1000 + i)
+        embs.append(embed(ids, tmask)[0])
+    torch.cuda.synchronize()
+
+    def request(i, lengths):
+        return Request(emb=embs[i], temperature=temp, eos_token=625, max_new_token=lengths[i],
+                       min_new_token=lengths[i], logits_processors=procs, manual_seed=5000 + i,
+                       stream_batch=p.stream_batch)
+
+    def windows():
+        return StreamWindows(p.stream_speed, p.pass_first_n_batches)
+
+    def arrivals(rate, count, seed):
+        g = np.random.default_rng(seed)
+        return np.cumsum(g.exponential(1.0 / rate, count)).tolist()
+
+    def open_arm(at, lengths, cancel_after=None):
+        """(a): each request submitted at its arrival; one consumer thread per job records its chunks."""
+        chunks = {i: [] for i in range(len(at))}
+        eng = gpt._open_slot_engine(ChatEngine, S, cap, True, None, models, True)
+        threads, jobs = [], []
+        t0 = time.perf_counter()
+
+        def consume(i, job):
+            for c, _ in job:
+                chunks[i].append((time.perf_counter() - t0, c.shape[1]))
+                if cancel_after is not None and i in cancel_after and len(chunks[i]) == 1:
+                    threading.Timer(cancel_after[i], job.cancel).start()
+
+        for i, a in enumerate(at):
+            time.sleep(max(0.0, a - (time.perf_counter() - t0)))
+            job = OpenEngine.submit(eng, request(i, lengths), True, windows())
+            jobs.append(job)
+            th = threading.Thread(target=consume, args=(i, job))
+            th.start()
+            threads.append(th)
+        for th in threads:
+            th.join()
+        eng.close()
+        return dict(chunks=chunks, steps=eng.stats.decode_steps, cancelled=sum(j.cancelled() for j in jobs))
+
+    def call_arm(at, lengths):
+        """(b): the requests that arrived while a call ran start together in the next call."""
+        chunks = {i: [] for i in range(len(at))}
+        steps, nxt = 0, 0
+        t0 = time.perf_counter()
+        while nxt < len(at):
+            time.sleep(max(0.0, at[nxt] - (time.perf_counter() - t0)))
+            now = time.perf_counter() - t0
+            batch = [i for i in range(nxt, len(at)) if at[i] <= now]
+            nxt = batch[-1] + 1
+            for k, c, _ in stream_continuous(gpt, dec, [request(i, lengths) for i in batch],
+                                             [windows() for _ in batch], True, slots=S, max_new_cap=cap):
+                chunks[batch[k]].append((time.perf_counter() - t0, c.shape[1]))
+            steps += gpt.last_schedule_stats.decode_steps
+        return dict(chunks=chunks, steps=steps, cancelled=0)
+
+    sr = 24000.0
+    pct = lambda v, q: round(float(np.percentile(np.asarray(v), q)), 4)  # noqa: E731
+
+    def summary(r, at, lengths):
+        first, done, under = [], [], 0
+        for i, ch in r["chunks"].items():
+            ch = [(t, m) for t, m in ch if m > 0]
+            if not ch:
+                continue
+            first.append(ch[0][0] - at[i])
+            done.append(ch[-1][0] - at[i])
+            played = ch[0][1] / sr  # audio handed out before each later chunk, played from the first chunk on
+            for t, m in ch[1:]:
+                under += t > ch[0][0] + played
+                played += m / sr
+        span = max(t for ch in r["chunks"].values() for t, _ in ch) - at[0]
+        useful = sum(lengths)
+        q = lambda v: {"p50": pct(v, 50), "p95": pct(v, 95), "max": round(max(v), 4)}  # noqa: E731
+        return {"span_s": round(span, 3), "first_chunk_s": q(first), "last_chunk_s": q(done),
+                "tokens_per_s": round(useful / span, 1), "decode_steps": r["steps"],
+                "mean_slot_occupancy": round((useful - len(lengths)) / (S * max(1, r["steps"])), 4),
+                "underruns": under, "cancelled": r["cancelled"]}
+
+    def median_run(rs):
+        return sorted(rs, key=lambda x: x["span_s"])[len(rs) // 2]
+
+    short = [min(t, 96) for t in tok[: 2 * S]]
+    for _ in range(max(1, min(args.warmup, 2))):
+        open_arm([0.0] * len(short), short)
+        call_arm([0.0] * len(short), short)
+    name, limit = gpu_card(local_rank)
+    rates = [float(x) for x in args.online.split(",")]
+    lines = []
+    for k, rate in enumerate(rates):
+        at = arrivals(rate, n, seed=11 + k)
+        runs = {"a": [], "b": []}
+        for _ in range(args.steps):
+            runs["a"].append(summary(open_arm(at, tok), at, tok))
+            runs["b"].append(summary(call_arm(at, tok), at, tok))
+        line = {"metric": "continuous_online", "card": name, "power_limit": limit, "rate_per_s": rate,
+                "requests": n, "slots": S, "useful_tokens": sum(tok), "repeats": args.steps,
+                "stream_batch": p.stream_batch, "stream_speed": p.stream_speed,
+                "pass_first_n_batches": p.pass_first_n_batches}
+        for arm in ("a", "b"):
+            line[arm] = median_run(runs[arm])
+            line[arm]["span_all_s"] = [r["span_s"] for r in runs[arm]]
+        lines.append(line)
+    if args.cancel is not None:
+        rate = max(rates)
+        at = arrivals(rate, n, seed=11 + rates.index(rate))
+        g = np.random.default_rng(23)
+        victims = sorted(g.choice(n, int(round(args.cancel * n)), replace=False).tolist())
+        after = {i: float(g.uniform(0.0, 1.0)) for i in victims}
+        runs = {"cancel": [], "full": []}
+        for _ in range(args.steps):
+            runs["cancel"].append(summary(open_arm(at, tok, after), at, tok))
+            runs["full"].append(summary(open_arm(at, tok), at, tok))
+        line = {"metric": "continuous_online_cancel", "card": name, "power_limit": limit, "rate_per_s": rate,
+                "requests": n, "slots": S, "cancel_fraction": args.cancel, "cancelled_requests": len(victims),
+                "repeats": args.steps}
+        for arm in ("cancel", "full"):
+            r = median_run(runs[arm])
+            line[arm] = {"span_s": r["span_s"], "decode_steps": r["decode_steps"], "cancelled": r["cancelled"],
+                         "span_all_s": [x["span_s"] for x in runs[arm]]}
+        lines.append(line)
+    return lines
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--requests", type=int, default=128)
@@ -430,6 +602,10 @@ def main():
     ap.add_argument("--dump-outputs", default=None, metavar="DIR")
     ap.add_argument("--stream", action="store_true", help="also measure streamed audio (a second JSON line)")
     ap.add_argument("--refine", action="store_true", help="also measure refinement + speech (one more JSON line)")
+    ap.add_argument("--online", default=None, metavar="RATE[,RATE...]",
+                    help="also measure streamed requests arriving at these rates (requests/s; one JSON line each)")
+    ap.add_argument("--cancel", type=float, default=None, metavar="FRACTION",
+                    help="with --online: one more line with this fraction of the requests cancelled")
     args = ap.parse_args()
     if args.steps < 1:
         ap.error("--steps must be >= 1")
@@ -439,6 +615,9 @@ def main():
         print(json.dumps(run_stream(args, rank)), flush=True)
     if args.refine:
         print(json.dumps(run_refine(args, rank)), flush=True)
+    if args.online:
+        for line in run_online(args, rank):
+            print(json.dumps(line), flush=True)
 
 
 if __name__ == "__main__":
