@@ -66,6 +66,7 @@ EXPORTS = (
     "ctb_dvae_blob_floats", "ctb_vocos_blob_floats", "ctb_decoder_create", "ctb_decoder_destroy",
     "ctb_dvae_decode", "ctb_vocos_decode", "ctb_decode_rows",
     "ctb_dvae_encoder_blob_floats", "ctb_dvae_encoder_create", "ctb_dvae_encoder_destroy", "ctb_dvae_encode",
+    "ctb_dvae_encode_rows",
 )
 
 
@@ -129,6 +130,7 @@ def load(build_if_missing: bool = True):
         lib.ctb_dvae_encoder_create.argtypes = [C.POINTER(ConvStackConfig), vp, i64, C.POINTER(vp)]
         lib.ctb_dvae_encoder_destroy.argtypes = [vp]
         lib.ctb_dvae_encode.argtypes = [vp, vp, i64, vp, i32, C.POINTER(i32), vp, vp, vp]
+        lib.ctb_dvae_encode_rows.argtypes = [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, i32, C.POINTER(i32), vp, vp]
         if lib.ctb_abi_version() != 3:
             raise CtbError("ABI version mismatch")
         _lib = lib

@@ -9,8 +9,10 @@ SURVEY.md 2 rows 7, 8, 10, 11) are *injected*: ``load()`` takes them from an ins
 """
 from __future__ import annotations
 
+import copy
 import logging
 import os
+import queue
 import re
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Union
@@ -18,13 +20,26 @@ from typing import Dict, List, Optional, Union
 import numpy as np
 import torch
 
+from . import _lib
 from .config import Config
-from .decoder import decode_to_wavs_window, DVAE, Vocos, decode_to_wavs, stream_window
+from .decoder import ENC_NFFT, decode_to_wavs_window, DVAE, Vocos, decode_to_wavs, stream_window
 from .embed import Embed
 from .engine import Job, OpenEngine
 from .gpt import GPT
 from .norm import Normalizer
 from .processors import gen_logits
+
+
+_SPLIT_REFINE = ("split_text=True with skip_refine_text=False is not supported on the slot engine (each sentence "
+                 "would wait for its refinement and for the paragraph's speaker sample)")
+
+
+def split_sentences(text: str) -> List[str]:
+    """``infer``'s sentence split (``split_text=True``): the lines of a text with a newline, else its sentences
+    ending in '。' or '. ' (reference core.py:237-241)."""
+    if "\n" in text:
+        return text.split("\n")
+    return [t for t in re.split(r"(?<=。)|(?<=\.\s)", text) if t]
 
 
 class Chat:
@@ -179,10 +194,7 @@ class Chat:
         params_infer_code = params_infer_code or Chat.InferCodeParams()
         self.context.set(False)
         if split_text and isinstance(text, str):
-            if "\n" in text:
-                text = text.split("\n")
-            else:
-                text = [t for t in re.split(r"(?<=。)|(?<=\.\s)", text) if t]
+            text = split_sentences(text)
             self.logger.info("split text into %d parts", len(text))
         if len(text) == 0:
             return []
@@ -204,7 +216,7 @@ class Chat:
 
     def infer_continuous(self, texts, params_infer_code=None, use_decoder=True, slots=None, stream=False, lang=None,
                          skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
-                         params_refine_text=None, refine_on_engine=False):
+                         params_refine_text=None, refine_on_engine=False, split_text=False):
         """Synthesise many texts with continuous batching (``GPT.generate_continuous``): each text is one request,
         ``params_infer_code`` is one ``InferCodeParams`` for all texts or a list with one per text (speaker, seed,
         temperature, top-P/K, penalty, token limits).  Generator of ``(index, wav)`` in completion order; ``wav`` is
@@ -217,18 +229,28 @@ class Chat:
         request of its own on the slot engine instead, and its speech codes follow as soon as its refinement ends:
         ``wav`` is then what ``infer([texts[index]], split_text=False, skip_refine_text=False)`` returns with that
         text's params.  A seeded refinement depends on the batch it is drawn in, so the two modes give different
-        seeded results; the batched one stays the default."""
+        seeded results; the batched one stays the default.
+
+        ``split_text=True`` makes each text a paragraph, split into sentences as ``infer`` splits it, with one voice
+        across its sentences (see ``ChatEngine.submit``): ``wav`` is then what ``infer(texts[index], split_text=True,
+        max_split_batch=1, skip_refine_text=True)[0]`` returns with that text's params, which are not modified.  The
+        paragraphs run on an open engine (``open_engine``); ``slots`` defaults to the handle's ``max_batch``."""
         if stream:
             raise ValueError("infer_continuous: stream=True is not supported; each waveform is yielded when complete "
                              "(infer_continuous_stream streams)")
         texts, params = self._continuous_params(texts, params_infer_code)
+        if split_text:
+            if not skip_refine_text:
+                raise ValueError(_SPLIT_REFINE)
+            return self._paragraphs(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
+                                    do_homophone_replacement, False)
         return self._infer_continuous(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
                                       do_homophone_replacement, self._refine_params(texts, params_refine_text),
                                       refine_on_engine)
 
     def infer_continuous_stream(self, texts, params_infer_code=None, use_decoder=True, slots=None, lang=None,
                                 skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
-                                params_refine_text=None, refine_on_engine=False):
+                                params_refine_text=None, refine_on_engine=False, split_text=False):
         """Streaming synthesis of many texts with continuous batching (``GPT.generate_continuous_stream``).
         Generator of ``(index, chunk, last)``, ``chunk`` a ``[1, n]`` float32 array; for each text the chunks are
         those ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=True)`` yields with that
@@ -236,8 +258,15 @@ class Chat:
         its final chunk.  A seeded text whose first code is EOS yields one empty final chunk.  All windows due at one
         engine poll are decoded in one ragged call (``TokenDecoder.decode_rows``), straight from the engine's
         buffers.  Arguments as for ``infer_continuous``; with ``refine_on_engine=True`` the chunks are those of
-        ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=False)``."""
+        ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=False)``.  With ``split_text=True``
+        each text is a paragraph, streamed sentence by sentence as ``ChatEngine.submit(split_text=True,
+        stream=True)`` streams it."""
         texts, params = self._continuous_params(texts, params_infer_code)
+        if split_text:
+            if not skip_refine_text:
+                raise ValueError(_SPLIT_REFINE)
+            return self._paragraphs(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
+                                    do_homophone_replacement, True)
         return self._infer_continuous_stream(texts, params, use_decoder, slots, lang, skip_refine_text,
                                              do_text_normalization, do_homophone_replacement,
                                              self._refine_params(texts, params_refine_text), refine_on_engine)
@@ -279,6 +308,47 @@ class Chat:
                 raise ValueError("params_refine_text: one RefineTextParams per text")
             return list(params_refine_text)
         return [params_refine_text or Chat.RefineTextParams()] * len(texts)
+
+    def _paragraphs(self, texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
+                    do_homophone_replacement, stream):
+        """``infer_continuous*(split_text=True)``: every text a paragraph job on one open engine, submitted in order.
+        Generator of ``(index, wav)`` in completion order, or of ``(index, chunk, last)`` as the chunks come."""
+        if not skip_refine_text:
+            raise ValueError(_SPLIT_REFINE)
+        assert self.has_loaded(use_decoder=use_decoder)
+        self.context.set(False)
+        if not texts:
+            return
+        out: queue.Queue = queue.Queue()
+        cap = max(p.max_new_token for p in params)
+        with self.open_engine(slots, max_new_cap=cap, use_decoder=use_decoder) as eng:
+            try:
+                jobs = [eng.submit(t, params_infer_code=p, stream=stream, lang=lang, split_text=True,
+                                   do_text_normalization=do_text_normalization,
+                                   do_homophone_replacement=do_homophone_replacement, _sink=(out, k))
+                        for k, (t, p) in enumerate(zip(texts, params))]
+                left = len(jobs)
+                while left:
+                    try:
+                        k, item = out.get(timeout=0.05)
+                    except queue.Empty:
+                        if eng._stopped:  # the worker failed: close() raises its error
+                            eng.close()
+                        if self.context.get():
+                            self.logger.warning("generation is interrupted")
+                            eng.close(cancel=True)
+                            return
+                        continue
+                    if item is None:  # job k ended: its result, or its error raised here
+                        left -= 1
+                        wav = jobs[k].result()
+                        if not stream:
+                            yield k, wav
+                    elif stream:
+                        yield (k, *item)
+            except GeneratorExit:
+                eng.close(cancel=True)
+                raise
 
     def _continuous_requests(self, texts, params, use_decoder, lang, skip_refine_text, do_text_normalization,
                              do_homophone_replacement, refine, refine_on_engine=False):
@@ -621,6 +691,91 @@ def _decode_windows(dev, jobs, model: DVAE, use_decoder: bool, ragged: bool = Tr
     return out
 
 
+class _Paragraph:
+    """A paragraph job's state on ``ChatEngine``: its reference stage, which request speaks which sentence, and the
+    in-order assembly of the sentences' audio (``add``).  ``sink`` = (queue, key): the chunks and the end of the job are
+    also posted there, for ``Chat.infer_continuous*(split_text=True)``."""
+
+    def __init__(self, n: int, stream_params, sink=None):
+        self.n, self.sink = n, sink
+        self.windows = ([StreamWindows(stream_params.stream_speed, stream_params.pass_first_n_batches)
+                         for _ in range(n)] if stream_params is not None else None)
+        self.ref = None
+        self.order: Dict[object, int] = {}  # Request -> sentence number
+        self.job: Optional[Job] = None
+        self.parts: List[list] = [[] for _ in range(n)]
+        self.closed = [False] * n
+        self.next = 0  # the first sentence whose audio is not all out
+        self._ended = False
+
+    def add(self, k: int, chunk: np.ndarray, last: bool) -> None:
+        """Sentence k's next chunk (its whole stripped waveform when not streaming); ``last``: its final one."""
+        self.parts[k].append(chunk)
+        self.closed[k] = self.closed[k] or last
+        out = []
+        while self.next < self.n:
+            if self.windows is not None:
+                out += self.parts[self.next]
+                self.parts[self.next] = []
+            if not self.closed[self.next]:
+                break
+            self.next += 1
+        done = self.next == self.n
+        job = self.job
+        if self.windows is not None:
+            for j, c in enumerate(out):
+                item = (c, done and j == len(out) - 1)
+                job._put(item)
+                if self.sink is not None:
+                    self.sink[0].put((self.sink[1], item))
+            if done:
+                job._finish(None)
+        elif done:
+            job._finish(np.concatenate([c[0] for part in self.parts for c in part]))
+        if done:
+            self.ended()
+
+    def ended(self) -> None:
+        if self.sink is not None and not self._ended:
+            self.sink[0].put((self.sink[1], None))
+        self._ended = True
+
+
+class _SpeakerSampler:
+    """``Request.prepare`` of the paragraphs' reference stages on one engine: the whole sequences of the reference stages
+    that end at a poll are decoded in one ``decode_rows`` call, straight from the engine's buffers, and the waveforms
+    are read in place by one ``encode_rows`` call; ``take`` hands each stage's speaker-prompt string to its ``then``."""
+
+    def __init__(self, chat: "Chat", model: DVAE, use_decoder: bool):
+        self.chat, self.model, self.use_decoder = chat, model, use_decoder
+        self._out: Dict[object, object] = {}
+
+    def __call__(self, dev, items) -> None:
+        rows = []
+        for r, s, n in items:
+            if n == 0:  # infer() gets no reference waveform from a seeded sentence 0 that ends empty
+                self._out[r] = RuntimeError("sentence 0 of the paragraph ended empty: there is no audio to sample a "
+                                            "speaker from")
+            elif 512 * n - 256 <= ENC_NFFT // 2:
+                self._out[r] = _lib.CtbError(f"reflect padding needs more than {ENC_NFFT // 2} samples (sentence 0 "
+                                             f"of the paragraph has {n} token)")
+            else:
+                rows.append((r, s, n))
+        if not rows:
+            return
+        buf = dev.hid_out if self.use_decoder else dev.ids_out
+        wavs = self.model.engine.decode_rows([buf[s, :n] for _, s, n in rows], 1 if self.use_decoder else 2)
+        codes = self.chat.dvae.audio_encoder.encode_rows(wavs)
+        for (r, _, _), c in zip(rows, codes):
+            self._out[r] = self.chat.speaker.encode_prompt(c)
+
+    def take(self, r):
+        v = self._out.pop(r)
+        if isinstance(v, BaseException):
+            raise v
+        return v
+
+
 class ChatEngine(OpenEngine):
     """``Chat.open_engine``: an open slot engine whose jobs are texts (see there).  At each poll every window due for a
     streaming job and the whole sequence of every non-streaming job that completed go into one ``decode_rows`` call."""
@@ -629,16 +784,38 @@ class ChatEngine(OpenEngine):
                  max_new_cap: Optional[int] = None):
         self.chat, self.use_decoder = chat, use_decoder
         self.model = chat.decoder if use_decoder else chat.dvae
+        self._sampler = _SpeakerSampler(chat, self.model, use_decoder)
         super().__init__(make_device, chunk, check, device, on_close, max_new_cap)
 
     def submit(self, text: str, params_infer_code=None, stream=False, skip_refine_text=True, params_refine_text=None,
-               lang=None, do_text_normalization=True, do_homophone_replacement=True) -> Job:
+               lang=None, do_text_normalization=True, do_homophone_replacement=True, split_text=False,
+               _sink=None) -> Job:
         """Queue one text -> ``Job``: ``result()`` is the waveform ``infer_continuous`` yields for it, or with
         ``stream=True`` the job iterates the ``(chunk, last)`` pairs ``infer_continuous_stream`` yields for it.
         ``skip_refine_text=False`` refines the text on the engine first (``refine_on_engine=True``).  A cancelled
-        job's ``result()`` raises ``concurrent.futures.CancelledError`` and its stream ends."""
+        job's ``result()`` raises ``concurrent.futures.CancelledError`` and its stream ends.
+
+        ``split_text=True``: the text is a paragraph, split into sentences by ``infer``'s rule (``split_sentences``),
+        and keeps one voice across them as ``infer`` does.  With one sentence, or with an explicit ``spk_smp``, each
+        sentence is one request with these params.  Otherwise sentence 0 first runs once alone (the reference stage);
+        its whole, unstripped waveform is encoded by the DVAE encode branch into the speaker sample ``spk_smp``
+        (``Job.spk_smp`` once known), with ``txt_smp`` = sentence 0, and every sentence, sentence 0 included, is then
+        a request of its own with a copy of the params carrying them.  The reference stages ending at one poll are
+        decoded in one ``decode_rows`` call and encoded in one ``encode_rows`` call.  ``result()`` is the sentences'
+        waveforms, each silence-stripped, concatenated in order: what ``infer(text, split_text=True,
+        max_split_batch=1, skip_refine_text=True)[0]`` returns (the caller's params are not modified here, while
+        ``infer`` stores the sample on them).  Streamed, the chunks are each sentence's chunks in sentence order,
+        those of ``infer([sentence], stream=True, split_text=False)`` with the sample on its params; a later
+        sentence's chunks are held until the earlier one's final chunk is out, and ``last`` marks only the final
+        chunk of the last sentence.  Unlike ``infer(stream=True)``, whose stream position runs on across its batches,
+        each sentence's stream starts at its own first sample.  A reference stage too short to encode or that ended
+        empty, or a sentence whose prompt breaks the engine's limits, fails that job only.  Needs
+        ``skip_refine_text=True``."""
         chat = self.chat
         params = params_infer_code or Chat.InferCodeParams()
+        if split_text:
+            return self._submit_paragraph(text, params, stream, skip_refine_text, lang, do_text_normalization,
+                                          do_homophone_replacement, _sink)
         if not skip_refine_text and self.max_new_cap is not None and params.max_new_token > self.max_new_cap:
             # the speech stage is made only when the refinement ends: check its limit here, in the caller's thread
             raise ValueError(f"max_new_token {params.max_new_token} exceeds max_new_cap={self.max_new_cap}")
@@ -652,24 +829,77 @@ class ChatEngine(OpenEngine):
         windows = StreamWindows(params.stream_speed, params.pass_first_n_batches) if stream else None
         return super().submit(request, stream, windows)
 
+    def _submit_paragraph(self, text, params, stream, skip_refine_text, lang, do_text_normalization,
+                          do_homophone_replacement, sink) -> Job:
+        if not skip_refine_text:
+            raise ValueError(_SPLIT_REFINE)
+        chat = self.chat
+        if self.max_new_cap is not None and params.max_new_token > self.max_new_cap:
+            raise ValueError(f"max_new_token {params.max_new_token} exceeds max_new_cap={self.max_new_cap}")
+        sentences = [chat.normalizer(t, do_text_normalization, do_homophone_replacement, lang)
+                     for t in split_sentences(text)]
+        if not sentences:
+            raise ValueError("split_text=True: the text has no sentence")
+        para = _Paragraph(len(sentences), params if stream else None, sink)
+        if len(sentences) == 1 or params.spk_smp is not None:
+            reqs = [chat._code_request(t, copy.copy(params)) for t in sentences]
+            para.order = {r: k for k, r in enumerate(reqs)}
+            job = super().submit(reqs, stream, para)
+        else:
+            if chat.dvae.audio_encoder is None:
+                raise RuntimeError("this DVAE checkpoint carries no encoder / VQ weights: cannot sample a speaker")
+            para.ref = chat._code_request(sentences[0], copy.copy(params))
+            para.ref.prepare = self._sampler
+
+            def then(out, para=para):
+                spk = self._sampler.take(para.ref)
+                para.job.spk_smp = spk
+                p = copy.copy(params)
+                p.spk_smp, p.txt_smp = spk, sentences[0]
+                reqs = [chat._code_request(t, p) for t in sentences]
+                para.order = {r: k for k, r in enumerate(reqs)}
+                return reqs
+
+            para.ref.then = then
+            job = super().submit(para.ref, stream, para)
+        para.job = job
+        return job
+
     def _serve(self, dev, requests, batch, jobs) -> None:
         wjobs = []  # (job, slot, n_tokens, a, b, flush, last), as stream_continuous builds them
         for (i, s, n, last), (job, final) in zip(batch, jobs):
+            para = job.state if isinstance(job.state, _Paragraph) else None
             if i in self.stats.failed:
                 job._fail(self.stats.failed[i])
+                if para is not None:
+                    para.ended()
             elif job.done():
                 continue
             elif i in self.stats.cancelled:
                 job._stop()
+                if para is not None:
+                    para.ended()
             elif requests[i].infer_text:  # a refinement stage: its follow-up carries the text on
                 continue
+            elif para is not None:
+                if requests[i] is para.ref:  # the reference stage: its audio only becomes the speaker sample
+                    continue
+                k = para.order[requests[i]]
+                if para.windows is not None:
+                    ws = para.windows[k].windows(n, last)
+                    wjobs += [((job, k), s, n, a, b, flush, last and j == len(ws) - 1) for j, (a, b, flush) in
+                              enumerate(ws)]
+                elif last:
+                    wjobs.append(((job, k), s, n, 0, 512 * n - 256, True, True))
             elif job.stream:
                 ws = job.state.windows(n, last)
                 wjobs += [(job, s, n, a, b, flush, last and k == len(ws) - 1) for k, (a, b, flush) in enumerate(ws)]
             elif last:  # the whole sequence, silent samples dropped: what infer_continuous yields
                 wjobs.append((job, s, n, 0, 512 * n - 256, True, True))
         for job, chunk, last in _decode_windows(dev, wjobs, self.model, self.use_decoder):
-            if job.stream:
+            if isinstance(job, tuple):  # a sentence of a paragraph
+                job[0].state.add(job[1], chunk, last)
+            elif job.stream:
                 job._put((chunk, last))
                 if last:
                     job._finish(None)

@@ -458,13 +458,19 @@ struct ctb_encoder {
   int64_t max_samples;
   int max_frames;
   float *padded, *spec, *mel_tm, *bufX, *bufY, *bufA, *bufB, *bufH;
+  // what the buffers hold (enc_reserve): cap_frames STFT / mel / bufX frames (bufY..bufH: half as many token rows),
+  // cap_padded samples of reflect-padded audio
+  size_t cap_frames, cap_padded;
+  int* rows_meta;  // ctb_dvae_encode_rows: [B] frame counts + [B] token counts, grown with B
+  int rows_meta_cap;
 };
 
 extern "C" int64_t ctb_dvae_encoder_blob_floats(const ctb_convstack_config* c) { return c ? enc_layout(*c).total : -1; }
 
 extern "C" int ctb_dvae_encoder_destroy(ctb_encoder* h) {
   if (!h) return CTB_OK;
-  void* ptrs[] = {h->W_hi, h->W_lo, h->padded, h->spec, h->mel_tm, h->bufX, h->bufY, h->bufA, h->bufB, h->bufH};
+  void* ptrs[] = {h->W_hi, h->W_lo, h->padded, h->spec, h->mel_tm, h->bufX, h->bufY, h->bufA, h->bufB, h->bufH,
+                  h->rows_meta};
   for (void* p : ptrs) if (p) cudaFree(p);
   delete h;
   return CTB_OK;
@@ -507,7 +513,40 @@ extern "C" int ctb_dvae_encoder_create(const ctb_convstack_config* c, const floa
     k_split_tf32<<<1024, 256>>>(h->W, h->W_hi, h->W_lo, h->L.total);
     CTB_CUDA(cudaDeviceSynchronize());
   }
+  h->cap_frames = F;
+  h->cap_padded = (F + 3) * ENC_HOP;
   *out = h;
+  return CTB_OK;
+}
+
+// grow the activation buffers to `frames` frames (bufY..bufH: frames / 2 token rows) and `padded` samples; the contents
+// are scratch.  They never shrink below what ctb_dvae_encode needs for max_samples.
+static int enc_reserve(ctb_encoder* h, size_t frames, size_t padded, cudaStream_t s) {
+  if (frames <= h->cap_frames && padded <= h->cap_padded) return CTB_OK;
+  CTB_CUDA(cudaStreamSynchronize(s));
+  float** bufs[] = {&h->padded, &h->spec, &h->mel_tm, &h->bufX, &h->bufY, &h->bufA, &h->bufB, &h->bufH};
+  for (float** b : bufs) if (*b) { cudaFree(*b); *b = nullptr; }
+  h->cap_frames = h->cap_padded = 0;
+  const ctb_convstack_config& c = h->c;
+  const size_t F1 = (size_t)h->max_frames + 1;  // the lone call's 2 * FP frames
+  const size_t R = std::max(F1, (frames + frames / 8 + 1) & ~(size_t)1);
+  const size_t P = std::max((F1 + 2) * ENC_HOP, padded + padded / 8);
+  cudaError_t e = cudaSuccess;
+  auto A = [&](float** p, size_t n) { if (e == cudaSuccess) e = cudaMalloc((void**)p, n * sizeof(float)); };
+  A(&h->padded, P);
+  A(&h->spec, R * ENC_LDMAG);
+  A(&h->mel_tm, R * MEL_PAD);
+  A(&h->bufX, R * c.idim);
+  A(&h->bufY, R / 2 * c.idim);
+  A(&h->bufA, R / 2 * std::max(c.hidden, c.bn_dim));
+  A(&h->bufB, R / 2 * std::max(std::max(c.hidden, c.bn_dim), c.odim));
+  A(&h->bufH, R / 2 * 4 * c.hidden);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return set_err(CTB_ERR_NOMEM, "encoder buffers for %zu frames: %s", R, cudaGetErrorString(e));
+  }
+  h->cap_frames = R;
+  h->cap_padded = P;
   return CTB_OK;
 }
 
@@ -529,6 +568,8 @@ extern "C" int ctb_dvae_encode(ctb_encoder* h, const float* wav_dev, int64_t n_s
   if (T > ids_capacity_tokens) return set_err(CTB_ERR_ARG, "ids buffer holds %d tokens, %d needed", ids_capacity_tokens, T);
   const GemmCtx gc{h->W, h->W_hi, h->W_lo, h->use_tc};
   int rc;
+  // a no-op unless a failed ctb_dvae_encode_rows growth left the handle without buffers
+  if ((rc = enc_reserve(h, h->max_frames, (size_t)(h->max_frames + 3) * ENC_HOP, s))) return rc;
   // framing (reflect padding) -> |STFT| as a double-precision direct DFT -> mel filterbank, log, / coef
   const int64_t total = (int64_t)(F + 3) * ENC_HOP;
   k_reflect_pad<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(wav_dev, h->padded, n_samples, total, ENC_NFFT / 2);
@@ -567,6 +608,96 @@ extern "C" int ctb_dvae_encode(ctb_encoder* h, const float* wav_dev, int64_t n_s
   q.bound_input = ((c.vq_levels >> 16) & 1) ? 0 : 1;
   q.w = W + L.vq_w; q.b = W + L.vq_b;
   k_fsq_quant<<<T * c.vq_groups, 128, 0, s>>>(q);
+  CTB_LAUNCH_CHECK();
+  return CTB_OK;
+}
+
+// Ragged batch of the encode branch.  Row k's frames live at a frame stride FW (the widest row's F, rounded up to even,
+// so a frame pair never straddles two rows) and its tokens at a stride FW / 2.  Every buffer a tapped conv reads holds
+// exact +0 in row k's frames f >= F_k (tokens t >= T_k), which is what TMA's out-of-bounds fill (or the FMA kernel's
+// range check) gives the lone call; every output element then keeps its operands and reduction order.
+extern "C" int ctb_dvae_encode_rows(ctb_encoder* h, int32_t B, const float* const* wavs_dev, const int64_t* n_samples,
+                                    int32_t* ids_dev, int32_t ids_ld, int32_t* n_tokens_out, float* margin_dev,
+                                    void* stream) {
+  if (!h || !wavs_dev || !n_samples || !ids_dev || !n_tokens_out) return set_err(CTB_ERR_ARG, "null argument");
+  if (B < 1) return set_err(CTB_ERR_ARG, "B=%d", B);
+  int Fmax = 0;
+  for (int k = 0; k < B; ++k) {
+    if (!wavs_dev[k]) return set_err(CTB_ERR_ARG, "row %d: null wav", k);
+    if (n_samples[k] <= ENC_NFFT / 2)
+      return set_err(CTB_ERR_ARG, "row %d: reflect padding needs more than %d samples", k, ENC_NFFT / 2);
+    if (n_samples[k] > h->max_samples)
+      return set_err(CTB_ERR_ARG, "row %d: %lld samples exceed this handle (max_samples=%lld)", k,
+                     (long long)n_samples[k], (long long)h->max_samples);
+    const int F = (int)(n_samples[k] / ENC_HOP) + 1;
+    if (F / 2 > ids_ld) return set_err(CTB_ERR_ARG, "row %d: ids_ld %d < %d tokens", k, ids_ld, F / 2);
+    Fmax = std::max(Fmax, F);
+  }
+  const ctb_convstack_config& c = h->c;
+  const EncOff& L = h->L;
+  const float* W = h->W;
+  cudaStream_t s = (cudaStream_t)stream;
+  const int FW = (Fmax + 1) & ~1, TW = FW / 2;
+  int rc;
+  if ((rc = enc_reserve(h, (size_t)B * FW, (size_t)B * (FW + 3) * ENC_HOP, s))) return rc;
+  // one upload of the row table: [B] frame counts then [B] token counts (staged from pageable memory before
+  // cudaMemcpyAsync returns; stream order protects the device copy)
+  if (B > h->rows_meta_cap) {
+    CTB_CUDA(cudaStreamSynchronize(s));
+    if (h->rows_meta) { cudaFree(h->rows_meta); h->rows_meta = nullptr; h->rows_meta_cap = 0; }
+    CTB_CUDA(cudaMalloc((void**)&h->rows_meta, (size_t)B * 2 * sizeof(int)));
+    h->rows_meta_cap = B;
+  }
+  std::vector<int> meta((size_t)2 * B);
+  for (int k = 0; k < B; ++k) {
+    meta[k] = (int)(n_samples[k] / ENC_HOP) + 1;
+    meta[B + k] = n_tokens_out[k] = meta[k] / 2;
+  }
+  CTB_CUDA(cudaMemcpyAsync(h->rows_meta, meta.data(), meta.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  const int* fr = h->rows_meta;
+  const int* tn = h->rows_meta + B;
+  const GemmCtx gc{h->W, h->W_hi, h->W_lo, h->use_tc};
+  // framing, |STFT| and log-mel are frame-local: the lone kernels run per row, and the mel frames past F_k are +0
+  for (int k = 0; k < B; ++k) {
+    const int F = meta[k];
+    float* padded = h->padded + (size_t)k * (FW + 3) * ENC_HOP;
+    float* spec = h->spec + (size_t)k * FW * ENC_LDMAG;
+    float* mel = h->mel_tm + (size_t)k * FW * MEL_PAD;
+    const int64_t total = (int64_t)(F + 3) * ENC_HOP;
+    k_reflect_pad<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(wavs_dev[k], padded, n_samples[k], total, ENC_NFFT / 2);
+    CTB_LAUNCH_CHECK();
+    k_stft_mag<ENC_NFFT><<<dim3(F, (ENC_NBIN + 255) / 256), 256, 0, s>>>(padded, W + L.window, ENC_HOP, ENC_NBIN, spec,
+                                                                         ENC_LDMAG);
+    CTB_LAUNCH_CHECK();
+    k_mel_log<MEL_PAD><<<F, MEL_PAD, ENC_NBIN * sizeof(float), s>>>(spec, ENC_LDMAG, ENC_NBIN, W + L.fb, W + L.coef, MEL,
+                                                                     mel);
+    CTB_LAUNCH_CHECK();
+    if (F < FW) CTB_CUDA(cudaMemsetAsync(mel + (size_t)F * MEL_PAD, 0, (size_t)(FW - F) * MEL_PAD * sizeof(float), s));
+  }
+  // ds0 writes +0 in frames f >= F_k, so each row's frame pairs past its own are zero, the frame at F_k of an odd F_k
+  // included (the lone call's memset).  ds1 writes +0 in token rows t >= T_k: the lone call computes rows T..FP-1 but
+  // its stack reads them only as out-of-bounds zeros.
+  if ((rc = gemm<GE_GELU>(s, gc, h->mel_tm, MEL_PAD, B * FW, c.idim, 3 * MEL_PAD, 3, MEL_PAD, 1, 1, FW, W + L.ds0_w,
+                          W + L.ds0_b, nullptr, nullptr, 0, h->bufX, c.idim, fr))) return rc;
+  if ((rc = gemm<GE_GELU>(s, gc, h->bufX, 2 * c.idim, B * TW, c.idim, 3 * 2 * c.idim, 3, 2 * c.idim, 1, 1, TW,
+                          W + L.ds1_w, W + L.ds1_b, nullptr, nullptr, 0, h->bufY, c.idim, tn))) return rc;
+  if ((rc = gemm<GE_GELU>(s, gc, h->bufY, c.idim, B * TW, c.bn_dim, 3 * c.idim, 3, c.idim, 1, 1, TW, W + L.in0_w,
+                          W + L.in0_b, nullptr, nullptr, 0, h->bufB, c.bn_dim, tn))) return rc;
+  if ((rc = gemm<GE_BIAS>(s, gc, h->bufB, c.bn_dim, B * TW, c.hidden, 3 * c.bn_dim, 3, c.bn_dim, 1, 1, TW, W + L.in2_w,
+                          W + L.in2_b, nullptr, nullptr, 0, h->bufA, c.hidden, tn))) return rc;
+  for (int i = 0; i < c.n_layer; ++i)
+    if ((rc = convnext(s, gc, W, L.blk[i], h->bufA, h->bufB, h->bufH, B * TW, TW, c.hidden, 4 * c.hidden, c.dilation,
+                       tn))) return rc;
+  if ((rc = gemm<GE_NONE>(s, gc, h->bufA, c.hidden, B * TW, c.odim, c.hidden, 1, c.hidden, 1, 0, TW, W + L.conv_out_w,
+                          nullptr, nullptr, nullptr, 0, h->bufB, c.odim, tn))) return rc;
+  FsqQuantP q{};
+  q.x = h->bufB; q.ids = ids_dev; q.margin = margin_dev; q.T = ids_ld; q.G = c.vq_groups; q.R = c.vq_residual;
+  q.levels = c.vq_levels & 0xff; q.nlev = 4; q.per_group = c.vq_dim / c.vq_groups;
+  q.scale_base = (float)(((c.vq_levels >> 8) & 0xff) ? ((c.vq_levels >> 8) & 0xff) : (q.levels - 1));
+  q.bound_input = ((c.vq_levels >> 16) & 1) ? 0 : 1;
+  q.w = W + L.vq_w; q.b = W + L.vq_b;
+  q.tn = tn; q.F = TW;
+  k_fsq_quant<true><<<dim3(TW * c.vq_groups, B), 128, 0, s>>>(q);
   CTB_LAUNCH_CHECK();
   return CTB_OK;
 }

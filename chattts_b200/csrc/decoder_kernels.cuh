@@ -462,6 +462,9 @@ struct FsqQuantP {
   float scale_base; int bound_input;
   const float* w;   // [G][nlev][per_group]
   const float* b;   // [G][nlev]
+  // ragged mode (ctb_dvae_encode_rows): row b's x is [F rows, G * per_group] at x + b * F * G * per_group, its ids and
+  // margins [G * R, T] (T = the row stride) at + b * G * R * T; only its first tn[b] tokens are quantised
+  const int* tn; int F;
 };
 __device__ __forceinline__ float fsq_bound(float z, int levels) {
   const float half_l = (float)(levels - 1) * (1.0f + 1e-3f) * 0.5f;
@@ -469,9 +472,17 @@ __device__ __forceinline__ float fsq_bound(float z, int levels) {
   const float shift = atanhf(offset / half_l);
   return tanhf(z + shift) * half_l - offset;
 }
+// RAGGED: grid (F * G, B); blocks past a row's tn[b] tokens return at once.  A token's arithmetic is the lone kernel's.
+template <bool RAGGED = false>
 __global__ void __launch_bounds__(128) k_fsq_quant(const FsqQuantP p) {
   const int t = blockIdx.x / p.G, g = blockIdx.x % p.G;
-  const float* x = p.x + ((size_t)t * p.G + g) * p.per_group;
+  size_t xoff = 0, ioff = 0;
+  if (RAGGED) {
+    if (t >= p.tn[blockIdx.y]) return;
+    xoff = (size_t)blockIdx.y * p.F * p.G * p.per_group;
+    ioff = (size_t)blockIdx.y * p.G * p.R * p.T;
+  }
+  const float* x = p.x + xoff + ((size_t)t * p.G + g) * p.per_group;
   __shared__ float s_part[4][8];
   float acc[8];
   for (int k = 0; k < p.nlev; ++k) acc[k] = 0.f;
@@ -505,8 +516,8 @@ __global__ void __launch_bounds__(128) k_fsq_quant(const FsqQuantP p) {
       idx += ((int)q + p.levels / 2) * mul;
       mul *= p.levels;
     }
-    p.ids[((size_t)g * p.R + r) * p.T + t] = idx;
-    if (p.margin) p.margin[((size_t)g * p.R + r) * p.T + t] = mg;
+    p.ids[ioff + ((size_t)g * p.R + r) * p.T + t] = idx;
+    if (p.margin) p.margin[ioff + ((size_t)g * p.R + r) * p.T + t] = mg;
     sc /= p.scale_base;
   }
 }

@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import threading
 from typing import Dict, List, Optional, Sequence, Union
 
 import numpy as np
@@ -308,6 +309,9 @@ class AudioEncoder:
             self._cfg.vq_levels |= 1 << 16
         assert blob.numel() == lib.ctb_dvae_encoder_blob_floats(C.byref(self._cfg)), "encoder blob layout mismatch"
         self._blob = blob.to(self.device, torch.float32).contiguous()
+        # the handle is not re-entrant: an open engine's worker and Chat.sample_audio_speaker may share it
+        self._lock = threading.Lock()
+        self._done: Optional[torch.cuda.Event] = None
         self._handle = C.c_void_p()
         with torch.cuda.device(self.device):
             _lib.check(lib.ctb_dvae_encoder_create(C.byref(self._cfg), C.c_void_p(self._blob.data_ptr()), max_samples,
@@ -321,6 +325,48 @@ class AudioEncoder:
             pass
 
     def encode(self, wav: torch.Tensor, want_mel: bool = False, want_margin: bool = False):
+        with self._lock, torch.cuda.device(self.device):
+            self._after_last_call()
+            out = self._encode(wav, want_mel, want_margin)
+            self._record_call()
+            return out
+
+    def _after_last_call(self):
+        """Callers on different CUDA streams share the handle's scratch: order this call after the previous one."""
+        if self._done is not None:
+            torch.cuda.current_stream().wait_event(self._done)
+
+    def _record_call(self):
+        self._done = torch.cuda.Event()
+        self._done.record(torch.cuda.current_stream())
+
+    def encode_rows(self, wavs: Sequence[torch.Tensor], want_margin: bool = False):
+        """Independent waveforms -> codes in one ``ctb_dvae_encode_rows`` call: a list of ``[G*R, T_k]`` int32 (views
+        into one buffer), row k bit-identical to ``encode(wavs[k])``; with ``want_margin`` a list of ``(ids, margin)``.
+        Rows already on the device as contiguous fp32 (e.g. ``TokenDecoder.decode_rows`` outputs) are read in place."""
+        wavs = [w.view(-1) if w.dtype == torch.float32 and w.is_contiguous() and w.device == self.device
+                else w.to(self.device, torch.float32).contiguous().view(-1) for w in wavs]
+        if not wavs:
+            return []
+        lib = _lib.load()
+        rows, B = self.vq.G * self.vq.R, len(wavs)
+        ld = max(1, max((w.numel() // ENC_HOP + 1) // 2 for w in wavs))
+        ids = torch.empty(B, rows, ld, dtype=torch.int32, device=self.device)
+        margin = torch.empty(B, rows, ld, dtype=torch.float32, device=self.device) if want_margin else None
+        ptrs = (C.c_void_p * B)(*[w.data_ptr() for w in wavs])
+        ns = (C.c_int64 * B)(*[w.numel() for w in wavs])
+        n_tok = (C.c_int32 * B)()
+        with self._lock, torch.cuda.device(self.device):
+            self._after_last_call()
+            _lib.check(lib.ctb_dvae_encode_rows(self._handle, B, ptrs, ns, C.c_void_p(ids.data_ptr()), ld, n_tok,
+                                                C.c_void_p(margin.data_ptr()) if want_margin else None,
+                                                C.c_void_p(torch.cuda.current_stream().cuda_stream)))
+            self._record_call()
+        if want_margin:
+            return [(ids[k, :, : n_tok[k]], margin[k, :, : n_tok[k]]) for k in range(B)]
+        return [ids[k, :, : n_tok[k]] for k in range(B)]
+
+    def _encode(self, wav: torch.Tensor, want_mel: bool, want_margin: bool):
         lib = _lib.load()
         wav = wav.to(self.device, torch.float32).contiguous().view(-1)
         n = wav.numel()

@@ -42,7 +42,13 @@ class Request:
 
     ``then``: called with the request's outputs when it ends at EOS or ``max_new_token`` (a seeded request that ended
     empty included; not on an interrupt); the ``Request`` it returns, if any, is queued ahead of every waiting request
-    under the next unused request index."""
+    under the next unused request index.  It may also return a list of requests (a fan-out): all of them are queued
+    ahead of the waiting requests, in list order, under consecutive indices.
+
+    ``prepare``: per-poll device work the follow-ups depend on.  When requests with a ``then`` end at a poll, each
+    distinct ``prepare`` among them is called once, before any of their ``then``, as ``prepare(dev, [(request, slot,
+    n_tokens)])`` with every one of them that names it (slot None for a seeded request that ended empty); the slots'
+    outputs are valid in ``dev``'s buffers.  This is how the work of every request ending at one poll is batched."""
 
     emb: torch.Tensor
     temperature: Sequence[float]
@@ -54,7 +60,8 @@ class Request:
     ensure_non_empty: bool = True
     stream_batch: int = 24
     infer_text: bool = False
-    then: Optional[Callable[[object], Optional["Request"]]] = None
+    then: Optional[Callable[[object], object]] = None
+    prepare: Optional[Callable[[object, list], None]] = None
 
     def __post_init__(self):
         if self.emb.dim() == 3:
@@ -90,6 +97,7 @@ class ScheduleStats:
     tokens: int = 0
     interrupted: bool = False
     children: Dict[int, int] = field(default_factory=dict)  # request index -> index of the follow-up it returned
+    fanout: Dict[int, List[int]] = field(default_factory=dict)  # request index -> indices of the list ``then`` returned
     cancelled: Set[int] = field(default_factory=set)  # request indices stopped by an ``Arrivals.cancel``
     keys: Dict[int, object] = field(default_factory=dict)  # open source: index of a submitted request -> its key
     failed: Dict[int, BaseException] = field(default_factory=dict)  # open source: request index -> its follow-up's error
@@ -98,16 +106,17 @@ class ScheduleStats:
 class Arrivals:
     """The request source of an open engine: requests submitted and cancelled from any thread, taken by the scheduling
     loop at each poll.  Each submission carries a key (an open engine's ``Job``; by default the request itself), so one
-    ``Request`` may be submitted several times under different keys; ``cancel(key)`` stops whichever stage of that
-    submission's follow-up chain is live."""
+    ``Request`` may be submitted several times under different keys; ``cancel(key)`` stops every stage of that
+    submission that is live (its follow-ups and fan-outs included).  A submission may be a list of requests, queued
+    in list order, which are stages of one submission from the start."""
 
     def __init__(self):
         self._cv = threading.Condition()
-        self._new: List[Tuple[object, Request]] = []
+        self._new: List[Tuple[object, object]] = []  # (key, Request or list of Requests)
         self._cancel: List[object] = []
         self.closed = False
 
-    def submit(self, r: Request, key=None) -> None:
+    def submit(self, r, key=None) -> None:
         with self._cv:
             if self.closed:
                 raise RuntimeError("the engine is closed")
@@ -124,7 +133,7 @@ class Arrivals:
             self.closed = True
             self._cv.notify()
 
-    def take(self, block: bool) -> Tuple[List[Tuple[object, Request]], List[object], bool]:
+    def take(self, block: bool) -> Tuple[List[Tuple[object, object]], List[object], bool]:
         """``([(key, request)] submitted, [key] cancelled, closed)`` since the last call; with ``block``, waits until
         there is one of them."""
         with self._cv:
@@ -134,29 +143,59 @@ class Arrivals:
             return new, cancel, self.closed
 
 
+def _prepare(requests: List[Request], done, dev, stats: ScheduleStats, source: Optional[Arrivals] = None) -> None:
+    """One call of each distinct ``Request.prepare`` among the requests ``done`` (``(index, slot, n_tokens, _)``) that
+    ended at this poll with a ``then``.  With an open ``source`` a failure is recorded in ``stats.failed`` for every
+    request of that call (their ``then`` is not called) instead of stopping the loop."""
+    groups: Dict[Callable, list] = {}
+    for i, s, n, _ in done:
+        r = requests[i]
+        if r.then is not None and r.prepare is not None:
+            groups.setdefault(r.prepare, []).append((i, s, n))
+    for fn, items in groups.items():
+        try:
+            fn(dev, [(requests[i], s, n) for i, s, n in items])
+        except Exception as e:
+            if source is None:
+                raise
+            for i, _, _ in items:
+                stats.failed[i] = e
+
+
 def _follow_up(requests: List[Request], i: int, slot: Optional[int], n: int, dev, check, stats: ScheduleStats,
                source: Optional[Arrivals] = None):
-    """Request ``i`` ended: its follow-up's index as a list (empty without one).  With an open ``source`` a follow-up
-    that fails (``then`` raises or ``check`` rejects it) is recorded in ``stats.failed`` instead of stopping the loop."""
+    """Request ``i`` ended: the indices of its follow-ups (empty without one).  With an open ``source`` a follow-up
+    that fails (``then`` raises or ``check`` rejects one of a fan-out) is recorded in ``stats.failed`` instead of
+    stopping the loop."""
     then = requests[i].then
-    if then is None:
+    if then is None or i in stats.failed:
         return []
     try:
         child = then(dev.empty(i) if slot is None else dev.harvest(slot, n))
         if child is None:
             return []
-        if not isinstance(child, Request):
-            raise TypeError("Request.then must return a Request or None")
+        kids = list(child) if isinstance(child, (list, tuple)) else [child]
+        if not all(isinstance(c, Request) for c in kids):
+            raise TypeError("Request.then must return a Request, a list of Requests or None")
         if check is not None:
-            check(child)
+            for c in kids:
+                check(c)
     except Exception as e:
         if source is None:
             raise
         stats.failed[i] = e
         return []
-    requests.append(child)
-    stats.children[i] = len(requests) - 1
-    return [len(requests) - 1]
+    if not kids:
+        return []
+    first = len(requests)
+    for c in kids:
+        requests.append(c)
+    idx = list(range(first, first + len(kids)))
+    if isinstance(child, Request):
+        stats.children[i] = idx[0]
+    else:
+        stats.fanout[i] = idx
+    return idx
 
 
 def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: Optional[ScheduleStats] = None,
@@ -175,13 +214,23 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
     queue and ends empty without touching a slot; a cancelled running request is stopped with ``dev.cancel`` right
     after the status read, so it ends with the ``end_idx`` tokens that read reported (a request the same read shows
     finished is finished); neither calls its ``then``, and cancelling a request whose follow-up was already made
-    cancels the follow-up.  Cancelled requests are listed in ``stats.cancelled``.  With nothing running and nothing
+    cancels the follow-up.  A submission's live stages are all cancelled together (a fan-out runs several).  Cancelled
+    requests are listed in ``stats.cancelled``.  With nothing running and nothing
     waiting the loop blocks in ``source.take`` instead of decoding, and it ends once the source is closed and drained."""
     stats = stats if stats is not None else ScheduleStats()
     waiting = deque(range(len(requests)))
     owner: List[Optional[int]] = [None] * dev.slots
-    live: Dict[object, int] = {}  # open source: submission key -> index of its live stage
+    live: Dict[object, Set[int]] = {}  # open source: submission key -> indices of its live stages
     root: Dict[int, object] = {}  # and back
+
+    def retire(i: int) -> Set[int]:  # stage i is no longer live: the submission's remaining live stages
+        key = root.pop(i)
+        stages = live[key]
+        stages.discard(i)
+        if not stages:
+            del live[key]
+        return stages
+
     doomed: Set[int] = set()  # running requests to stop after the next status read
     while True:
         taken: list = []
@@ -189,21 +238,22 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
             idle = not waiting and all(o is None for o in owner)
             new, cancels, closed = source.take(block=idle)
             for key, r in new:
-                requests.append(r)
-                i = len(requests) - 1
-                live[key], root[i], stats.keys[i] = i, key, key
-                waiting.append(i)
+                stages = live.setdefault(key, set())
+                for x in (r if isinstance(r, (list, tuple)) else [r]):
+                    requests.append(x)
+                    i = len(requests) - 1
+                    stages.add(i)
+                    root[i], stats.keys[i] = key, key
+                    waiting.append(i)
             for key in cancels:
-                i = live.get(key)
-                if i is None:  # ended already
-                    continue
-                if i in waiting:
-                    waiting.remove(i)
-                    del live[root.pop(i)]
-                    stats.cancelled.add(i)
-                    taken.append((i, None, 0, False))
-                else:
-                    doomed.add(i)
+                for i in sorted(live.get(key, ())):  # nothing left when it ended already
+                    if i in waiting:
+                        waiting.remove(i)
+                        retire(i)
+                        stats.cancelled.add(i)
+                        taken.append((i, None, 0, False))
+                    else:
+                        doomed.add(i)
             if idle and closed and not new and not taken:
                 return
         free = [s for s in range(dev.slots) if owner[s] is None]
@@ -221,6 +271,7 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
         polled = list(owner)
         ended = taken
         follow: List[int] = []
+        done = []  # (index, slot, n_tokens, cancelled at this read) of the requests that may have a follow-up
         freed = False
         stop = [s for s in range(dev.slots) if owner[s] in doomed and st.state[s] != _lib.SLOT_FINISHED]
         if stop:
@@ -234,7 +285,7 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
             was_doomed = i in doomed
             doomed.discard(i)
             if s in stop:  # no follow-up after a cancel
-                del live[root.pop(i)]
+                retire(i)
                 stats.cancelled.add(i)
                 stats.tokens += st.end_idx[s]
                 ended.append((i, s, st.end_idx[s], False))
@@ -246,21 +297,25 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
                     stats.requeued += 1
                     continue
                 ended.append((i, None, 0, True))
-                kids = _follow_up(requests, i, None, 0, dev, check, stats, source)
+                done.append((i, None, 0, was_doomed))
             else:
                 stats.tokens += st.end_idx[s]
                 ended.append((i, s, st.end_idx[s], bool(st.finish[s])))
-                kids = _follow_up(requests, i, s, st.end_idx[s], dev, check, stats, source)
-            if i in root:  # the submitted request's live stage moves on to its follow-up, or it is done
-                key = root.pop(i)
-                if kids and was_doomed:  # finished at the read that applies its cancel: the follow-up is cancelled
-                    stats.cancelled.add(kids[0])
-                    ended.append((kids[0], None, 0, False))
+                done.append((i, s, st.end_idx[s], was_doomed))
+        _prepare(requests, done, dev, stats, source)
+        for i, s, n, was_doomed in done:
+            kids = _follow_up(requests, i, s, n, dev, check, stats, source)
+            if i in root:  # the submitted request's live stage moves on to its follow-ups, or it is done
+                key = root[i]
+                retire(i)
+                if kids and was_doomed:  # finished at the read that applies its cancel: the follow-ups are cancelled
+                    for k in kids:
+                        stats.cancelled.add(k)
+                        ended.append((k, None, 0, False))
                     kids = []
-                if kids:
-                    live[key], root[kids[0]] = kids[0], key
-                else:
-                    del live[key]
+                for k in kids:
+                    live.setdefault(key, set()).add(k)
+                    root[k] = key
             follow += kids
         waiting.extendleft(reversed(follow))  # ahead of the waiting requests, in slot order
         if freed and waiting:
@@ -486,6 +541,7 @@ class Job:
         self._items: Optional[queue.Queue] = queue.Queue() if stream else None
         self._cancelled = False
         self.state = None
+        self.spk_smp: Optional[str] = None  # Chat.open_engine paragraphs: the speaker sampled from sentence 0
 
     def cancel(self) -> None:
         self._engine._source.cancel(self)
@@ -562,12 +618,15 @@ class OpenEngine:
         self._thread.start()
 
     # ---------------------------------------------------------------- callers
-    def submit(self, request: Request, stream: bool = False, state=None) -> Job:
-        """Queue ``request``; ``state`` is kept on the job for ``_serve`` (``Job.state``)."""
-        if not isinstance(request, Request):
+    def submit(self, request, stream: bool = False, state=None) -> Job:
+        """Queue ``request`` (or a non-empty list of requests, stages of one job from the start); ``state`` is kept on
+        the job for ``_serve`` (``Job.state``)."""
+        reqs = list(request) if isinstance(request, (list, tuple)) else [request]
+        if not reqs or not all(isinstance(r, Request) for r in reqs):
             raise TypeError("requests must be chattts_b200.engine.Request objects")
         if self._check is not None:
-            self._check(request)
+            for r in reqs:
+                self._check(r)
         job = Job(self, stream)
         job.state = state
         with self._lock:
@@ -639,18 +698,22 @@ class OpenEngine:
                 job = self._job_at.get(i)
                 if job is None:  # a submitted request's first yield
                     job = self._job_at[i] = self.stats.keys.pop(i)
-                child = self.stats.children.get(i) if last else None
-                if child is not None:
-                    self._job_at[child] = job
-                jobs.append((job, child is None))
+                kids = []
+                if last:
+                    child = self.stats.children.get(i)
+                    kids = ([] if child is None else [child]) + self.stats.fanout.get(i, [])
+                for c in kids:
+                    self._job_at[c] = job
+                jobs.append((job, not kids))
             self._serve(dev, requests, batch, jobs)
             for (i, _, _, last), (job, final) in zip(batch, jobs):
                 if last:  # every stage's outputs are handed out once its final yield is served: release it
                     del self._job_at[i], requests[i]
                     self.stats.children.pop(i, None)
+                    self.stats.fanout.pop(i, None)
                     self.stats.cancelled.discard(i)
                     self.stats.failed.pop(i, None)
-                    if final:
+                    if final and job.done():  # a job of several final stages (a fan-out) ends with the last one
                         with self._lock:
                             self._pending.discard(job)
 

@@ -295,6 +295,16 @@ int ctb_dvae_encoder_destroy(ctb_encoder* h);
  * decision margin the parity tests use to tell a real mismatch from fp32 reordering noise. */
 int ctb_dvae_encode(ctb_encoder* h, const float* wav_dev, int64_t n_samples, int32_t* ids_dev,
                     int32_t ids_capacity_tokens, int32_t* n_tokens_out, float* mel_dev, float* margin_dev, void* stream);
+/* Ragged batch of independent waveforms -> codes in one pass.  Row k is encoded exactly as ctb_dvae_encode encodes it
+ * alone: its ids and margins are bit-identical, on either back end (CTB_DECODER_FMA).
+ *   wavs_dev, n_samples: host arrays of B entries (they may be released on return); wavs_dev[k] -> n_k fp32 samples at
+ *                        24 kHz on the device, read in place (e.g. a row of ctb_decode_rows' wav_dev)
+ *   ids_dev [B, G*R, ids_ld] int32; margin_dev (optional) the same shape in fp32
+ *   n_tokens_out: host array of B entries, T_k = (n_k / 256 + 1) / 2
+ * CTB_ERR_ARG for B < 1, a null argument, n_k <= 512, n_k > max_samples or T_k > ids_ld.  The handle's scratch grows on
+ * demand to B rows of the widest one (CTB_ERR_NOMEM if it cannot).  Not re-entrant with the handle's other calls. */
+int ctb_dvae_encode_rows(ctb_encoder* h, int32_t B, const float* const* wavs_dev, const int64_t* n_samples,
+                         int32_t* ids_dev, int32_t ids_ld, int32_t* n_tokens_out, float* margin_dev, void* stream);
 
 #ifdef __cplusplus
 }

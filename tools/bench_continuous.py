@@ -3,6 +3,7 @@
 
     python tools/bench_continuous.py [--requests N] [--slots S] [--steps K] [--warmup W] [--dump-outputs DIR] [--stream]
                                      [--refine] [--online RATE[,RATE...] [--cancel FRACTION]]
+    python tools/bench_continuous.py --paragraphs N [--slots S] [--steps K] [--warmup W]
 
 N requests (default 128), each one utterance with its own seeded prompt (8..128 tokens) and forced length (64..1024
 tokens, min_new = max_new: synthetic weights have no meaningful EOS), run through the slot engine with S slots
@@ -18,6 +19,8 @@ engine, the speech request admitted as the request's refinement ends (``Request.
 speech codes on the engine; (c) the speech codes alone on the engine (the first line's workload).  Per arm: wall time,
 useful speech-tokens/s, decode steps, mean slot occupancy and the time from start to each request's first speech token
 (p50 / p95 / max; the token is sampled by the admission's prefill and counted at the status read that follows it).
+
+``--paragraphs N`` prints only one JSON line: N split-text paragraphs on the open engine (see ``run_paragraphs``).
 
 ``--stream`` then prints a second JSON line: the same requests streamed as audio (hidden path, DVAE decoder and Vocos
 from synthetic weights, InferCodeParams' default stream_batch / stream_speed / pass_first_n_batches), timed
@@ -593,6 +596,139 @@ def run_online(args, local_rank: int = 0):
     return lines
 
 
+class _CharTokenizer:
+    """A tokenizer stand-in for ``--paragraphs`` (the real one needs the model assets): one id per character."""
+    len, break_0_ids, eos_token, spk_emb_ids = 21178, 21150, 21001, 21143
+
+    def encode(self, text, num_vq, prompt=None, device="cpu"):
+        rows = [[(ord(ch) * 37 + 11) % 20000 + 1 for ch in t] or [1] for t in text]
+        P = 0 if prompt is None else int(prompt.size(1))
+        T = max(len(r) for r in rows) + P
+        ids = torch.zeros(len(rows), T, num_vq, dtype=torch.long)
+        mask = torch.zeros(len(rows), T, dtype=torch.bool)
+        for b, r in enumerate(rows):
+            ids[b, T - P - len(r): T - P] = torch.tensor(r)[:, None]
+            mask[b, T - P - len(r):] = True
+        text_mask = mask.clone()
+        if P:
+            ids[:, T - P:] = prompt.t().long()[None]
+            text_mask[:, T - P:] = False
+        return ids.to(device), mask.to(device), text_mask.to(device)
+
+    def decode(self, tokens):
+        return ["".join(chr(97 + int(t) % 26) for t in row) for row in tokens]
+
+
+def run_paragraphs(args, local_rank: int = 0):
+    """Paragraphs of 2-6 sentences (seeded; each paragraph's sentences forced to one seeded length of 48..256 tokens),
+    all submitted at once.  Arms, alternated, ``--steps`` repeats each: (a) ``ChatEngine.submit(split_text=True,
+    stream=True)`` on one open engine of S slots; (b) the same with one lone ``encode`` per speaker sample instead of
+    one ``encode_rows`` call per poll; (c) ``Chat.infer(paragraph, stream=True)`` one paragraph after another.
+    Per arm (median repeat by wall time): wall time, first- and last-chunk latency per paragraph, and for (a)/(b) the
+    share of the wall time spent in the speaker-sample encode (device-synchronised around each call)."""
+    import numpy as np
+
+    from chattts_b200 import Chat
+    from chattts_b200.core import split_sentences
+    from chattts_b200.speaker import Speaker
+    from chattts_b200.synth import synth_all
+
+    dev = torch.device("cuda", local_rank)
+    torch.cuda.set_device(dev)
+    S, n = args.slots, args.paragraphs
+    g = np.random.default_rng(31)
+    texts, lengths = [], []
+    for k in range(n):
+        m = int(g.integers(2, 7))
+        texts.append(" ".join(f"sentence {j} of paragraph {k} says something." for j in range(m)))
+        lengths.append(int(g.integers(48, 257)))
+    c = Chat()
+    assert c.load_states(synth_all(0), tokenizer=_CharTokenizer(), speaker=Speaker(768, None), device=dev,
+                         max_batch=S, max_context=1024)
+    enc = c.dvae.audio_encoder
+    batched = enc.encode_rows
+    encode_s = [0.0]
+
+    def timed(fn):
+        def call(wavs, *a, **kw):
+            torch.cuda.synchronize()
+            t = time.perf_counter()
+            out = fn(wavs, *a, **kw)
+            torch.cuda.synchronize()
+            encode_s[0] += time.perf_counter() - t
+            return out
+        return call
+
+    def lone(wavs, *a, **kw):  # arm (b): what the engine would do without the ragged encode
+        return [enc.encode(w) for w in wavs]
+
+    def params(k):
+        return c.InferCodeParams(manual_seed=900 + k, max_new_token=lengths[k], min_new_token=lengths[k],
+                                 show_tqdm=False)
+
+    def engine_arm(rows):
+        enc.encode_rows = timed(rows)
+        encode_s[0] = 0.0
+        times = {k: [] for k in range(n)}
+        t0 = time.perf_counter()
+        try:
+            with c.open_engine(slots=S, max_new_cap=max(lengths)) as eng:
+                jobs = [eng.submit(t, params_infer_code=params(k), stream=True, split_text=True)
+                        for k, t in enumerate(texts)]
+                threads = []
+                for k, job in enumerate(jobs):
+                    def consume(k=k, job=job):
+                        for ch, _ in job:
+                            if ch.shape[1]:
+                                times[k].append(time.perf_counter() - t0)
+                    threads.append(threading.Thread(target=consume))
+                    threads[-1].start()
+                for th in threads:
+                    th.join()
+        finally:
+            del enc.encode_rows
+        return times, time.perf_counter() - t0, encode_s[0]
+
+    def infer_arm():
+        times = {k: [] for k in range(n)}
+        t0 = time.perf_counter()
+        for k, t in enumerate(texts):
+            for ch in c.infer(t, stream=True, skip_refine_text=True, params_infer_code=params(k)):
+                if ch.shape[1]:
+                    times[k].append(time.perf_counter() - t0)
+        return times, time.perf_counter() - t0, None
+
+    def summary(r):
+        times, wall, enc_s = r
+        q = lambda v: {"p50": round(float(np.percentile(v, 50)), 4), "p95": round(float(np.percentile(v, 95)), 4),
+                       "max": round(float(max(v)), 4)}  # noqa: E731
+        out = {"wall_s": round(wall, 3), "first_chunk_s": q([t[0] for t in times.values() if t]),
+               "last_chunk_s": q([t[-1] for t in times.values() if t])}
+        if enc_s is not None:
+            out["encode_s"] = round(enc_s, 4)
+            out["encode_share"] = round(enc_s / wall, 4)
+        return out
+
+    import threading
+
+    for _ in range(max(1, args.warmup)):
+        engine_arm(batched)
+        engine_arm(lone)
+    runs = {"a": [], "b": [], "c": []}
+    for _ in range(args.steps):
+        runs["a"].append(summary(engine_arm(batched)))
+        runs["b"].append(summary(engine_arm(lone)))
+        runs["c"].append(summary(infer_arm()))
+    name, limit = gpu_card(local_rank)
+    line = {"metric": "continuous_paragraphs", "card": name, "power_limit": limit, "paragraphs": n, "slots": S,
+            "sentences": sum(len(split_sentences(t)) for t in texts), "forced_tokens": [min(lengths), max(lengths)],
+            "repeats": args.steps}
+    for arm, rs in runs.items():
+        line[arm] = sorted(rs, key=lambda x: x["wall_s"])[len(rs) // 2]
+        line[arm]["wall_all_s"] = [x["wall_s"] for x in rs]
+    return line
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--requests", type=int, default=128)
@@ -606,10 +742,15 @@ def main():
                     help="also measure streamed requests arriving at these rates (requests/s; one JSON line each)")
     ap.add_argument("--cancel", type=float, default=None, metavar="FRACTION",
                     help="with --online: one more line with this fraction of the requests cancelled")
+    ap.add_argument("--paragraphs", type=int, default=None, metavar="N",
+                    help="only measure N split-text paragraphs on the open engine (one JSON line)")
     args = ap.parse_args()
     if args.steps < 1:
         ap.error("--steps must be >= 1")
     rank = int(os.environ.get("LOCAL_RANK", "0"))
+    if args.paragraphs:
+        print(json.dumps(run_paragraphs(args, rank)), flush=True)
+        return
     print(json.dumps(run_continuous(args, rank)), flush=True)
     if args.stream:
         print(json.dumps(run_stream(args, rank)), flush=True)
