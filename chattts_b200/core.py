@@ -30,10 +30,6 @@ from .norm import Normalizer
 from .processors import gen_logits
 
 
-_SPLIT_REFINE = ("split_text=True with skip_refine_text=False is not supported on the slot engine (each sentence "
-                 "would wait for its refinement and for the paragraph's speaker sample)")
-
-
 def split_sentences(text: str) -> List[str]:
     """``infer``'s sentence split (``split_text=True``): the lines of a text with a newline, else its sentences
     ending in '。' or '. ' (reference core.py:237-241)."""
@@ -216,7 +212,7 @@ class Chat:
 
     def infer_continuous(self, texts, params_infer_code=None, use_decoder=True, slots=None, stream=False, lang=None,
                          skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
-                         params_refine_text=None, refine_on_engine=False, split_text=False):
+                         params_refine_text=None, refine_on_engine=False, split_text=False, max_split_batch=1):
         """Synthesise many texts with continuous batching (``GPT.generate_continuous``): each text is one request,
         ``params_infer_code`` is one ``InferCodeParams`` for all texts or a list with one per text (speaker, seed,
         temperature, top-P/K, penalty, token limits).  Generator of ``(index, wav)`` in completion order; ``wav`` is
@@ -233,24 +229,26 @@ class Chat:
 
         ``split_text=True`` makes each text a paragraph, split into sentences as ``infer`` splits it, with one voice
         across its sentences (see ``ChatEngine.submit``): ``wav`` is then what ``infer(texts[index], split_text=True,
-        max_split_batch=1, skip_refine_text=True)[0]`` returns with that text's params, which are not modified.  The
-        paragraphs run on an open engine (``open_engine``); ``slots`` defaults to the handle's ``max_batch``."""
+        max_split_batch=max_split_batch, skip_refine_text=True)[0]`` returns with that text's params, which are not
+        modified; with ``skip_refine_text=False`` each sentence is refined on the engine first, and ``wav`` is what
+        ``infer(texts[index], max_split_batch=max_split_batch, params_refine_text=...)[0]`` returns (seeded: bit for
+        bit on the code path).  The paragraphs run on an open engine (``open_engine``); ``slots`` defaults to the
+        handle's ``max_batch``."""
         if stream:
             raise ValueError("infer_continuous: stream=True is not supported; each waveform is yielded when complete "
                              "(infer_continuous_stream streams)")
         texts, params = self._continuous_params(texts, params_infer_code)
         if split_text:
-            if not skip_refine_text:
-                raise ValueError(_SPLIT_REFINE)
             return self._paragraphs(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
-                                    do_homophone_replacement, False)
+                                    do_homophone_replacement, False, self._refine_params(texts, params_refine_text),
+                                    max_split_batch)
         return self._infer_continuous(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
                                       do_homophone_replacement, self._refine_params(texts, params_refine_text),
                                       refine_on_engine)
 
     def infer_continuous_stream(self, texts, params_infer_code=None, use_decoder=True, slots=None, lang=None,
                                 skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
-                                params_refine_text=None, refine_on_engine=False, split_text=False):
+                                params_refine_text=None, refine_on_engine=False, split_text=False, max_split_batch=1):
         """Streaming synthesis of many texts with continuous batching (``GPT.generate_continuous_stream``).
         Generator of ``(index, chunk, last)``, ``chunk`` a ``[1, n]`` float32 array; for each text the chunks are
         those ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=True)`` yields with that
@@ -260,13 +258,12 @@ class Chat:
         buffers.  Arguments as for ``infer_continuous``; with ``refine_on_engine=True`` the chunks are those of
         ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=False)``.  With ``split_text=True``
         each text is a paragraph, streamed sentence by sentence as ``ChatEngine.submit(split_text=True,
-        stream=True)`` streams it."""
+        stream=True)`` streams it, refined first with ``skip_refine_text=False``."""
         texts, params = self._continuous_params(texts, params_infer_code)
         if split_text:
-            if not skip_refine_text:
-                raise ValueError(_SPLIT_REFINE)
             return self._paragraphs(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
-                                    do_homophone_replacement, True)
+                                    do_homophone_replacement, True, self._refine_params(texts, params_refine_text),
+                                    max_split_batch)
         return self._infer_continuous_stream(texts, params, use_decoder, slots, lang, skip_refine_text,
                                              do_text_normalization, do_homophone_replacement,
                                              self._refine_params(texts, params_refine_text), refine_on_engine)
@@ -310,23 +307,24 @@ class Chat:
         return [params_refine_text or Chat.RefineTextParams()] * len(texts)
 
     def _paragraphs(self, texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
-                    do_homophone_replacement, stream):
+                    do_homophone_replacement, stream, refine, max_split_batch):
         """``infer_continuous*(split_text=True)``: every text a paragraph job on one open engine, submitted in order.
         Generator of ``(index, wav)`` in completion order, or of ``(index, chunk, last)`` as the chunks come."""
-        if not skip_refine_text:
-            raise ValueError(_SPLIT_REFINE)
         assert self.has_loaded(use_decoder=use_decoder)
         self.context.set(False)
         if not texts:
             return
         out: queue.Queue = queue.Queue()
         cap = max(p.max_new_token for p in params)
+        if not skip_refine_text:
+            cap = max(cap, max(r.max_new_token for r in refine))
         with self.open_engine(slots, max_new_cap=cap, use_decoder=use_decoder) as eng:
             try:
                 jobs = [eng.submit(t, params_infer_code=p, stream=stream, lang=lang, split_text=True,
-                                   do_text_normalization=do_text_normalization,
+                                   skip_refine_text=skip_refine_text, params_refine_text=r,
+                                   max_split_batch=max_split_batch, do_text_normalization=do_text_normalization,
                                    do_homophone_replacement=do_homophone_replacement, _sink=(out, k))
-                        for k, (t, p) in enumerate(zip(texts, params))]
+                        for k, (t, p, r) in enumerate(zip(texts, params, refine))]
                 left = len(jobs)
                 while left:
                     try:
@@ -407,8 +405,9 @@ class Chat:
                 out.destroy()
                 yield k, wav[np.abs(wav) > thr]  # quirk Q20, as infer() returns it
 
-    def _code_request(self, text, params):
-        """The request ``_infer_code([text], ...)`` would decode as a batch of one."""
+    def _code_request(self, text, params, noise_batch=None):
+        """The request ``_infer_code([text], ...)`` would decode as a batch of one (``noise_batch`` = (B, b): as row b
+        of a batch of B)."""
         from .engine import Request
 
         temperature = params.temperature if isinstance(params.temperature, list) else [params.temperature] * self.config.gpt.num_vq
@@ -427,10 +426,12 @@ class Chat:
         return Request(emb=emb[0][valid.to(emb.device)], temperature=temperature, eos_token=num_code,
                        max_new_token=params.max_new_token, min_new_token=params.min_new_token,
                        logits_processors=(*processors, *warpers), manual_seed=params.manual_seed,
-                       ensure_non_empty=params.ensure_non_empty, stream_batch=params.stream_batch)
+                       ensure_non_empty=params.ensure_non_empty, stream_batch=params.stream_batch,
+                       noise_batch=noise_batch)
 
-    def _refine_request(self, text, params):
-        """The text request ``_refine_text([text], ...)`` would generate as a batch of one."""
+    def _refine_request(self, text, params, noise_batch=None):
+        """The text request ``_refine_text([text], ...)`` would generate as a batch of one (``noise_batch`` = (B, b): as
+        row b of a batch of B)."""
         from .engine import Request
 
         input_ids, attention_mask, text_mask = self.tokenizer.encode(
@@ -442,7 +443,8 @@ class Chat:
         return Request(emb=emb[0][valid.to(emb.device)], temperature=[params.temperature],
                        eos_token=self.tokenizer.eos_token, max_new_token=params.max_new_token,
                        min_new_token=params.min_new_token, logits_processors=(*processors, *warpers),
-                       manual_seed=params.manual_seed, ensure_non_empty=params.ensure_non_empty, infer_text=True)
+                       manual_seed=params.manual_seed, ensure_non_empty=params.ensure_non_empty, infer_text=True,
+                       noise_batch=noise_batch)
 
     def _chained_request(self, text, params, refine):
         """The text's refinement request, whose follow-up is the speech-code request of the refined text."""
@@ -776,6 +778,50 @@ class _SpeakerSampler:
         return v
 
 
+class _RefineGraph:
+    """The stage graph of a refined paragraph (``ChatEngine.submit(split_text=True, skip_refine_text=False)``).
+
+    Each of the n sentences is refined by a text request of its own, whose ``then`` is ``then(k)``; ``refined[k]`` is
+    its text once it has ended (``refined_text(outputs)``).  With a reference stage (``reference`` given: n > 1 and no
+    ``spk_smp``), refinement 0's follow-up is ``reference(r_0)``, the code request of the refined sentence 0 alone,
+    and the reference stage's ``then`` takes the speaker sample with ``sample(request)``.  Sentence k's code request,
+    ``code(k, r_k, (spk_smp, txt_smp) or None)``, needs both ``r_k`` and the sample, and is made exactly once, by
+    whichever of the two stages ends last (the join): refinement k's ``then`` returns it when the sample is known and
+    None otherwise, and the reference stage's ``then`` returns the code requests of every sentence refined by then, in
+    sentence order.  Without a reference stage each refinement's ``then`` returns its code request.  A refinement that
+    ended empty raises in its ``then``, which fails the job, as a seeded first-step EOS makes ``infer`` raise."""
+
+    def __init__(self, n: int, refined_text, code, reference=None, sample=None):
+        self.n, self.refined_text, self.code, self.reference, self.sample = n, refined_text, code, reference, sample
+        self.refined: List[Optional[str]] = [None] * n
+        self.ref = None  # the reference stage's request, once refinement 0 has ended
+        self.spk = None  # (spk_smp, txt_smp), once the reference stage has ended
+        self._made = [False] * n
+
+    def then(self, k: int):
+        def then(out):
+            if int(out.ids[0].shape[0]) == 0:
+                raise RuntimeError(f"the refinement of sentence {k} of the paragraph ended empty")
+            self.refined[k] = self.refined_text(out)
+            if self.reference is None:
+                return self._make(k)
+            if k == 0:
+                self.ref = self.reference(self.refined[0])
+                self.ref.then = self._reference_then
+                return self.ref
+            return self._make(k) if self.spk is not None else None
+        return then
+
+    def _reference_then(self, out):
+        self.spk = (self.sample(self.ref), self.refined[0])
+        return [self._make(k) for k in range(self.n) if self.refined[k] is not None]
+
+    def _make(self, k: int):
+        assert not self._made[k], f"sentence {k}'s code request was made twice"
+        self._made[k] = True
+        return self.code(k, self.refined[k], self.spk)
+
+
 class ChatEngine(OpenEngine):
     """``Chat.open_engine``: an open slot engine whose jobs are texts (see there).  At each poll every window due for a
     streaming job and the whole sequence of every non-streaming job that completed go into one ``decode_rows`` call."""
@@ -789,7 +835,7 @@ class ChatEngine(OpenEngine):
 
     def submit(self, text: str, params_infer_code=None, stream=False, skip_refine_text=True, params_refine_text=None,
                lang=None, do_text_normalization=True, do_homophone_replacement=True, split_text=False,
-               _sink=None) -> Job:
+               max_split_batch=1, _sink=None) -> Job:
         """Queue one text -> ``Job``: ``result()`` is the waveform ``infer_continuous`` yields for it, or with
         ``stream=True`` the job iterates the ``(chunk, last)`` pairs ``infer_continuous_stream`` yields for it.
         ``skip_refine_text=False`` refines the text on the engine first (``refine_on_engine=True``).  A cancelled
@@ -809,13 +855,26 @@ class ChatEngine(OpenEngine):
         sentence's chunks are held until the earlier one's final chunk is out, and ``last`` marks only the final
         chunk of the last sentence.  Unlike ``infer(stream=True)``, whose stream position runs on across its batches,
         each sentence's stream starts at its own first sample.  A reference stage too short to encode or that ended
-        empty, or a sentence whose prompt breaks the engine's limits, fails that job only.  Needs
-        ``skip_refine_text=True``."""
+        empty, or a sentence whose prompt breaks the engine's limits, fails that job only; its other live stages are
+        cancelled at the next poll.
+
+        ``max_split_batch`` = m: sentence k samples as row ``k mod m`` of ``infer``'s code batch of
+        ``min(m, n - m * (k // m))`` sentences (``Request.noise_batch``), so a seeded paragraph is what ``infer(...,
+        max_split_batch=m)`` returns; the default 1 is the batch of one of each sentence.
+
+        ``skip_refine_text=False`` with ``split_text=True`` refines every sentence on the engine first, each as row
+        ``k mod max_batch`` of ``infer``'s refinement batch, with ``params_refine_text``; ``Job.refined`` lists the
+        refined sentences as they end.  The reference stage speaks the refined sentence 0, and each sentence's code
+        request starts as soon as both its refinement and the speaker sample are done (see ``_RefineGraph``).
+        ``result()`` is then what ``infer(text, use_decoder=False, max_split_batch=m, params_refine_text=...)[0]``
+        returns, bit for bit on the code path when seeded (with the default arguments and m = 4: ``infer(text)``).
+        A refinement that ends empty fails the job, as it makes ``infer`` raise."""
         chat = self.chat
         params = params_infer_code or Chat.InferCodeParams()
         if split_text:
-            return self._submit_paragraph(text, params, stream, skip_refine_text, lang, do_text_normalization,
-                                          do_homophone_replacement, _sink)
+            return self._submit_paragraph(text, params, stream, skip_refine_text,
+                                          params_refine_text or Chat.RefineTextParams(), max_split_batch, lang,
+                                          do_text_normalization, do_homophone_replacement, _sink)
         if not skip_refine_text and self.max_new_cap is not None and params.max_new_token > self.max_new_cap:
             # the speech stage is made only when the refinement ends: check its limit here, in the caller's thread
             raise ValueError(f"max_new_token {params.max_new_token} exceeds max_new_cap={self.max_new_cap}")
@@ -829,39 +888,68 @@ class ChatEngine(OpenEngine):
         windows = StreamWindows(params.stream_speed, params.pass_first_n_batches) if stream else None
         return super().submit(request, stream, windows)
 
-    def _submit_paragraph(self, text, params, stream, skip_refine_text, lang, do_text_normalization,
-                          do_homophone_replacement, sink) -> Job:
-        if not skip_refine_text:
-            raise ValueError(_SPLIT_REFINE)
+    def _submit_paragraph(self, text, params, stream, skip_refine_text, refine, max_split_batch, lang,
+                          do_text_normalization, do_homophone_replacement, sink) -> Job:
         chat = self.chat
         if self.max_new_cap is not None and params.max_new_token > self.max_new_cap:
             raise ValueError(f"max_new_token {params.max_new_token} exceeds max_new_cap={self.max_new_cap}")
+        m = int(max_split_batch)
+        if m < 1:
+            raise ValueError("max_split_batch must be >= 1")
         sentences = [chat.normalizer(t, do_text_normalization, do_homophone_replacement, lang)
                      for t in split_sentences(text)]
         if not sentences:
             raise ValueError("split_text=True: the text has no sentence")
-        para = _Paragraph(len(sentences), params if stream else None, sink)
-        if len(sentences) == 1 or params.spk_smp is not None:
-            reqs = [chat._code_request(t, copy.copy(params)) for t in sentences]
-            para.order = {r: k for k, r in enumerate(reqs)}
-            job = super().submit(reqs, stream, para)
-        else:
-            if chat.dvae.audio_encoder is None:
-                raise RuntimeError("this DVAE checkpoint carries no encoder / VQ weights: cannot sample a speaker")
-            para.ref = chat._code_request(sentences[0], copy.copy(params))
+        n = len(sentences)
+        if min(m, n) > chat.gpt.max_batch:
+            raise ValueError(f"max_split_batch={m}: a batch of {min(m, n)} sentences exceeds this handle's "
+                             f"max_batch={chat.gpt.max_batch}")
+        para = _Paragraph(n, params if stream else None, sink)
+        spk_stage = n > 1 and params.spk_smp is None
+        if spk_stage and chat.dvae.audio_encoder is None:
+            raise RuntimeError("this DVAE checkpoint carries no encoder / VQ weights: cannot sample a speaker")
+
+        def code(k, t, sample):  # sentence k's request: a copy of the params carrying the sample, row k mod m
+            p = copy.copy(params)
+            if sample is not None:
+                p.spk_smp, p.txt_smp = sample
+            r = chat._code_request(t, p, noise_batch=(min(m, n - m * (k // m)), k % m))
+            para.order[r] = k
+            return r
+
+        def reference(t):  # the reference stage: sentence 0 alone, as infer() synthesises it
+            para.ref = chat._code_request(t, copy.copy(params))
             para.ref.prepare = self._sampler
+            return para.ref
 
-            def then(out, para=para):
-                spk = self._sampler.take(para.ref)
-                para.job.spk_smp = spk
-                p = copy.copy(params)
-                p.spk_smp, p.txt_smp = spk, sentences[0]
-                reqs = [chat._code_request(t, p) for t in sentences]
-                para.order = {r: k for k, r in enumerate(reqs)}
-                return reqs
+        def sample(ref):
+            spk = self._sampler.take(ref)
+            para.job.spk_smp = spk
+            return spk
 
-            para.ref.then = then
-            job = super().submit(para.ref, stream, para)
+        if not skip_refine_text:
+            B = chat.gpt.max_batch  # infer() refines a paragraph's sentences in batches of up to max_batch
+            graph = _RefineGraph(n, chat._refined_text, code, reference if spk_stage else None,
+                                 sample if spk_stage else None)
+            reqs = []
+            for k, t in enumerate(sentences):
+                r = chat._refine_request(t, refine, noise_batch=(min(B, n - B * (k // B)), k % B))
+                r.then = graph.then(k)
+                r.stream_batch = params.stream_batch
+                reqs.append(r)
+            job = super().submit(reqs, stream, para)
+            job.refined = graph.refined
+        elif not spk_stage:
+            job = super().submit([code(k, t, None) for k, t in enumerate(sentences)], stream, para)
+        else:
+            ref = reference(sentences[0])
+
+            def then(out):
+                smp = (sample(ref), sentences[0])
+                return [code(k, t, smp) for k, t in enumerate(sentences)]
+
+            ref.then = then
+            job = super().submit(ref, stream, para)
         para.job = job
         return job
 

@@ -48,7 +48,13 @@ class Request:
     ``prepare``: per-poll device work the follow-ups depend on.  When requests with a ``then`` end at a poll, each
     distinct ``prepare`` among them is called once, before any of their ``then``, as ``prepare(dev, [(request, slot,
     n_tokens)])`` with every one of them that names it (slot None for a seeded request that ended empty); the slots'
-    outputs are valid in ``dev``'s buffers.  This is how the work of every request ending at one poll is batched."""
+    outputs are valid in ``dev``'s buffers.  This is how the work of every request ending at one poll is batched.
+
+    ``noise_batch``: ``(B, b)`` - a seeded request samples as row ``b`` of a static ``GPT.generate`` batch of ``B``
+    with the same seed: it draws rows ``b * rows ... (b + 1) * rows - 1`` of that batch's Exp(1) noise (``rows``: 1
+    for text, ``num_vq`` for codes) instead of the rows of a batch of one.  Nothing else the sampler computes depends
+    on the row, as long as the repetition penalty covers the row (``check_noise_batch``).  ``None`` and ``(1, 0)`` are
+    a batch of one; an unseeded request ignores it."""
 
     emb: torch.Tensor
     temperature: Sequence[float]
@@ -62,6 +68,7 @@ class Request:
     infer_text: bool = False
     then: Optional[Callable[[object], object]] = None
     prepare: Optional[Callable[[object, list], None]] = None
+    noise_batch: Optional[Tuple[int, int]] = None
 
     def __post_init__(self):
         if self.emb.dim() == 3:
@@ -76,6 +83,47 @@ class Request:
             raise ValueError("stream_batch must be >= 1")
         if self.infer_text and torch.as_tensor(self.temperature).numel() != 1:
             raise ValueError("a text request takes one temperature")
+        if self.noise_batch is not None:
+            B, b = (int(x) for x in self.noise_batch)
+            self.noise_batch = (B, b)
+            check_noise_batch(self, 1 if self.infer_text else None)
+
+
+def check_noise_batch(r: Request, rows: Optional[int], max_batch: Optional[int] = None) -> None:
+    """Raise ``ValueError`` unless ``r.noise_batch`` = ``(B, b)`` names a row of a static batch the request can sample
+    as: ``0 <= b < B``, ``B`` at most ``max_batch``, and with a repetition penalty every one of the row's ``rows``
+    noise rows below the penalty's ``max_input_ids`` (the static sampler drops the penalty from rows at or past it,
+    the engine never does).  ``rows`` None skips the penalty check."""
+    if r.noise_batch is None:
+        return
+    B, b = r.noise_batch
+    if B < 1 or not 0 <= b < B:
+        raise ValueError(f"noise_batch {r.noise_batch}: needs 0 <= b < B")
+    if max_batch is not None and B > max_batch:
+        raise ValueError(f"noise_batch {r.noise_batch}: B exceeds this handle's max_batch={max_batch}")
+    if rows is None:
+        return
+    for proc in r.logits_processors:
+        if hasattr(proc, "penalty") and hasattr(proc, "past_window") and hasattr(proc, "max_input_ids"):
+            if (b + 1) * rows > int(proc.max_input_ids):
+                raise ValueError(f"noise_batch {r.noise_batch}: row {b} of the static batch would lose its repetition "
+                                 f"penalty (rows {b * rows}..{(b + 1) * rows - 1}, max_input_ids "
+                                 f"{proc.max_input_ids})")
+
+
+def noise_rows(reqs: Sequence[Request], rows: int, cols: int, cache: Dict[tuple, torch.Tensor]) -> torch.Tensor:
+    """The Exp(1) noise of the seeded requests ``reqs`` ([len(reqs) * rows, cols], on the host): for each one, rows
+    ``b * rows ... (b + 1) * rows - 1`` of ``exp_noise(B * rows, cols, manual_seed)``, ``(B, b)`` its ``noise_batch``
+    (default a batch of one).  The full batch's noise is built once per ``(B, rows, cols, seed)`` in ``cache`` and the
+    rows are sliced from it."""
+    parts = []
+    for r in reqs:
+        B, b = r.noise_batch or (1, 0)
+        key = (B, rows, cols, r.manual_seed)
+        if key not in cache:
+            cache[key] = exp_noise(B * rows, cols, r.manual_seed)
+        parts.append(cache[key][b * rows: (b + 1) * rows])
+    return torch.cat(parts)
 
 
 @dataclass
@@ -414,6 +462,7 @@ class EngineDevice:
     def admit(self, batch: List[Tuple[int, int]]) -> None:
         # one prefill per kind: seeded requests bring their Exp(1) rows, unseeded ones sample with device Philox; code
         # and text requests are admitted by separate calls
+        noise: Dict[tuple, torch.Tensor] = {}  # one static batch's noise per (B, rows, cols, seed) in this admission
         for seeded, text in ((True, False), (True, True), (False, False), (False, True)):
             group = [(s, i) for s, i in batch if (self.requests[i].manual_seed is not None) == seeded
                      and bool(self.requests[i].infer_text) == text]
@@ -425,9 +474,9 @@ class EngineDevice:
             alone = [(s, i) for s, i in group if T0 + self.requests[i].max_new_token > self.gpt.max_context]
             rest = [p for p in group if p not in alone]
             for part in ([rest] if rest else []) + [[p] for p in alone]:
-                self._admit(part, seeded, text)
+                self._admit(part, seeded, text, noise)
 
-    def _admit(self, group, seeded: bool, text: bool) -> None:
+    def _admit(self, group, seeded: bool, text: bool, cache: Dict[tuple, torch.Tensor]) -> None:
         gpt, n = self.gpt, len(group)
         reqs = [self.requests[i] for _, i in group]
         T0 = max(MIN_PROMPT_COLS, max(int(r.emb.shape[0]) for r in reqs))
@@ -444,9 +493,9 @@ class EngineDevice:
             philox = 0 if seeded else int(torch.randint(0, 2 ** 62, (1,)).item())
             cfgs[k] = build_sampler_config(r.logits_processors, temps, int(r.eos_token), r.min_new_token, philox)
         noise = None
-        if seeded:  # the rows GPT.generate draws for a batch of one with this seed
+        if seeded:  # the rows GPT.generate draws for this request's row of its batch (noise_batch) with this seed
             rows, cols = (1, gpt.num_text_tokens) if text else (gpt.num_vq, gpt.num_audio_tokens)
-            noise = torch.cat([exp_noise(rows, cols, r.manual_seed) for r in reqs]).to(self.dev)
+            noise = noise_rows(reqs, rows, cols, cache).to(self.dev)
         slots = (C.c_int32 * n)(*[s for s, _ in group])
         max_new = (C.c_int32 * n)(*[r.max_new_token for r in reqs])
         for s, _ in group:
@@ -542,6 +591,7 @@ class Job:
         self._cancelled = False
         self.state = None
         self.spk_smp: Optional[str] = None  # Chat.open_engine paragraphs: the speaker sampled from sentence 0
+        self.refined: Optional[List[Optional[str]]] = None  # refined paragraphs: each sentence's text once refined
 
     def cancel(self) -> None:
         self._engine._source.cancel(self)
@@ -712,7 +762,8 @@ class OpenEngine:
                     self.stats.children.pop(i, None)
                     self.stats.fanout.pop(i, None)
                     self.stats.cancelled.discard(i)
-                    self.stats.failed.pop(i, None)
+                    if self.stats.failed.pop(i, None) is not None:
+                        self._source.cancel(job)  # a failed job's other live stages are stopped at the next poll
                     if final and job.done():  # a job of several final stages (a fan-out) ends with the last one
                         with self._lock:
                             self._pending.discard(job)

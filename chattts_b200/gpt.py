@@ -339,7 +339,7 @@ class GPT:
         """Checks shared by the slot-engine generators -> (requests, slots, chunk, context, max_new_cap, check), where
         ``check`` validates a follow-up request as the up-front ones are.  The poll interval is `chunk`, else
         CTB_DECODE_CHUNK, else `default_chunk` (None: the smallest ``stream_batch``)."""
-        from .engine import MIN_PROMPT_COLS, Request
+        from .engine import MIN_PROMPT_COLS, Request, check_noise_batch
 
         self._check_free(name)
         if infer_text:
@@ -368,6 +368,7 @@ class GPT:
                                  f"(max_context={self.max_context}; prompts up to 1024 tokens)")
             if r.max_new_token > cap:
                 raise ValueError(f"max_new_token {r.max_new_token} exceeds max_new_cap={cap}")
+            check_noise_batch(r, 1 if r.infer_text else self.num_vq, self.max_batch)
 
         for r in requests:
             check(r)

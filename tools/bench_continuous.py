@@ -3,7 +3,7 @@
 
     python tools/bench_continuous.py [--requests N] [--slots S] [--steps K] [--warmup W] [--dump-outputs DIR] [--stream]
                                      [--refine] [--online RATE[,RATE...] [--cancel FRACTION]]
-    python tools/bench_continuous.py --paragraphs N [--slots S] [--steps K] [--warmup W]
+    python tools/bench_continuous.py --paragraphs N [--refine] [--slots S] [--steps K] [--warmup W]
 
 N requests (default 128), each one utterance with its own seeded prompt (8..128 tokens) and forced length (64..1024
 tokens, min_new = max_new: synthetic weights have no meaningful EOS), run through the slot engine with S slots
@@ -20,7 +20,8 @@ speech codes on the engine; (c) the speech codes alone on the engine (the first 
 useful speech-tokens/s, decode steps, mean slot occupancy and the time from start to each request's first speech token
 (p50 / p95 / max; the token is sampled by the admission's prefill and counted at the status read that follows it).
 
-``--paragraphs N`` prints only one JSON line: N split-text paragraphs on the open engine (see ``run_paragraphs``).
+``--paragraphs N`` prints only one JSON line: N split-text paragraphs on the open engine (see ``run_paragraphs``);
+with ``--refine`` every sentence is refined first, against ``Chat.infer``'s default mode (``run_paragraphs_refine``).
 
 ``--stream`` then prints a second JSON line: the same requests streamed as audio (hidden path, DVAE decoder and Vocos
 from synthetic weights, InferCodeParams' default stream_batch / stream_speed / pass_first_n_batches), timed
@@ -729,6 +730,114 @@ def run_paragraphs(args, local_rank: int = 0):
     return line
 
 
+def run_paragraphs_refine(args, local_rank: int = 0):
+    """``--paragraphs N --refine``: the paragraphs of ``run_paragraphs``, each sentence refined first (seeded, forced to
+    one seeded length of 16..48 tokens per paragraph).  Arms, alternated, ``--steps`` repeats each: (a)
+    ``ChatEngine.submit(split_text=True, skip_refine_text=False, max_split_batch=4, stream=True)`` on one open engine
+    of S slots; (b) ``Chat.infer(paragraph, stream=True)`` with its default arguments (the same refinement and batches
+    of 4 sentences), one paragraph after another.  Per arm (median repeat by wall time): wall time, first- and
+    last-chunk latency per paragraph, and the host time spent building seeded Exp(1) noise (``exp_noise``)."""
+    import threading
+
+    import numpy as np
+
+    import chattts_b200.engine as engine_mod
+    import chattts_b200.gpt as gpt_mod
+    from chattts_b200 import Chat
+    from chattts_b200.core import split_sentences
+    from chattts_b200.speaker import Speaker
+    from chattts_b200.synth import synth_all
+
+    dev = torch.device("cuda", local_rank)
+    torch.cuda.set_device(dev)
+    S, n = args.slots, args.paragraphs
+    g = np.random.default_rng(31)
+    texts, lengths, rlengths = [], [], []
+    for k in range(n):
+        m = int(g.integers(2, 7))
+        texts.append(" ".join(f"sentence {j} of paragraph {k} says something." for j in range(m)))
+        lengths.append(int(g.integers(48, 257)))
+        rlengths.append(int(g.integers(16, 49)))
+    c = Chat()
+    assert c.load_states(synth_all(0), tokenizer=_CharTokenizer(), speaker=Speaker(768, None), device=dev,
+                         max_batch=S, max_context=1024)
+    noise_s = [0.0]
+
+    def timed_noise(fn):
+        def call(*a, **kw):
+            t = time.perf_counter()
+            out = fn(*a, **kw)
+            noise_s[0] += time.perf_counter() - t
+            return out
+        return call
+
+    def params(k):
+        return c.InferCodeParams(manual_seed=900 + k, max_new_token=lengths[k], min_new_token=lengths[k],
+                                 show_tqdm=False)
+
+    def refine(k):
+        return c.RefineTextParams(manual_seed=500 + k, max_new_token=rlengths[k], min_new_token=rlengths[k],
+                                  show_tqdm=False)
+
+    def engine_arm():
+        times = {k: [] for k in range(n)}
+        t0 = time.perf_counter()
+        cap = max(max(lengths), max(rlengths))
+        with c.open_engine(slots=S, max_new_cap=cap) as eng:
+            jobs = [eng.submit(t, params_infer_code=params(k), stream=True, split_text=True, skip_refine_text=False,
+                               params_refine_text=refine(k), max_split_batch=4) for k, t in enumerate(texts)]
+            threads = []
+            for k, job in enumerate(jobs):
+                def consume(k=k, job=job):
+                    for ch, _ in job:
+                        if ch.shape[1]:
+                            times[k].append(time.perf_counter() - t0)
+                threads.append(threading.Thread(target=consume))
+                threads[-1].start()
+            for th in threads:
+                th.join()
+        return times, time.perf_counter() - t0
+
+    def infer_arm():
+        times = {k: [] for k in range(n)}
+        t0 = time.perf_counter()
+        for k, t in enumerate(texts):
+            for ch in c.infer(t, stream=True, params_refine_text=refine(k), params_infer_code=params(k)):
+                if ch.shape[1]:
+                    times[k].append(time.perf_counter() - t0)
+        return times, time.perf_counter() - t0
+
+    def run(arm, module):
+        real = module.exp_noise
+        module.exp_noise = timed_noise(real)
+        noise_s[0] = 0.0
+        try:
+            times, wall = arm()
+        finally:
+            module.exp_noise = real
+        q = lambda v: {"p50": round(float(np.percentile(v, 50)), 4), "p95": round(float(np.percentile(v, 95)), 4),
+                       "max": round(float(max(v)), 4)}  # noqa: E731
+        return {"wall_s": round(wall, 3), "first_chunk_s": q([t[0] for t in times.values() if t]),
+                "last_chunk_s": q([t[-1] for t in times.values() if t]), "noise_s": round(noise_s[0], 4)}
+
+    for _ in range(max(1, args.warmup)):
+        run(engine_arm, engine_mod)
+        run(infer_arm, gpt_mod)
+    runs = {"a": [], "b": []}
+    for _ in range(args.steps):
+        runs["a"].append(run(engine_arm, engine_mod))
+        runs["b"].append(run(infer_arm, gpt_mod))
+    name, limit = gpu_card(local_rank)
+    line = {"metric": "continuous_paragraphs_refine", "card": name, "power_limit": limit, "paragraphs": n,
+            "slots": S, "sentences": sum(len(split_sentences(t)) for t in texts),
+            "forced_tokens": [min(lengths), max(lengths)], "forced_refine_tokens": [min(rlengths), max(rlengths)],
+            "max_split_batch": 4, "repeats": args.steps}
+    for arm, rs in runs.items():
+        line[arm] = sorted(rs, key=lambda x: x["wall_s"])[len(rs) // 2]
+        line[arm]["wall_all_s"] = [x["wall_s"] for x in rs]
+    return line
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--requests", type=int, default=128)
@@ -737,7 +846,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--dump-outputs", default=None, metavar="DIR")
     ap.add_argument("--stream", action="store_true", help="also measure streamed audio (a second JSON line)")
-    ap.add_argument("--refine", action="store_true", help="also measure refinement + speech (one more JSON line)")
+    ap.add_argument("--refine", action="store_true", help="also measure refinement + speech (one more JSON line); "
+                    "with --paragraphs: refine every sentence (the paragraphs line of run_paragraphs_refine)")
     ap.add_argument("--online", default=None, metavar="RATE[,RATE...]",
                     help="also measure streamed requests arriving at these rates (requests/s; one JSON line each)")
     ap.add_argument("--cancel", type=float, default=None, metavar="FRACTION",
@@ -749,7 +859,8 @@ def main():
         ap.error("--steps must be >= 1")
     rank = int(os.environ.get("LOCAL_RANK", "0"))
     if args.paragraphs:
-        print(json.dumps(run_paragraphs(args, rank)), flush=True)
+        run = run_paragraphs_refine if args.refine else run_paragraphs
+        print(json.dumps(run(args, rank)), flush=True)
         return
     print(json.dumps(run_continuous(args, rank)), flush=True)
     if args.stream:
