@@ -48,8 +48,7 @@ constexpr int FL_A_X = 0;                                       // [BMAX][768]  
 constexpr int FL_A_XO = FL_A_X + FL_BMAX * KC;                  // [BMAX][768]  residual stream after O-proj
 constexpr int FL_A_ACT = FL_A_XO + FL_BMAX * KC;                // [BMAX][3072] silu(gate) * up
 constexpr int FL_A_P = FL_A_ACT + FL_BMAX * 4 * KC;             // [BMAX][12][SMAX][66] attention partials
-constexpr int FL_A_AO = FL_A_P + FL_BMAX * FL_HEADS * FL_SMAX * FL_PW;  // [BMAX][768] merged attention output
-constexpr int FL_A_END = FL_A_AO + FL_BMAX * KC;
+constexpr int FL_A_END = FL_A_P + FL_BMAX * FL_HEADS * FL_SMAX * FL_PW;
 constexpr int FL_REP_STRIDE = ((FL_A_END + 1023) / 1024) * 1024;
 constexpr int FL_A_Q = 0, FL_A_KN = FL_BMAX * KC, FL_A_VN = 2 * FL_BMAX * KC;
 constexpr int FL_QKV_WORDS = 3 * FL_BMAX * KC;
@@ -60,8 +59,11 @@ constexpr int FL_TAIL_WORDS = FL_A_IDX + 64;
 constexpr size_t FL_PARITY_WORDS = (size_t)FL_RMAX * FL_REP_STRIDE + FL_TAIL_WORDS;
 constexpr size_t FL_ARENA_WORDS = 2 * FL_PARITY_WORDS;
 constexpr unsigned FL_EPOCH_STEP = 256;  // tags of one launch: base + 8 * layer + kind
+// CTB_MEGA_TRACE buffer (words): CTA 0's phase stamps and cycle probes below FL_TR_EV, then FL_TR_EVN per-CTA event
+// stamps of one layer for each of up to 192 CTAs (the grids k_flow runs on)
+constexpr int FL_TR_EV = 4096, FL_TR_EVN = 32, FL_TR_WORDS = FL_TR_EV + 192 * FL_TR_EVN;
 
-enum FlowTagKind { FT_X = 0, FT_QKV = 1, FT_P = 2, FT_XO = 3, FT_ACT = 4, FT_LOGITS = 5, FT_IDX = 6, FT_AO = 7 };
+enum FlowTagKind { FT_X = 0, FT_QKV = 1, FT_P = 2, FT_XO = 3, FT_ACT = 4, FT_LOGITS = 5, FT_IDX = 6 };
 enum FlowStage { FS_Q0 = 0, FS_Q1 = 1, FS_KV = 2, FS_O = 3, FS_GU0 = 4, FS_GU1 = 5, FS_GU2 = 6, FS_D0 = 7, FS_D1 = 8, FS_NLAYER = 9 };
 
 // barrier among the 8 consumer warps only (the loader warp never joins it)
@@ -356,8 +358,7 @@ __device__ __forceinline__ void fl_refill_all(const FlowP& p, FlowW& w) {
 // ---------------------------------------------------------------- phase helpers
 // Poll p.B x 768 LL words into xs (raw), zero rows >= B, block barrier.
 template <int BT>
-__device__ __forceinline__ void fl_stage768(const FlowP& p, const unsigned long long* src, uint32_t tag, float* xs, FlowWd& wd, FlowW& fw,
-                                            const int* rowmask = nullptr) {
+__device__ __forceinline__ void fl_stage768(const FlowP& p, const unsigned long long* src, uint32_t tag, float* xs, FlowWd& wd, FlowW& fw) {
   const int tid = threadIdx.x;
   unsigned long long v[BT][3];
   wd.spins = 0;
@@ -365,13 +366,13 @@ __device__ __forceinline__ void fl_stage768(const FlowP& p, const unsigned long 
     bool ok = true;
 #pragma unroll
     for (int b = 0; b < BT; ++b)
-      if (b < p.B && (rowmask == nullptr || rowmask[b])) {
+      if (b < p.B) {
 #pragma unroll
         for (int k = 0; k < 3; ++k) v[b][k] = ll_ld(src + b * KC + tid + 256 * k);
       }
 #pragma unroll
     for (int b = 0; b < BT; ++b)
-      if (b < p.B && (rowmask == nullptr || rowmask[b])) {
+      if (b < p.B) {
 #pragma unroll
         for (int k = 0; k < 3; ++k) ok = ok && (ll_tag(v[b][k]) == tag);
       }
@@ -381,8 +382,91 @@ __device__ __forceinline__ void fl_stage768(const FlowP& p, const unsigned long 
 #pragma unroll
   for (int b = 0; b < BT; ++b) {
 #pragma unroll
-    for (int k = 0; k < 3; ++k) xs[b * KC + tid + 256 * k] = (b < p.B && (rowmask == nullptr || rowmask[b])) ? ll_val(v[b][k]) : 0.f;
+    for (int k = 0; k < 3; ++k) xs[b * KC + tid + 256 * k] = b < p.B ? ll_val(v[b][k]) : 0.f;
   }
+  fl_bar();
+}
+
+// Stage the attention output of the p.B rows into xs, merging the ns = min(chunks, S) split partials of every
+// (row, head) with k_step's expressions in k_step's order (s = 0 .. ns-1): every CTA computes the same bits.  Rows
+// without attention units (inactive prompt columns) get 0.  Block barrier at the end.
+//
+// The elements tid + 256 k (k < 3) of a warp belong to three heads, (warp >> 1) + 4 k, so every warp stages on its
+// own.  The partials are 12 * ns * 66 words per row: spinning on all of them would load L2 several times as hard as
+// staging 768 merged words.  Lane k * FL_SMAX + s spins on the {m, l} pair of split s of the warp's head k only; the
+// merge weights go lane to lane by shuffles, and the o words are read once the pairs are in and re-read only if a
+// tag is stale (they are stored by other producer threads than m / l, so every word is checked).
+template <int BT>
+__device__ __forceinline__ void fl_stage_attn(const FlowP& p, const unsigned long long* P, uint32_t tag, float* xs, FlowWd& wd, int S,
+                                              const int* s_pos, const int* s_active) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int pk = lane / FL_SMAX, ps = lane % FL_SMAX, pbase = min(pk, 2) * FL_SMAX;
+#pragma unroll 1
+  for (int b = 0; b < BT; ++b) {
+    if (b >= p.B) break;
+    float v[3] = {0.f, 0.f, 0.f};
+    if (s_active[b]) {
+      const int ns = min((s_pos[b] + FL_CH) / FL_CH, S);
+      const unsigned long long* Pb = P + (size_t)b * FL_HEADS * FL_SMAX * FL_PW + (size_t)(warp >> 1) * FL_SMAX * FL_PW;
+      const bool pl = pk < 3 && ps < ns;
+      float m = -INFINITY, lv = 0.f;
+      wd.spins = 0;
+      while (true) {
+        bool ok = true;
+        if (pl) {
+          unsigned long long w1, w2;
+          ll_ld2(Pb + (size_t)(4 * pk * FL_SMAX + ps) * FL_PW + 64, w1, w2);
+          ok = ll_tag(w1) == tag && ll_tag(w2) == tag;
+          m = ll_val(w1); lv = ll_val(w2);
+        }
+        if (__all_sync(0xffffffffu, ok)) break;
+        if (__any_sync(0xffffffffu, fl_giveup(wd, 0x400))) { wd.dead = 1; break; }
+      }
+      float GM = -INFINITY;  // of this lane's head
+#pragma unroll
+      for (int s = 0; s < FL_SMAX; ++s) {
+        const float ms = __shfl_sync(0xffffffffu, m, pbase + s);
+        if (s < ns) GM = fmaxf(GM, ms);
+      }
+      const float wgt = pl ? expf(m - GM) : 0.f;
+      unsigned long long w[3][FL_SMAX];
+      while (true) {
+        bool ok = true;
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+#pragma unroll
+          for (int s = 0; s < FL_SMAX; ++s)
+            if (s < ns) w[k][s] = ll_ld(Pb + (size_t)(4 * k * FL_SMAX + s) * FL_PW + (tid & 63));
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+#pragma unroll
+          for (int s = 0; s < FL_SMAX; ++s)
+            if (s < ns) ok = ok && ll_tag(w[k][s]) == tag;
+        if (__all_sync(0xffffffffu, ok)) break;
+        if (__any_sync(0xffffffffu, fl_giveup(wd, 0x401))) { wd.dead = 1; break; }
+      }
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        float GL = 0.f, GO = 0.f;
+#pragma unroll
+        for (int s = 0; s < FL_SMAX; ++s) {
+          const float ws = __shfl_sync(0xffffffffu, wgt, k * FL_SMAX + s);
+          const float ls = __shfl_sync(0xffffffffu, lv, k * FL_SMAX + s);
+          if (s < ns) {
+            GL = fmaf(ws, ls, GL);
+            GO = fmaf(ws, ll_val(w[k][s]), GO);
+          }
+        }
+        v[k] = GO / GL;
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) xs[b * KC + tid + 256 * k] = v[k];
+  }
+#pragma unroll
+  for (int b = 0; b < BT; ++b)
+    if (b >= p.B)
+      for (int k = 0; k < 3; ++k) xs[b * KC + tid + 256 * k] = 0.f;
   fl_bar();
 }
 
@@ -635,7 +719,8 @@ __device__ __noinline__ int fl_sample_row(const ctb_sampler_config& c, const flo
   const int kk = c.top_k > 0 ? min(max(c.top_k, c.min_tokens_to_keep), V) : 0;
   const int min_keep = min(c.min_tokens_to_keep, V);
   uint32_t thr_key = 0;
-  if (use_p || kk > 0) {
+  // greedy replaces thr_key by the arg-max key below, so the top-p / top-k threshold is dead work there (uniform branch)
+  if (!c.greedy && (use_p || kk > 0)) {
     double den = 0.0;
     if (use_p) {
       double dv[4];
@@ -786,8 +871,8 @@ __global__ void __launch_bounds__(FL_THREADS, 1) k_flow(const __grid_constant__ 
   uint32_t base = (uint32_t)ldg_cg(reinterpret_cast<const int*>(p.epoch));
   int tr = 0;
 #define FL_TRACE() do { if (p.trace && blockIdx.x == 0 && tid == 0 && tr < 250) p.trace[tr++] = globaltimer_ns(); } while (0)
-  // per-CTA event stamps of one layer (profiling aid; trace[256 + cta * 16 + k])
-#define FL_EV(k) do { if (p.trace && l == 10 && tid == 0) p.trace[256 + blockIdx.x * 16 + (k)] = globaltimer_ns(); } while (0)
+  // per-CTA event stamps of one layer (profiling aid; trace[FL_TR_EV + cta * FL_TR_EVN + k], read by tools/flow_trace.py)
+#define FL_EV(k) do { if (p.trace && l == 10 && tid == 0) p.trace[FL_TR_EV + blockIdx.x * FL_TR_EVN + (k)] = globaltimer_ns(); } while (0)
   // cycle stamps inside the gate/up phase of CTA 0 / warp 0 (profiling aid; trace[3000 + k])
 #define FL_CK(k) do { if (p.trace && l == 10 && tid == 0 && blockIdx.x == 0) p.trace[3000 + (k)] = (unsigned long long)clock64(); } while (0)
 
@@ -1103,52 +1188,18 @@ __global__ void __launch_bounds__(FL_THREADS, 1) k_flow(const __grid_constant__ 
             M = cm;
           }
         }
-        // The splits of a (row, head) meet at the split-0 unit, which publishes the merged 64 outputs: the O-proj phase of
-        // all CTAs then stages 768 words per row instead of every CTA reading (and merging) every partial.
-        const int ns_u = min(g.u_nchunk, g.S);
+        // Every unit publishes its partial; the O-proj phase of every CTA merges the splits of a (row, head) itself while
+        // it stages its input (fl_stage_attn), so the partials cross CTAs once instead of meeting at a split-0 unit first.
+        FL_EV(14);
         if (tid < 64) {
-          unsigned long long* P = par + FL_A_P + ((size_t)(b * FL_HEADS + h) * FL_SMAX) * FL_PW;  // replica 0 only
-          float v = 0.f;
-          if (ns_u > 1 && g.u_split > 0) {
-            ll_st(P + (size_t)g.u_split * FL_PW + tid, O, tagl + FT_P);
-            if (tid == 0) { ll_st(P + (size_t)g.u_split * FL_PW + 64, M, tagl + FT_P); ll_st(P + (size_t)g.u_split * FL_PW + 65, L, tagl + FT_P); }
-          } else {
-            // split 0 (or the only split): same expressions and order as k_step's merge (s = 0 .. ns-1)
-            float om[FL_SMAX], mm[FL_SMAX], lm[FL_SMAX];
-            om[0] = O; mm[0] = M; lm[0] = L;
-            if (ns_u > 1) {
-              wd.spins = 0;
-              while (true) {
-                bool ok = true;
-#pragma unroll
-                for (int sp = 1; sp < FL_SMAX; ++sp)
-                  if (sp < ns_u) {
-                    const unsigned long long w0 = ll_ld(P + (size_t)sp * FL_PW + tid);
-                    unsigned long long w1, w2;
-                    ll_ld2(P + (size_t)sp * FL_PW + 64, w1, w2);
-                    ok = ok && ll_tag(w0) == tagl + FT_P && ll_tag(w1) == tagl + FT_P && ll_tag(w2) == tagl + FT_P;
-                    om[sp] = ll_val(w0); mm[sp] = ll_val(w1); lm[sp] = ll_val(w2);
-                  }
-                if (__all_sync(0xffffffffu, ok)) break;
-                if (__any_sync(0xffffffffu, fl_giveup(wd, 0x400))) { wd.dead = 1; break; }
-              }
-            }
-            float GM = -INFINITY;
-#pragma unroll
-            for (int sp = 0; sp < FL_SMAX; ++sp)
-              if (sp < ns_u) GM = fmaxf(GM, mm[sp]);
-            float GL = 0.f, GO = 0.f;
-#pragma unroll
-            for (int sp = 0; sp < FL_SMAX; ++sp)
-              if (sp < ns_u) {
-                const float w = expf(mm[sp] - GM);
-                GL = fmaf(w, lm[sp], GL);
-                GO = fmaf(w, om[sp], GO);
-              }
-            v = GO / GL;
-            for (int r = 0; r < R; ++r) ll_st(par + (size_t)r * FL_REP_STRIDE + FL_A_AO + (size_t)b * KC + h * 64 + tid, v, tagl + FT_AO);
+          unsigned long long* P = par + FL_A_P + ((size_t)(b * FL_HEADS + h) * FL_SMAX + g.u_split) * FL_PW;
+          for (int r = 0; r < R; ++r) {
+            unsigned long long* Pr = P + (size_t)r * FL_REP_STRIDE;
+            ll_st(Pr + tid, O, tagl + FT_P);
+            if (tid == 0) { ll_st(Pr + 64, M, tagl + FT_P); ll_st(Pr + 65, L, tagl + FT_P); }
           }
         }
+        FL_EV(15);
         if (pend_kv) fl_ring_release(p, fw);
       }
       FL_TRACE();
@@ -1158,7 +1209,7 @@ __global__ void __launch_bounds__(FL_THREADS, 1) k_flow(const __grid_constant__ 
       fl_bar();  // xs (raw x) is no longer read by any warp of this CTA
       if (l + 1 < p.L || p.sample) fl_nw_fetch(s_nw1, l + 1 < p.L ? Wl + p.layer_stride + p.o_ln1 : p.W + p.o_final_norm, &s_nwbar[0], pol_w);
       const bool o_rdy = fl_o_valid(g) ? fl_ring_peek_n(p, fw, 1) : true;
-      fl_stage768<BT>(p, myr + FL_A_AO, tagl + FT_AO, xs, wd, fw, s_active);
+      fl_stage_attn<BT>(p, myr + FL_A_P, tagl + FT_P, xs, wd, g.S, s_pos, s_active);
       fl_refill_all(p, fw);
       FL_EV(6);
       if (fl_o_valid(g)) {
@@ -1209,6 +1260,7 @@ __global__ void __launch_bounds__(FL_THREADS, 1) k_flow(const __grid_constant__ 
 #pragma unroll
         for (int j = 0; j < FL_GU; ++j) sl[j] = reinterpret_cast<const float4*>(fl_ring_slot_at(fw, j)) + lane;
         if (!gu_rdy) fl_ring_wait_n(p, fw, ngu, wd);
+        FL_EV(16);
         FL_CK(1);
         float acc[8 * BT];
 #pragma unroll
@@ -1309,6 +1361,7 @@ __global__ void __launch_bounds__(FL_THREADS, 1) k_flow(const __grid_constant__ 
         const float* s0 = fl_ring_slot_at(fw, 0);
         const float* s1 = nr1 > 0 ? fl_ring_slot_at(fw, 1) : s0;
         if (!d_rdy) fl_ring_wait_n(p, fw, nr1 > 0 ? 2 : 1, wd);
+        FL_EV(17);
         float acc[8 * BT];
 #pragma unroll
         for (int k = 0; k < 8 * BT; ++k) acc[k] = 0.f;

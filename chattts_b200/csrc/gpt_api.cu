@@ -299,7 +299,7 @@ extern "C" int ctb_gpt_create(const ctb_gpt_config* c, const float* weights_dev,
   TRY(dalloc(&h->finish, Bp));
   TRY(dalloc(&h->st, 1));
   TRY(dalloc(&h->bar, 4));
-  if (getenv("CTB_MEGA_TRACE")) TRY(dalloc(&h->trace, 4096));
+  if (getenv("CTB_MEGA_TRACE")) TRY(dalloc(&h->trace, FL_TR_WORDS));
   h->flow_ok = getenv("CTB_NO_FLOW") == nullptr && g_num_sms >= 128 && g_num_sms <= 191 && c->intermediate_size == 4 * KC &&
                c->num_heads == c->num_kv_heads && c->num_heads * c->head_dim == KC && c->num_heads <= FL_HEADS;
   if (h->flow_ok) {
@@ -1227,7 +1227,7 @@ extern "C" int ctb_gpt_embed_prompt(ctb_gpt* h, const int64_t* ids_dev, const ui
 
 extern "C" int ctb_gpt_debug_trace(ctb_gpt* h, unsigned long long* host_out, int n) {
   if (!h || !h->trace) return set_err(CTB_ERR_STATE, "trace disabled (set CTB_MEGA_TRACE=1 before ctb_gpt_create)");
-  CTB_CUDA(cudaMemcpy(host_out, h->trace, sizeof(unsigned long long) * (size_t)std::min(n, 4096), cudaMemcpyDeviceToHost));
+  CTB_CUDA(cudaMemcpy(host_out, h->trace, sizeof(unsigned long long) * (size_t)std::min(n, FL_TR_WORDS), cudaMemcpyDeviceToHost));
   return CTB_OK;
 }
 

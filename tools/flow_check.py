@@ -132,10 +132,12 @@ def main():
           f" layer={sum(avg):.0f}  heads={t[101] - t[100]}  total={t[101] - t[0]}", flush=True)
     print("layer0:", per[0], "layer1:", per[1], flush=True)
     # per-CTA event stamps of layer 10 (see FL_EV in flow.cuh)
-    buf2 = (C.c_ulonglong * 4096)()
-    _lib.check(lib.ctb_gpt_debug_trace(tr._handle, buf2, 4096))
+    from flow_trace import flow_consts
+    _, ev0, evn, words = flow_consts()
+    buf2 = (C.c_ulonglong * words)()
+    _lib.check(lib.ctb_gpt_debug_trace(tr._handle, buf2, words))
     import numpy as np
-    ev = np.array([[buf2[256 + c * 16 + k] for k in range(14)] for c in range(148)], dtype=np.int64)
+    ev = np.array([[buf2[ev0 + c * evn + k] for k in range(14)] for c in range(132)], dtype=np.int64)
     t0 = ev[:, 0].min()
     names = ["A.start", "X.staged", "Q.slot", "A.end", "q.arrived", "B.end", "C.merged", "O.slot", "C.end", "XO.staged",
              "D.end", "ACT.polled", "E.partial", "E.end"]
@@ -153,7 +155,7 @@ def main():
         int(buf2[3013]) - int(buf2[3012]), int(buf2[3014]) - int(buf2[3013]), int(buf2[3015]), int(buf2[3016])))
     print("  CTA 0:", (ev[0] - t0).tolist())
     print("  CTA 100:", (ev[100] - t0).tolist())
-    print("  CTA 147:", (ev[147] - t0).tolist(), flush=True)
+    print("  CTA 131:", (ev[131] - t0).tolist(), flush=True)
 
 
 if __name__ == "__main__":
