@@ -42,6 +42,22 @@ class GptStatus(C.Structure):
                 ("any_finished_first_step", C.c_int32), ("reserved", C.c_int32)]
 
 
+#: precision flags of ctb_gpt_engine_begin_ex (CTB_ENGINE_FP16_* in the header)
+ENGINE_FP16_WEIGHTS, ENGINE_FP16_KV = 1, 2
+
+
+def engine_flags(dtype) -> int:
+    """The ctb_gpt_engine_begin_ex flags of a slot engine's ``dtype``: torch.float32 (0) or torch.float16 (fp16 layer
+    weights and KV cache).  Anything else raises ValueError; nothing touches the device."""
+    import torch
+
+    if dtype is None or dtype == torch.float32:
+        return 0
+    if dtype == torch.float16:
+        return ENGINE_FP16_WEIGHTS | ENGINE_FP16_KV
+    raise ValueError(f"slot engine dtype must be torch.float32 or torch.float16, not {dtype!r}")
+
+
 #: slot states reported by ctb_gpt_engine_status (CTB_SLOT_* in the header)
 SLOT_IDLE, SLOT_RUNNING, SLOT_FINISHED = 0, 1, 2
 
@@ -62,7 +78,7 @@ EXPORTS = (
     "ctb_abi_version", "ctb_last_error", "ctb_launch_count", "ctb_gpt_layout_query", "ctb_gpt_create",
     "ctb_gpt_destroy", "ctb_gpt_begin", "ctb_gpt_decode", "ctb_gpt_status_query", "ctb_gpt_profile_kernel", "ctb_gpt_debug_trace", "ctb_gpt_embed_prompt", "ctb_sample",
     "ctb_gpt_engine_begin", "ctb_gpt_engine_admit", "ctb_gpt_engine_admit_text", "ctb_gpt_engine_status",
-    "ctb_gpt_engine_cancel",
+    "ctb_gpt_engine_cancel", "ctb_gpt_engine_begin_ex",
     "ctb_dvae_blob_floats", "ctb_vocos_blob_floats", "ctb_decoder_create", "ctb_decoder_destroy",
     "ctb_dvae_decode", "ctb_vocos_decode", "ctb_decode_rows",
     "ctb_dvae_encoder_blob_floats", "ctb_dvae_encoder_create", "ctb_dvae_encoder_destroy", "ctb_dvae_encode",
@@ -110,6 +126,7 @@ def load(build_if_missing: bool = True):
         lib.ctb_gpt_debug_trace.argtypes = [vp, vp, i32]
         lib.ctb_gpt_embed_prompt.argtypes = [vp, vp, vp, i32, i32, vp, vp]
         lib.ctb_gpt_engine_begin.argtypes = [vp, i32, i32, vp, vp, vp]
+        lib.ctb_gpt_engine_begin_ex.argtypes = [vp, i32, i32, i32, vp, vp, vp]
         lib.ctb_gpt_engine_admit.argtypes = [vp, i32, vp, i32, vp, vp, C.POINTER(SamplerConfig), vp, vp, vp]
         lib.ctb_gpt_engine_admit_text.argtypes = lib.ctb_gpt_engine_admit.argtypes
         lib.ctb_gpt_engine_status.argtypes = [vp, C.POINTER(GptStatus), vp, vp, vp, vp]

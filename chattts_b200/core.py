@@ -212,7 +212,8 @@ class Chat:
 
     def infer_continuous(self, texts, params_infer_code=None, use_decoder=True, slots=None, stream=False, lang=None,
                          skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
-                         params_refine_text=None, refine_on_engine=False, split_text=False, max_split_batch=1):
+                         params_refine_text=None, refine_on_engine=False, split_text=False, max_split_batch=1,
+                         dtype=torch.float32):
         """Synthesise many texts with continuous batching (``GPT.generate_continuous``): each text is one request,
         ``params_infer_code`` is one ``InferCodeParams`` for all texts or a list with one per text (speaker, seed,
         temperature, top-P/K, penalty, token limits).  Generator of ``(index, wav)`` in completion order; ``wav`` is
@@ -233,7 +234,12 @@ class Chat:
         modified; with ``skip_refine_text=False`` each sentence is refined on the engine first, and ``wav`` is what
         ``infer(texts[index], max_split_batch=max_split_batch, params_refine_text=...)[0]`` returns (seeded: bit for
         bit on the code path).  The paragraphs run on an open engine (``open_engine``); ``slots`` defaults to the
-        handle's ``max_batch``."""
+        handle's ``max_batch``.
+
+        ``dtype=torch.float16`` runs every request on a half-precision engine (``GPT.generate_continuous``): fp16
+        layer weights and KV cache, as the reference's ``use_vllm=True`` serves; the waveforms then follow that model.
+        Path 2 (DVAE / Vocos) is unchanged."""
+        _lib.engine_flags(dtype)  # an unsupported dtype raises here, before any device work
         if stream:
             raise ValueError("infer_continuous: stream=True is not supported; each waveform is yielded when complete "
                              "(infer_continuous_stream streams)")
@@ -241,14 +247,15 @@ class Chat:
         if split_text:
             return self._paragraphs(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
                                     do_homophone_replacement, False, self._refine_params(texts, params_refine_text),
-                                    max_split_batch)
+                                    max_split_batch, dtype)
         return self._infer_continuous(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
                                       do_homophone_replacement, self._refine_params(texts, params_refine_text),
-                                      refine_on_engine)
+                                      refine_on_engine, dtype)
 
     def infer_continuous_stream(self, texts, params_infer_code=None, use_decoder=True, slots=None, lang=None,
                                 skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
-                                params_refine_text=None, refine_on_engine=False, split_text=False, max_split_batch=1):
+                                params_refine_text=None, refine_on_engine=False, split_text=False, max_split_batch=1,
+                                dtype=torch.float32):
         """Streaming synthesis of many texts with continuous batching (``GPT.generate_continuous_stream``).
         Generator of ``(index, chunk, last)``, ``chunk`` a ``[1, n]`` float32 array; for each text the chunks are
         those ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=True)`` yields with that
@@ -258,22 +265,25 @@ class Chat:
         buffers.  Arguments as for ``infer_continuous``; with ``refine_on_engine=True`` the chunks are those of
         ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=False)``.  With ``split_text=True``
         each text is a paragraph, streamed sentence by sentence as ``ChatEngine.submit(split_text=True,
-        stream=True)`` streams it, refined first with ``skip_refine_text=False``."""
+        stream=True)`` streams it, refined first with ``skip_refine_text=False``.  ``dtype`` as in
+        ``infer_continuous``."""
+        flags = _lib.engine_flags(dtype)
         texts, params = self._continuous_params(texts, params_infer_code)
         if split_text:
             return self._paragraphs(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
                                     do_homophone_replacement, True, self._refine_params(texts, params_refine_text),
-                                    max_split_batch)
+                                    max_split_batch, dtype)
         return self._infer_continuous_stream(texts, params, use_decoder, slots, lang, skip_refine_text,
                                              do_text_normalization, do_homophone_replacement,
-                                             self._refine_params(texts, params_refine_text), refine_on_engine)
+                                             self._refine_params(texts, params_refine_text), refine_on_engine, flags)
 
     def refine_continuous(self, texts, params_refine_text=None, slots=None, lang=None, do_text_normalization=True,
-                          do_homophone_replacement=True):
+                          do_homophone_replacement=True, dtype=torch.float32):
         """Refine many texts on the slot engine, each as a request of its own: generator of ``(index, refined_text)``
         in completion order.  ``refined_text`` is what ``infer([texts[index]], refine_text_only=True,
         split_text=False, params_refine_text=...)[0]`` returns for that text; ``params_refine_text`` is one
-        ``RefineTextParams`` or one per text."""
+        ``RefineTextParams`` or one per text.  ``dtype`` as in ``infer_continuous``."""
+        _lib.engine_flags(dtype)
         if isinstance(texts, str):
             texts = [texts]
         texts = list(texts)
@@ -284,7 +294,8 @@ class Chat:
             return
         texts = [self.normalizer(t, do_text_normalization, do_homophone_replacement, lang) for t in texts]
         requests = [self._refine_request(t, r) for t, r in zip(texts, refine)]
-        for i, out in self.gpt.generate_continuous(requests, slots=slots, return_hidden=False, context=self.context):
+        for i, out in self.gpt.generate_continuous(requests, slots=slots, return_hidden=False, context=self.context,
+                                                   dtype=dtype):
             yield i, self._refined_text(out)
 
     @staticmethod
@@ -307,7 +318,7 @@ class Chat:
         return [params_refine_text or Chat.RefineTextParams()] * len(texts)
 
     def _paragraphs(self, texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
-                    do_homophone_replacement, stream, refine, max_split_batch):
+                    do_homophone_replacement, stream, refine, max_split_batch, dtype=torch.float32):
         """``infer_continuous*(split_text=True)``: every text a paragraph job on one open engine, submitted in order.
         Generator of ``(index, wav)`` in completion order, or of ``(index, chunk, last)`` as the chunks come."""
         assert self.has_loaded(use_decoder=use_decoder)
@@ -318,7 +329,7 @@ class Chat:
         cap = max(p.max_new_token for p in params)
         if not skip_refine_text:
             cap = max(cap, max(r.max_new_token for r in refine))
-        with self.open_engine(slots, max_new_cap=cap, use_decoder=use_decoder) as eng:
+        with self.open_engine(slots, max_new_cap=cap, use_decoder=use_decoder, dtype=dtype) as eng:
             try:
                 jobs = [eng.submit(t, params_infer_code=p, stream=stream, lang=lang, split_text=True,
                                    skip_refine_text=skip_refine_text, params_refine_text=r,
@@ -375,7 +386,8 @@ class Chat:
         return [self._code_request(t, p) for t, p in zip(texts, params)], cap
 
     def _infer_continuous_stream(self, texts, params, use_decoder, slots, lang, skip_refine_text,
-                                 do_text_normalization, do_homophone_replacement, refine, refine_on_engine=False):
+                                 do_text_normalization, do_homophone_replacement, refine, refine_on_engine=False,
+                                 flags=0):
         requests, cap = self._continuous_requests(texts, params, use_decoder, lang, skip_refine_text,
                                                   do_text_normalization, do_homophone_replacement, refine,
                                                   refine_on_engine)
@@ -383,10 +395,10 @@ class Chat:
             return
         windows = [StreamWindows(p.stream_speed, p.pass_first_n_batches) for p in params]
         yield from stream_continuous(self.gpt, self.decoder if use_decoder else self.dvae, requests, windows,
-                                     use_decoder, slots, self.context, max_new_cap=cap)
+                                     use_decoder, slots, self.context, max_new_cap=cap, flags=flags)
 
     def _infer_continuous(self, texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
-                          do_homophone_replacement, refine, refine_on_engine=False):
+                          do_homophone_replacement, refine, refine_on_engine=False, dtype=torch.float32):
         requests, cap = self._continuous_requests(texts, params, use_decoder, lang, skip_refine_text,
                                                   do_text_normalization, do_homophone_replacement, refine,
                                                   refine_on_engine)
@@ -395,7 +407,7 @@ class Chat:
         thr = np.float32(1e-5)
         with torch.no_grad():
             for i, out in self.gpt.generate_continuous(requests, slots=slots, return_hidden=use_decoder,
-                                                       context=self.context, max_new_cap=cap):
+                                                       context=self.context, max_new_cap=cap, dtype=dtype):
                 k = _text_index(self.gpt, requests, i)
                 if k is None:  # a refinement stage: its follow-up carries the text on
                     out.destroy()
@@ -458,15 +470,18 @@ class Chat:
         ids = out.ids[0]
         return self.tokenizer.decode([ids[ids.less(self.tokenizer.break_0_ids)]])[0]
 
-    def open_engine(self, slots: Optional[int] = None, max_new_cap: int = 2048, use_decoder: bool = True):
+    def open_engine(self, slots: Optional[int] = None, max_new_cap: int = 2048, use_decoder: bool = True,
+                    dtype=torch.float32):
         """A long-lived slot engine (``GPT.open_engine``) that synthesises texts submitted from any thread while it
         decodes: ``engine.submit(text, params_infer_code=None, stream=False, skip_refine_text=True, ...) -> Job``,
         ``Job.cancel()`` for one text, ``close(cancel=False)`` or a ``with`` block to drain it (``close(cancel=True)``
         is its interrupt; ``Chat.context`` is not read).  ``slots`` defaults to the handle's ``max_batch``; every
-        stage's ``max_new_token`` must be at most ``max_new_cap``.  See ``ChatEngine.submit``."""
+        stage's ``max_new_token`` must be at most ``max_new_cap``.  See ``ChatEngine.submit``.  ``dtype`` as in
+        ``infer_continuous``: every stage of every job runs on that engine."""
+        flags = _lib.engine_flags(dtype)
         assert self.has_loaded(use_decoder=use_decoder)
         return self.gpt._open_slot_engine(ChatEngine, self.gpt.max_batch if slots is None else slots, max_new_cap,
-                                          use_decoder, None, self, use_decoder)
+                                          use_decoder, None, self, use_decoder, flags=flags)
 
     def interrupt(self):
         self.context.set(True)
@@ -631,7 +646,7 @@ def _text_index(gpt: GPT, requests, i: int) -> Optional[int]:
 
 def stream_continuous(gpt: GPT, model: DVAE, requests, windows: List[StreamWindows], use_decoder: bool, slots=None,
                       context=None, ragged: bool = True, stats: Optional[Dict[str, float]] = None,
-                      max_new_cap: Optional[int] = None):
+                      max_new_cap: Optional[int] = None, flags: int = 0):
     """Streamed audio of many requests on the slot engine: generator of ``(request_index, chunk [1, n] float32, last)``.
     Text requests stream nothing; a follow-up's chunks come under its parent's index, with its parent's windows.
 
@@ -640,10 +655,11 @@ def stream_continuous(gpt: GPT, model: DVAE, requests, windows: List[StreamWindo
     the DVAE decoder) or codes (``model`` = the code DVAE, ``use_decoder=False``) in one ``decode_rows`` call, and the
     window is cut out of its row.  ``ragged=False`` decodes the windows one ``decode_to_wavs_window`` call each
     instead (the straightforward form tools/bench_continuous.py compares against).  ``stats['path2_s']`` (optional)
-    accumulates the host time spent decoding and copying the audio."""
+    accumulates the host time spent decoding and copying the audio.  ``flags``: the engine's
+    ctb_gpt_engine_begin_ex precision flags."""
     import time
 
-    for dev, batch in gpt._stream_polls(requests, slots, use_decoder, context, max_new_cap=max_new_cap):
+    for dev, batch in gpt._stream_polls(requests, slots, use_decoder, context, max_new_cap=max_new_cap, flags=flags):
         t_start = time.perf_counter()
         jobs = []  # (text, slot, n_tokens, a, b, flush, last)
         for i, s, n, last in batch:

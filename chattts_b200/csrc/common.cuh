@@ -1,5 +1,6 @@
 // Shared device/host helpers for the chattts_b200 kernels (sm_90a only).
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -101,6 +102,24 @@ __device__ __forceinline__ float4 ldg_cg(const float4* p) { return __ldcg(p); }
 __device__ __forceinline__ float ldg_cg(const float* p) { return __ldcg(p); }
 __device__ __forceinline__ int ldg_cg(const int* p) { return __ldcg(p); }
 __device__ __forceinline__ int ldg_cg(const uint8_t* p) { return (int)__ldcg(p); }
+
+// 8 consecutive K or V values as fp32: two 16-byte loads from an fp32 cache, one from an fp16 cache
+__device__ __forceinline__ void ld_kv8(const float* p, float4& a, float4& b) {
+  a = ldg_cg(reinterpret_cast<const float4*>(p));
+  b = ldg_cg(reinterpret_cast<const float4*>(p + 4));
+}
+__device__ __forceinline__ void ld_kv8(const __half* p, float4& a, float4& b) {
+  const uint4 u = __ldcg(reinterpret_cast<const uint4*>(p));
+  const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
+  const float2 f1 = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+  const float2 f2 = __half22float2(*reinterpret_cast<const __half2*>(&u.z));
+  const float2 f3 = __half22float2(*reinterpret_cast<const __half2*>(&u.w));
+  a = make_float4(f0.x, f0.y, f1.x, f1.y);
+  b = make_float4(f2.x, f2.y, f3.x, f3.y);
+}
+// a K/V pair appended to the cache (fp16: rounded to nearest even)
+__device__ __forceinline__ void st_kv2(float* p, float a, float b) { *reinterpret_cast<float2*>(p) = make_float2(a, b); }
+__device__ __forceinline__ void st_kv2(__half* p, float a, float b) { *reinterpret_cast<__half2*>(p) = __floats2half2_rn(a, b); }
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

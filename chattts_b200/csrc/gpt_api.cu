@@ -53,8 +53,8 @@ struct ctb_gpt {
   int32_t* idx;
   uint8_t *active, *finish;
   LoopState* st;
-  size_t kv_layer_floats;
-  size_t kv_pages;      // pages per layer currently in the pool
+  size_t kv_layer_elems;  // elements (fp32, or fp16 for a CTB_ENGINE_FP16_KV engine) of one layer's share of the pool
+  size_t kv_bytes;        // size of the pool
   int bt_B; size_t bt_per_row;  // shape the uploaded block table was built for
   // per generate() call
   int B, T0, max_new, infer_text, started;
@@ -107,7 +107,20 @@ struct ctb_gpt {
   int eng_text;
   cudaGraphExec_t graph_exec_text;
   uint64_t graph_kernels_text;
+  // ---- half-precision slot engine (ctb_gpt_engine_begin_ex)
+  int prec;                   // CTB_ENGINE_FP16_* bits of the current engine (0 for fp32 engines and generate())
+  bool tc_base;               // tensor-core activation scratch, head copies and their tensor maps exist (tc_setup_base)
+  __half *w16_qkv, *w16_wo, *w16_gu, *w16_wd;  // fp16 decode copies of the layer matrices (built once, kept)
+  CUtensorMap *m16_wqkv, *m16_wo, *m16_wgu, *m16_wd;
+  float* gw16;                // the same rounded values as fp32 in the blob's layer layout: prefill W_hi
+  float* pf_wzero;            // prefill W_lo of the rounded weights (exactly zero), as large as the largest matrix
 };
+
+static size_t kv_elem_bytes(const ctb_gpt* h) { return (h->prec & CTB_ENGINE_FP16_KV) ? 2 : 4; }
+// layer l's share of the KV pool, in the element type the current call's kernels use
+static float* kv_layer(const ctb_gpt* h, int l) {
+  return reinterpret_cast<float*>(reinterpret_cast<char*>(h->kv) + (size_t)l * h->kv_layer_elems * kv_elem_bytes(h));
+}
 
 // floats of one slot's noise in the engine's buffer: room for a code request's or a text request's rows
 static size_t noise_stride(const ctb_gpt* h) {
@@ -165,9 +178,31 @@ __global__ void k_build_tc_weight(const float* __restrict__ W, const float* __re
   for (int k = threadIdx.x; k < K; k += blockDim.x)
     out[(size_t)pr * K + k] = scale ? __fmul_rn(W[(size_t)r * K + k], scale[k]) : W[(size_t)r * K + k];
 }
+
+__global__ void k_build_tc_weight16(const float* __restrict__ W, const float* __restrict__ scale, __half* __restrict__ out16,
+                                    float* __restrict__ out32, int rows, int K, int mode, int qk_rows, int hd, int I,
+                                    int* __restrict__ bad) {
+  const int r = blockIdx.x;
+  if (r >= rows) return;
+  int pr = r;  // the row permutation of k_build_tc_weight
+  if (mode == 1 && r < qk_rows) {
+    const int h = r / hd, j = r % hd, half = hd / 2;
+    pr = h * hd + (j < half ? 2 * j : 2 * (j - half) + 1);
+  } else if (mode == 2) {
+    pr = (r < I) ? 2 * r : 2 * (r - I) + 1;
+  }
+  for (int k = threadIdx.x; k < K; k += blockDim.x) {
+    const float v = scale ? __fmul_rn(W[(size_t)r * K + k], scale[k]) : W[(size_t)r * K + k];
+    if (fabsf(v) > 65504.f) *bad = 1;
+    const __half w = __float2half_rn(v);
+    out16[(size_t)pr * K + k] = w;
+    out32[(size_t)r * K + k] = __half2float(w);
+  }
+}
 }  // namespace ctb
 
-static int encode_map_2d(CUtensorMap* m, const float* base, uint64_t rows, uint64_t K, uint32_t box_rows) {
+static int encode_map_2d(CUtensorMap* m, const void* base, uint64_t rows, uint64_t K, uint32_t box_rows,
+                         bool f16 = false) {
   static PFN_cuTensorMapEncodeTiled_v12000 enc = nullptr;
   if (!enc) {
     void* fp = nullptr;
@@ -177,41 +212,39 @@ static int encode_map_2d(CUtensorMap* m, const float* base, uint64_t rows, uint6
       return set_err(CTB_ERR_CUDA, "cuTensorMapEncodeTiled unavailable");
     enc = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fp);
   }
+  // fp32: 128-byte rows of 32 k, swizzled for wgmma; fp16 (weights the kernel widens): dense 64-byte rows
   const cuuint64_t dims[2] = {K, rows};
-  const cuuint64_t strides[1] = {K * 4};
+  const cuuint64_t strides[1] = {K * (f16 ? 2 : 4)};
   const cuuint32_t box[2] = {32, box_rows};
   const cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+  CUresult r = enc(m, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base),
+                   dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   f16 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return set_err(CTB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)r);
   return CTB_OK;
 }
 
-template <int EPI, int NPAD, int CS>
+template <int EPI, int NPAD, int CS, int PREC = 0>
 static int set_tc_attr() {
-  return ensure_smem_attr((const void*)k_tc_dec<EPI, NPAD, CS>, TdCfg<NPAD>::SMEM_BYTES);
+  return ensure_smem_attr((const void*)k_tc_dec<EPI, NPAD, CS, PREC>, TdCfg<NPAD, (PREC & TD_W16) != 0>::SMEM_BYTES);
 }
 
 // cluster sizes of the split-K (K slices per 128-row tile)
 constexpr int CS_QKV = 4, CS_O = 8, CS_GU = 2, CS_DOWN = 8, CS_HEADS = 4;
 
+static int tc_setup_base(ctb_gpt* h);
+
+// the fp32 wgmma step: norm-folded, permuted fp32 copies of Wqkv and [Wgate; Wup] (Wo and Wdown are read in place)
 static int tc_setup(ctb_gpt* h) {
   const ctb_gpt_config& c = h->cfg;
   const ctb_gpt_layout& L = h->lay;
   const size_t d = c.hidden_size, I = c.intermediate_size;
   const size_t nqkv = (size_t)(c.num_heads + 2 * c.num_kv_heads) * c.head_dim;
   int rc;
+  if ((rc = tc_setup_base(h))) return rc;
   if ((rc = dalloc(&h->tc_wqkv, (size_t)c.num_layers * nqkv * d))) return rc;
   if ((rc = dalloc(&h->tc_wgu, (size_t)c.num_layers * 2 * I * d))) return rc;
-  if ((rc = dalloc(&h->tc_heads_code, (size_t)c.num_vq * c.num_audio_tokens * d))) return rc;
-  if ((rc = dalloc(&h->tc_heads_text, (size_t)c.num_text_tokens * d))) return rc;
-  if ((rc = dalloc(&h->x_hi, 32 * d))) return rc;
-  if ((rc = dalloc(&h->x_lo, 32 * d))) return rc;
-  if ((rc = dalloc(&h->attn_hi, 32 * d))) return rc;
-  if ((rc = dalloc(&h->attn_lo, 32 * d))) return rc;
-  if ((rc = dalloc(&h->h_hi, 32 * I))) return rc;
-  if ((rc = dalloc(&h->h_lo, 32 * I))) return rc;
   h->m_wqkv = new CUtensorMap[c.num_layers]; h->m_wo = new CUtensorMap[c.num_layers];
   h->m_wgu = new CUtensorMap[c.num_layers]; h->m_wd = new CUtensorMap[c.num_layers];
   const int qk_rows = (c.num_heads + c.num_kv_heads) * c.head_dim;
@@ -226,6 +259,29 @@ static int tc_setup(ctb_gpt* h) {
     if ((rc = encode_map_2d(&h->m_wgu[l], wg, 2 * I, d, 128))) return rc;
     if ((rc = encode_map_2d(&h->m_wd[l], Wl + L.wdown, d, I, 128))) return rc;
   }
+  CTB_CUDA(cudaDeviceSynchronize());
+#define TCATTR(E, C) if ((rc = set_tc_attr<E, 16, C>())) return rc; if ((rc = set_tc_attr<E, 32, C>())) return rc;
+  TCATTR(DE_QKV, CS_QKV) TCATTR(DE_OPROJ, CS_O) TCATTR(DE_GATEUP, CS_GU) TCATTR(DE_DOWN, CS_DOWN)
+#undef TCATTR
+  return CTB_OK;
+}
+
+// what every wgmma step shares: the tf32-split activation scratch of 32 rows, the fp32 norm-folded head copies and the
+// tensor maps over them
+static int tc_setup_base(ctb_gpt* h) {
+  if (h->tc_base) return CTB_OK;
+  const ctb_gpt_config& c = h->cfg;
+  const ctb_gpt_layout& L = h->lay;
+  const size_t d = c.hidden_size, I = c.intermediate_size;
+  int rc;
+  if ((rc = dalloc(&h->tc_heads_code, (size_t)c.num_vq * c.num_audio_tokens * d))) return rc;
+  if ((rc = dalloc(&h->tc_heads_text, (size_t)c.num_text_tokens * d))) return rc;
+  if ((rc = dalloc(&h->x_hi, 32 * d))) return rc;
+  if ((rc = dalloc(&h->x_lo, 32 * d))) return rc;
+  if ((rc = dalloc(&h->attn_hi, 32 * d))) return rc;
+  if ((rc = dalloc(&h->attn_lo, 32 * d))) return rc;
+  if ((rc = dalloc(&h->h_hi, 32 * I))) return rc;
+  if ((rc = dalloc(&h->h_lo, 32 * I))) return rc;
   const int nhc = c.num_vq * c.num_audio_tokens;
   k_build_tc_weight<<<nhc, 256>>>(h->W + L.head_code, h->W + L.final_norm, h->tc_heads_code, nhc, (int)d, 0, 0, 0, 0);
   k_build_tc_weight<<<c.num_text_tokens, 256>>>(h->W + L.head_text, h->W + L.final_norm, h->tc_heads_text,
@@ -242,8 +298,80 @@ static int tc_setup(ctb_gpt* h) {
     if ((rc = encode_map_2d(&h->m_h[n][0], h->h_hi, 32, I, npad))) return rc;
     if ((rc = encode_map_2d(&h->m_h[n][1], h->h_lo, 32, I, npad))) return rc;
   }
-#define TCATTR(E, C) if ((rc = set_tc_attr<E, 16, C>())) return rc; if ((rc = set_tc_attr<E, 32, C>())) return rc;
-  TCATTR(DE_QKV, CS_QKV) TCATTR(DE_OPROJ, CS_O) TCATTR(DE_GATEUP, CS_GU) TCATTR(DE_DOWN, CS_DOWN) TCATTR(DE_HEADS, CS_HEADS)
+  if ((rc = set_tc_attr<DE_HEADS, 16, CS_HEADS>())) return rc;
+  if ((rc = set_tc_attr<DE_HEADS, 32, CS_HEADS>())) return rc;
+  h->tc_base = true;
+  return CTB_OK;
+}
+
+static void fp16_free(ctb_gpt* h) {
+  void* ptrs[] = {h->w16_qkv, h->w16_wo, h->w16_gu, h->w16_wd, h->gw16, h->pf_wzero};
+  for (void* p : ptrs) if (p) cudaFree(p);
+  h->w16_qkv = h->w16_wo = h->w16_gu = h->w16_wd = nullptr; h->gw16 = h->pf_wzero = nullptr;
+  delete[] h->m16_wqkv; delete[] h->m16_wo; delete[] h->m16_wgu; delete[] h->m16_wd;
+  h->m16_wqkv = h->m16_wo = h->m16_wgu = h->m16_wd = nullptr;
+}
+
+// The half-precision engine's weights, built by the first such engine and kept for the life of the handle: fp16
+// decode copies of the four layer matrices (Wqkv and [Wgate; Wup] norm-folded in fp32 first, then rounded; Wo and
+// Wdown rounded) and the same values as fp32 for the prefill GEMMs.  A value outside fp16's range refuses them.
+static int fp16_setup(ctb_gpt* h) {
+  if (h->w16_qkv) return CTB_OK;
+  const ctb_gpt_config& c = h->cfg;
+  const ctb_gpt_layout& L = h->lay;
+  const size_t d = c.hidden_size, I = c.intermediate_size, nq = (size_t)c.num_heads * c.head_dim;
+  const size_t nqkv = (size_t)(c.num_heads + 2 * c.num_kv_heads) * c.head_dim;
+  const int nl = c.num_layers, qk_rows = (c.num_heads + c.num_kv_heads) * c.head_dim;
+  int rc;
+  if ((rc = tc_setup_base(h))) return rc;
+  int* bad = nullptr;
+  if ((rc = dalloc(&h->w16_qkv, nl * nqkv * d)) || (rc = dalloc(&h->w16_wo, nl * d * nq)) ||
+      (rc = dalloc(&h->w16_gu, nl * 2 * I * d)) || (rc = dalloc(&h->w16_wd, nl * d * I)) ||
+      (rc = dalloc(&h->gw16, (size_t)L.layer_stride * nl)) ||
+      (rc = dalloc(&h->pf_wzero, std::max(std::max(nqkv * d, d * nq), std::max(2 * I * d, d * I)))) ||
+      (rc = dalloc(&bad, (size_t)4 * nl))) {
+    fp16_free(h);
+    if (bad) cudaFree(bad);
+    return rc;
+  }
+  for (int l = 0; l < nl; ++l) {
+    const float* Wl = h->W + L.layer0 + (int64_t)l * L.layer_stride;
+    float* gl = h->gw16 + (int64_t)l * L.layer_stride;
+    k_build_tc_weight16<<<(unsigned)nqkv, 256>>>(Wl + L.wqkv, Wl + L.ln1, h->w16_qkv + l * nqkv * d, gl + L.wqkv,
+                                                 (int)nqkv, (int)d, 1, qk_rows, c.head_dim, 0, bad + 4 * l);
+    k_build_tc_weight16<<<(unsigned)d, 256>>>(Wl + L.wo, nullptr, h->w16_wo + l * d * nq, gl + L.wo, (int)d, (int)nq, 0,
+                                              0, 0, 0, bad + 4 * l + 1);
+    k_build_tc_weight16<<<(unsigned)(2 * I), 256>>>(Wl + L.wgate_up, Wl + L.ln2, h->w16_gu + l * 2 * I * d,
+                                                    gl + L.wgate_up, (int)(2 * I), (int)d, 2, 0, 0, (int)I, bad + 4 * l + 2);
+    k_build_tc_weight16<<<(unsigned)d, 256>>>(Wl + L.wdown, nullptr, h->w16_wd + l * d * I, gl + L.wdown, (int)d, (int)I,
+                                              0, 0, 0, 0, bad + 4 * l + 3);
+  }
+  std::vector<int> hbad((size_t)4 * nl);
+  const cudaError_t e = cudaMemcpy(hbad.data(), bad, hbad.size() * sizeof(int), cudaMemcpyDeviceToHost);
+  cudaFree(bad);
+  if (e != cudaSuccess) { fp16_free(h); return set_err(CTB_ERR_CUDA, "fp16 weight copies: %s", cudaGetErrorString(e)); }
+  static const char* names[4] = {"self_attn.qkv (x input_layernorm)", "self_attn.o_proj",
+                                 "mlp.gate_up (x post_attention_layernorm)", "mlp.down_proj"};
+  for (int i = 0; i < 4 * nl; ++i)
+    if (hbad[i]) {
+      fp16_free(h);
+      return set_err(CTB_ERR_ARG, "fp16 engine: layer %d %s has a weight with |w| > 65504 (outside fp16's range)", i / 4,
+                     names[i % 4]);
+    }
+  h->m16_wqkv = new CUtensorMap[nl]; h->m16_wo = new CUtensorMap[nl];
+  h->m16_wgu = new CUtensorMap[nl]; h->m16_wd = new CUtensorMap[nl];
+  for (int l = 0; l < nl; ++l) {
+    if ((rc = encode_map_2d(&h->m16_wqkv[l], h->w16_qkv + l * nqkv * d, nqkv, d, 128, true)) ||
+        (rc = encode_map_2d(&h->m16_wo[l], h->w16_wo + l * d * nq, d, nq, 128, true)) ||
+        (rc = encode_map_2d(&h->m16_wgu[l], h->w16_gu + l * 2 * I * d, 2 * I, d, 128, true)) ||
+        (rc = encode_map_2d(&h->m16_wd[l], h->w16_wd + l * d * I, d, I, 128, true))) {
+      fp16_free(h);
+      return rc;
+    }
+  }
+#define TCATTR(E, C, P) if ((rc = set_tc_attr<E, 16, C, P>())) return rc; if ((rc = set_tc_attr<E, 32, C, P>())) return rc;
+  TCATTR(DE_QKV, CS_QKV, 1) TCATTR(DE_QKV, CS_QKV, 3) TCATTR(DE_OPROJ, CS_O, 1) TCATTR(DE_GATEUP, CS_GU, 1)
+  TCATTR(DE_DOWN, CS_DOWN, 1)
 #undef TCATTR
   return CTB_OK;
 }
@@ -287,7 +415,7 @@ extern "C" int ctb_gpt_create(const ctb_gpt_config* c, const float* weights_dev,
   TRY(dalloc(&h->logits, Bp * nlog));
   // The KV pool is sized by what a generate() call can actually touch (ctb_gpt_begin -> kv_reserve), not by
   // max_batch x max_context: a handle that allows 32 rows x 4096 tokens costs nothing until such a call arrives.
-  h->kv = nullptr; h->kv_layer_floats = 0; h->kv_pages = 0;
+  h->kv = nullptr; h->kv_layer_elems = 0; h->kv_bytes = 0;
   TRY(dalloc(&h->part, (size_t)c->max_batch * c->num_heads * h->nsplit_max * (c->head_dim + 2)));
   TRY(dalloc(&h->block_table, (size_t)c->max_batch * h->pages_per_row));
   TRY(dalloc(&h->seq_len, Bp));
@@ -345,6 +473,7 @@ extern "C" int ctb_gpt_destroy(ctb_gpt* h) {
                   h->rows, h->cfgs, h->eng_noise, h->eng_slot, h->eng_text_logits, h->eng_text_idx};
   delete[] h->m_wqkv; delete[] h->m_wo; delete[] h->m_wgu; delete[] h->m_wd;
   for (void* p : ptrs) if (p) cudaFree(p);
+  fp16_free(h);
   delete h;
   return CTB_OK;
 }
@@ -475,7 +604,7 @@ static int launch_layer_kernel(ctb_gpt* h, const StepCtx& x, int l, int kind, cu
   const ctb_gpt_layout& L = h->lay;
   const int d = c.hidden_size, I = c.intermediate_size, hd = c.head_dim;
   const float* Wl = h->W + L.layer0 + (int64_t)l * L.layer_stride;
-  float* kvl = h->kv + (size_t)l * h->kv_layer_floats;
+  float* kvl = kv_layer(h, l);
   GemvP p = x.g;
   switch (kind) {
     case 0:
@@ -492,7 +621,10 @@ static int launch_layer_kernel(ctb_gpt* h, const StepCtx& x, int l, int kind, cu
       // so large batches need no cross-CTA merge at all
       const int want = (2 * g_num_sms + c.num_heads * h->B - 1) / (c.num_heads * h->B);
       dim3 agrid(std::max(1, std::min(want, (max_ctx + ATT_CHUNK - 1) / ATT_CHUNK)), c.num_heads, h->B);
-      CTB_CUDA(launch_pdl(k_attn, agrid, dim3(ATT_THREADS), 0, s, a));
+      if (h->prec & CTB_ENGINE_FP16_KV)
+        CTB_CUDA(launch_pdl(k_attn<__half>, agrid, dim3(ATT_THREADS), 0, s, a));
+      else
+        CTB_CUDA(launch_pdl(k_attn<float>, agrid, dim3(ATT_THREADS), 0, s, a));
       CTB_LAUNCH_CHECK();
       return CTB_OK;
     }
@@ -555,15 +687,16 @@ static int launch_sampler(ctb_gpt* h, const StepCtx& x, cudaStream_t s) {
   return launch_sample(sp, s);
 }
 
-template <int EPI, int CS>
+template <int EPI, int CS, int PREC = 0>
 static int launch_tc(int npad, const CUtensorMap& mw, const CUtensorMap& mxh, const CUtensorMap& mxl, const TcDecP& p,
                      cudaStream_t s) {
+  constexpr bool W16 = (PREC & TD_W16) != 0;
   const int tiles = (p.nrows + 127) / 128;
   dim3 grid(tiles * CS);
   if (npad == 16)
-    CTB_CUDA(launch_pdl_cluster(k_tc_dec<EPI, 16, CS>, grid, dim3(TD_THREADS), (size_t)TdCfg<16>::SMEM_BYTES, s, (unsigned)CS, mw, mxh, mxl, p));
+    CTB_CUDA(launch_pdl_cluster(k_tc_dec<EPI, 16, CS, PREC>, grid, dim3(TD_THREADS), (size_t)TdCfg<16, W16>::SMEM_BYTES, s, (unsigned)CS, mw, mxh, mxl, p));
   else
-    CTB_CUDA(launch_pdl_cluster(k_tc_dec<EPI, 32, CS>, grid, dim3(TD_THREADS), (size_t)TdCfg<32>::SMEM_BYTES, s, (unsigned)CS, mw, mxh, mxl, p));
+    CTB_CUDA(launch_pdl_cluster(k_tc_dec<EPI, 32, CS, PREC>, grid, dim3(TD_THREADS), (size_t)TdCfg<32, W16>::SMEM_BYTES, s, (unsigned)CS, mw, mxh, mxl, p));
   CTB_LAUNCH_CHECK();
   return CTB_OK;
 }
@@ -579,7 +712,10 @@ static TcDecP make_tc(ctb_gpt* h) {
   return p;
 }
 
-static int launch_layer_kernel_tc(ctb_gpt* h, int l, int kind, cudaStream_t s) {
+// PREC: the engine's CTB_ENGINE_FP16_* bits (only the QKV GEMM sees the KV bit)
+template <int PREC>
+static int launch_layer_kernel_tc_t(ctb_gpt* h, int l, int kind, cudaStream_t s) {
+  constexpr int PW = PREC & TD_W16;
   const ctb_gpt_config& c = h->cfg;
   const int n = h->B > 16 ? 1 : 0, npad = n ? 32 : 16;
   const int d = c.hidden_size, I = c.intermediate_size;
@@ -587,19 +723,28 @@ static int launch_layer_kernel_tc(ctb_gpt* h, int l, int kind, cudaStream_t s) {
   switch (kind) {
     case 0:
       p.K = d; p.kslice = d / CS_QKV; p.nrows = (c.num_heads + 2 * c.num_kv_heads) * c.head_dim; p.xraw = h->x;
-      p.kv = h->kv + (size_t)l * h->kv_layer_floats;
-      return launch_tc<DE_QKV, CS_QKV>(npad, h->m_wqkv[l], h->m_x[n][0], h->m_x[n][1], p, s);
+      p.kv = kv_layer(h, l);
+      return launch_tc<DE_QKV, CS_QKV, PREC>(npad, PW ? h->m16_wqkv[l] : h->m_wqkv[l], h->m_x[n][0], h->m_x[n][1], p, s);
     case 2:
       p.K = c.num_heads * c.head_dim; p.kslice = p.K / CS_O; p.nrows = d; p.xraw = nullptr;
-      return launch_tc<DE_OPROJ, CS_O>(npad, h->m_wo[l], h->m_attn[n][0], h->m_attn[n][1], p, s);
+      return launch_tc<DE_OPROJ, CS_O, PW>(npad, PW ? h->m16_wo[l] : h->m_wo[l], h->m_attn[n][0], h->m_attn[n][1], p, s);
     case 3:
       p.K = d; p.kslice = d / CS_GU; p.nrows = 2 * I; p.xraw = h->x;
-      return launch_tc<DE_GATEUP, CS_GU>(npad, h->m_wgu[l], h->m_x[n][0], h->m_x[n][1], p, s);
+      return launch_tc<DE_GATEUP, CS_GU, PW>(npad, PW ? h->m16_wgu[l] : h->m_wgu[l], h->m_x[n][0], h->m_x[n][1], p, s);
     case 4:
       p.K = I; p.kslice = I / CS_DOWN; p.nrows = d; p.xraw = nullptr;
-      return launch_tc<DE_DOWN, CS_DOWN>(npad, h->m_wd[l], h->m_h[n][0], h->m_h[n][1], p, s);
+      return launch_tc<DE_DOWN, CS_DOWN, PW>(npad, PW ? h->m16_wd[l] : h->m_wd[l], h->m_h[n][0], h->m_h[n][1], p, s);
   }
   return set_err(CTB_ERR_ARG, "bad tc kernel kind %d", kind);
+}
+
+static int launch_layer_kernel_tc(ctb_gpt* h, int l, int kind, cudaStream_t s) {
+  switch (h->prec) {
+    case 0: return launch_layer_kernel_tc_t<0>(h, l, kind, s);
+    case CTB_ENGINE_FP16_WEIGHTS: return launch_layer_kernel_tc_t<CTB_ENGINE_FP16_WEIGHTS>(h, l, kind, s);
+    case CTB_ENGINE_FP16_KV: return launch_layer_kernel_tc_t<CTB_ENGINE_FP16_KV>(h, l, kind, s);
+    default: return launch_layer_kernel_tc_t<CTB_ENGINE_FP16_WEIGHTS | CTB_ENGINE_FP16_KV>(h, l, kind, s);
+  }
 }
 
 static int launch_heads_tc(ctb_gpt* h, cudaStream_t s) {
@@ -648,7 +793,7 @@ static int launch_step_mega(ctb_gpt* h, int col, bool sample, cudaStream_t s) {
   m.L = c.num_layers; m.d = c.hidden_size; m.I = c.intermediate_size; m.Hq = c.num_heads; m.Hkv = c.num_kv_heads;
   m.hd = c.head_dim; m.eps = c.rms_eps; m.scaling = 1.0f / sqrtf((float)c.head_dim);
   m.x = h->x; m.qbuf = h->qbuf; m.attn = h->attn; m.mlp = h->mlp; m.logits = h->logits; m.kv = h->kv; m.part = h->part;
-  m.kv_layer_floats = h->kv_layer_floats; m.block_table = h->block_table; m.pages_per_row = h->pages_per_row;
+  m.kv_layer_floats = h->kv_layer_elems; m.block_table = h->block_table; m.pages_per_row = h->pages_per_row;
   m.seq_len = h->seq_len; m.counter = h->counter; m.nsplit_max = h->nsplit_max; m.st = h->st; m.bar = h->bar;
   m.decode = col < 0; m.col = col < 0 ? 0 : col; m.T0 = h->T0; m.sample = sample ? 1 : 0;
   m.emb = h->emb; m.mask = h->mask; m.ids_out = h->ids_out; m.max_new = h->max_new; m.num_vq = c.num_vq;
@@ -693,7 +838,7 @@ static int launch_step_flow(ctb_gpt* h, int col, bool sample, cudaStream_t s, in
   m.o_cos = L.rope_cos; m.o_sin = L.rope_sin;
   m.L = c.num_layers; m.I = c.intermediate_size; m.Hq = c.num_heads; m.hd = c.head_dim; m.eps = c.rms_eps;
   m.scaling = 1.0f / sqrtf((float)c.head_dim);
-  m.logits = h->logits; m.kv = h->kv; m.kv_layer_floats = h->kv_layer_floats; m.block_table = h->block_table;
+  m.logits = h->logits; m.kv = h->kv; m.kv_layer_floats = h->kv_layer_elems; m.block_table = h->block_table;
   m.pages_per_row = h->pages_per_row; m.seq_len = h->seq_len; m.st = h->st;
   m.decode = col < 0; m.col = col < 0 ? 0 : col; m.T0 = h->T0; m.sample = sample ? 1 : 0;
   m.emb = h->emb; m.mask = h->mask; m.ids_out = h->ids_out; m.max_new = h->max_new; m.num_vq = c.num_vq;
@@ -820,16 +965,18 @@ static int prefill_reserve(ctb_gpt* h, size_t rows) {
   const ctb_gpt_config& c = h->cfg;
   const size_t d = c.hidden_size, I = c.intermediate_size, nqkv = (size_t)(c.num_heads + 2 * c.num_kv_heads) * c.head_dim;
   int rc;
-  if (!h->gw_hi) {
+  if (!h->gw_hi && !(h->prec & CTB_ENGINE_FP16_WEIGHTS)) {  // a half-precision engine's prefill reads h->gw16
     const size_t n = (size_t)h->lay.layer_stride * c.num_layers;
     if ((rc = dalloc(&h->gw_hi, n))) return rc;
     if ((rc = dalloc(&h->gw_lo, n))) return rc;
     k_split_tf32_t<0><<<2048, 256>>>(h->W + h->lay.layer0, h->gw_hi, h->gw_lo, (int64_t)n);
+    CTB_CUDA(cudaDeviceSynchronize());
+  }
+  if (!h->pf_ones) {
     if ((rc = dalloc(&h->pf_ones, 2 * I))) return rc;
     if ((rc = dalloc(&h->pf_zeros, 2 * I))) return rc;
     std::vector<float> ones(2 * I, 1.0f);
     CTB_CUDA(cudaMemcpy(h->pf_ones, ones.data(), ones.size() * sizeof(float), cudaMemcpyHostToDevice));
-    CTB_CUDA(cudaDeviceSynchronize());
   }
   if (rows > h->pf_rows) {
     float** bufs[] = {&h->pf_resid, &h->pf_xn, &h->pf_qkv, &h->pf_q, &h->pf_attn, &h->pf_gu, &h->pf_h};
@@ -869,29 +1016,34 @@ static int prefill_batched(ctb_gpt* h, int B, int T0, const float* emb, const ui
   pp.pages_per_row = h->pages_per_row; pp.rope_cos = h->W + L.rope_cos; pp.rope_sin = h->W + L.rope_sin;
   pp.permute_qk = h->use_tc ? 1 : 0; pp.attn = h->pf_attn; pp.scaling = 1.0f / sqrtf((float)c.head_dim);
   const int rms_blocks = (M + 7) / 8;
+  // a half-precision engine: the rounded weights (norms folded in before rounding) with W_lo = 0 and unit norms
+  const bool w16 = (h->prec & CTB_ENGINE_FP16_WEIGHTS) != 0, kv16 = (h->prec & CTB_ENGINE_FP16_KV) != 0;
   for (int l = 0; l < c.num_layers; ++l) {
     const int64_t lo = (int64_t)l * L.layer_stride;
     const float* Wl = h->W + L.layer0 + lo;
-    const float *Whi = h->gw_hi + lo, *Wlo = h->gw_lo + lo;
-    pp.kv = h->kv + (size_t)l * h->kv_layer_floats;
-    k_rms_rows<<<rms_blocks, 256, 0, s>>>(h->pf_resid, Wl + L.ln1, h->pf_xn, M, d, c.rms_eps);
+    const float *Whi = (w16 ? h->gw16 : h->gw_hi) + lo, *Wlo = w16 ? nullptr : h->gw_lo + lo;
+    auto wlo = [&](int64_t off) { return w16 ? h->pf_wzero : Wlo + off; };
+    pp.kv = kv_layer(h, l);
+    k_rms_rows<<<rms_blocks, 256, 0, s>>>(h->pf_resid, w16 ? h->pf_ones : Wl + L.ln1, h->pf_xn, M, d, c.rms_eps);
     CTB_LAUNCH_CHECK();
-    if ((rc = tc_gemm_launch<GE_NONE>(s, h->pf_xn, d, B, T0, nqkv, d, 1, d, 1, 0, Whi + L.wqkv, Wlo + L.wqkv, nullptr,
+    if ((rc = tc_gemm_launch<GE_NONE>(s, h->pf_xn, d, B, T0, nqkv, d, 1, d, 1, 0, Whi + L.wqkv, wlo(L.wqkv), nullptr,
                                       nullptr, nullptr, 0, h->pf_qkv, nqkv))) return rc;
-    k_prefill_rope_kv<<<dim3(T0, B), 256, 0, s>>>(pp);
+    if (kv16) k_prefill_rope_kv<__half><<<dim3(T0, B), 256, 0, s>>>(pp);
+    else k_prefill_rope_kv<float><<<dim3(T0, B), 256, 0, s>>>(pp);
     CTB_LAUNCH_CHECK();
-    k_prefill_attn<<<dim3((T0 + PF_ATT_WARPS - 1) / PF_ATT_WARPS, c.num_heads, B), PF_ATT_WARPS * 32,
-                     (size_t)PF_ATT_WARPS * T0 * sizeof(float), s>>>(pp);
+    const dim3 agrid((T0 + PF_ATT_WARPS - 1) / PF_ATT_WARPS, c.num_heads, B);
+    if (kv16) k_prefill_attn<__half><<<agrid, PF_ATT_WARPS * 32, (size_t)PF_ATT_WARPS * T0 * sizeof(float), s>>>(pp);
+    else k_prefill_attn<float><<<agrid, PF_ATT_WARPS * 32, (size_t)PF_ATT_WARPS * T0 * sizeof(float), s>>>(pp);
     CTB_LAUNCH_CHECK();
-    if ((rc = tc_gemm_launch<GE_SCALE_RES>(s, h->pf_attn, d, B, T0, d, d, 1, d, 1, 0, Whi + L.wo, Wlo + L.wo, h->pf_zeros,
+    if ((rc = tc_gemm_launch<GE_SCALE_RES>(s, h->pf_attn, d, B, T0, d, d, 1, d, 1, 0, Whi + L.wo, wlo(L.wo), h->pf_zeros,
                                            h->pf_ones, h->pf_resid, d, h->pf_resid, d))) return rc;
-    k_rms_rows<<<rms_blocks, 256, 0, s>>>(h->pf_resid, Wl + L.ln2, h->pf_xn, M, d, c.rms_eps);
+    k_rms_rows<<<rms_blocks, 256, 0, s>>>(h->pf_resid, w16 ? h->pf_ones : Wl + L.ln2, h->pf_xn, M, d, c.rms_eps);
     CTB_LAUNCH_CHECK();
-    if ((rc = tc_gemm_launch<GE_NONE>(s, h->pf_xn, d, B, T0, 2 * I, d, 1, d, 1, 0, Whi + L.wgate_up, Wlo + L.wgate_up,
+    if ((rc = tc_gemm_launch<GE_NONE>(s, h->pf_xn, d, B, T0, 2 * I, d, 1, d, 1, 0, Whi + L.wgate_up, wlo(L.wgate_up),
                                       nullptr, nullptr, nullptr, 0, h->pf_gu, 2 * I))) return rc;
     k_silu_mul<<<(unsigned)(((size_t)M * I + 255) / 256), 256, 0, s>>>(h->pf_gu, h->pf_h, M, I);
     CTB_LAUNCH_CHECK();
-    if ((rc = tc_gemm_launch<GE_SCALE_RES>(s, h->pf_h, I, B, T0, d, I, 1, I, 1, 0, Whi + L.wdown, Wlo + L.wdown,
+    if ((rc = tc_gemm_launch<GE_SCALE_RES>(s, h->pf_h, I, B, T0, d, I, 1, I, 1, 0, Whi + L.wdown, wlo(L.wdown),
                                            h->pf_zeros, h->pf_ones, h->pf_resid, d, h->pf_resid, d))) return rc;
   }
   k_prefill_finish<<<B, 256, 0, s>>>(h->pf_resid, h->x, h->use_tc ? h->x_hi : nullptr, h->use_tc ? h->x_lo : nullptr,
@@ -904,27 +1056,29 @@ static int prefill_batched(ctb_gpt* h, int B, int T0, const float* emb, const ui
   return launch_finalize(h, s);
 }
 
-// Pages for B rows of up to `tokens` tokens each: grow the pool if needed (page = 16 tokens x K|V x heads x 64 floats per
-// layer) and assign row b the pages [b * need, (b + 1) * need) - kernels only ever see the block table.
+// Pages for B rows of up to `tokens` tokens each: grow the pool if needed (page = 16 tokens x K|V x heads x 64 values per
+// layer, fp32 or fp16 by the call's CTB_ENGINE_FP16_KV bit; the pool is sized in bytes, so calls of either type reuse
+// it) and assign row b the pages [b * need, (b + 1) * need) - kernels only ever see the block table.
 static int kv_reserve(ctb_gpt* h, int B, int tokens, cudaStream_t s) {
   const ctb_gpt_config& c = h->cfg;
   const size_t per_row = ((size_t)tokens + kPageTokens - 1) / kPageTokens;
   const size_t need = per_row * (size_t)B;
-  const size_t page_floats = (size_t)2 * c.num_kv_heads * kPageTokens * c.head_dim;
-  if (need > h->kv_pages) {
+  const size_t page_elems = (size_t)2 * c.num_kv_heads * kPageTokens * c.head_dim;
+  const size_t page_bytes = page_elems * kv_elem_bytes(h) * c.num_layers;  // one page of every layer
+  if (need * page_bytes > h->kv_bytes) {
     CTB_CUDA(cudaStreamSynchronize(s));
-    if (h->kv) { cudaFree(h->kv); h->kv = nullptr; h->kv_pages = 0; }
+    if (h->kv) { cudaFree(h->kv); h->kv = nullptr; h->kv_bytes = 0; }
     const size_t pages = need + need / 8;  // a little head-room against re-allocation on slightly longer calls
-    if (cudaMalloc(reinterpret_cast<void**>(&h->kv), pages * page_floats * c.num_layers * sizeof(float)) != cudaSuccess) {
+    if (cudaMalloc(reinterpret_cast<void**>(&h->kv), pages * page_bytes) != cudaSuccess) {
       cudaGetLastError();
       return set_err(CTB_ERR_NOMEM, "KV pool: %zu pages x %d layers (%.1f GB) do not fit", pages, c.num_layers,
-                     (double)(pages * page_floats * c.num_layers * 4) / 1e9);
+                     (double)(pages * page_bytes) / 1e9);
     }
-    CTB_CUDA(cudaMemsetAsync(h->kv, 0, pages * page_floats * c.num_layers * sizeof(float), s));
-    h->kv_pages = pages;
-    h->kv_layer_floats = pages * page_floats;
+    CTB_CUDA(cudaMemsetAsync(h->kv, 0, pages * page_bytes, s));
+    h->kv_bytes = pages * page_bytes;
     h->bt_B = 0;
   }
+  h->kv_layer_elems = h->kv_bytes / page_bytes * page_elems;
   if (h->bt_B == B && h->bt_per_row == per_row) return CTB_OK;  // table already describes this shape: nothing to upload
   std::vector<int> bt((size_t)B * h->pages_per_row, 0);
   for (int b = 0; b < B; ++b)
@@ -946,7 +1100,7 @@ extern "C" int ctb_gpt_begin(ctb_gpt* h, int32_t B, int32_t T0, const float* emb
   if (sampler->min_tokens_to_keep < 1) return set_err(CTB_ERR_ARG, "min_tokens_to_keep must be >= 1");
   cudaStream_t s = (cudaStream_t)stream;
   h->B = B; h->T0 = T0; h->max_new = max_new_token; h->infer_text = infer_text ? 1 : 0;
-  h->engine = 0; h->phase = RS_RUNNING;
+  h->engine = 0; h->phase = RS_RUNNING; h->prec = 0;
   h->use_tc = h->tc_ready && B >= h->tc_min_batch;
   h->sampler = *sampler; h->q_noise = q_noise_dev; h->emb = emb_dev; h->mask = mask_dev;
   h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev;
@@ -1037,13 +1191,33 @@ extern "C" int ctb_gpt_decode(ctb_gpt* h, int32_t n_steps, void* stream) {
 // ------------------------------------------------------------------ slot engine (continuous batching)
 extern "C" int ctb_gpt_engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t* ids_out_dev,
                                     float* hiddens_out_dev, void* stream) {
+  return ctb_gpt_engine_begin_ex(h, S, max_new_cap, 0, ids_out_dev, hiddens_out_dev, stream);
+}
+
+static_assert((int)TD_W16 == CTB_ENGINE_FP16_WEIGHTS && (int)TD_KV16 == CTB_ENGINE_FP16_KV, "precision bits");
+
+extern "C" int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t flags, int32_t* ids_out_dev,
+                                       float* hiddens_out_dev, void* stream) {
   if (!h || !ids_out_dev) return set_err(CTB_ERR_ARG, "null argument");
   const ctb_gpt_config& c = h->cfg;
   if (S < 2 || S > c.max_batch) return set_err(CTB_ERR_ARG, "S=%d outside [2,%d]", S, c.max_batch);
   if (max_new_cap < 1 || max_new_cap >= c.max_context)
     return set_err(CTB_ERR_ARG, "max_new_cap=%d outside [1,%d)", max_new_cap, c.max_context);
+  if (flags & ~(CTB_ENGINE_FP16_WEIGHTS | CTB_ENGINE_FP16_KV)) return set_err(CTB_ERR_ARG, "unknown engine flags 0x%x", flags);
+  if (flags && S > 32) return set_err(CTB_ERR_ARG, "S=%d: a half-precision engine serves up to 32 slots", S);
+  if (flags && getenv("CTB_GPT_FMA"))
+    return set_err(CTB_ERR_ARG, "a half-precision engine runs on the wgmma step, which CTB_GPT_FMA=1 disables");
   cudaStream_t s = (cudaStream_t)stream;
   int rc;
+  if (flags) {
+    // the half-precision engine always runs the wgmma step: build what this handle lacks (a handle whose max_batch is
+    // below 9 or above 32 has no tensor-core state yet)
+    if ((flags & CTB_ENGINE_FP16_WEIGHTS) ? (rc = fp16_setup(h)) : (!h->tc_wqkv && (rc = tc_setup(h)))) return rc;
+    if ((flags & CTB_ENGINE_FP16_KV) && !(flags & CTB_ENGINE_FP16_WEIGHTS)) {
+      if ((rc = set_tc_attr<DE_QKV, 16, CS_QKV, CTB_ENGINE_FP16_KV>())) return rc;
+      if ((rc = set_tc_attr<DE_QKV, 32, CS_QKV, CTB_ENGINE_FP16_KV>())) return rc;
+    }
+  }
   if (!h->rows) {
     if ((rc = dalloc(&h->rows, (size_t)h->bpad_max))) return rc;
     if ((rc = dalloc(&h->cfgs, (size_t)c.max_batch))) return rc;
@@ -1053,10 +1227,10 @@ extern "C" int ctb_gpt_engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, 
     if ((rc = dalloc(&h->eng_text_idx, (size_t)c.max_batch))) return rc;
   }
   // S rows of audio codes or text, each slot owning a fixed page range of max_context tokens; PDL chain (S <= 8) or wgmma
-  // step (S >= 9) - the one-kernel steps are never selected (use_flow, enqueue_step)
-  h->engine = 1; h->phase = RS_RUNNING;
+  // step (S >= 9, and every half-precision engine) - the one-kernel steps are never selected (use_flow, enqueue_step)
+  h->engine = 1; h->phase = RS_RUNNING; h->prec = flags;
   h->B = S; h->T0 = 0; h->max_new = max_new_cap; h->infer_text = 0;
-  h->use_tc = h->tc_ready && S >= h->tc_min_batch;
+  h->use_tc = flags ? true : h->tc_ready && S >= h->tc_min_batch;
   h->q_noise = h->eng_noise; h->emb = nullptr; h->mask = nullptr;
   h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev; h->eng_text = 0;
   if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }

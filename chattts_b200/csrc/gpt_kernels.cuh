@@ -570,7 +570,7 @@ __global__ void k_input(const InputP p) {
 struct AttnP {
   const LoopState* st; int check_finished;
   const float* q;        // [Bpad, Hq*hd]
-  const float* kv;       // this layer's pool
+  const float* kv;       // this layer's pool (elements of k_attn's KVT)
   const int* block_table; int pages_per_row;
   const int* pos; const uint8_t* active;
   float* out;            // [Bpad, Hq*hd]
@@ -585,8 +585,10 @@ struct AttnP {
 // Each warp owns ATT_CHUNK/4 keys of the CTA's chunk: 8 lanes per key row, all K and V rows of the warp
 // are requested up front (one memory round trip), softmax statistics stay in registers; the four warps
 // merge through shared memory and the CTA publishes (m, l, o[64]); the last CTA of a (row, head)
-// merges the splits (flash-decoding).
+// merges the splits (flash-decoding).  KVT: the cache's element type (float, or __half for a half-precision slot
+// engine: each 8-dim slice is one 16-byte load widened to fp32; the arithmetic is the same).
 #ifdef CTB_GPT_KERNELS_IMPL
+template <typename KVT>
 __global__ void __launch_bounds__(ATT_THREADS) k_attn(const AttnP p) {
   pdl_trigger();
   pdl_wait();
@@ -631,12 +633,9 @@ __global__ void __launch_bounds__(ATT_THREADS) k_attn(const AttnP p) {
       k0[i] = k1[i] = v0[i] = v1[i] = make_float4(0.f, 0.f, 0.f, 0.f);
       if (t < n) {
         const int page = bt[t / kPageTokens];
-        const float* kr = p.kv + kv_off(page, 0, hk, t % kPageTokens, p.Hkv, HD) + sub * 8;
-        const float* vr = p.kv + kv_off(page, 1, hk, t % kPageTokens, p.Hkv, HD) + sub * 8;
-        k0[i] = ldg_cg(reinterpret_cast<const float4*>(kr));
-        k1[i] = ldg_cg(reinterpret_cast<const float4*>(kr + 4));
-        v0[i] = ldg_cg(reinterpret_cast<const float4*>(vr));
-        v1[i] = ldg_cg(reinterpret_cast<const float4*>(vr + 4));
+        const KVT* kv = reinterpret_cast<const KVT*>(p.kv);
+        ld_kv8(kv + kv_off(page, 0, hk, t % kPageTokens, p.Hkv, HD) + sub * 8, k0[i], k1[i]);
+        ld_kv8(kv + kv_off(page, 1, hk, t % kPageTokens, p.Hkv, HD) + sub * 8, v0[i], v1[i]);
       }
     }
     float sc[ITER], m = -INFINITY;

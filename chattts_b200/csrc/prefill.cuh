@@ -9,6 +9,8 @@
 //   then k_prefill_finish hands the last column's residual to the decode-loop state (x, seq_len) and the
 //   regular heads -> sampler -> finalize kernels produce the first token.
 #pragma once
+#include <type_traits>
+
 #include "gpt_kernels.cuh"
 
 namespace ctb {
@@ -55,7 +57,9 @@ struct PrefillP {
   const int* slot;          // [B] decode row (block-table row) of prompt b; nullptr: row b
 };
 
-// RoPE + KV append for every valid prompt token; grid (T0, B), 256 threads over (which, head, j)
+// RoPE + KV append for every valid prompt token; grid (T0, B), 256 threads over (which, head, j).  KVT: the cache's
+// element type (__half: K and V are rounded to nearest even as they are appended).
+template <typename KVT>
 __global__ void k_prefill_rope_kv(const PrefillP p) {
   const int c = blockIdx.x, b = blockIdx.y;
   if (!p.mask[(size_t)b * p.T0 + c]) return;
@@ -83,8 +87,8 @@ __global__ void k_prefill_rope_kv(const PrefillP p) {
       float* dst = p.q + ((size_t)b * p.T0 + c) * nq + h * p.hd;
       dst[i0] = o0; dst[i1] = o1;
     } else {
-      float* dst = p.kv + kv_off(page, which - 1, h, pos % kPageTokens, p.Hkv, p.hd);
-      dst[i0] = o0; dst[i1] = o1;
+      KVT* dst = reinterpret_cast<KVT*>(p.kv) + kv_off(page, which - 1, h, pos % kPageTokens, p.Hkv, p.hd);
+      dst[i0] = KVT(o0); dst[i1] = KVT(o1);
     }
   }
 }
@@ -94,7 +98,9 @@ __global__ void k_prefill_rope_kv(const PrefillP p) {
 // as the decode kernels), warp max; pass 2: exponentials + sum; pass 3: P.V with lane = two output dims, keys in order.
 // (Round 1 walked the queries of a (row, head) serially in one 128-thread CTA: 12 CTAs on 132 SMs and O(T^2) per CTA -
 // fine for 16-token prompts, hopeless for speaker-prompt prefixes of hundreds of tokens.)
+// KVT: the cache's element type, widened to fp32 as it is read.
 constexpr int PF_ATT_WARPS = 8;
+template <typename KVT>
 __global__ void __launch_bounds__(PF_ATT_WARPS * 32) k_prefill_attn(const PrefillP p) {
   constexpr int HD = 64;
   const int h = blockIdx.y, b = blockIdx.z, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -110,14 +116,31 @@ __global__ void __launch_bounds__(PF_ATT_WARPS * 32) k_prefill_attn(const Prefil
   float4 q[HD / 4];
 #pragma unroll
   for (int i = 0; i < HD / 4; ++i) q[i] = __ldg(reinterpret_cast<const float4*>(p.q + qrow) + i);
+  const KVT* kv = reinterpret_cast<const KVT*>(p.kv);
   float m = -INFINITY;
   for (int k = lane; k <= t; k += 32) {
-    const float4* kr = reinterpret_cast<const float4*>(p.kv + kv_off(bt[k / kPageTokens], 0, hk, k % kPageTokens, p.Hkv, HD));
     float s = 0.f;
+    if constexpr (std::is_same<KVT, float>::value) {
+      const float4* kr = reinterpret_cast<const float4*>(kv + kv_off(bt[k / kPageTokens], 0, hk, k % kPageTokens, p.Hkv, HD));
 #pragma unroll
-    for (int i = 0; i < HD / 4; ++i) {
-      const float4 kk = kr[i];
-      s = fmaf(q[i].x, kk.x, s); s = fmaf(q[i].y, kk.y, s); s = fmaf(q[i].z, kk.z, s); s = fmaf(q[i].w, kk.w, s);
+      for (int i = 0; i < HD / 4; ++i) {
+        const float4 kk = kr[i];
+        s = fmaf(q[i].x, kk.x, s); s = fmaf(q[i].y, kk.y, s); s = fmaf(q[i].z, kk.z, s); s = fmaf(q[i].w, kk.w, s);
+      }
+    } else {
+      const uint4* kr = reinterpret_cast<const uint4*>(kv + kv_off(bt[k / kPageTokens], 0, hk, k % kPageTokens, p.Hkv, HD));
+#pragma unroll
+      for (int i = 0; i < HD / 8; ++i) {
+        const uint4 u = kr[i];
+        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&w[2 * j]));
+          const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&w[2 * j + 1]));
+          const float4 qq = q[2 * i + j];
+          s = fmaf(qq.x, a.x, s); s = fmaf(qq.y, a.y, s); s = fmaf(qq.z, b.x, s); s = fmaf(qq.w, b.y, s);
+        }
+      }
     }
     s *= p.scaling;
     s_p[k] = s;
@@ -131,7 +154,10 @@ __global__ void __launch_bounds__(PF_ATT_WARPS * 32) k_prefill_attn(const Prefil
   float o0 = 0.f, o1 = 0.f;
 #pragma unroll 4
   for (int k = 0; k <= t; ++k) {
-    const float2 v = *reinterpret_cast<const float2*>(p.kv + kv_off(bt[k / kPageTokens], 1, hk, k % kPageTokens, p.Hkv, HD) + 2 * lane);
+    const KVT* vp = kv + kv_off(bt[k / kPageTokens], 1, hk, k % kPageTokens, p.Hkv, HD) + 2 * lane;
+    float2 v;
+    if constexpr (std::is_same<KVT, float>::value) v = *reinterpret_cast<const float2*>(vp);
+    else v = __half22float2(*reinterpret_cast<const __half2*>(vp));
     const float pk = s_p[k];
     o0 = fmaf(pk, v.x, o0); o1 = fmaf(pk, v.y, o1);
   }

@@ -15,6 +15,11 @@
 //     are made adjacent by a row permutation applied once when the tensor-core weight copy is built.
 //   * 4-stage TMA/mbarrier ring; weight tiles of the first stages are requested BEFORE griddepcontrol.wait
 //     (PDL), activations after it.
+//   * half-precision slot engine (PREC & TD_W16): the weight copy is fp16 (8 KiB tiles by TMA, unswizzled).  The
+//     worker warpgroup widens a tile into the fp32 128-byte-swizzled tile the descriptors read; an fp16 value is
+//     exactly a tf32 value, so W_lo = 0 and one MMA per k-step, W x [x_hi ; x_lo], is the whole product.  k order,
+//     split-K and epilogues are those of the fp32 kernel (same results on fp16-representable weights).
+//     PREC & TD_KV16: the QKV epilogue appends K/V to an fp16 cache.
 #pragma once
 #include "gpt_kernels.cuh"
 #include "tc_common.cuh"
@@ -22,15 +27,21 @@
 namespace ctb {
 
 enum DecEpi { DE_QKV = 0, DE_OPROJ = 1, DE_GATEUP = 2, DE_DOWN = 3, DE_HEADS = 4 };
+enum DecPrec { TD_W16 = 1, TD_KV16 = 2 };  // the bits of CTB_ENGINE_FP16_WEIGHTS / CTB_ENGINE_FP16_KV
 
 constexpr int TD_STAGES = 3;  // 3 x 36-48 KiB: two CTAs (this kernel + its PDL successor) fit one SM
 constexpr int TD_THREADS = 160;  // warps 0-3: one warpgroup (rms, W split, wgmma, epilogue); warp 4: TMA
 constexpr int TD_A_BYTES = 128 * 32 * 4;  // 16 KiB weight tile (128 rows x 32 k)
+constexpr int TD_A16_BYTES = 128 * 32 * 2;  // 8 KiB fp16 weight tile as TMA lands it
 
-template <int NPAD>
+template <int NPAD, bool W16 = false>
 struct TdCfg {
   static constexpr int X_BYTES = NPAD * 128;                       // one x tile (NPAD rows x 32 k)
-  static constexpr int STAGE_BYTES = 2 * TD_A_BYTES + 2 * X_BYTES;  // W | W_lo | x_hi | x_lo
+  // fp32: W | W_lo | x_hi | x_lo      fp16: W (widened) | x_hi | x_lo | W16
+  static constexpr int X_OFF = W16 ? TD_A_BYTES : 2 * TD_A_BYTES;
+  static constexpr int W16_OFF = X_OFF + 2 * X_BYTES;
+  static constexpr int W_TX = W16 ? TD_A16_BYTES : TD_A_BYTES;  // weight bytes TMA brings per stage
+  static constexpr int STAGE_BYTES = W16 ? W16_OFF + TD_A16_BYTES : 2 * TD_A_BYTES + 2 * X_BYTES;
   static constexpr int SMEM_BYTES = TD_STAGES * STAGE_BYTES + 1024 + 512;
 };
 
@@ -48,11 +59,12 @@ struct TcDecP {
   const RowState* rows; int want;  // HEADS in slot-engine mode: only rows matching `want` (nullptr: every row)
 };
 
-template <int EPI, int NPAD, int CS>
+template <int EPI, int NPAD, int CS, int PREC>
 __global__ void __launch_bounds__(TD_THREADS, 1)
 k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_xhi,
          const __grid_constant__ CUtensorMap map_xlo, const TcDecP p) {
-  using Cfg = TdCfg<NPAD>;
+  constexpr bool W16 = (PREC & TD_W16) != 0;
+  using Cfg = TdCfg<NPAD, W16>;
   pdl_trigger();
   extern __shared__ uint8_t td_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(td_smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -89,25 +101,26 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
     // ===================== TMA producer
     if (lane == 0) {
       const int pre = min(nk, TD_STAGES);
+      constexpr int W_DST = W16 ? Cfg::W16_OFF : 0;
       for (int t = 0; t < pre; ++t) {  // weights do not depend on earlier kernels
         uint8_t* st = smem + t * Cfg::STAGE_BYTES;
-        mbar_expect_tx(&full[t], TD_A_BYTES + 2 * Cfg::X_BYTES);
-        tma_load_2d(st, &map_w, &full[t], kbase + t * 32, r_tile);
+        mbar_expect_tx(&full[t], Cfg::W_TX + 2 * Cfg::X_BYTES);
+        tma_load_2d(st + W_DST, &map_w, &full[t], kbase + t * 32, r_tile);
       }
       pdl_wait();  // activations below were written by the previous kernel
       for (int t = 0; t < pre; ++t) {
         uint8_t* st = smem + t * Cfg::STAGE_BYTES;
-        tma_load_2d(st + 2 * TD_A_BYTES, &map_xhi, &full[t], kbase + t * 32, 0);
-        tma_load_2d(st + 2 * TD_A_BYTES + Cfg::X_BYTES, &map_xlo, &full[t], kbase + t * 32, 0);
+        tma_load_2d(st + Cfg::X_OFF, &map_xhi, &full[t], kbase + t * 32, 0);
+        tma_load_2d(st + Cfg::X_OFF + Cfg::X_BYTES, &map_xlo, &full[t], kbase + t * 32, 0);
       }
       for (int t = pre; t < nk; ++t) {
         const int s = t % TD_STAGES, it = t / TD_STAGES;
         mbar_wait(&empty[s], (it - 1) & 1);
         uint8_t* st = smem + s * Cfg::STAGE_BYTES;
-        mbar_expect_tx(&full[s], TD_A_BYTES + 2 * Cfg::X_BYTES);
-        tma_load_2d(st, &map_w, &full[s], kbase + t * 32, r_tile);
-        tma_load_2d(st + 2 * TD_A_BYTES, &map_xhi, &full[s], kbase + t * 32, 0);
-        tma_load_2d(st + 2 * TD_A_BYTES + Cfg::X_BYTES, &map_xlo, &full[s], kbase + t * 32, 0);
+        mbar_expect_tx(&full[s], Cfg::W_TX + 2 * Cfg::X_BYTES);
+        tma_load_2d(st + W_DST, &map_w, &full[s], kbase + t * 32, r_tile);
+        tma_load_2d(st + Cfg::X_OFF, &map_xhi, &full[s], kbase + t * 32, 0);
+        tma_load_2d(st + Cfg::X_OFF + Cfg::X_BYTES, &map_xlo, &full[s], kbase + t * 32, 0);
       }
     }
   } else {
@@ -168,20 +181,37 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
       const int s = t % TD_STAGES, it = t / TD_STAGES;
       mbar_wait(&full[s], it & 1);
       float4* a = reinterpret_cast<float4*>(smem + s * Cfg::STAGE_BYTES);
-      float4* lo = reinterpret_cast<float4*>(smem + s * Cfg::STAGE_BYTES + TD_A_BYTES);
+      if constexpr (W16) {
+        // [128 rows][32 k] fp16, 64 B per row -> fp32 rows of 128 B, 16-byte chunk c stored at chunk c ^ (row & 7)
+        // (the 128-byte swizzle TMA applies to the fp32 tiles)
+        const uint4* w16 = reinterpret_cast<const uint4*>(smem + s * Cfg::STAGE_BYTES + Cfg::W16_OFF);
 #pragma unroll
-      for (int j = 0; j < TD_A_BYTES / 16 / 128; ++j) {
-        const int i = threadIdx.x + 128 * j;
-        const float4 v = a[i];
-        float4 h, l;
-        h.x = to_tf32(v.x); h.y = to_tf32(v.y); h.z = to_tf32(v.z); h.w = to_tf32(v.w);
-        l.x = to_tf32(v.x - h.x); l.y = to_tf32(v.y - h.y); l.z = to_tf32(v.z - h.z); l.w = to_tf32(v.w - h.w);
-        a[i] = h; lo[i] = l;
+        for (int j = 0; j < TD_A16_BYTES / 16 / 128; ++j) {
+          const int i = threadIdx.x + 128 * j, r = i >> 2, c = 2 * (i & 3);
+          const uint4 u = w16[i];
+          const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
+          const float2 f1 = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+          const float2 f2 = __half22float2(*reinterpret_cast<const __half2*>(&u.z));
+          const float2 f3 = __half22float2(*reinterpret_cast<const __half2*>(&u.w));
+          a[r * 8 + (c ^ (r & 7))] = make_float4(f0.x, f0.y, f1.x, f1.y);
+          a[r * 8 + ((c + 1) ^ (r & 7))] = make_float4(f2.x, f2.y, f3.x, f3.y);
+        }
+      } else {
+        float4* lo = reinterpret_cast<float4*>(smem + s * Cfg::STAGE_BYTES + TD_A_BYTES);
+#pragma unroll
+        for (int j = 0; j < TD_A_BYTES / 16 / 128; ++j) {
+          const int i = threadIdx.x + 128 * j;
+          const float4 v = a[i];
+          float4 h, l;
+          h.x = to_tf32(v.x); h.y = to_tf32(v.y); h.z = to_tf32(v.z); h.w = to_tf32(v.w);
+          l.x = to_tf32(v.x - h.x); l.y = to_tf32(v.y - h.y); l.z = to_tf32(v.z - h.z); l.w = to_tf32(v.w - h.w);
+          a[i] = h; lo[i] = l;
+        }
       }
       fence_async_smem();  // generic-proxy writes -> visible to the tensor core (async proxy)
       warpgroup_bar(2);
       const uint32_t st = smem_u32(smem + s * Cfg::STAGE_BYTES);
-      const uint32_t w_hi = st, w_lo = st + TD_A_BYTES, x_hl = st + 2 * TD_A_BYTES;
+      const uint32_t w_hi = st, w_lo = st + TD_A_BYTES, x_hl = st + Cfg::X_OFF;
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
@@ -190,13 +220,13 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
         for (int hf = 0; hf < 2; ++hf) {
           const uint32_t ro = hf * (TD_A_BYTES / 2);  // 64 rows x 128 B
           // cols [0,NPAD) += W_hi x_hi ; cols [NPAD,2NPAD) += W_hi x_lo   (x_hi | x_lo tiles are contiguous)
-          // cols [0,NPAD) += W_lo x_hi
+          // cols [0,NPAD) += W_lo x_hi   (fp32 weights only)
           if constexpr (NPAD == 16) {
             wgmma_tf32_n32(acc[hf], wgmma_desc_sw128(w_hi + ro + ko), wgmma_desc_sw128(x_hl + ko), (t | k) ? 1u : 0u);
-            wgmma_tf32_n16(acc[hf], wgmma_desc_sw128(w_lo + ro + ko), wgmma_desc_sw128(x_hl + ko), 1u);
+            if constexpr (!W16) wgmma_tf32_n16(acc[hf], wgmma_desc_sw128(w_lo + ro + ko), wgmma_desc_sw128(x_hl + ko), 1u);
           } else {
             wgmma_tf32_n64(acc[hf], wgmma_desc_sw128(w_hi + ro + ko), wgmma_desc_sw128(x_hl + ko), (t | k) ? 1u : 0u);
-            wgmma_tf32_n32(acc[hf], wgmma_desc_sw128(w_lo + ro + ko), wgmma_desc_sw128(x_hl + ko), 1u);
+            if constexpr (!W16) wgmma_tf32_n32(acc[hf], wgmma_desc_sw128(w_lo + ro + ko), wgmma_desc_sw128(x_hl + ko), 1u);
           }
         }
       }
@@ -264,8 +294,9 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
           *reinterpret_cast<float2*>(p.qbuf + (size_t)b * nq + h * p.hd + pp) = make_float2(o0, o1);
         } else {
           const int page = __ldg(p.block_table + b * p.pages_per_row + pos / kPageTokens);
-          float* dst = p.kv + kv_off(page, which - 1, h, pos % kPageTokens, p.Hkv, p.hd);
-          *reinterpret_cast<float2*>(dst + pp) = make_float2(o0, o1);
+          const size_t off = kv_off(page, which - 1, h, pos % kPageTokens, p.Hkv, p.hd) + pp;
+          if constexpr ((PREC & TD_KV16) != 0) st_kv2(reinterpret_cast<__half*>(p.kv) + off, o0, o1);
+          else *reinterpret_cast<float2*>(p.kv + off) = make_float2(o0, o1);
         }
       } else if (EPI == DE_OPROJ || EPI == DE_DOWN) {
         float* xr = p.xres + (size_t)b * p.d + R;
@@ -300,5 +331,11 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
 //   unchanged; mode 2: [gate; up] -> interleaved (gate_n -> 2n, up_n -> 2n+1)
 __global__ void k_build_tc_weight(const float* __restrict__ W, const float* __restrict__ scale, float* __restrict__ out,
                                   int rows, int K, int mode, int qk_rows, int hd, int I);
+// the half-precision engine's copies of one layer matrix: v = W[r * K + k] * (scale ? scale[k] : 1) in fp32, then
+// out16[perm(r) * K + k] = fp16_rne(v) (decode layout, as above) and out32[r * K + k] = fp16_rne(v) as fp32 (the
+// blob's layout, for the prefill GEMMs); *bad = 1 if some |v| > 65504 (not representable in fp16)
+__global__ void k_build_tc_weight16(const float* __restrict__ W, const float* __restrict__ scale, __half* __restrict__ out16,
+                                    float* __restrict__ out32, int rows, int K, int mode, int qk_rows, int hd, int I,
+                                    int* __restrict__ bad);
 
 }  // namespace ctb

@@ -442,7 +442,8 @@ def stream_schedule(requests: List[Request], dev, chunk: int, context=None, stat
 class EngineDevice:
     """The device layer of ``schedule`` on a GPT handle (ctb_gpt_engine_begin / _admit / _status, ctb_gpt_decode)."""
 
-    def __init__(self, gpt, requests: Sequence[Request], slots: int, max_new_cap: int, return_hidden: bool = True):
+    def __init__(self, gpt, requests: Sequence[Request], slots: int, max_new_cap: int, return_hidden: bool = True,
+                 flags: int = 0):
         self.gpt, self.requests, self.slots = gpt, requests, slots
         self.lib = _lib.load()
         dev = gpt.device_gpt
@@ -451,8 +452,8 @@ class EngineDevice:
         self.ids_out = torch.zeros(slots, max_new_cap, gpt.num_vq, dtype=torch.int32, device=dev)
         self.hid_out = (torch.zeros(slots, max_new_cap, gpt.config.hidden_size, dtype=torch.float32, device=dev)
                         if return_hidden else None)
-        _lib.check(self.lib.ctb_gpt_engine_begin(
-            gpt._handle, slots, max_new_cap, C.c_void_p(self.ids_out.data_ptr()),
+        _lib.check(self.lib.ctb_gpt_engine_begin_ex(
+            gpt._handle, slots, max_new_cap, flags, C.c_void_p(self.ids_out.data_ptr()),
             C.c_void_p(self.hid_out.data_ptr()) if self.hid_out is not None else None, self.stream))
         self._state = (C.c_int32 * slots)()
         self._end = torch.zeros(slots, dtype=torch.int32)

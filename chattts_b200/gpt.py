@@ -229,7 +229,7 @@ class GPT:
     @torch.no_grad()
     def generate_continuous(self, requests, slots: Optional[int] = None, return_hidden=True, infer_text=False,
                             stream=False, return_attn=False, context=None, chunk: Optional[int] = None,
-                            max_new_cap: Optional[int] = None):
+                            max_new_cap: Optional[int] = None, dtype=torch.float32):
         """Generate audio codes or text for many utterances on a slot engine (chattts_b200.engine): up to ``slots``
         requests (default: ``max_batch``, at most the number of requests) decode together, and a waiting request takes
         the place of a finished one at the next poll (every ``chunk`` steps, default CTB_DECODE_CHUNK or 32).  Each
@@ -244,8 +244,14 @@ class GPT:
         Follow-ups (``Request.then``) are yielded under new indices, ``len(requests)`` on; ``last_schedule_stats
         .children`` maps each request index to its follow-up's.  ``max_new_cap`` (default: the largest
         ``max_new_token`` of ``requests``) bounds every request's ``max_new_token``, follow-ups included: the engine's
-        output buffers are sized by it."""
-        from .engine import EngineDevice, ScheduleStats, schedule
+        output buffers are sized by it.
+
+        ``dtype=torch.float16`` runs a half-precision engine (ctb_gpt_engine_begin_ex): the four matrices of every
+        layer and the KV cache in fp16, everything else fp32 (the model the reference serves with
+        ``Chat.load(use_vllm=True)``).  Its ids then follow that model, not ``generate``'s fp32 one."""
+        from .engine import ScheduleStats, schedule
+
+        flags = _lib.engine_flags(dtype)
 
         if stream:
             raise ValueError("generate_continuous: stream=True is not supported; results are yielded per request "
@@ -255,7 +261,7 @@ class GPT:
         if not requests:
             return
         with torch.cuda.device(self.device_gpt):
-            dev = EngineDevice(self, requests, S, cap, return_hidden)
+            dev = self._engine_device(requests, S, cap, return_hidden, flags)
             self.last_schedule_stats = stats = ScheduleStats()  # admissions, decode steps (tools/bench_continuous.py)
             for i, slot, n in schedule(requests, dev, chunk, context, stats, check):
                 yield i, (dev.empty(i) if slot is None else dev.harvest(slot, n))
@@ -265,7 +271,7 @@ class GPT:
     @torch.no_grad()
     def generate_continuous_stream(self, requests, slots: Optional[int] = None, return_hidden=True, context=None,
                                    chunk: Optional[int] = None, infer_text=False, return_attn=False,
-                                   max_new_cap: Optional[int] = None):
+                                   max_new_cap: Optional[int] = None, dtype=torch.float32):
         """Streaming form of ``generate_continuous``: generator of ``(request_index, GenerationOutputs, last)``.
 
         For each request the yields are exactly those ``generate(stream=True, stream_batch=r.stream_batch)`` makes for
@@ -277,31 +283,34 @@ class GPT:
         served as in ``generate_continuous``.
 
         ``ids`` are copies.  ``hiddens`` are views into the engine's buffer, like the narrowed views ``generate``
-        hands out: they stay valid until this generator is resumed (copy them to keep them)."""
+        hands out: they stay valid until this generator is resumed (copy them to keep them).  ``dtype`` as in
+        ``generate_continuous``."""
+        flags = _lib.engine_flags(dtype)
         for dev, batch in self._stream_polls(requests, slots, return_hidden, context, chunk, infer_text, return_attn,
-                                             max_new_cap):
+                                             max_new_cap, flags):
             for i, slot, n, last in batch:
                 yield i, (dev.empty(i) if slot is None else dev.harvest(slot, n, copy=False)), last
 
     def _stream_polls(self, requests, slots=None, return_hidden=True, context=None, chunk=None, infer_text=False,
-                      return_attn=False, max_new_cap=None):
+                      return_attn=False, max_new_cap=None, flags=0):
         """``(EngineDevice, [(request_index, slot, n_tokens, last)])`` once per poll (engine.stream_schedule): every
         yield due at that poll, while the engine's buffers hold all of them."""
-        from .engine import EngineDevice, ScheduleStats, stream_schedule
+        from .engine import ScheduleStats, stream_schedule
 
         requests, S, chunk, context, cap, check = self._engine_args(
             "generate_continuous_stream", requests, slots, infer_text, return_attn, context, chunk, None, max_new_cap)
         if not requests:
             return
         with torch.cuda.device(self.device_gpt):
-            dev = EngineDevice(self, requests, S, cap, return_hidden)
+            dev = self._engine_device(requests, S, cap, return_hidden, flags)
             self.last_schedule_stats = stats = ScheduleStats()
             for batch in stream_schedule(requests, dev, chunk, context, stats, check):
                 yield dev, batch
             if stats.interrupted:
                 self.logger.warning("generation is interrupted")
 
-    def open_engine(self, slots: int, max_new_cap: int, return_hidden=True, chunk: Optional[int] = None):
+    def open_engine(self, slots: int, max_new_cap: int, return_hidden=True, chunk: Optional[int] = None,
+                    dtype=torch.float32):
         """A slot engine that takes requests while it decodes: ``submit(request, stream=False) -> engine.Job`` from
         any thread, ``Job.cancel()`` for one request, ``close(cancel=False)`` (or a ``with`` block) to drain it.
 
@@ -311,21 +320,30 @@ class GPT:
         (copies), and simply ends when cancelled.  ``submit`` checks the request against this handle and
         ``max_new_cap`` in the caller's thread.  One worker thread owns the handle and its stream; while the engine
         is open ``generate``, ``generate_continuous*`` and another ``open_engine`` raise.  The poll interval is
-        ``chunk`` steps (default CTB_DECODE_CHUNK, else 24)."""
+        ``chunk`` steps (default CTB_DECODE_CHUNK, else 24).  ``dtype`` as in ``generate_continuous``."""
         from .engine import GptEngine
 
-        return self._open_slot_engine(GptEngine, slots, max_new_cap, return_hidden, chunk)
+        return self._open_slot_engine(GptEngine, slots, max_new_cap, return_hidden, chunk,
+                                      flags=_lib.engine_flags(dtype))
 
-    def _open_slot_engine(self, cls, slots, max_new_cap, return_hidden, chunk, *args):
-        """An ``engine.OpenEngine`` subclass ``cls`` that owns this handle until it is closed."""
-        from .engine import EngineDevice
-
+    def _open_slot_engine(self, cls, slots, max_new_cap, return_hidden, chunk, *args, flags=0):
+        """An ``engine.OpenEngine`` subclass ``cls`` that owns this handle until it is closed (``flags``: the
+        ctb_gpt_engine_begin_ex precision flags)."""
         _, S, chunk, _, cap, check = self._engine_args("open_engine", [], slots, False, False, None, chunk, None,
                                                        max_new_cap)
-        engine = cls(lambda requests: EngineDevice(self, requests, S, cap, return_hidden), chunk, check,
+        engine = cls(lambda requests: self._engine_device(requests, S, cap, return_hidden, flags), chunk, check,
                      self.device_gpt, self._close_engine, *args, max_new_cap=cap)
         self._open = engine
         return engine
+
+    def _engine_device(self, requests, S, cap, return_hidden, flags):
+        """The ``engine.EngineDevice`` of one slot engine; an fp32 engine gets the five-argument form that stand-in
+        devices implement."""
+        from . import engine
+
+        if flags:
+            return engine.EngineDevice(self, requests, S, cap, return_hidden, flags=flags)
+        return engine.EngineDevice(self, requests, S, cap, return_hidden)
 
     def _close_engine(self):
         self._open = None

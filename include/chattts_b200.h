@@ -156,6 +156,28 @@ int ctb_gpt_status_query(ctb_gpt* h, ctb_gpt_status* out, int32_t* end_idx_host,
 int ctb_gpt_engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t* ids_out_dev, float* hiddens_out_dev,
                          void* stream);
 
+/* ctb_gpt_engine_begin with precision flags (flags = 0 is ctb_gpt_engine_begin).  The half-precision engine is the
+ * model the reference serves with its vLLM fork (dtype "auto" runs a float32 checkpoint in float16), except that the
+ * heads stay fp32 as in every reference mode:
+ *   CTB_ENGINE_FP16_WEIGHTS  the four matrices of every layer are stored in fp16, rounded to nearest even: Wqkv and
+ *                            [Wgate; Wup] after the fp32 fold of input_layernorm / post_attention_layernorm into
+ *                            their columns (the activations then enter as x * rsqrt(mean(x^2) + eps)), Wo and Wdown as
+ *                            they are.  Prefill uses the same rounded values.
+ *   CTB_ENGINE_FP16_KV       K (after RoPE) and V are rounded to fp16 as they are appended; every attention, prompt
+ *                            and decode, reads the rounded values.  K/V overflow is not checked (nor is it in the
+ *                            reference's fp16 modes).
+ * Embeddings, RMSNorm statistics, RoPE, activations, attention arithmetic, the heads, the sampler and the hidden
+ * states in hiddens_out_dev stay fp32.  A flagged engine always runs the wgmma step with 16 (S <= 16) or 32 padded
+ * rows and builds what the handle lacks for it; the fp16 copies (377.5 MB for the 20 layers, plus their 755 MB fp32
+ * image read by the prefill GEMMs) are built by the first CTB_ENGINE_FP16_WEIGHTS engine and kept until
+ * ctb_gpt_destroy.  The KV pool is sized in bytes and shared by every call on the handle.
+ * Errors (CTB_ERR_ARG): unknown flag bits; S > 32 with a flag set; a flag set while CTB_GPT_FMA=1; a layer weight
+ * (norm folded) with |w| > 65504, named by layer and matrix in ctb_last_error - the handle is left as it was. */
+#define CTB_ENGINE_FP16_WEIGHTS 1
+#define CTB_ENGINE_FP16_KV 2
+int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t flags, int32_t* ids_out_dev,
+                            float* hiddens_out_dev, void* stream);
+
 /* Admit n requests into the idle or finished slots slots[0..n) (host array): prefill their prompts (token-parallel,
  * left padded, 8 <= T0 <= 1024: pad shorter prompts with masked columns) into those slots and sample each one's first
  * token; no other slot's state, outputs or KV pages are touched.

@@ -2,6 +2,7 @@
 """Continuous-batching benchmark: the slot engine against static batches, one JSON line.
 
     python tools/bench_continuous.py [--requests N] [--slots S] [--steps K] [--warmup W] [--dump-outputs DIR] [--stream]
+                                     [--dtype float16]
                                      [--refine] [--online RATE[,RATE...] [--cancel FRACTION]]
     python tools/bench_continuous.py --paragraphs N [--refine] [--slots S] [--steps K] [--warmup W]
 
@@ -11,6 +12,8 @@ tokens, min_new = max_new: synthetic weights have no meaningful EOS), run throug
 run to their longest row (``GPT.generate``).  Reports useful speech-tokens/s of both arms (the tokens the requests
 asked for), mean slot occupancy, the card and its power limit.  ``--steps`` = timed repeats of each arm, alternating.
 ``--dump-outputs DIR`` writes both arms' ids (concatenated in request order) and the lengths as DIR/<name>.npy.
+``--dtype float16`` adds a third arm, alternated with the others: the half-precision slot engine (fp16 layer weights
+and KV cache) on the same requests.
 
 ``--refine`` prints one more JSON line: each request is a text-refinement stage (16..160 forced text tokens) followed by
 its speech codes (the forced lengths above), through S slots, timed alternately in three arms: (a) both stages on the
@@ -113,8 +116,8 @@ def run_continuous(args, local_rank: int = 0):
     reqs = [Request(emb=embs[i], temperature=temp, eos_token=625, max_new_token=tok[i], min_new_token=tok[i],
                     logits_processors=procs, manual_seed=5000 + i) for i in range(n)]
 
-    def engine_arm(rs):
-        out = {i: o.ids[0] for i, o in gpt.generate_continuous(rs, slots=S, return_hidden=False)}
+    def engine_arm(rs, dtype=torch.float32):
+        out = {i: o.ids[0] for i, o in gpt.generate_continuous(rs, slots=S, return_hidden=False, dtype=dtype)}
         torch.cuda.synchronize()
         return out, gpt.last_schedule_stats
 
@@ -139,16 +142,24 @@ def run_continuous(args, local_rank: int = 0):
 
     # warm-up: both arms on a short version of the workload (graph capture, buffer growth, module loads)
     short = [min(t, 64) for t in tok]
+    fp16 = args.dtype == "float16"  # a third arm: the half-precision engine on the same requests
     for _ in range(max(1, min(args.warmup, 2))):
-        engine_arm([Request(emb=r.emb, temperature=temp, eos_token=625, max_new_token=64, min_new_token=64,
-                            logits_processors=procs, manual_seed=r.manual_seed) for r in reqs[: 2 * S]])
+        warm = [Request(emb=r.emb, temperature=temp, eos_token=625, max_new_token=64, min_new_token=64,
+                        logits_processors=procs, manual_seed=r.manual_seed) for r in reqs[: 2 * S]]
+        engine_arm(warm)
+        if fp16:
+            engine_arm(warm, torch.float16)
         static_arm(list(range(2 * S)), short)
     useful = sum(tok)
-    t_eng, t_sta = [], []
+    t_eng, t_sta, t_e16 = [], [], []
     for _ in range(args.steps):
         t0 = time.perf_counter()
         eng, stats = engine_arm(reqs)
         t_eng.append(time.perf_counter() - t0)
+        if fp16:
+            t0 = time.perf_counter()
+            eng16, stats16 = engine_arm(reqs, torch.float16)
+            t_e16.append(time.perf_counter() - t0)
         t0 = time.perf_counter()
         sta, static_steps = static_arm(list(range(n)), tok)
         t_sta.append(time.perf_counter() - t0)
@@ -159,6 +170,14 @@ def run_continuous(args, local_rank: int = 0):
     name, limit = gpu_card(local_rank)
     med = lambda v: sorted(v)[len(v) // 2]  # noqa: E731
     te, ts = med(t_eng), med(t_sta)
+    extra = {}
+    if fp16:
+        t16 = med(t_e16)
+        extra = {"engine_fp16": {"tokens_per_s": round(useful / t16, 1), "seconds": round(t16, 3),
+                                 "seconds_all": [round(t, 3) for t in t_e16], "decode_steps": stats16.decode_steps,
+                                 "admissions": stats16.admissions,
+                                 "ids_equal_to_fp32_engine": sum(torch.equal(eng16[i], eng[i]) for i in range(n))},
+                 "fp16_over_fp32_engine": round(te / t16, 3)}
     return {
         "metric": "continuous_useful_speech_tokens_per_s", "unit": "tokens/s", "card": name, "power_limit": limit,
         "requests": n, "slots": S, "prompt_tokens": [min(plen), max(plen)], "forced_tokens": [min(tok), max(tok)],
@@ -170,7 +189,7 @@ def run_continuous(args, local_rank: int = 0):
         "static": {"tokens_per_s": round(useful / ts, 1), "seconds": round(ts, 3),
                    "seconds_all": [round(t, 3) for t in t_sta], "decode_steps": static_steps,
                    "mean_slot_occupancy": round(useful / (S * static_steps), 4)},
-        "speedup": round(ts / te, 3),
+        "speedup": round(ts / te, 3), **extra,
     }
 
 
@@ -844,6 +863,8 @@ def main():
     ap.add_argument("--slots", type=int, default=32, help="engine slots = static batch rows")
     ap.add_argument("--steps", type=int, default=3, help="timed repeats of each arm")
     ap.add_argument("--warmup", type=int, default=1)
+    ap.add_argument("--dtype", choices=("float32", "float16"), default="float32",
+                    help="float16: also time the half-precision slot engine on the same requests (a third arm)")
     ap.add_argument("--dump-outputs", default=None, metavar="DIR")
     ap.add_argument("--stream", action="store_true", help="also measure streamed audio (a second JSON line)")
     ap.add_argument("--refine", action="store_true", help="also measure refinement + speech (one more JSON line); "
