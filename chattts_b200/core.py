@@ -214,10 +214,11 @@ class Chat:
                          skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
                          params_refine_text=None, refine_on_engine=False, split_text=False, max_split_batch=1,
                          dtype=torch.float32):
-        """Synthesise many texts with continuous batching (``GPT.generate_continuous``): each text is one request,
-        ``params_infer_code`` is one ``InferCodeParams`` for all texts or a list with one per text (speaker, seed,
-        temperature, top-P/K, penalty, token limits).  Generator of ``(index, wav)`` in completion order; ``wav`` is
-        what ``infer([texts[index]], split_text=False, skip_refine_text=True)`` returns for that text with its params.
+        """Synthesise many texts with continuous batching: each text is one job on an open slot engine
+        (``open_engine``), all queued at once; ``params_infer_code`` is one ``InferCodeParams`` for all texts or a list
+        with one per text (speaker, seed, temperature, top-P/K, penalty, token limits).  Generator of ``(index, wav)``
+        in completion order; ``wav`` is what ``infer([texts[index]], split_text=False, skip_refine_text=True)``
+        returns for that text with its params.
         Normalisation and the optional text refinement run as in ``infer``; ``params_refine_text`` is one
         ``RefineTextParams`` or one per text.
 
@@ -233,8 +234,11 @@ class Chat:
         max_split_batch=max_split_batch, skip_refine_text=True)[0]`` returns with that text's params, which are not
         modified; with ``skip_refine_text=False`` each sentence is refined on the engine first, and ``wav`` is what
         ``infer(texts[index], max_split_batch=max_split_batch, params_refine_text=...)[0]`` returns (seeded: bit for
-        bit on the code path).  The paragraphs run on an open engine (``open_engine``); ``slots`` defaults to the
-        handle's ``max_batch``.
+        bit on the code path).
+
+        ``slots`` defaults to max(2, min(max_batch, len(texts))), with ``split_text`` to the handle's ``max_batch``.
+        ``Chat.interrupt()`` ends the running texts with what they have, or with ``split_text`` cancels every
+        unfinished paragraph (see ``_continuous``).
 
         ``dtype=torch.float16`` runs every request on a half-precision engine (``GPT.generate_continuous``): fp16
         layer weights and KV cache, as the reference's ``use_vllm=True`` serves; the waveforms then follow that model.
@@ -244,21 +248,16 @@ class Chat:
             raise ValueError("infer_continuous: stream=True is not supported; each waveform is yielded when complete "
                              "(infer_continuous_stream streams)")
         texts, params = self._continuous_params(texts, params_infer_code)
-        if split_text:
-            return self._paragraphs(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
-                                    do_homophone_replacement, False, self._refine_params(texts, params_refine_text),
-                                    max_split_batch, dtype)
-        return self._infer_continuous(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
-                                      do_homophone_replacement, self._refine_params(texts, params_refine_text),
-                                      refine_on_engine, dtype)
+        return self._continuous(texts, params, self._refine_params(texts, params_refine_text), False, use_decoder,
+                                slots, lang, skip_refine_text, do_text_normalization, do_homophone_replacement,
+                                refine_on_engine, split_text, max_split_batch, dtype)
 
     def infer_continuous_stream(self, texts, params_infer_code=None, use_decoder=True, slots=None, lang=None,
                                 skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
                                 params_refine_text=None, refine_on_engine=False, split_text=False, max_split_batch=1,
                                 dtype=torch.float32):
-        """Streaming synthesis of many texts with continuous batching (``GPT.generate_continuous_stream``).
-        Generator of ``(index, chunk, last)``, ``chunk`` a ``[1, n]`` float32 array; for each text the chunks are
-        those ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=True)`` yields with that
+        """Streaming synthesis of many texts with continuous batching on an open slot engine.  Generator of ``(index,
+        chunk, last)``, ``chunk`` a ``[1, n]`` float32 array; for each text the chunks are those ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=True)`` yields with that
         text's params (its own ``stream_batch``, ``stream_speed`` and ``pass_first_n_batches``), and ``last`` marks
         its final chunk.  A seeded text whose first code is EOS yields one empty final chunk.  All windows due at one
         engine poll are decoded in one ragged call (``TokenDecoder.decode_rows``), straight from the engine's
@@ -267,15 +266,11 @@ class Chat:
         each text is a paragraph, streamed sentence by sentence as ``ChatEngine.submit(split_text=True,
         stream=True)`` streams it, refined first with ``skip_refine_text=False``.  ``dtype`` as in
         ``infer_continuous``."""
-        flags = _lib.engine_flags(dtype)
+        _lib.engine_flags(dtype)
         texts, params = self._continuous_params(texts, params_infer_code)
-        if split_text:
-            return self._paragraphs(texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
-                                    do_homophone_replacement, True, self._refine_params(texts, params_refine_text),
-                                    max_split_batch, dtype)
-        return self._infer_continuous_stream(texts, params, use_decoder, slots, lang, skip_refine_text,
-                                             do_text_normalization, do_homophone_replacement,
-                                             self._refine_params(texts, params_refine_text), refine_on_engine, flags)
+        return self._continuous(texts, params, self._refine_params(texts, params_refine_text), True, use_decoder,
+                                slots, lang, skip_refine_text, do_text_normalization, do_homophone_replacement,
+                                refine_on_engine, split_text, max_split_batch, dtype)
 
     def refine_continuous(self, texts, params_refine_text=None, slots=None, lang=None, do_text_normalization=True,
                           do_homophone_replacement=True, dtype=torch.float32):
@@ -317,105 +312,83 @@ class Chat:
             return list(params_refine_text)
         return [params_refine_text or Chat.RefineTextParams()] * len(texts)
 
-    def _paragraphs(self, texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
-                    do_homophone_replacement, stream, refine, max_split_batch, dtype=torch.float32):
-        """``infer_continuous*(split_text=True)``: every text a paragraph job on one open engine, submitted in order.
-        Generator of ``(index, wav)`` in completion order, or of ``(index, chunk, last)`` as the chunks come."""
+    def _continuous(self, texts, params, refine, stream, use_decoder, slots, lang, skip_refine_text,
+                    do_text_normalization, do_homophone_replacement, refine_on_engine, split_text, max_split_batch,
+                    dtype):
+        """``infer_continuous*``: every text one ``ChatEngine`` job on one open engine.  Generator of ``(index, wav)``
+        in completion order, or of ``(index, chunk, last)`` as the chunks come.
+
+        Batched refinement (``skip_refine_text=False`` without ``refine_on_engine`` or ``split_text``) refines the
+        normalised texts in static batches of up to ``max_batch`` before the engine opens, and the refined texts are
+        spoken as they are: they are not normalised again.  The first stage of every text is queued in one step, so
+        the engine's first admission fills min(slots, len(texts)) slots.  ``slots`` defaults to max(2, min(max_batch,
+        len(texts))), with ``split_text`` to ``max_batch``; the poll interval is CTB_DECODE_CHUNK, else 24 with
+        ``split_text``, else the smallest ``stream_batch`` of the texts when streaming, else 32.
+
+        ``Chat.interrupt()``: a text's audio ends early only where it has no later part to wait for.  Without
+        ``split_text`` the engine stops at its first poll that sees the interrupt: every text whose speech stage is
+        running ends with the tokens it has (its silence-stripped waveform, or its final chunk with ``last=True``),
+        and a text still waiting or refining yields nothing.  With ``split_text`` a paragraph cut short would miss
+        sentences, so within one poll every unfinished paragraph is cancelled and yields nothing more.  Either way
+        "generation is interrupted" is logged and the generator ends with the handle free.  An invalid text raises
+        here; closing the generator early or an error in the engine cancels every job and frees the handle too."""
         assert self.has_loaded(use_decoder=use_decoder)
         self.context.set(False)
         if not texts:
             return
-        out: queue.Queue = queue.Queue()
-        cap = max(p.max_new_token for p in params)
-        if not skip_refine_text:
-            cap = max(cap, max(r.max_new_token for r in refine))
-        with self.open_engine(slots, max_new_cap=cap, use_decoder=use_decoder, dtype=dtype) as eng:
-            try:
-                jobs = [eng.submit(t, params_infer_code=p, stream=stream, lang=lang, split_text=True,
-                                   skip_refine_text=skip_refine_text, params_refine_text=r,
-                                   max_split_batch=max_split_batch, do_text_normalization=do_text_normalization,
-                                   do_homophone_replacement=do_homophone_replacement, _sink=(out, k))
-                        for k, (t, p, r) in enumerate(zip(texts, params, refine))]
-                left = len(jobs)
-                while left:
-                    try:
-                        k, item = out.get(timeout=0.05)
-                    except queue.Empty:
-                        if eng._stopped:  # the worker failed: close() raises its error
-                            eng.close()
-                        if self.context.get():
-                            self.logger.warning("generation is interrupted")
-                            eng.close(cancel=True)
-                            return
-                        continue
-                    if item is None:  # job k ended: its result, or its error raised here
-                        left -= 1
-                        wav = jobs[k].result()
-                        if not stream:
-                            yield k, wav
-                    elif stream:
-                        yield (k, *item)
-            except GeneratorExit:
-                eng.close(cancel=True)
-                raise
 
-    def _continuous_requests(self, texts, params, use_decoder, lang, skip_refine_text, do_text_normalization,
-                             do_homophone_replacement, refine, refine_on_engine=False):
-        """Normalisation, optional refinement and one engine request per text (as ``_infer`` prepares them) ->
-        (requests, max_new_cap).  With ``refine_on_engine`` (and refinement on) each request refines its text and
-        names the text's speech-code request as its follow-up."""
-        assert self.has_loaded(use_decoder=use_decoder)
-        self.context.set(False)
-        if not texts:
-            return [], 0
-        texts = [self.normalizer(t, do_text_normalization, do_homophone_replacement, lang) for t in texts]
+        def normalize(t):
+            return self.normalizer(t, do_text_normalization, do_homophone_replacement, lang)
+
         cap = max(p.max_new_token for p in params)
-        if not skip_refine_text and refine_on_engine:
-            requests = [self._chained_request(t, p, r) for t, p, r in zip(texts, params, refine)]
-            return requests, max(cap, max(r.max_new_token for r in requests))
-        if not skip_refine_text:
+        if not skip_refine_text and (refine_on_engine or split_text):
+            cap = max(cap, max(r.max_new_token for r in refine))
+        elif not skip_refine_text:
             if any(r is not refine[0] for r in refine):
                 raise ValueError("one RefineTextParams per text needs refine_on_engine=True (batched refinement "
                                  "draws every text of a batch with one set of parameters)")
+            texts = [normalize(t) for t in texts]
             tokens = []
             for lo in range(0, len(texts), self.gpt.max_batch):
                 refined = self._refine_text(texts[lo: lo + self.gpt.max_batch], self.device, refine[0])
                 tokens += [i[i.less(self.tokenizer.break_0_ids)] for i in refined.ids]
                 refined.destroy()
-            texts = self.tokenizer.decode(tokens)
-        return [self._code_request(t, p) for t, p in zip(texts, params)], cap
-
-    def _infer_continuous_stream(self, texts, params, use_decoder, slots, lang, skip_refine_text,
-                                 do_text_normalization, do_homophone_replacement, refine, refine_on_engine=False,
-                                 flags=0):
-        requests, cap = self._continuous_requests(texts, params, use_decoder, lang, skip_refine_text,
-                                                  do_text_normalization, do_homophone_replacement, refine,
-                                                  refine_on_engine)
-        if not requests:
-            return
-        windows = [StreamWindows(p.stream_speed, p.pass_first_n_batches) for p in params]
-        yield from stream_continuous(self.gpt, self.decoder if use_decoder else self.dvae, requests, windows,
-                                     use_decoder, slots, self.context, max_new_cap=cap, flags=flags)
-
-    def _infer_continuous(self, texts, params, use_decoder, slots, lang, skip_refine_text, do_text_normalization,
-                          do_homophone_replacement, refine, refine_on_engine=False, dtype=torch.float32):
-        requests, cap = self._continuous_requests(texts, params, use_decoder, lang, skip_refine_text,
-                                                  do_text_normalization, do_homophone_replacement, refine,
-                                                  refine_on_engine)
-        if not requests:
-            return
-        thr = np.float32(1e-5)
-        with torch.no_grad():
-            for i, out in self.gpt.generate_continuous(requests, slots=slots, return_hidden=use_decoder,
-                                                       context=self.context, max_new_cap=cap, dtype=dtype):
-                k = _text_index(self.gpt, requests, i)
-                if k is None:  # a refinement stage: its follow-up carries the text on
-                    out.destroy()
+            texts, skip_refine_text = self.tokenizer.decode(tokens), True
+            normalize = str  # the refined texts are spoken as they are
+        if slots is None:
+            slots = self.gpt.max_batch if split_text else max(2, min(self.gpt.max_batch, len(texts)))
+        env = os.environ.get("CTB_DECODE_CHUNK")
+        chunk = int(env) if env else 24 if split_text else min(p.stream_batch for p in params) if stream else 32
+        out: queue.Queue = queue.Queue()  # (k, (chunk, last)), or (k, None) once text k's job has ended
+        with self.gpt._open_slot_engine(ChatEngine, slots, cap, use_decoder, chunk, self, use_decoder,
+                                        None if split_text else self.context,
+                                        flags=_lib.engine_flags(dtype)) as eng:
+            subs = [eng._job(t, p, stream, skip_refine_text, r, split_text, max_split_batch, normalize, (out, k))
+                    for k, (t, p, r) in enumerate(zip(texts, params, refine))]
+            eng._enqueue(subs)
+            jobs = [job for job, _ in subs]
+            left = len(jobs)
+            while left:
+                if split_text and self.context.get():
+                    eng.close(cancel=True)
+                    self.logger.warning("generation is interrupted")
+                    return
+                stopped = eng._stopped  # read first: whatever the worker posted before it stopped is in `out` now
+                try:
+                    k, item = out.get(timeout=0.05)
+                except queue.Empty:
+                    if stopped:  # on an error, or on an interrupt it saw
+                        eng.close()  # raises the worker's error, if it had one
+                        self.logger.warning("generation is interrupted")
+                        return
                     continue
-                res = out.hiddens if use_decoder else out.ids
-                wav = self._decode_to_wavs(res, use_decoder)[0] if int(res[0].shape[0]) > 0 else np.zeros(0, np.float32)
-                out.destroy()
-                yield k, wav[np.abs(wav) > thr]  # quirk Q20, as infer() returns it
+                if item is None:  # job k ended: its result, or its error raised here
+                    left -= 1
+                    wav = jobs[k].result()
+                    if not stream:
+                        yield k, wav
+                elif stream:
+                    yield (k, *item)
 
     def _code_request(self, text, params, noise_batch=None):
         """The request ``_infer_code([text], ...)`` would decode as a batch of one (``noise_batch`` = (B, b): as row b
@@ -457,13 +430,6 @@ class Chat:
                        min_new_token=params.min_new_token, logits_processors=(*processors, *warpers),
                        manual_seed=params.manual_seed, ensure_non_empty=params.ensure_non_empty, infer_text=True,
                        noise_batch=noise_batch)
-
-    def _chained_request(self, text, params, refine):
-        """The text's refinement request, whose follow-up is the speech-code request of the refined text."""
-        req = self._refine_request(text, refine)
-        req.then = lambda out: self._code_request(self._refined_text(out), params)
-        req.stream_batch = params.stream_batch  # the engine polls at the smallest stream_batch of its requests
-        return req
 
     def _refined_text(self, out) -> str:
         """The text ``_infer`` makes of one refined row: ids below ``break_0_ids``, decoded."""
@@ -636,54 +602,18 @@ class StreamWindows:
         return out
 
 
-def _text_index(gpt: GPT, requests, i: int) -> Optional[int]:
-    """Engine request index -> index of the text it speaks (a follow-up speaks its parent's text); None for a text
-    request (a refinement stage)."""
-    if i < len(requests):
-        return None if requests[i].infer_text else i
-    return {c: p for p, c in gpt.last_schedule_stats.children.items()}[i]
-
-
-def stream_continuous(gpt: GPT, model: DVAE, requests, windows: List[StreamWindows], use_decoder: bool, slots=None,
-                      context=None, ragged: bool = True, stats: Optional[Dict[str, float]] = None,
-                      max_new_cap: Optional[int] = None, flags: int = 0):
-    """Streamed audio of many requests on the slot engine: generator of ``(request_index, chunk [1, n] float32, last)``.
-    Text requests stream nothing; a follow-up's chunks come under its parent's index, with its parent's windows.
-
-    At every engine poll the windows of every GPT yield due then (``GPT._stream_polls``) are decoded together: each
-    window's token range (``decoder.stream_window``) is read straight from the engine's hidden states (``model`` =
-    the DVAE decoder) or codes (``model`` = the code DVAE, ``use_decoder=False``) in one ``decode_rows`` call, and the
-    window is cut out of its row.  ``ragged=False`` decodes the windows one ``decode_to_wavs_window`` call each
-    instead (the straightforward form tools/bench_continuous.py compares against).  ``stats['path2_s']`` (optional)
-    accumulates the host time spent decoding and copying the audio.  ``flags``: the engine's
-    ctb_gpt_engine_begin_ex precision flags."""
-    import time
-
-    for dev, batch in gpt._stream_polls(requests, slots, use_decoder, context, max_new_cap=max_new_cap, flags=flags):
-        t_start = time.perf_counter()
-        jobs = []  # (text, slot, n_tokens, a, b, flush, last)
-        for i, s, n, last in batch:
-            t = _text_index(gpt, requests, i)
-            if t is None:
-                continue
-            ws = windows[t].windows(n, last)
-            jobs += [(t, s, n, a, b, flush, last and k == len(ws) - 1) for k, (a, b, flush) in enumerate(ws)]
-        out = _decode_windows(dev, jobs, model, use_decoder, ragged)
-        if stats is not None:
-            stats["path2_s"] = stats.get("path2_s", 0.0) + time.perf_counter() - t_start
-        yield from out
-
-
-def _decode_windows(dev, jobs, model: DVAE, use_decoder: bool, ragged: bool = True):
+def _decode_windows(dev, jobs, model: DVAE, use_decoder: bool):
     """One poll's path-2 work on the slot engine ``dev``: ``jobs`` are ``(key, slot, n_tokens, a, b, flush, last)``,
     samples [a, b) of the decode of the slot's first ``n_tokens`` tokens (``flush``: drop its silent samples) ->
-    ``[(key, chunk [1, m] float32, last)]`` in the same order.  Every non-empty window goes into one ``decode_rows``
-    call (``ragged=False``: one ``decode_to_wavs_window`` call each)."""
+    ``[(key, chunk [1, m] float32, last)]`` in the same order.  Each window's token range (``decoder.stream_window``)
+    is read straight from the engine's hidden states (``model`` = the DVAE decoder) or codes (``model`` = the code
+    DVAE, ``use_decoder=False``); every non-empty window goes into one ``decode_rows`` call and is cut out of its
+    row."""
     thr = np.float32(1e-5)
     buf = dev.hid_out if use_decoder else dev.ids_out
     due = [k for k, j in enumerate(jobs) if j[4] > j[3]]
     chunks: Dict[int, np.ndarray] = {}
-    if due and ragged:
+    if due:
         rows, cuts = [], []
         for k in due:
             _, s, n, a, b = jobs[k][:5]
@@ -696,10 +626,6 @@ def _decode_windows(dev, jobs, model: DVAE, use_decoder: bool, ragged: bool = Tr
         for k, (c0, c1) in zip(due, cuts):
             chunks[k] = flat[None, off: off + c1 - c0]
             off += c1 - c0
-    elif due:
-        for k in due:
-            _, s, n, a, b = jobs[k][:5]
-            chunks[k] = decode_to_wavs_window([buf[s, :n]], use_decoder, model, model, a, b)
     out = []
     for k, (i, _, _, _, _, flush, last) in enumerate(jobs):
         chunk = chunks.get(k, np.zeros((1, 0), dtype=np.float32))
@@ -710,9 +636,9 @@ def _decode_windows(dev, jobs, model: DVAE, use_decoder: bool, ragged: bool = Tr
 
 
 class _Paragraph:
-    """A paragraph job's state on ``ChatEngine``: its reference stage, which request speaks which sentence, and the
-    in-order assembly of the sentences' audio (``add``).  ``sink`` = (queue, key): the chunks and the end of the job are
-    also posted there, for ``Chat.infer_continuous*(split_text=True)``."""
+    """A job's state on ``ChatEngine`` (a text without ``split_text`` is a paragraph of one sentence): its reference
+    stage, which request speaks which sentence, and the in-order assembly of the sentences' audio (``add``).  ``sink`` =
+    (queue, key): the chunks and the end of the job are also posted there, for ``Chat.infer_continuous*``."""
 
     def __init__(self, n: int, stream_params, sink=None):
         self.n, self.sink = n, sink
@@ -805,10 +731,12 @@ class _RefineGraph:
     whichever of the two stages ends last (the join): refinement k's ``then`` returns it when the sample is known and
     None otherwise, and the reference stage's ``then`` returns the code requests of every sentence refined by then, in
     sentence order.  Without a reference stage each refinement's ``then`` returns its code request.  A refinement that
-    ended empty raises in its ``then``, which fails the job, as a seeded first-step EOS makes ``infer`` raise."""
+    ended empty raises in its ``then``, which fails the job, as a seeded first-step EOS makes ``infer`` raise; with
+    ``speak_empty`` (a text submitted without ``split_text``) the empty refined text is spoken instead."""
 
-    def __init__(self, n: int, refined_text, code, reference=None, sample=None):
+    def __init__(self, n: int, refined_text, code, reference=None, sample=None, speak_empty=False):
         self.n, self.refined_text, self.code, self.reference, self.sample = n, refined_text, code, reference, sample
+        self.speak_empty = speak_empty
         self.refined: List[Optional[str]] = [None] * n
         self.ref = None  # the reference stage's request, once refinement 0 has ended
         self.spk = None  # (spk_smp, txt_smp), once the reference stage has ended
@@ -816,7 +744,7 @@ class _RefineGraph:
 
     def then(self, k: int):
         def then(out):
-            if int(out.ids[0].shape[0]) == 0:
+            if int(out.ids[0].shape[0]) == 0 and not self.speak_empty:
                 raise RuntimeError(f"the refinement of sentence {k} of the paragraph ended empty")
             self.refined[k] = self.refined_text(out)
             if self.reference is None:
@@ -842,16 +770,16 @@ class ChatEngine(OpenEngine):
     """``Chat.open_engine``: an open slot engine whose jobs are texts (see there).  At each poll every window due for a
     streaming job and the whole sequence of every non-streaming job that completed go into one ``decode_rows`` call."""
 
-    def __init__(self, make_device, chunk, check, device, on_close, chat: "Chat", use_decoder: bool,
+    def __init__(self, make_device, chunk, check, device, on_close, chat: "Chat", use_decoder: bool, context=None,
                  max_new_cap: Optional[int] = None):
         self.chat, self.use_decoder = chat, use_decoder
         self.model = chat.decoder if use_decoder else chat.dvae
         self._sampler = _SpeakerSampler(chat, self.model, use_decoder)
-        super().__init__(make_device, chunk, check, device, on_close, max_new_cap)
+        super().__init__(make_device, chunk, check, device, on_close, max_new_cap, context)
 
     def submit(self, text: str, params_infer_code=None, stream=False, skip_refine_text=True, params_refine_text=None,
                lang=None, do_text_normalization=True, do_homophone_replacement=True, split_text=False,
-               max_split_batch=1, _sink=None) -> Job:
+               max_split_batch=1) -> Job:
         """Queue one text -> ``Job``: ``result()`` is the waveform ``infer_continuous`` yields for it, or with
         ``stream=True`` the job iterates the ``(chunk, last)`` pairs ``infer_continuous_stream`` yields for it.
         ``skip_refine_text=False`` refines the text on the engine first (``refine_on_engine=True``).  A cancelled
@@ -884,36 +812,31 @@ class ChatEngine(OpenEngine):
         request starts as soon as both its refinement and the speaker sample are done (see ``_RefineGraph``).
         ``result()`` is then what ``infer(text, use_decoder=False, max_split_batch=m, params_refine_text=...)[0]``
         returns, bit for bit on the code path when seeded (with the default arguments and m = 4: ``infer(text)``).
-        A refinement that ends empty fails the job, as it makes ``infer`` raise."""
-        chat = self.chat
-        params = params_infer_code or Chat.InferCodeParams()
-        if split_text:
-            return self._submit_paragraph(text, params, stream, skip_refine_text,
-                                          params_refine_text or Chat.RefineTextParams(), max_split_batch, lang,
-                                          do_text_normalization, do_homophone_replacement, _sink)
-        if not skip_refine_text and self.max_new_cap is not None and params.max_new_token > self.max_new_cap:
-            # the speech stage is made only when the refinement ends: check its limit here, in the caller's thread
-            raise ValueError(f"max_new_token {params.max_new_token} exceeds max_new_cap={self.max_new_cap}")
-        text = chat.normalizer(text, do_text_normalization, do_homophone_replacement, lang)
-        # the prompt is embedded here, on the caller's stream: ctb_gpt_embed_prompt is the one handle call that may run
-        # beside the worker (it only reads the weights); submit orders the engine's stream after the caller's
-        if skip_refine_text:
-            request = chat._code_request(text, params)
-        else:
-            request = chat._chained_request(text, params, params_refine_text or Chat.RefineTextParams())
-        windows = StreamWindows(params.stream_speed, params.pass_first_n_batches) if stream else None
-        return super().submit(request, stream, windows)
+        A refinement that ends empty fails the job, as it makes ``infer`` raise.  Without ``split_text`` the text is
+        a paragraph of one sentence, and a refinement that ends empty goes on to speak the empty refined text."""
 
-    def _submit_paragraph(self, text, params, stream, skip_refine_text, refine, max_split_batch, lang,
-                          do_text_normalization, do_homophone_replacement, sink) -> Job:
+        def normalize(t):
+            return self.chat.normalizer(t, do_text_normalization, do_homophone_replacement, lang)
+
+        job, requests = self._job(text, params_infer_code or Chat.InferCodeParams(), stream, skip_refine_text,
+                                  params_refine_text or Chat.RefineTextParams(), split_text, max_split_batch, normalize)
+        self._enqueue([(job, requests)])
+        return job
+
+    def _job(self, text, params, stream, skip_refine_text, refine, split_text, max_split_batch, normalize, sink=None):
+        """``submit``'s job, not queued yet, and its first requests -> ``(Job, requests)``; ``normalize`` maps each
+        sentence to the text it speaks, ``sink`` as in ``_Paragraph``."""
         chat = self.chat
         if self.max_new_cap is not None and params.max_new_token > self.max_new_cap:
+            # a speech stage made by a follow-up is only checked when it is made: check the limit here, in the caller's
+            # thread
             raise ValueError(f"max_new_token {params.max_new_token} exceeds max_new_cap={self.max_new_cap}")
         m = int(max_split_batch)
         if m < 1:
             raise ValueError("max_split_batch must be >= 1")
-        sentences = [chat.normalizer(t, do_text_normalization, do_homophone_replacement, lang)
-                     for t in split_sentences(text)]
+        # the prompts are embedded here, on the caller's stream: ctb_gpt_embed_prompt is the one handle call that may
+        # run beside the worker (it only reads the weights); _enqueue orders the engine's stream after the caller's
+        sentences = [normalize(t) for t in (split_sentences(text) if split_text else [text])]
         if not sentences:
             raise ValueError("split_text=True: the text has no sentence")
         n = len(sentences)
@@ -946,66 +869,49 @@ class ChatEngine(OpenEngine):
         if not skip_refine_text:
             B = chat.gpt.max_batch  # infer() refines a paragraph's sentences in batches of up to max_batch
             graph = _RefineGraph(n, chat._refined_text, code, reference if spk_stage else None,
-                                 sample if spk_stage else None)
+                                 sample if spk_stage else None, speak_empty=not split_text)
             reqs = []
             for k, t in enumerate(sentences):
                 r = chat._refine_request(t, refine, noise_batch=(min(B, n - B * (k // B)), k % B))
                 r.then = graph.then(k)
-                r.stream_batch = params.stream_batch
+                r.stream_batch = params.stream_batch  # the engine polls at the smallest stream_batch of its requests
                 reqs.append(r)
-            job = super().submit(reqs, stream, para)
-            job.refined = graph.refined
         elif not spk_stage:
-            job = super().submit([code(k, t, None) for k, t in enumerate(sentences)], stream, para)
+            reqs = [code(k, t, None) for k, t in enumerate(sentences)]
         else:
-            ref = reference(sentences[0])
+            ref = reqs = reference(sentences[0])
 
             def then(out):
                 smp = (sample(ref), sentences[0])
                 return [code(k, t, smp) for k, t in enumerate(sentences)]
 
             ref.then = then
-            job = super().submit(ref, stream, para)
-        para.job = job
-        return job
+        para.job = self._new_job(reqs, stream, para)
+        if not skip_refine_text:
+            para.job.refined = graph.refined
+        return para.job, reqs
 
     def _serve(self, dev, requests, batch, jobs) -> None:
-        wjobs = []  # (job, slot, n_tokens, a, b, flush, last), as stream_continuous builds them
+        wjobs = []  # ((paragraph, sentence), slot, n_tokens, a, b, flush, last)
         for (i, s, n, last), (job, final) in zip(batch, jobs):
-            para = job.state if isinstance(job.state, _Paragraph) else None
+            para = job.state
             if i in self.stats.failed:
                 job._fail(self.stats.failed[i])
-                if para is not None:
-                    para.ended()
+                para.ended()
             elif job.done():
                 continue
             elif i in self.stats.cancelled:
                 job._stop()
-                if para is not None:
-                    para.ended()
-            elif requests[i].infer_text:  # a refinement stage: its follow-up carries the text on
-                continue
-            elif para is not None:
-                if requests[i] is para.ref:  # the reference stage: its audio only becomes the speaker sample
-                    continue
+                para.ended()
+            elif requests[i].infer_text or requests[i] is para.ref:
+                continue  # a refinement, or the reference stage, whose audio only becomes the speaker sample
+            else:
                 k = para.order[requests[i]]
                 if para.windows is not None:
                     ws = para.windows[k].windows(n, last)
-                    wjobs += [((job, k), s, n, a, b, flush, last and j == len(ws) - 1) for j, (a, b, flush) in
+                    wjobs += [((para, k), s, n, a, b, flush, last and j == len(ws) - 1) for j, (a, b, flush) in
                               enumerate(ws)]
-                elif last:
-                    wjobs.append(((job, k), s, n, 0, 512 * n - 256, True, True))
-            elif job.stream:
-                ws = job.state.windows(n, last)
-                wjobs += [(job, s, n, a, b, flush, last and k == len(ws) - 1) for k, (a, b, flush) in enumerate(ws)]
-            elif last:  # the whole sequence, silent samples dropped: what infer_continuous yields
-                wjobs.append((job, s, n, 0, 512 * n - 256, True, True))
-        for job, chunk, last in _decode_windows(dev, wjobs, self.model, self.use_decoder):
-            if isinstance(job, tuple):  # a sentence of a paragraph
-                job[0].state.add(job[1], chunk, last)
-            elif job.stream:
-                job._put((chunk, last))
-                if last:
-                    job._finish(None)
-            else:
-                job._finish(chunk[0])
+                elif last:  # the whole sequence, silent samples dropped
+                    wjobs.append(((para, k), s, n, 0, 512 * n - 256, True, True))
+        for (para, k), chunk, last in _decode_windows(dev, wjobs, self.model, self.use_decoder):
+            para.add(k, chunk, last)

@@ -165,10 +165,14 @@ class Arrivals:
         self.closed = False
 
     def submit(self, r, key=None) -> None:
+        self.submit_all([(r if key is None else key, r)])
+
+    def submit_all(self, items: List[Tuple[object, object]]) -> None:
+        """Queue ``[(key, request or list of requests)]`` in one step: the loop takes all of them at the same poll."""
         with self._cv:
             if self.closed:
                 raise RuntimeError("the engine is closed")
-            self._new.append((r if key is None else key, r))
+            self._new += items
             self._cv.notify()
 
     def cancel(self, key) -> None:
@@ -647,14 +651,16 @@ class OpenEngine:
     admission, decode, status read, cancellation and harvest copy on the engine's CUDA stream.  ``submit`` and
     ``Job.cancel`` only queue under a lock, from any thread.  ``check`` validates a request in the caller's thread at
     ``submit`` (and each follow-up in the worker, where a failure fails that job only).  An error in the worker fails
-    every pending job with it, stops the engine and is raised again by ``close``.  Subclasses turn each poll's yields
-    into job results (``_serve``)."""
+    every pending job with it, stops the engine and is raised again by ``close``.  With a ``context`` (``GPT.Context``)
+    an interrupt is ``schedule``'s: at the first poll that sees it the running requests end with what they have, the
+    engine stops, and every job that has not ended by then is cancelled.  Subclasses turn each poll's yields into job
+    results (``_serve``)."""
 
     def __init__(self, make_device: Callable[[List[Request]], object], chunk: int,
                  check: Optional[Callable[[Request], None]] = None, device=None,
-                 on_close: Optional[Callable[[], None]] = None, max_new_cap: Optional[int] = None):
+                 on_close: Optional[Callable[[], None]] = None, max_new_cap: Optional[int] = None, context=None):
         self._make_device, self.chunk, self._check, self._on_close = make_device, int(chunk), check, on_close
-        self.device, self.max_new_cap = device, max_new_cap
+        self.device, self.max_new_cap, self._context = device, max_new_cap, context
         cuda = device is not None and torch.device(device).type == "cuda"
         self._stream = torch.cuda.Stream(device) if cuda else None
         self._source = Arrivals()
@@ -672,6 +678,12 @@ class OpenEngine:
     def submit(self, request, stream: bool = False, state=None) -> Job:
         """Queue ``request`` (or a non-empty list of requests, stages of one job from the start); ``state`` is kept on
         the job for ``_serve`` (``Job.state``)."""
+        job = self._new_job(request, stream, state)
+        self._enqueue([(job, request)])
+        return job
+
+    def _new_job(self, request, stream: bool, state) -> Job:
+        """The job of ``submit(request, stream, state)``, its requests checked, not queued yet."""
         reqs = list(request) if isinstance(request, (list, tuple)) else [request]
         if not reqs or not all(isinstance(r, Request) for r in reqs):
             raise TypeError("requests must be chattts_b200.engine.Request objects")
@@ -680,14 +692,17 @@ class OpenEngine:
                 self._check(r)
         job = Job(self, stream)
         job.state = state
+        return job
+
+    def _enqueue(self, subs: List[Tuple[Job, object]]) -> None:
+        """Queue ``[(job, request or list of requests)]`` in one step: the worker takes all of them at the same poll."""
         with self._lock:
             if self._stopped:
                 raise RuntimeError("the engine is closed") from self._error
-            if self._stream is not None:  # the prompt was made on the caller's stream
+            if self._stream is not None:  # the prompts were made on the caller's stream
                 self._stream.wait_stream(torch.cuda.current_stream(self.device))
-            self._pending.add(job)
-            self._source.submit(request, job)
-        return job
+            self._pending.update(job for job, _ in subs)
+            self._source.submit_all(subs)
 
     def close(self, cancel: bool = False) -> None:
         """Wait for every submitted job (``cancel=True``: cancel them all first), then join the worker.  Raises the
@@ -737,13 +752,17 @@ class OpenEngine:
                 self._source.close()
                 jobs = list(self._pending)
                 self._pending.clear()
-            for job in jobs:
-                if not job.done():
-                    job._fail(self._error or RuntimeError("the engine stopped"))
+            for job in jobs:  # without an error the loop ended early only on an interrupt
+                if job.done():
+                    continue
+                if self._error is not None:
+                    job._fail(self._error)
+                else:
+                    job._stop()
 
     def _loop(self, requests: _RequestTable) -> None:
         dev = self._make_device(requests)
-        for batch in stream_schedule(requests, dev, self.chunk, None, self.stats, self._check, self._source):
+        for batch in stream_schedule(requests, dev, self.chunk, self._context, self.stats, self._check, self._source):
             jobs = []
             for i, s, n, last in batch:
                 job = self._job_at.get(i)

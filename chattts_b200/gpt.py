@@ -285,18 +285,9 @@ class GPT:
         ``ids`` are copies.  ``hiddens`` are views into the engine's buffer, like the narrowed views ``generate``
         hands out: they stay valid until this generator is resumed (copy them to keep them).  ``dtype`` as in
         ``generate_continuous``."""
-        flags = _lib.engine_flags(dtype)
-        for dev, batch in self._stream_polls(requests, slots, return_hidden, context, chunk, infer_text, return_attn,
-                                             max_new_cap, flags):
-            for i, slot, n, last in batch:
-                yield i, (dev.empty(i) if slot is None else dev.harvest(slot, n, copy=False)), last
-
-    def _stream_polls(self, requests, slots=None, return_hidden=True, context=None, chunk=None, infer_text=False,
-                      return_attn=False, max_new_cap=None, flags=0):
-        """``(EngineDevice, [(request_index, slot, n_tokens, last)])`` once per poll (engine.stream_schedule): every
-        yield due at that poll, while the engine's buffers hold all of them."""
         from .engine import ScheduleStats, stream_schedule
 
+        flags = _lib.engine_flags(dtype)
         requests, S, chunk, context, cap, check = self._engine_args(
             "generate_continuous_stream", requests, slots, infer_text, return_attn, context, chunk, None, max_new_cap)
         if not requests:
@@ -305,7 +296,8 @@ class GPT:
             dev = self._engine_device(requests, S, cap, return_hidden, flags)
             self.last_schedule_stats = stats = ScheduleStats()
             for batch in stream_schedule(requests, dev, chunk, context, stats, check):
-                yield dev, batch
+                for i, slot, n, last in batch:
+                    yield i, (dev.empty(i) if slot is None else dev.harvest(slot, n, copy=False)), last
             if stats.interrupted:
                 self.logger.warning("generation is interrupted")
 

@@ -212,6 +212,26 @@ def test_infer_continuous_refine_on_engine_equals_infer_per_text(use_decoder):
             assert np.array_equal(got[i], ref), i
 
 
+@pytest.mark.parametrize("use_decoder", [False, True])
+def test_infer_continuous_batched_refinement_equals_infer_of_the_refined_texts(use_decoder):
+    """The default mode: the texts are refined in static batches, as ``infer(refine_text_only=True)`` refines them,
+    and each refined text is then spoken as ``infer`` speaks it."""
+    c = chat()
+    refine, params = _refine_params(c)[0], _code_params(c)
+    refined = c.infer(TEXTS, refine_text_only=True, split_text=False, params_refine_text=refine)
+    got = dict(c.infer_continuous(TEXTS, params_infer_code=params, params_refine_text=refine, slots=3,
+                                  use_decoder=use_decoder, skip_refine_text=False))
+    assert sorted(got) == list(range(len(TEXTS)))
+    for i, t in enumerate(refined):
+        ref = c.infer([t], split_text=False, skip_refine_text=True, use_decoder=use_decoder,
+                      params_infer_code=params[i])[0]
+        assert got[i].shape == ref.shape, (i, got[i].shape, ref.shape)
+        if use_decoder:
+            assert float(np.sqrt(np.mean((got[i] - ref) ** 2))) < 1e-4, i
+        else:
+            assert np.array_equal(got[i], ref), i
+
+
 @pytest.mark.parametrize("use_decoder", [True, False])
 def test_infer_continuous_stream_refine_on_engine_equals_static_stream(use_decoder):
     c = chat()

@@ -1,6 +1,7 @@
 """Refined split-text paragraphs without a GPU: the stage graph's join (``core._RefineGraph``) in the scheduling policy
 against a stub device, a ``ChatEngine`` on a stub device and a stand-in ``Chat`` (failures, cancels in every phase,
 nothing left held), and ``Request.noise_batch``: its rows and its validation."""
+import time
 from types import SimpleNamespace
 
 import pytest
@@ -320,6 +321,192 @@ def test_max_split_batch_over_max_batch_is_refused_at_submit():
             eng.submit(PARA, params_infer_code=p, split_text=True, max_split_batch=0)
         eng.submit("a. b", params_infer_code=p, split_text=True, max_split_batch=5, skip_refine_text=False,
                    params_refine_text=r).cancel()  # two sentences: a batch of 2
+
+
+# ---------------------------------------------------------------------------------------------------- Chat's driver
+class _DriverStub(_Stub):
+    """_Stub that records each decode's chunk and calls ``on_decode(number of decodes so far)`` after each one.  The
+    hidden path reads the id buffer (the stand-in decoders only count tokens)."""
+
+    def __init__(self, slots, requests, chat, on_admit, on_decode):
+        super().__init__(slots, requests, chat, on_admit)
+        self.on_decode, self.chunks, self.hid_out = on_decode, [], self.ids_out
+
+    def decode(self, n):
+        self.chunks.append(n)
+        super().decode(n)
+        self.on_decode(self.decodes)
+
+
+@pytest.fixture
+def driver(monkeypatch):
+    """``make(fake, ...)``: a real ``Chat`` whose models are the ``_FakeChat``'s and whose GPT handle serves its
+    engines on ``_DriverStub`` devices, so ``infer_continuous*`` runs its own driver unchanged."""
+    import ctypes as C
+
+    import chattts_b200.engine as engine
+    from chattts_b200.gpt import GPT
+
+    made = []
+
+    def make(fake, max_batch=4, on_admit=lambda r: None, on_decode=lambda c, k: None, stub=_DriverStub):
+        c = Chat()
+        c.gpt = GPT({"hidden_size": 4}, embed=None, device_gpt=torch.device("cpu"), max_batch=max_batch,
+                    max_context=300)
+        c.gpt._handle = C.c_void_p(1)  # never reaches the library: the device layer is a stub
+        made.append(c.gpt)
+        c.vocos = c.embed = c.tokenizer = c.device = None
+        c.decoder = c.dvae = fake.dvae
+        c.speaker, c.normalizer = fake.speaker, fake.normalizer
+        c._code_request, c._refine_request, c._refined_text = fake._code_request, fake._refine_request, \
+            fake._refined_text
+        devs = []
+
+        def device(gpt, requests, S, cap, hidden):
+            devs.append(stub(S, requests, fake, on_admit, lambda k: on_decode(c, k)))
+            return devs[-1]
+
+        monkeypatch.setattr(engine, "EngineDevice", device)
+        return c, devs
+
+    yield make
+    for gpt in made:
+        gpt._handle = C.c_void_p()
+
+
+TEXTS = ["t0", "t1", "t2", "t3", "t4", "t5"]
+
+
+def _text_chat(code=150, refine=9, **kw):
+    return _FakeChat({t: refine for t in TEXTS}, {t: code for t in TEXTS}, **kw)
+
+
+@pytest.mark.parametrize("n", [3, 6])
+@pytest.mark.parametrize("split_text", [False, True])
+def test_the_first_admission_holds_a_first_stage_of_every_text_it_can(driver, n, split_text):
+    fake = _text_chat()
+    texts = TEXTS[:n]
+    if split_text:  # two sentences each: a paragraph's first stage is its reference stage
+        texts = [t + ". x" for t in texts]
+        fake.code_len.update({t: 20 for t in ["x", *(t + ". " for t in TEXTS)]})
+    c, devs = driver(fake)
+    p = Chat.InferCodeParams(manual_seed=1, max_new_token=200)
+    got = dict(c.infer_continuous(texts, params_infer_code=p, split_text=split_text))
+    assert sorted(got) == list(range(n))
+    assert len(devs[0].admissions[0]) == min(4, n)  # every slot the call has, or one per text
+
+
+@pytest.mark.parametrize("case", ["plain", "stream", "one text", "split", "split stream", "env"])
+def test_default_slots_and_poll_interval(driver, monkeypatch, case):
+    fake = _text_chat(code=20)
+    fake.code_len.update({"x": 20, "y": 20})
+    c, devs = driver(fake)
+    texts, split = (TEXTS[:1] if case == "one text" else TEXTS[:3]), case.startswith("split")
+    if split:
+        texts = ["x"] * 3  # one sentence each
+    if case == "env":
+        monkeypatch.setenv("CTB_DECODE_CHUNK", "5")
+    else:
+        monkeypatch.delenv("CTB_DECODE_CHUNK", raising=False)
+    params = [Chat.InferCodeParams(manual_seed=1, max_new_token=200, stream_batch=b) for b in (16, 12, 20)][:len(texts)]
+    if case.endswith("stream"):
+        list(c.infer_continuous_stream(texts, params_infer_code=params, split_text=split))
+    else:
+        list(c.infer_continuous(texts, params_infer_code=params, split_text=split))
+    want_slots = {"one text": 2, "split": 4, "split stream": 4}.get(case, 3)
+    want_chunk = {"stream": 12, "split": 24, "split stream": 24, "env": 5}.get(case, 32)
+    assert devs[0].slots == want_slots and set(devs[0].chunks) == {want_chunk}
+
+
+@pytest.mark.parametrize("stream", [False, True])
+def test_an_interrupt_ends_the_running_texts_with_what_they_have(driver, caplog, stream):
+    fake = _text_chat(code=150)
+
+    def on_decode(c, k):
+        if k == 2:
+            c.interrupt()
+
+    c, devs = driver(fake, on_decode=on_decode)
+    p = Chat.InferCodeParams(manual_seed=1, max_new_token=200, stream_speed=3000, pass_first_n_batches=0)
+    call = c.infer_continuous_stream if stream else c.infer_continuous
+    with caplog.at_level("WARNING"):
+        events = list(call(TEXTS[:4], params_infer_code=p, slots=2))
+    assert "generation is interrupted" in caplog.text
+    partial = 512 * (1 + 2 * (24 if stream else 32)) - 256  # the prefill's token and two polls' chunks
+    if stream:
+        finals = [(i, x) for i, x, last in events if last]
+        assert sorted(i for i, _ in finals) == [0, 1] and {i for i, *_ in events} == {0, 1}
+        assert all(sum(x.shape[1] for j, x, _ in events if j == i) == partial for i in (0, 1))
+    else:
+        assert sorted(i for i, _ in events) == [0, 1] and all(w.shape == (partial,) for _, w in events)
+    assert c.gpt._open is None and len(devs[0].chunks) == 2  # the handle is free, and nothing decoded after the read
+
+
+def test_batched_refinement_speaks_the_refined_texts_as_they_are(driver):
+    fake = _text_chat(code=20)
+    fake.normalizer = lambda text, *a: "N:" + text  # not the identity, so a second pass would show
+    c, _ = driver(fake)
+    refined_in = []
+
+    def refine_text(texts, device, params):  # batch b's row k refines to ids [100 b + k]
+        refined_in.append(list(texts))
+        return SimpleNamespace(ids=[torch.tensor([100 * len(refined_in) + k]) for k in range(len(texts))],
+                               destroy=lambda: None)
+
+    c._refine_text = refine_text
+    c.tokenizer = SimpleNamespace(break_0_ids=10 ** 6, decode=lambda tokens: [f"r{int(t[0])}" for t in tokens])
+    want = ["r100", "r101", "r102", "r103", "r200", "r201"]
+    fake.code_len.update({t: 20 for t in want})
+    p = Chat.InferCodeParams(manual_seed=1, max_new_token=200)
+    got = dict(c.infer_continuous(TEXTS, params_infer_code=p, skip_refine_text=False,
+                                  params_refine_text=Chat.RefineTextParams(manual_seed=2)))
+    assert sorted(got) == list(range(6))
+    assert refined_in == [["N:" + t for t in TEXTS[:4]], ["N:" + t for t in TEXTS[4:]]]  # batches of max_batch
+    assert [t for t, _, _ in fake.codes] == want
+
+
+@pytest.mark.parametrize("stream", [False, True])
+def test_a_text_whose_refinement_ends_empty_speaks_the_empty_refinement(driver, stream):
+    fake = _text_chat(code=20, refine=0)  # seeded: every refinement samples EOS first
+    fake.code_len.update({"R" + t: 20 for t in TEXTS})
+    c, _ = driver(fake)
+    p = Chat.InferCodeParams(manual_seed=1, max_new_token=200)
+    kw = dict(params_infer_code=p, skip_refine_text=False, refine_on_engine=True,
+              params_refine_text=Chat.RefineTextParams(manual_seed=2, max_new_token=50))
+    if stream:
+        got = {i for i, _, last in c.infer_continuous_stream(TEXTS[:2], **kw) if last}
+    else:
+        got = {i for i, w in c.infer_continuous(TEXTS[:2], **kw) if w.shape == (512 * 20 - 256,)}
+    assert got == {0, 1} and [t for t, _, _ in fake.codes] == ["Rt0", "Rt1"]
+
+
+class _SlowStub(_DriverStub):
+    def decode(self, n):
+        time.sleep(0.02)  # a poll takes longer than the driver's wait for the next chunk
+        super().decode(n)
+
+
+@pytest.mark.parametrize("stream", [False, True])
+def test_an_interrupt_cancels_every_unfinished_paragraph(driver, caplog, stream):
+    # the reference stages and sentence 0 end in one poll of 24 steps each: sentence 0's chunks are out before the
+    # interrupt, while the other sentences need 7 polls
+    fake = _chat(code=(9, 150, 150, 150, 150))
+
+    def on_decode(c, k):
+        if k == 3:
+            c.interrupt()
+
+    c, devs = driver(fake, on_decode=on_decode, stub=_SlowStub)
+    p = Chat.InferCodeParams(manual_seed=1, max_new_token=200)
+    call = c.infer_continuous_stream if stream else c.infer_continuous
+    with caplog.at_level("WARNING"):
+        events = list(call([PARA, PARA], params_infer_code=p, split_text=True))
+    assert "generation is interrupted" in caplog.text
+    if stream:
+        assert events and not any(last for *_, last in events)
+    else:
+        assert events == []
+    assert max(d.decodes for d in devs) < 3 + 6 and c.gpt._open is None and _idle(devs)
 
 
 # ---------------------------------------------------------------------------------------------------- noise_batch

@@ -28,18 +28,18 @@ with ``--refine`` every sentence is refined first, against ``Chat.infer``'s defa
 
 ``--stream`` then prints a second JSON line: the same requests streamed as audio (hidden path, DVAE decoder and Vocos
 from synthetic weights, InferCodeParams' default stream_batch / stream_speed / pass_first_n_batches), timed
-alternately in three arms: (a) the streaming engine with one ragged ``decode_rows`` call per poll, (b) the same engine
-with one ``decode_to_wavs_window`` call per window, (c) the non-streaming engine without path 2.  Per arm: wall time,
+alternately in two arms: (a) every request a streaming job of one open engine (``ChatEngine``), all submitted at once,
+with one ragged ``decode_rows`` call per poll, (c) the non-streaming engine without path 2.  For (a): wall time,
 useful speech-tokens/s, seconds of audio delivered per wall second, time to first chunk from admission and from start
 (p50 / p95 / max), playback underruns (chunks that arrive after the request's earlier chunks have finished playing,
-counted from its first chunk) and the share of wall time in path 2.  (a) and (b) must yield the same chunks; with
+counted from its first chunk) and the share of wall time in path 2 (host time in ``core._decode_windows``).  With
 ``--dump-outputs`` the chunks of (a) are written as stream_chunks.npy (concatenated in yield order),
 stream_chunk_index.npy and stream_chunk_lengths.npy.
 
 ``--online 12,24`` prints one more line per rate: the same requests streamed (hidden path, 32 slots, InferCodeParams'
 defaults) but arriving over time, seeded Poisson arrivals at that many requests/s; (a) the open engine, each request
-submitted at its arrival, against (b) consecutive ``stream_continuous`` calls, each starting every request that arrived
-while the previous one ran.  Per arm: time from arrival to first and to last chunk (p50 / p95 / max), useful tokens/s
+submitted at its arrival, against (b) one open engine after another, each starting every request that arrived while
+the previous one ran (all submitted, then closed).  Per arm: time from arrival to first and to last chunk (p50 / p95 / max), useful tokens/s
 over the span from the first arrival to the last chunk, decode steps, mean slot occupancy and underruns.  ``--cancel F``
 adds a line with a seeded fraction F of the requests cancelled 0..1 s after their first chunk (open engine, highest
 rate), against the same arrivals without cancellation: decode steps and span.
@@ -79,6 +79,33 @@ def gpu_card(index: int):
         return name, limit
     except Exception:
         return torch.cuda.get_device_name(index), None
+
+
+def request_job(eng, request, p, sink=None):
+    """``request`` (an engine ``Request``) as one streaming job of ``eng`` (a ``ChatEngine``) with the windows of ``p``
+    (``InferCodeParams``), not queued yet: ``(Job, request)`` for ``eng._enqueue``."""
+    from chattts_b200.core import _Paragraph
+
+    para = _Paragraph(1, p, sink)
+    para.order[request] = 0
+    para.job = eng._new_job(request, True, para)
+    return para.job, request
+
+
+def stream_requests(eng, requests, p):
+    """Every request one streaming job of ``eng``, all queued in one step: generator of ``(position, chunk)`` as the
+    chunks come, until every job has ended."""
+    import queue
+
+    out = queue.Queue()
+    eng._enqueue([request_job(eng, r, p, (out, k)) for k, r in enumerate(requests)])
+    left = len(requests)
+    while left:
+        k, item = out.get(timeout=600)
+        if item is None:
+            left -= 1
+        else:
+            yield k, item[0]
 
 
 def continuous_workload(n: int, seed: int):
@@ -194,11 +221,14 @@ def run_continuous(args, local_rank: int = 0):
 
 
 def run_stream(args, local_rank: int = 0):
-    """Streamed audio on the slot engine, three arms timed alternately in this process (see the module docstring)."""
+    """Streamed audio on the slot engine, two arms timed alternately in this process (see the module docstring)."""
+    import types
+
     import numpy as np
 
+    import chattts_b200.core as core
     from chattts_b200.config import Config
-    from chattts_b200.core import Chat, StreamWindows, stream_continuous
+    from chattts_b200.core import Chat, ChatEngine
     from chattts_b200.decoder import DVAE, Vocos
     from chattts_b200.embed import Embed
     from chattts_b200.engine import EngineDevice, Request
@@ -240,19 +270,29 @@ def run_stream(args, local_rank: int = 0):
         admit(self, batch)
 
     EngineDevice.admit = timed_admit
+    path2 = [0.0]
+    decode_windows = core._decode_windows
 
-    def stream_arm(lengths, ragged):
+    def timed_windows(*a, **kw):  # the host time of each poll's path-2 work: decode and copy the audio
+        t = time.perf_counter()
+        out = decode_windows(*a, **kw)
+        path2[0] += time.perf_counter() - t
+        return out
+
+    core._decode_windows = timed_windows
+    models = types.SimpleNamespace(decoder=dec, dvae=dec)  # what ChatEngine reads of a Chat
+
+    def stream_arm(lengths):
         admitted.clear()
-        stats, chunks, arrive = {}, [], []
-        windows = [StreamWindows(p.stream_speed, p.pass_first_n_batches) for _ in lengths]
+        path2[0] = 0.0
+        chunks, arrive = [], []
         t0 = time.perf_counter()
-        for i, chunk, _ in stream_continuous(gpt, dec, requests(lengths), windows, True, slots=S, ragged=ragged,
-                                             stats=stats):
-            chunks.append((i, chunk))
-            arrive.append(time.perf_counter())
+        with gpt._open_slot_engine(ChatEngine, S, max(lengths), True, p.stream_batch, models, True) as eng:
+            for i, chunk in stream_requests(eng, requests(lengths), p):
+                chunks.append((i, chunk))
+                arrive.append(time.perf_counter())
         wall = time.perf_counter() - t0
-        return dict(wall=wall, t0=t0, chunks=chunks, arrive=arrive, admitted=dict(admitted),
-                    path2=stats.get("path2_s", 0.0))
+        return dict(wall=wall, t0=t0, chunks=chunks, arrive=arrive, admitted=dict(admitted), path2=path2[0])
 
     def plain_arm(lengths):
         t0 = time.perf_counter()
@@ -263,19 +303,13 @@ def run_stream(args, local_rank: int = 0):
 
     short = [min(t, 96) for t in tok[: 2 * S]]
     for _ in range(max(1, min(args.warmup, 2))):
-        stream_arm(short, True)
-        stream_arm(short, False)
+        stream_arm(short)
         plain_arm(short)
-    runs = {"a": [], "b": [], "c": []}
+    runs = {"a": [], "c": []}
     for _ in range(args.steps):
-        runs["a"].append(stream_arm(tok, True))
-        runs["b"].append(stream_arm(tok, False))
+        runs["a"].append(stream_arm(tok))
         runs["c"].append(plain_arm(tok))
-    ca, cb = runs["a"][-1]["chunks"], runs["b"][-1]["chunks"]
-    per = lambda ch: {i: [c for j, c in ch if j == i] for i in range(n)}  # noqa: E731
-    pa, pb = per(ca), per(cb)
-    assert all(len(pa[i]) == len(pb[i]) and all(np.array_equal(x, y) for x, y in zip(pa[i], pb[i])) for i in range(n)), \
-        "arms (a) and (b) yield different chunks"
+    ca = runs["a"][-1]["chunks"]
     if args.dump_outputs:
         dump_outputs(args.dump_outputs, {
             "stream_chunks": np.concatenate([c[0] for _, c in ca]) if ca else np.zeros(0, np.float32),
@@ -309,17 +343,15 @@ def run_stream(args, local_rank: int = 0):
     out = {"metric": "continuous_stream", "card": None, "power_limit": None, "requests": n, "slots": S,
            "stream_batch": p.stream_batch, "stream_speed": p.stream_speed,
            "pass_first_n_batches": p.pass_first_n_batches, "useful_tokens": useful, "repeats": args.steps}
-    for arm in ("a", "b"):
-        rs = runs[arm]
-        pick = sorted(rs, key=lambda r: r["wall"])[len(rs) // 2]  # the median run
-        out[arm] = summary(pick)
-        out[arm]["seconds_all"] = [round(r["wall"], 3) for r in rs]
+    rs = runs["a"]
+    out["a"] = summary(sorted(rs, key=lambda r: r["wall"])[len(rs) // 2])  # the median run
+    out["a"]["seconds_all"] = [round(r["wall"], 3) for r in rs]
     tc = med([r["wall"] for r in runs["c"]])
     out["c"] = {"seconds": round(tc, 3), "tokens_per_s": round(useful / tc, 1),
                 "seconds_all": [round(r["wall"], 3) for r in runs["c"]]}
-    out["a_over_b_speedup"] = round(out["b"]["seconds"] / out["a"]["seconds"], 3)
     out["card"], out["power_limit"] = gpu_card(local_rank)
     EngineDevice.admit = admit
+    core._decode_windows = decode_windows
     return out
 
 
@@ -455,8 +487,7 @@ def run_refine(args, local_rank: int = 0):
 def run_online(args, local_rank: int = 0):
     """Requests arriving over time (seeded Poisson arrivals at each rate of ``--online``), streamed as audio: (a) the
     open engine (``GPT.open_engine`` / ``ChatEngine``: every request submitted at its arrival) against (b) what a
-    server can do without it: the requests that arrived while one ``stream_continuous`` call ran start together in the
-    next call.  Arms alternate, ``--steps`` repeats each; the median run by span is reported.  One JSON line per rate,
+    server can do without it: the requests that arrived while one engine ran start together on the next one.  Arms alternate, ``--steps`` repeats each; the median run by span is reported.  One JSON line per rate,
     and with ``--cancel F`` one more: arm (a) at the highest rate with a seeded fraction F of the requests cancelled
     at a seeded time (0..1 s) after their first chunk, against the same arrivals without cancellation."""
     import threading
@@ -465,10 +496,10 @@ def run_online(args, local_rank: int = 0):
     import numpy as np
 
     from chattts_b200.config import Config
-    from chattts_b200.core import Chat, ChatEngine, StreamWindows, stream_continuous
+    from chattts_b200.core import Chat, ChatEngine
     from chattts_b200.decoder import DVAE, Vocos
     from chattts_b200.embed import Embed
-    from chattts_b200.engine import OpenEngine, Request
+    from chattts_b200.engine import Request
     from chattts_b200.gpt import GPT
     from chattts_b200.processors import gen_logits
     from chattts_b200.prompts import synth_prompt_batch
@@ -500,9 +531,6 @@ def run_online(args, local_rank: int = 0):
                        min_new_token=lengths[i], logits_processors=procs, manual_seed=5000 + i,
                        stream_batch=p.stream_batch)
 
-    def windows():
-        return StreamWindows(p.stream_speed, p.pass_first_n_batches)
-
     def arrivals(rate, count, seed):
         g = np.random.default_rng(seed)
         return np.cumsum(g.exponential(1.0 / rate, count)).tolist()
@@ -522,7 +550,8 @@ def run_online(args, local_rank: int = 0):
 
         for i, a in enumerate(at):
             time.sleep(max(0.0, a - (time.perf_counter() - t0)))
-            job = OpenEngine.submit(eng, request(i, lengths), True, windows())
+            job, r = request_job(eng, request(i, lengths), p)
+            eng._enqueue([(job, r)])
             jobs.append(job)
             th = threading.Thread(target=consume, args=(i, job))
             th.start()
@@ -533,7 +562,8 @@ def run_online(args, local_rank: int = 0):
         return dict(chunks=chunks, steps=eng.stats.decode_steps, cancelled=sum(j.cancelled() for j in jobs))
 
     def call_arm(at, lengths):
-        """(b): the requests that arrived while a call ran start together in the next call."""
+        """(b): the requests that arrived while one engine ran start together on the next one (all submitted, then
+        closed)."""
         chunks = {i: [] for i in range(len(at))}
         steps, nxt = 0, 0
         t0 = time.perf_counter()
@@ -542,10 +572,10 @@ def run_online(args, local_rank: int = 0):
             now = time.perf_counter() - t0
             batch = [i for i in range(nxt, len(at)) if at[i] <= now]
             nxt = batch[-1] + 1
-            for k, c, _ in stream_continuous(gpt, dec, [request(i, lengths) for i in batch],
-                                             [windows() for _ in batch], True, slots=S, max_new_cap=cap):
-                chunks[batch[k]].append((time.perf_counter() - t0, c.shape[1]))
-            steps += gpt.last_schedule_stats.decode_steps
+            with gpt._open_slot_engine(ChatEngine, S, cap, True, None, models, True) as eng:
+                for k, c in stream_requests(eng, [request(i, lengths) for i in batch], p):
+                    chunks[batch[k]].append((time.perf_counter() - t0, c.shape[1]))
+            steps += eng.stats.decode_steps
         return dict(chunks=chunks, steps=steps, cancelled=0)
 
     sr = 24000.0
