@@ -42,17 +42,19 @@ def gfsq_embed(ids: torch.Tensor, s: State, G: int = 2, R: int = 2, levels=(5, 5
                ) -> torch.Tensor:
     """[3p] GFSQ._embed (dvae.py:87-97) -> GroupedResidualFSQ.get_output_from_indices.
     ids [B, G*R, T] -> feat [B, dim, T].  Codebook c = g*R + r; residual r is scaled by
-    ``scale_base ** -r`` (``levels - 1`` = 4 in the releases ChatTTS was built against)."""
+    ``scale_base ** -r`` (``levels - 1`` = 4 in the releases ChatTTS was built against).
+    The codes are evaluated in the dtype of the ``project_out`` weights, on the device of ``ids``."""
     B, _, T = ids.shape
+    dt = s["vq_layer.quantizer.rvqs.0.project_out.weight"].dtype
     x = ids.transpose(1, 2).reshape(B, T, G, R).permute(2, 0, 1, 3)  # [G, B, T, R]
-    basis = torch.cumprod(torch.tensor([1] + list(levels[:-1])), 0)
-    lv = torch.tensor(levels)
+    basis = torch.cumprod(torch.tensor([1] + list(levels[:-1])), 0).to(ids.device)
+    lv = torch.tensor(levels).to(ids.device)
     outs = []
     for g in range(G):
         z = 0
         for r in range(R):
             li = (x[g, :, :, r, None] // basis) % lv        # [B, T, 4] level indices
-            code = (li.float() - (lv // 2).float()) / (lv // 2).float()
+            code = (li.to(dt) - (lv // 2).to(dt)) / (lv // 2).to(dt)
             z = z + code * (float(scale_base) ** -r)
         outs.append(F.linear(z, s[f"vq_layer.quantizer.rvqs.{g}.project_out.weight"],
                              s[f"vq_layer.quantizer.rvqs.{g}.project_out.bias"]))

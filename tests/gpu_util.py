@@ -1,6 +1,8 @@
+import gc
 import os
 
 import numpy as np
+import pytest
 import torch
 
 from chattts_b200.config import Config
@@ -27,3 +29,21 @@ def build_gpt(seed=0, std=0.02, max_batch=32, max_context=640):
 
 def load_gold(name):
     return np.load(os.path.join(GOLD, name + ".npz"))
+
+
+def release_on_teardown(*caches):
+    """A module-scoped autouse fixture that empties ``caches`` (the module's dicts of engine handles, models and device
+    tensors) once its tests are done, so that the device memory they hold is free for the modules that run after it.
+    Assign it to a module-level name: ``_release = release_on_teardown(_models, _refs)``."""
+
+    @pytest.fixture(scope="module", autouse=True)
+    def _release():
+        yield
+        for c in caches:
+            c.clear()
+        gc.collect()
+        if torch.cuda.is_available():
+            torch.cuda.synchronize()
+            torch.cuda.empty_cache()
+
+    return _release

@@ -17,6 +17,7 @@ from chattts_b200.processors import gen_logits
 from chattts_b200.prompts import synth_prompt_batch
 from chattts_b200.synth import synth_embed_state, synth_gpt_state
 from fp16_oracle import GPTOracleFp16, fp16_layer_state
+from gpu_util import release_on_teardown
 from oracle.gpt_oracle import SamplerParams
 
 pytestmark = pytest.mark.gpu
@@ -33,6 +34,7 @@ LENGTHS = [3, 17, 40, 5, 9, 26, 7, 33, 12, 4, 21, 38]
 MAX_NEW = [20, 45, 90, 33, 60, 25, 81, 40, 55, 70, 28, 64]
 MIXED = [(0.7, 20, 1.05), (None, 20, 1.0), (0.5, None, 1.05), (None, None, 1.0), (0.95, 3, 1.2), (0.7, 20, 1.0)]
 _handles = {}
+_release = release_on_teardown(_handles)
 
 
 def _build(state, max_batch=32, max_context=640):

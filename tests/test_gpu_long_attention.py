@@ -42,6 +42,7 @@ from chattts_b200.processors import gen_logits
 from chattts_b200.prompts import synth_prompt_batch
 from chattts_b200.synth import synth_embed_state, synth_gpt_state
 from f64_oracle import F64Oracle, peaked_state, sample_trace
+from gpu_util import release_on_teardown
 from oracle.gpt_oracle import SamplerParams, exp_noise
 
 pytestmark = pytest.mark.gpu
@@ -66,6 +67,7 @@ PARAMS = [(0.7, 20, 1.05), (None, 20, 1.0), (0.5, None, 1.05), (0.7, 20, 1.0), (
 TEMPS = [[0.3, 0.5, 0.7, 1.0], [0.7] * 4, [1.0, 0.3, 0.3, 0.5], [0.5] * 4, [0.3] * 4, [1.0] * 4]
 
 _models, _oracles, _refs = {}, {}, {}
+_release = release_on_teardown(_models, _oracles, _refs)  # two 32 x 2048 engines, float64 oracles
 
 
 def _model(kind):
