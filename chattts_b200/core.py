@@ -57,13 +57,16 @@ class Chat:
     # ------------------------------------------------------------------ loading
     def load(self, source="local", force_redownload=False, compile: bool = False, custom_path=None,
              device: Optional[torch.device] = None, coef: Optional[torch.Tensor] = None, use_flash_attn=False,
-             use_vllm=False, experimental: bool = False, spk_stat: Optional[str] = None) -> bool:
+             use_vllm=False, experimental: bool = False, spk_stat: Optional[str] = None, max_batch: int = 32,
+             max_context: int = 4096) -> bool:
         """core.py:137-163.  ``compile`` / ``use_flash_attn`` / ``use_vllm`` / ``experimental`` are accepted and
         ignored (one back end, SURVEY.md quirk Q14).  The asset files are located like the reference does for
         ``source="local"`` (working directory or ``custom_path``) and ``"custom"``; downloading / sha256 checking
         (core.py:66-135) is left to the reference package, which ``source="huggingface"`` therefore still needs.
         ``spk_stat`` (config.py:132, the base16384 std|mean table random speakers are drawn from) is taken from the
-        argument, else from an importable reference package; without it only ``sample_random_speaker`` is unavailable."""
+        argument, else from an importable reference package; without it only ``sample_random_speaker`` is unavailable.
+        ``max_batch`` / ``max_context`` size the handles as in ``load_states``: a slot engine serves up to
+        ``max_batch`` slots (up to 64 on the wgmma step, half-precision engines included)."""
         root = self.download_models(source, force_redownload, custom_path)
         if root is None:
             return False
@@ -95,7 +98,8 @@ class Chat:
         dev = device or torch.device("cuda")
         self.normalizer = Normalizer(homophones, self.logger)
         return self.load_states(states, tokenizer=Tokenizer(paths["tokenizer_path"]),
-                                speaker=Speaker(self.config.gpt.hidden_size, spk_stat, dev), device=dev, coef=coef)
+                                speaker=Speaker(self.config.gpt.hidden_size, spk_stat, dev), device=dev, coef=coef,
+                                max_batch=max_batch, max_context=max_context)
 
     def download_models(self, source="local", force_redownload=False, custom_path=None) -> Optional[str]:
         """core.py:66-135, without the downloader: returns the folder that holds ``asset/`` or ``None``."""
@@ -236,13 +240,13 @@ class Chat:
         ``infer(texts[index], max_split_batch=max_split_batch, params_refine_text=...)[0]`` returns (seeded: bit for
         bit on the code path).
 
-        ``slots`` defaults to max(2, min(max_batch, len(texts))), with ``split_text`` to the handle's ``max_batch``.
-        ``Chat.interrupt()`` ends the running texts with what they have, or with ``split_text`` cancels every
+        ``slots`` defaults to max(2, min(max_batch, len(texts))), with ``split_text`` to the handle's ``max_batch``
+        (``load(max_batch=...)``); engines of 9..64 slots run the wgmma decode step.  ``Chat.interrupt()`` ends the running texts with what they have, or with ``split_text`` cancels every
         unfinished paragraph (see ``_continuous``).
 
         ``dtype=torch.float16`` runs every request on a half-precision engine (``GPT.generate_continuous``): fp16
         layer weights and KV cache, as the reference's ``use_vllm=True`` serves; the waveforms then follow that model.
-        Path 2 (DVAE / Vocos) is unchanged."""
+        It serves up to 64 slots.  Path 2 (DVAE / Vocos) is unchanged."""
         _lib.engine_flags(dtype)  # an unsupported dtype raises here, before any device work
         if stream:
             raise ValueError("infer_continuous: stream=True is not supported; each waveform is yielded when complete "
@@ -441,8 +445,8 @@ class Chat:
         """A long-lived slot engine (``GPT.open_engine``) that synthesises texts submitted from any thread while it
         decodes: ``engine.submit(text, params_infer_code=None, stream=False, skip_refine_text=True, ...) -> Job``,
         ``Job.cancel()`` for one text, ``close(cancel=False)`` or a ``with`` block to drain it (``close(cancel=True)``
-        is its interrupt; ``Chat.context`` is not read).  ``slots`` defaults to the handle's ``max_batch``; every
-        stage's ``max_new_token`` must be at most ``max_new_cap``.  See ``ChatEngine.submit``.  ``dtype`` as in
+        is its interrupt; ``Chat.context`` is not read).  ``slots`` defaults to the handle's ``max_batch`` (up to 64
+        for ``dtype=torch.float16``); every stage's ``max_new_token`` must be at most ``max_new_cap``.  See ``ChatEngine.submit``.  ``dtype`` as in
         ``infer_continuous``: every stage of every job runs on that engine."""
         flags = _lib.engine_flags(dtype)
         assert self.has_loaded(use_decoder=use_decoder)

@@ -88,10 +88,11 @@ struct ctb_gpt {
   unsigned* flow_epoch;
   int steps_enqueued;  // loop iterations enqueued since ctb_gpt_begin (host-side bound for ctb_gpt_decode)
   float *tc_wqkv, *tc_wgu, *tc_heads_code, *tc_heads_text;  // permuted / norm-folded weight copies
-  float *x_hi, *x_lo, *attn_hi, *attn_lo, *h_hi, *h_lo;      // [32][K] tf32-split activations
+  float *x_hi, *x_lo, *attn_hi, *attn_lo, *h_hi, *h_lo;      // [tc_rows][K] tf32-split activations
+  int tc_rows;                                               // 32, or 64 on a handle whose max_batch exceeds 32
   CUtensorMap *m_wqkv, *m_wo, *m_wgu, *m_wd;                 // [layers] host arrays
   CUtensorMap m_hcode, m_htext;
-  CUtensorMap m_x[2][2], m_attn[2][2], m_h[2][2];            // [npad16|32][hi|lo]
+  CUtensorMap m_x[3][2], m_attn[3][2], m_h[3][2];            // [npad16|32|64][hi|lo] (npad 64: tc_rows == 64 only)
   bool use_graph;
   // ---- slot engine (ctb_gpt_engine_*): B = S slots, max_new = the per-slot capacity of ids_out / hiddens_out
   int engine;                 // 1 between ctb_gpt_engine_begin and the next ctb_gpt_begin
@@ -260,14 +261,15 @@ static int tc_setup(ctb_gpt* h) {
     if ((rc = encode_map_2d(&h->m_wd[l], Wl + L.wdown, d, I, 128))) return rc;
   }
   CTB_CUDA(cudaDeviceSynchronize());
-#define TCATTR(E, C) if ((rc = set_tc_attr<E, 16, C>())) return rc; if ((rc = set_tc_attr<E, 32, C>())) return rc;
+#define TCATTR(E, C) if ((rc = set_tc_attr<E, 16, C>())) return rc; if ((rc = set_tc_attr<E, 32, C>())) return rc; \
+  if ((rc = set_tc_attr<E, 64, C>())) return rc;
   TCATTR(DE_QKV, CS_QKV) TCATTR(DE_OPROJ, CS_O) TCATTR(DE_GATEUP, CS_GU) TCATTR(DE_DOWN, CS_DOWN)
 #undef TCATTR
   return CTB_OK;
 }
 
-// what every wgmma step shares: the tf32-split activation scratch of 32 rows, the fp32 norm-folded head copies and the
-// tensor maps over them
+// what every wgmma step shares: the tf32-split activation scratch (32 rows; 64 on a handle whose max_batch exceeds 32,
+// for engines of up to 64 slots), the fp32 norm-folded head copies and the tensor maps over them
 static int tc_setup_base(ctb_gpt* h) {
   if (h->tc_base) return CTB_OK;
   const ctb_gpt_config& c = h->cfg;
@@ -276,12 +278,14 @@ static int tc_setup_base(ctb_gpt* h) {
   int rc;
   if ((rc = dalloc(&h->tc_heads_code, (size_t)c.num_vq * c.num_audio_tokens * d))) return rc;
   if ((rc = dalloc(&h->tc_heads_text, (size_t)c.num_text_tokens * d))) return rc;
-  if ((rc = dalloc(&h->x_hi, 32 * d))) return rc;
-  if ((rc = dalloc(&h->x_lo, 32 * d))) return rc;
-  if ((rc = dalloc(&h->attn_hi, 32 * d))) return rc;
-  if ((rc = dalloc(&h->attn_lo, 32 * d))) return rc;
-  if ((rc = dalloc(&h->h_hi, 32 * I))) return rc;
-  if ((rc = dalloc(&h->h_lo, 32 * I))) return rc;
+  const size_t R = c.max_batch > 32 ? 64 : 32;
+  if ((rc = dalloc(&h->x_hi, R * d))) return rc;
+  if ((rc = dalloc(&h->x_lo, R * d))) return rc;
+  if ((rc = dalloc(&h->attn_hi, R * d))) return rc;
+  if ((rc = dalloc(&h->attn_lo, R * d))) return rc;
+  if ((rc = dalloc(&h->h_hi, R * I))) return rc;
+  if ((rc = dalloc(&h->h_lo, R * I))) return rc;
+  h->tc_rows = (int)R;
   const int nhc = c.num_vq * c.num_audio_tokens;
   k_build_tc_weight<<<nhc, 256>>>(h->W + L.head_code, h->W + L.final_norm, h->tc_heads_code, nhc, (int)d, 0, 0, 0, 0);
   k_build_tc_weight<<<c.num_text_tokens, 256>>>(h->W + L.head_text, h->W + L.final_norm, h->tc_heads_text,
@@ -289,17 +293,18 @@ static int tc_setup_base(ctb_gpt* h) {
   CTB_CUDA(cudaDeviceSynchronize());
   if ((rc = encode_map_2d(&h->m_hcode, h->tc_heads_code, nhc, d, 128))) return rc;
   if ((rc = encode_map_2d(&h->m_htext, h->tc_heads_text, c.num_text_tokens, d, 128))) return rc;
-  for (int n = 0; n < 2; ++n) {
-    const uint32_t npad = n ? 32 : 16;
-    if ((rc = encode_map_2d(&h->m_x[n][0], h->x_hi, 32, d, npad))) return rc;
-    if ((rc = encode_map_2d(&h->m_x[n][1], h->x_lo, 32, d, npad))) return rc;
-    if ((rc = encode_map_2d(&h->m_attn[n][0], h->attn_hi, 32, d, npad))) return rc;
-    if ((rc = encode_map_2d(&h->m_attn[n][1], h->attn_lo, 32, d, npad))) return rc;
-    if ((rc = encode_map_2d(&h->m_h[n][0], h->h_hi, 32, I, npad))) return rc;
-    if ((rc = encode_map_2d(&h->m_h[n][1], h->h_lo, 32, I, npad))) return rc;
+  for (int n = 0; n < (R > 32 ? 3 : 2); ++n) {
+    const uint32_t npad = 16u << n;
+    if ((rc = encode_map_2d(&h->m_x[n][0], h->x_hi, R, d, npad))) return rc;
+    if ((rc = encode_map_2d(&h->m_x[n][1], h->x_lo, R, d, npad))) return rc;
+    if ((rc = encode_map_2d(&h->m_attn[n][0], h->attn_hi, R, d, npad))) return rc;
+    if ((rc = encode_map_2d(&h->m_attn[n][1], h->attn_lo, R, d, npad))) return rc;
+    if ((rc = encode_map_2d(&h->m_h[n][0], h->h_hi, R, I, npad))) return rc;
+    if ((rc = encode_map_2d(&h->m_h[n][1], h->h_lo, R, I, npad))) return rc;
   }
   if ((rc = set_tc_attr<DE_HEADS, 16, CS_HEADS>())) return rc;
   if ((rc = set_tc_attr<DE_HEADS, 32, CS_HEADS>())) return rc;
+  if ((rc = set_tc_attr<DE_HEADS, 64, CS_HEADS>())) return rc;
   h->tc_base = true;
   return CTB_OK;
 }
@@ -369,7 +374,8 @@ static int fp16_setup(ctb_gpt* h) {
       return rc;
     }
   }
-#define TCATTR(E, C, P) if ((rc = set_tc_attr<E, 16, C, P>())) return rc; if ((rc = set_tc_attr<E, 32, C, P>())) return rc;
+#define TCATTR(E, C, P) if ((rc = set_tc_attr<E, 16, C, P>())) return rc; if ((rc = set_tc_attr<E, 32, C, P>())) return rc; \
+  if ((rc = set_tc_attr<E, 64, C, P>())) return rc;
   TCATTR(DE_QKV, CS_QKV, 1) TCATTR(DE_QKV, CS_QKV, 3) TCATTR(DE_OPROJ, CS_O, 1) TCATTR(DE_GATEUP, CS_GU, 1)
   TCATTR(DE_DOWN, CS_DOWN, 1)
 #undef TCATTR
@@ -687,6 +693,9 @@ static int launch_sampler(ctb_gpt* h, const StepCtx& x, cudaStream_t s) {
   return launch_sample(sp, s);
 }
 
+// npad 16 for B <= 16, 32 for B <= 32, 64 for B <= 64 (a 64-row scratch only: tc_rows == 64)
+static int tc_npad_index(int B) { return B > 32 ? 2 : (B > 16 ? 1 : 0); }
+
 template <int EPI, int CS, int PREC = 0>
 static int launch_tc(int npad, const CUtensorMap& mw, const CUtensorMap& mxh, const CUtensorMap& mxl, const TcDecP& p,
                      cudaStream_t s) {
@@ -695,8 +704,10 @@ static int launch_tc(int npad, const CUtensorMap& mw, const CUtensorMap& mxh, co
   dim3 grid(tiles * CS);
   if (npad == 16)
     CTB_CUDA(launch_pdl_cluster(k_tc_dec<EPI, 16, CS, PREC>, grid, dim3(TD_THREADS), (size_t)TdCfg<16, W16>::SMEM_BYTES, s, (unsigned)CS, mw, mxh, mxl, p));
-  else
+  else if (npad == 32)
     CTB_CUDA(launch_pdl_cluster(k_tc_dec<EPI, 32, CS, PREC>, grid, dim3(TD_THREADS), (size_t)TdCfg<32, W16>::SMEM_BYTES, s, (unsigned)CS, mw, mxh, mxl, p));
+  else
+    CTB_CUDA(launch_pdl_cluster(k_tc_dec<EPI, 64, CS, PREC>, grid, dim3(TD_THREADS), (size_t)TdCfg<64, W16>::SMEM_BYTES, s, (unsigned)CS, mw, mxh, mxl, p));
   CTB_LAUNCH_CHECK();
   return CTB_OK;
 }
@@ -717,7 +728,7 @@ template <int PREC>
 static int launch_layer_kernel_tc_t(ctb_gpt* h, int l, int kind, cudaStream_t s) {
   constexpr int PW = PREC & TD_W16;
   const ctb_gpt_config& c = h->cfg;
-  const int n = h->B > 16 ? 1 : 0, npad = n ? 32 : 16;
+  const int n = tc_npad_index(h->B), npad = 16 << n;
   const int d = c.hidden_size, I = c.intermediate_size;
   TcDecP p = make_tc(h);
   switch (kind) {
@@ -749,7 +760,7 @@ static int launch_layer_kernel_tc(ctb_gpt* h, int l, int kind, cudaStream_t s) {
 
 static int launch_heads_tc(ctb_gpt* h, cudaStream_t s) {
   const ctb_gpt_config& c = h->cfg;
-  const int n = h->B > 16 ? 1 : 0, npad = n ? 32 : 16;
+  const int n = tc_npad_index(h->B), npad = 16 << n;
   TcDecP p = make_tc(h);
   const int rpi = h->infer_text ? 1 : c.num_vq;
   const int V = h->infer_text ? c.num_text_tokens : c.num_audio_tokens;
@@ -1121,9 +1132,9 @@ extern "C" int ctb_gpt_begin(ctb_gpt* h, int32_t B, int32_t T0, const float* emb
   if (h->use_tc) {
     const size_t d = h->cfg.hidden_size, I = h->cfg.intermediate_size;
     float* z768[] = {h->x_hi, h->x_lo, h->attn_hi, h->attn_lo};
-    for (float* zp : z768) CTB_CUDA(cudaMemsetAsync(zp, 0, 32 * d * sizeof(float), s));
-    CTB_CUDA(cudaMemsetAsync(h->h_hi, 0, 32 * I * sizeof(float), s));
-    CTB_CUDA(cudaMemsetAsync(h->h_lo, 0, 32 * I * sizeof(float), s));
+    for (float* zp : z768) CTB_CUDA(cudaMemsetAsync(zp, 0, h->tc_rows * d * sizeof(float), s));
+    CTB_CUDA(cudaMemsetAsync(h->h_hi, 0, h->tc_rows * I * sizeof(float), s));
+    CTB_CUDA(cudaMemsetAsync(h->h_lo, 0, h->tc_rows * I * sizeof(float), s));
   }
   int rc;
   // prefill: the prompt is walked column by column through the decode kernels (left padding
@@ -1204,18 +1215,21 @@ extern "C" int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_ca
   if (max_new_cap < 1 || max_new_cap >= c.max_context)
     return set_err(CTB_ERR_ARG, "max_new_cap=%d outside [1,%d)", max_new_cap, c.max_context);
   if (flags & ~(CTB_ENGINE_FP16_WEIGHTS | CTB_ENGINE_FP16_KV)) return set_err(CTB_ERR_ARG, "unknown engine flags 0x%x", flags);
-  if (flags && S > 32) return set_err(CTB_ERR_ARG, "S=%d: a half-precision engine serves up to 32 slots", S);
+  if (flags && S > 64) return set_err(CTB_ERR_ARG, "S=%d: a half-precision engine serves up to 64 slots", S);
   if (flags && getenv("CTB_GPT_FMA"))
     return set_err(CTB_ERR_ARG, "a half-precision engine runs on the wgmma step, which CTB_GPT_FMA=1 disables");
   cudaStream_t s = (cudaStream_t)stream;
   int rc;
-  if (flags) {
-    // the half-precision engine always runs the wgmma step: build what this handle lacks (a handle whose max_batch is
-    // below 9 or above 32 has no tensor-core state yet)
+  // the wgmma step serves every half-precision engine and fp32 engines of tc_min_batch..64 slots, whatever the handle's
+  // max_batch (CTB_GPT_FMA=1 keeps fp32 engines on the PDL chain); wider fp32 engines run the chain
+  const bool use_tc = flags ? true : getenv("CTB_GPT_FMA") == nullptr && S >= h->tc_min_batch && S <= 64;
+  if (use_tc) {
+    // build what this handle lacks (a handle whose max_batch is below 9 or above 32 has no tensor-core state yet)
     if ((flags & CTB_ENGINE_FP16_WEIGHTS) ? (rc = fp16_setup(h)) : (!h->tc_wqkv && (rc = tc_setup(h)))) return rc;
     if ((flags & CTB_ENGINE_FP16_KV) && !(flags & CTB_ENGINE_FP16_WEIGHTS)) {
       if ((rc = set_tc_attr<DE_QKV, 16, CS_QKV, CTB_ENGINE_FP16_KV>())) return rc;
       if ((rc = set_tc_attr<DE_QKV, 32, CS_QKV, CTB_ENGINE_FP16_KV>())) return rc;
+      if ((rc = set_tc_attr<DE_QKV, 64, CS_QKV, CTB_ENGINE_FP16_KV>())) return rc;
     }
   }
   if (!h->rows) {
@@ -1226,11 +1240,12 @@ extern "C" int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_ca
     if ((rc = dalloc(&h->eng_text_logits, (size_t)c.max_batch * c.num_text_tokens))) return rc;
     if ((rc = dalloc(&h->eng_text_idx, (size_t)c.max_batch))) return rc;
   }
-  // S rows of audio codes or text, each slot owning a fixed page range of max_context tokens; PDL chain (S <= 8) or wgmma
-  // step (S >= 9, and every half-precision engine) - the one-kernel steps are never selected (use_flow, enqueue_step)
+  // S rows of audio codes or text, each slot owning a fixed page range of max_context tokens; PDL chain (S <= 8 or S > 64)
+  // or wgmma step (9 <= S <= 64, and every half-precision engine) - the one-kernel steps are never selected (use_flow,
+  // enqueue_step)
   h->engine = 1; h->phase = RS_RUNNING; h->prec = flags;
   h->B = S; h->T0 = 0; h->max_new = max_new_cap; h->infer_text = 0;
-  h->use_tc = flags ? true : h->tc_ready && S >= h->tc_min_batch;
+  h->use_tc = use_tc;
   h->q_noise = h->eng_noise; h->emb = nullptr; h->mask = nullptr;
   h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev; h->eng_text = 0;
   if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
@@ -1249,9 +1264,9 @@ extern "C" int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_ca
   if (h->use_tc) {
     const size_t d = c.hidden_size, I = c.intermediate_size;
     float* z768[] = {h->x_hi, h->x_lo, h->attn_hi, h->attn_lo};
-    for (float* zp : z768) CTB_CUDA(cudaMemsetAsync(zp, 0, 32 * d * sizeof(float), s));
-    CTB_CUDA(cudaMemsetAsync(h->h_hi, 0, 32 * I * sizeof(float), s));
-    CTB_CUDA(cudaMemsetAsync(h->h_lo, 0, 32 * I * sizeof(float), s));
+    for (float* zp : z768) CTB_CUDA(cudaMemsetAsync(zp, 0, h->tc_rows * d * sizeof(float), s));
+    CTB_CUDA(cudaMemsetAsync(h->h_hi, 0, h->tc_rows * I * sizeof(float), s));
+    CTB_CUDA(cudaMemsetAsync(h->h_lo, 0, h->tc_rows * I * sizeof(float), s));
   }
   CTB_CUDA(cudaStreamSynchronize(s));  // idle_state is read by the copy engine
   h->started = 1;

@@ -29,7 +29,9 @@ namespace ctb {
 enum DecEpi { DE_QKV = 0, DE_OPROJ = 1, DE_GATEUP = 2, DE_DOWN = 3, DE_HEADS = 4 };
 enum DecPrec { TD_W16 = 1, TD_KV16 = 2 };  // the bits of CTB_ENGINE_FP16_WEIGHTS / CTB_ENGINE_FP16_KV
 
-constexpr int TD_STAGES = 3;  // 3 x 36-48 KiB: two CTAs (this kernel + its PDL successor) fit one SM
+// 3 stages of 28-40 KiB at NPAD 16 / 32: two CTAs (this kernel + its PDL successor) fit one SM; at NPAD 64 (40 KiB
+// fp16 / 48 KiB fp32 stages, 121.5 / 145.5 KiB in all) one CTA per SM
+constexpr int TD_STAGES = 3;
 constexpr int TD_THREADS = 160;  // warps 0-3: one warpgroup (rms, W split, wgmma, epilogue); warp 4: TMA
 constexpr int TD_A_BYTES = 128 * 32 * 4;  // 16 KiB weight tile (128 rows x 32 k)
 constexpr int TD_A16_BYTES = 128 * 32 * 2;  // 8 KiB fp16 weight tile as TMA lands it
@@ -224,9 +226,12 @@ k_tc_dec(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUte
           if constexpr (NPAD == 16) {
             wgmma_tf32_n32(acc[hf], wgmma_desc_sw128(w_hi + ro + ko), wgmma_desc_sw128(x_hl + ko), (t | k) ? 1u : 0u);
             if constexpr (!W16) wgmma_tf32_n16(acc[hf], wgmma_desc_sw128(w_lo + ro + ko), wgmma_desc_sw128(x_hl + ko), 1u);
-          } else {
+          } else if constexpr (NPAD == 32) {
             wgmma_tf32_n64(acc[hf], wgmma_desc_sw128(w_hi + ro + ko), wgmma_desc_sw128(x_hl + ko), (t | k) ? 1u : 0u);
             if constexpr (!W16) wgmma_tf32_n32(acc[hf], wgmma_desc_sw128(w_lo + ro + ko), wgmma_desc_sw128(x_hl + ko), 1u);
+          } else {
+            wgmma_tf32_n128(acc[hf], wgmma_desc_sw128(w_hi + ro + ko), wgmma_desc_sw128(x_hl + ko), (t | k) ? 1u : 0u);
+            if constexpr (!W16) wgmma_tf32_n64(acc[hf], wgmma_desc_sw128(w_lo + ro + ko), wgmma_desc_sw128(x_hl + ko), 1u);
           }
         }
       }

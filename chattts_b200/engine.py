@@ -29,6 +29,17 @@ from .processors import build_sampler_config, exp_noise
 
 #: shortest prompt the token-parallel prefill takes; shorter prompts are left padded with masked columns
 MIN_PROMPT_COLS = 8
+#: most prompt rows (prompts x padded width) one admission prefill takes.  Its activation scratch is sized per call and
+#: kept by the handle (3.8 GB for 64 prompts of 1,024 tokens); larger admissions run as consecutive prefills of up to
+#: this many rows, so an engine of 64 slots needs no more of it (1.9 GB) than one of 32 did.
+ADMIT_MAX_ROWS = 32 * 1024
+
+
+def admission_chunks(group: list, T0: int) -> List[list]:
+    """``group`` (one admission's prompts, padded to ``T0`` columns) as consecutive runs of at most
+    ``ADMIT_MAX_ROWS // T0`` prompts."""
+    n = max(1, ADMIT_MAX_ROWS // T0)
+    return [group[i: i + n] for i in range(0, len(group), n)]
 
 
 @dataclass(eq=False)
@@ -479,7 +490,8 @@ class EngineDevice:
             alone = [(s, i) for s, i in group if T0 + self.requests[i].max_new_token > self.gpt.max_context]
             rest = [p for p in group if p not in alone]
             for part in ([rest] if rest else []) + [[p] for p in alone]:
-                self._admit(part, seeded, text, noise)
+                for chunk in admission_chunks(part, T0):  # each prompt's results do not depend on its batch
+                    self._admit(chunk, seeded, text, noise)
 
     def _admit(self, group, seeded: bool, text: bool, cache: Dict[tuple, torch.Tensor]) -> None:
         gpt, n = self.gpt, len(group)

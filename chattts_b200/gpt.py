@@ -233,7 +233,8 @@ class GPT:
         """Generate audio codes or text for many utterances on a slot engine (chattts_b200.engine): up to ``slots``
         requests (default: ``max_batch``, at most the number of requests) decode together, and a waiting request takes
         the place of a finished one at the next poll (every ``chunk`` steps, default CTB_DECODE_CHUNK or 32).  Each
-        ``Request`` chooses its mode (``Request.infer_text``); code and text requests share the engine.
+        ``Request`` chooses its mode (``Request.infer_text``); code and text requests share the engine.  ``slots`` may
+        be up to the handle's ``max_batch``: engines of 9..64 slots run the wgmma decode step, wider ones the PDL chain.
 
         Generator of ``(request_index, GenerationOutputs)`` in completion order.  Each request's ids equal, bit for
         bit, ``generate`` on that request alone with the same arguments and ``manual_seed``.  A seeded request that
@@ -248,7 +249,8 @@ class GPT:
 
         ``dtype=torch.float16`` runs a half-precision engine (ctb_gpt_engine_begin_ex): the four matrices of every
         layer and the KV cache in fp16, everything else fp32 (the model the reference serves with
-        ``Chat.load(use_vllm=True)``).  Its ids then follow that model, not ``generate``'s fp32 one."""
+        ``Chat.load(use_vllm=True)``).  Its ids then follow that model, not ``generate``'s fp32 one.  It serves up to
+        64 slots (``CtbError`` above)."""
         from .engine import ScheduleStats, schedule
 
         flags = _lib.engine_flags(dtype)
@@ -312,7 +314,8 @@ class GPT:
         (copies), and simply ends when cancelled.  ``submit`` checks the request against this handle and
         ``max_new_cap`` in the caller's thread.  One worker thread owns the handle and its stream; while the engine
         is open ``generate``, ``generate_continuous*`` and another ``open_engine`` raise.  The poll interval is
-        ``chunk`` steps (default CTB_DECODE_CHUNK, else 24).  ``dtype`` as in ``generate_continuous``."""
+        ``chunk`` steps (default CTB_DECODE_CHUNK, else 24).  ``slots`` and ``dtype`` as in ``generate_continuous``
+        (up to ``max_batch`` slots; a half-precision engine up to 64)."""
         from .engine import GptEngine
 
         return self._open_slot_engine(GptEngine, slots, max_new_cap, return_hidden, chunk,

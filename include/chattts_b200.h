@@ -150,7 +150,9 @@ int ctb_gpt_status_query(ctb_gpt* h, ctb_gpt_status* out, int32_t* end_idx_host,
 #define CTB_SLOT_FINISHED 2
 
 /* Turn the handle into S slots (2 <= S <= max_batch), all idle.  Every slot owns a fixed KV page range of
- * max_context tokens (S x max_context tokens in all).
+ * max_context tokens (S x max_context tokens in all).  Engines of 9 <= S <= 64 slots run the wgmma step whatever the
+ * handle's max_batch (CTB_GPT_FMA=1 keeps them on the PDL chain), building its state on a handle that lacks it; the
+ * others run the PDL chain.
  *   ids_out_dev      [S, max_new_cap, num_vq] int32   slot b's tokens: ids_out_dev[b, 0 : end_idx[b]]
  *   hiddens_out_dev  [S, max_new_cap, d] fp32 or NULL  its last hidden states, same rows */
 int ctb_gpt_engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t* ids_out_dev, float* hiddens_out_dev,
@@ -167,11 +169,11 @@ int ctb_gpt_engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t* id
  *                            and decode, reads the rounded values.  K/V overflow is not checked (nor is it in the
  *                            reference's fp16 modes).
  * Embeddings, RMSNorm statistics, RoPE, activations, attention arithmetic, the heads, the sampler and the hidden
- * states in hiddens_out_dev stay fp32.  A flagged engine always runs the wgmma step with 16 (S <= 16) or 32 padded
- * rows and builds what the handle lacks for it; the fp16 copies (377.5 MB for the 20 layers, plus their 755 MB fp32
+ * states in hiddens_out_dev stay fp32.  A flagged engine always runs the wgmma step with 16 (S <= 16), 32 (S <= 32) or
+ * 64 padded rows and builds what the handle lacks for it; the fp16 copies (377.5 MB for the 20 layers, plus their 755 MB fp32
  * image read by the prefill GEMMs) are built by the first CTB_ENGINE_FP16_WEIGHTS engine and kept until
  * ctb_gpt_destroy.  The KV pool is sized in bytes and shared by every call on the handle.
- * Errors (CTB_ERR_ARG): unknown flag bits; S > 32 with a flag set; a flag set while CTB_GPT_FMA=1; a layer weight
+ * Errors (CTB_ERR_ARG): unknown flag bits; S > 64 with a flag set; a flag set while CTB_GPT_FMA=1; a layer weight
  * (norm folded) with |w| > 65504, named by layer and matrix in ctb_last_error - the handle is left as it was. */
 #define CTB_ENGINE_FP16_WEIGHTS 1
 #define CTB_ENGINE_FP16_KV 2
