@@ -222,7 +222,9 @@ class Chat:
         (``open_engine``), all queued at once; ``params_infer_code`` is one ``InferCodeParams`` for all texts or a list
         with one per text (speaker, seed, temperature, top-P/K, penalty, token limits).  Generator of ``(index, wav)``
         in completion order; ``wav`` is what ``infer([texts[index]], split_text=False, skip_refine_text=True)``
-        returns for that text with its params.
+        returns for that text with its params.  A code prompt (text plus ``spk_smp``) may be up to ``max_context`` -
+        ``max_new_token`` tokens; over 1,024 tokens it is prefilled with the tiled attention kernel, whose ids equal
+        ``infer``'s except at the sampler's near-ties (``GPT.generate_continuous``).
         Normalisation and the optional text refinement run as in ``infer``; ``params_refine_text`` is one
         ``RefineTextParams`` or one per text.
 
@@ -446,7 +448,9 @@ class Chat:
         decodes: ``engine.submit(text, params_infer_code=None, stream=False, skip_refine_text=True, ...) -> Job``,
         ``Job.cancel()`` for one text, ``close(cancel=False)`` or a ``with`` block to drain it (``close(cancel=True)``
         is its interrupt; ``Chat.context`` is not read).  ``slots`` defaults to the handle's ``max_batch`` (up to 64
-        for ``dtype=torch.float16``); every stage's ``max_new_token`` must be at most ``max_new_cap``.  See ``ChatEngine.submit``.  ``dtype`` as in
+        for ``dtype=torch.float16``); every stage's ``max_new_token`` must be at most ``max_new_cap``, and its prompt
+        plus ``max_new_token`` at most ``max_context`` (prompts over 1,024 tokens as in ``infer_continuous``).  See
+        ``ChatEngine.submit``.  ``dtype`` as in
         ``infer_continuous``: every stage of every job runs on that engine."""
         flags = _lib.engine_flags(dtype)
         assert self.has_loaded(use_decoder=use_decoder)

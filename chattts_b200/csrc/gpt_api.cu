@@ -1029,6 +1029,10 @@ static int prefill_batched(ctb_gpt* h, int B, int T0, const float* emb, const ui
   const int rms_blocks = (M + 7) / 8;
   // a half-precision engine: the rounded weights (norms folded in before rounding) with W_lo = 0 and unit norms
   const bool w16 = (h->prec & CTB_ENGINE_FP16_WEIGHTS) != 0, kv16 = (h->prec & CTB_ENGINE_FP16_KV) != 0;
+  if (T0 > PF_ATT_MAX_T0 &&
+      (rc = kv16 ? ensure_smem_attr((const void*)k_prefill_attn_tiled<__half>, PftSmem<__half>::BYTES)
+                 : ensure_smem_attr((const void*)k_prefill_attn_tiled<float>, PftSmem<float>::BYTES)))
+    return rc;
   for (int l = 0; l < c.num_layers; ++l) {
     const int64_t lo = (int64_t)l * L.layer_stride;
     const float* Wl = h->W + L.layer0 + lo;
@@ -1042,9 +1046,15 @@ static int prefill_batched(ctb_gpt* h, int B, int T0, const float* emb, const ui
     if (kv16) k_prefill_rope_kv<__half><<<dim3(T0, B), 256, 0, s>>>(pp);
     else k_prefill_rope_kv<float><<<dim3(T0, B), 256, 0, s>>>(pp);
     CTB_LAUNCH_CHECK();
-    const dim3 agrid((T0 + PF_ATT_WARPS - 1) / PF_ATT_WARPS, c.num_heads, B);
-    if (kv16) k_prefill_attn<__half><<<agrid, PF_ATT_WARPS * 32, (size_t)PF_ATT_WARPS * T0 * sizeof(float), s>>>(pp);
-    else k_prefill_attn<float><<<agrid, PF_ATT_WARPS * 32, (size_t)PF_ATT_WARPS * T0 * sizeof(float), s>>>(pp);
+    if (T0 > PF_ATT_MAX_T0) {
+      const dim3 tgrid((T0 + PFT_TILE - 1) / PFT_TILE, c.num_heads, B);
+      if (kv16) k_prefill_attn_tiled<__half><<<tgrid, PFT_THREADS, PftSmem<__half>::BYTES, s>>>(pp);
+      else k_prefill_attn_tiled<float><<<tgrid, PFT_THREADS, PftSmem<float>::BYTES, s>>>(pp);
+    } else {
+      const dim3 agrid((T0 + PF_ATT_WARPS - 1) / PF_ATT_WARPS, c.num_heads, B);
+      if (kv16) k_prefill_attn<__half><<<agrid, PF_ATT_WARPS * 32, (size_t)PF_ATT_WARPS * T0 * sizeof(float), s>>>(pp);
+      else k_prefill_attn<float><<<agrid, PF_ATT_WARPS * 32, (size_t)PF_ATT_WARPS * T0 * sizeof(float), s>>>(pp);
+    }
     CTB_LAUNCH_CHECK();
     if ((rc = tc_gemm_launch<GE_SCALE_RES>(s, h->pf_attn, d, B, T0, d, d, 1, d, 1, 0, Whi + L.wo, wlo(L.wo), h->pf_zeros,
                                            h->pf_ones, h->pf_resid, d, h->pf_resid, d))) return rc;
@@ -1282,7 +1292,9 @@ static int engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0,
   const ctb_gpt_config& c = h->cfg;
   const int S = h->B;
   if (n < 1 || n > S) return set_err(CTB_ERR_ARG, "n=%d outside [1,%d]", n, S);
-  if (T0 < 8 || T0 > 1024) return set_err(CTB_ERR_ARG, "T0=%d outside [8,1024]: left-pad shorter prompts to 8", T0);
+  // prompts over 1,024 columns take the tiled prefill attention; every slot owns max_context tokens of pages
+  if (T0 < 8 || T0 > c.max_context - 1)
+    return set_err(CTB_ERR_ARG, "T0=%d outside [8,%d]: left-pad shorter prompts to 8", T0, c.max_context - 1);
   cudaStream_t s = (cudaStream_t)stream;
   std::vector<RowState> rows((size_t)h->bpad_max);
   CTB_CUDA(cudaMemcpyAsync(rows.data(), h->rows, sizeof(RowState) * rows.size(), cudaMemcpyDeviceToHost, s));

@@ -4,7 +4,8 @@
 // for the GEMM tiler; pad columns are computed but never written to the KV cache nor attended to.
 //
 //   per layer:  k_rms_rows -> GEMM(Wqkv) -> k_prefill_rope_kv (RoPE, q buffer, paged-KV append)
-//               -> k_prefill_attn (causal over the row's valid tokens) -> GEMM(Wo)+residual
+//               -> k_prefill_attn (causal over the row's valid tokens; k_prefill_attn_tiled when T0 > 1024)
+//               -> GEMM(Wo)+residual
 //               -> k_rms_rows -> GEMM([Wgate;Wup]) -> k_silu_mul -> GEMM(Wdown)+residual
 //   then k_prefill_finish hands the last column's residual to the decode-loop state (x, seq_len) and the
 //   regular heads -> sampler -> finalize kernels produce the first token.
@@ -162,6 +163,195 @@ __global__ void __launch_bounds__(PF_ATT_WARPS * 32) k_prefill_attn(const Prefil
     o0 = fmaf(pk, v.x, o0); o1 = fmaf(pk, v.y, o1);
   }
   *reinterpret_cast<float2*>(p.attn + qrow + 2 * lane) = make_float2(o0 / l, o1 / l);  // V (and the output) is never permuted
+}
+
+// k_prefill_attn keeps a query's whole score row in shared memory (8 x T0 floats per CTA): prompts wider than this
+// take k_prefill_attn_tiled.  The choice depends on T0 alone, so a prompt of up to 1,024 columns is computed as before.
+constexpr int PF_ATT_MAX_T0 = 1024;
+
+// Tiled causal attention for prompts over PF_ATT_MAX_T0 columns: grid (ceil(T0 / 64), Hq, B), 256 threads.  A CTA takes
+// 64 consecutive queries t of one (row, head) and walks the key tiles 0 .. t / 64 (tiles wholly above the diagonal are
+// never loaded), each 64 keys = 4 pages of the row's block table, staged into shared memory once for all 64 queries with
+// cp.async and double-buffered.  Online softmax in fp32: running max and sum per query, the accumulator rescaled when
+// the max grows; causal mask inside the diagonal tile.  Thread (ty, tx) = (tid / 16, tid % 16) owns queries
+// 4 ty .. 4 ty + 3, and keys tx + 16 j of a tile for the scores, dims 4 tx .. 4 tx + 3 for P.V.  A score is the same
+// fmaf chain over the 64 dims as k_prefill_attn's.  Shared memory is fixed (PftSmem), whatever T0.  KVT: the cache's
+// element type, staged as it is stored and widened to fp32 as it is read.
+constexpr int PFT_TILE = 64, PFT_THREADS = 256;
+template <typename KVT>
+struct PftSmem {
+  static constexpr int QS = PFT_TILE + 4;                         // Q / P row stride (floats): 16-byte rows, one pad
+  static constexpr int KS = PFT_TILE + 16 / (int)sizeof(KVT);     // K / V row stride (elements): one 16-byte pad
+  static constexpr int CH = PFT_TILE * (int)sizeof(KVT) / 16;     // 16-byte chunks per K / V row
+  static constexpr int Q_FLOATS = PFT_TILE * QS;
+  static constexpr int KV_ELEMS = PFT_TILE * KS;                  // one K or V tile
+  static constexpr int BYTES = 2 * Q_FLOATS * 4 + 2 * 2 * KV_ELEMS * (int)sizeof(KVT);  // Q, P, 2 stages of K and V
+};
+
+__device__ __forceinline__ void pft_cp16(void* smem_dst, const void* gsrc, bool valid) {
+  // 16 bytes global -> shared; !valid: no read, 16 zero bytes
+  const uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d), "l"(gsrc), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void pft_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void pft_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// 8 consecutive staged values as fp32
+__device__ __forceinline__ void pft_ld8(const float* p, float4& a, float4& b) {
+  a = *reinterpret_cast<const float4*>(p); b = *reinterpret_cast<const float4*>(p + 4);
+}
+__device__ __forceinline__ void pft_ld8(const __half* p, float4& a, float4& b) {
+  const uint4 u = *reinterpret_cast<const uint4*>(p);
+  const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
+  const float2 f1 = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+  const float2 f2 = __half22float2(*reinterpret_cast<const __half2*>(&u.z));
+  const float2 f3 = __half22float2(*reinterpret_cast<const __half2*>(&u.w));
+  a = make_float4(f0.x, f0.y, f1.x, f1.y); b = make_float4(f2.x, f2.y, f3.x, f3.y);
+}
+// 4 consecutive staged values as fp32
+__device__ __forceinline__ float4 pft_ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
+__device__ __forceinline__ float4 pft_ld4(const __half* p) {
+  const uint2 u = *reinterpret_cast<const uint2*>(p);
+  const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
+  const float2 f1 = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+  return make_float4(f0.x, f0.y, f1.x, f1.y);
+}
+
+template <typename KVT>
+__global__ void __launch_bounds__(PFT_THREADS) k_prefill_attn_tiled(const PrefillP p) {
+  using SM = PftSmem<KVT>;
+  constexpr int HD = 64, T = PFT_TILE;
+  const int h = blockIdx.y, b = blockIdx.z, tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
+  const int n = p.nvalid[b];
+  const int qt = gridDim.x - 1 - blockIdx.x;  // the longest walks start first
+  if (qt * T >= n) return;                     // CTA-uniform, before any barrier
+  extern __shared__ __align__(16) unsigned char pft_smem[];
+  float* sQ = reinterpret_cast<float*>(pft_smem);
+  float* sP = sQ + SM::Q_FLOATS;
+  KVT* sKV = reinterpret_cast<KVT*>(sP + SM::Q_FLOATS);  // [stage][K, V][T][KS]
+  const int hk = h / (p.Hq / p.Hkv);
+  const int* bt = p.block_table + (p.slot ? p.slot[b] : b) * p.pages_per_row;
+  const int c0 = p.T0 - n;                     // first valid column (left padding)
+  const KVT* kv = reinterpret_cast<const KVT*>(p.kv);
+  const size_t row0 = (size_t)b * p.T0 + c0;   // column of query / key 0
+
+  // queries qt*64 .. qt*64+63 (zeros past the row's last)
+  for (int i = tid; i < T * 16; i += PFT_THREADS) {
+    const int r = i >> 4, c = i & 15, t = qt * T + r;
+    const float* src = t < n ? p.q + ((row0 + t) * p.Hq + h) * HD + c * 4 : p.q;
+    pft_cp16(sQ + r * SM::QS + c * 4, src, t < n);
+  }
+  // keys / values of tile kt into stage st (zeros past the row's last key)
+  auto load_kv = [&](int kt, int st) {
+    KVT* dst = sKV + (size_t)st * 2 * SM::KV_ELEMS;
+    for (int i = tid; i < 2 * T * SM::CH; i += PFT_THREADS) {
+      const int which = i / (T * SM::CH), r = (i / SM::CH) % T, c = i % SM::CH, k = kt * T + r;
+      constexpr int E = 16 / (int)sizeof(KVT);
+      const KVT* src = k < n ? kv + kv_off(bt[k / kPageTokens], which, hk, k % kPageTokens, p.Hkv, HD) + c * E : kv;
+      pft_cp16(dst + which * SM::KV_ELEMS + r * SM::KS + c * E, src, k < n);
+    }
+  };
+  load_kv(0, 0);
+  pft_commit();
+
+  float m[4], l[4], o[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    m[i] = -INFINITY; l[i] = 0.f;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) o[i][e] = 0.f;
+  }
+  for (int kt = 0; kt <= qt; ++kt) {
+    const int st = kt & 1;
+    if (kt < qt) { load_kv(kt + 1, st ^ 1); pft_commit(); pft_wait<1>(); }
+    else pft_wait<0>();
+    __syncthreads();
+    const KVT* sK = sKV + (size_t)st * 2 * SM::KV_ELEMS;
+    const KVT* sV = sK + SM::KV_ELEMS;
+    // scores of queries 4 ty + i against keys tx + 16 j
+    float s[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
+#pragma unroll 2
+    for (int d = 0; d < HD; d += 8) {
+      float4 qa[4], qb[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        qa[i] = *reinterpret_cast<const float4*>(sQ + (ty * 4 + i) * SM::QS + d);
+        qb[i] = *reinterpret_cast<const float4*>(sQ + (ty * 4 + i) * SM::QS + d + 4);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        float4 ka, kb;
+        pft_ld8(sK + (tx + 16 * j) * SM::KS + d, ka, kb);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          float a = s[i][j];
+          a = fmaf(qa[i].x, ka.x, a); a = fmaf(qa[i].y, ka.y, a); a = fmaf(qa[i].z, ka.z, a); a = fmaf(qa[i].w, ka.w, a);
+          a = fmaf(qb[i].x, kb.x, a); a = fmaf(qb[i].y, kb.y, a); a = fmaf(qb[i].z, kb.z, a); a = fmaf(qb[i].w, kb.w, a);
+          s[i][j] = a;
+        }
+      }
+    }
+    // causal mask, online softmax (a query's 64 scores are spread over the 16 lanes tx of its half-warp)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int t = min(qt * T + ty * 4 + i, n - 1);  // queries past the row's last see its keys, and are not written
+      float mx = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int k = kt * T + tx + 16 * j;
+        s[i][j] = k <= t ? s[i][j] * p.scaling : -INFINITY;
+        mx = fmaxf(mx, s[i][j]);
+      }
+#pragma unroll
+      for (int off = 8; off > 0; off >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+      const float mn = fmaxf(m[i], mx);            // finite: key kt * 64 <= t is never masked
+      const float alpha = expf(m[i] - mn);         // 0 on the first tile
+      float sum = 0.f;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float e = expf(s[i][j] - mn);
+        sP[(ty * 4 + i) * SM::QS + tx + 16 * j] = e;
+        sum += e;
+      }
+#pragma unroll
+      for (int off = 8; off > 0; off >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, off);
+      l[i] = l[i] * alpha + sum;
+      m[i] = mn;
+#pragma unroll
+      for (int e = 0; e < 4; ++e) o[i][e] *= alpha;
+    }
+    __syncthreads();
+    // o += P . V over the tile's keys in order
+#pragma unroll 2
+    for (int k = 0; k < T; k += 4) {
+      float4 pr[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) pr[i] = *reinterpret_cast<const float4*>(sP + (ty * 4 + i) * SM::QS + k);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        const float4 v = pft_ld4(sV + (k + kk) * SM::KS + tx * 4);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float pk = kk == 0 ? pr[i].x : kk == 1 ? pr[i].y : kk == 2 ? pr[i].z : pr[i].w;
+          o[i][0] = fmaf(pk, v.x, o[i][0]); o[i][1] = fmaf(pk, v.y, o[i][1]);
+          o[i][2] = fmaf(pk, v.z, o[i][2]); o[i][3] = fmaf(pk, v.w, o[i][3]);
+        }
+      }
+    }
+    __syncthreads();  // stage st and P are rewritten by the next tile
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int t = qt * T + ty * 4 + i;
+    if (t < n)  // V (and the output) is never permuted
+      *reinterpret_cast<float4*>(p.attn + ((row0 + t) * p.Hq + h) * HD + tx * 4) =
+          make_float4(o[i][0] / l[i], o[i][1] / l[i], o[i][2] / l[i], o[i][3] / l[i]);
+  }
 }
 
 // h = silu(gate) * up over [M, 2I] -> [M, I]

@@ -29,6 +29,9 @@ from .processors import build_sampler_config, exp_noise
 
 #: shortest prompt the token-parallel prefill takes; shorter prompts are left padded with masked columns
 MIN_PROMPT_COLS = 8
+#: widest prefill whose attention keeps the short-prompt kernel (k_prefill_attn); a longer prompt takes the tiled
+#: kernel and is prefilled on its own (``admission_groups``)
+LONG_PROMPT_COLS = 1024
 #: most prompt rows (prompts x padded width) one admission prefill takes.  Its activation scratch is sized per call and
 #: kept by the handle (3.8 GB for 64 prompts of 1,024 tokens); larger admissions run as consecutive prefills of up to
 #: this many rows, so an engine of 64 slots needs no more of it (1.9 GB) than one of 32 did.
@@ -42,11 +45,34 @@ def admission_chunks(group: list, T0: int) -> List[list]:
     return [group[i: i + n] for i in range(0, len(group), n)]
 
 
+def admission_groups(group: list, requests: Sequence["Request"], max_context: int) -> List[Tuple[list, int]]:
+    """``group`` (one admission's ``(slot, request index)`` pairs of one kind) as the prefills it runs as, each with
+    its padded width: ``[(pairs, T0)]``.
+
+    Prompts of up to ``LONG_PROMPT_COLS`` tokens share one width, and a request whose ``max_new_token`` no longer fits
+    its slot's ``max_context`` next to that width is admitted on its own.  A longer prompt is always prefilled on its
+    own, after them, so it never pads a short prompt to its width."""
+    def cols(pairs):
+        return max(MIN_PROMPT_COLS, max(int(requests[i].emb.shape[0]) for _, i in pairs))
+
+    short = [(s, i) for s, i in group if int(requests[i].emb.shape[0]) <= LONG_PROMPT_COLS]
+    out = []
+    if short:
+        T0 = cols(short)
+        alone = [(s, i) for s, i in short if T0 + requests[i].max_new_token > max_context]
+        rest = [p for p in short if p not in alone]
+        out += [(part, T0) for part in ([rest] if rest else [])] + [([p], T0) for p in alone]
+    return out + [([p], cols([p])) for p in group if int(requests[p[1]].emb.shape[0]) > LONG_PROMPT_COLS]
+
+
 @dataclass(eq=False)
 class Request:
     """One utterance for ``GPT.generate_continuous``.
 
-    ``emb``: [T, d] prompt embedding (every position valid, as a batch of one has no padding) or [1, T, d].
+    ``emb``: [T, d] prompt embedding (every position valid, as a batch of one has no padding) or [1, T, d];
+    ``T + max_new_token`` at most the handle's ``max_context``.  A prompt of more than ``LONG_PROMPT_COLS`` (1,024)
+    tokens is prefilled on its own with the tiled attention kernel (``GPT.generate_continuous`` on what that means
+    for equality with ``GPT.generate``).
     The other fields mean what the ``GPT.generate`` arguments of the same name mean; ``infer_text=True`` generates
     text tokens (one temperature, ``eos_token`` the tokenizer's EOS) and its outputs are those of
     ``GPT.generate(infer_text=True)`` for one row: 1-D int64 ids and no hidden states.
@@ -484,12 +510,7 @@ class EngineDevice:
                      and bool(self.requests[i].infer_text) == text]
             if not group:
                 continue
-            # the prompts share one padded width; a request whose max_new no longer fits its slot's max_context
-            # next to that width is admitted on its own
-            T0 = max(MIN_PROMPT_COLS, max(int(self.requests[i].emb.shape[0]) for _, i in group))
-            alone = [(s, i) for s, i in group if T0 + self.requests[i].max_new_token > self.gpt.max_context]
-            rest = [p for p in group if p not in alone]
-            for part in ([rest] if rest else []) + [[p] for p in alone]:
+            for part, T0 in admission_groups(group, self.requests, self.gpt.max_context):
                 for chunk in admission_chunks(part, T0):  # each prompt's results do not depend on its batch
                     self._admit(chunk, seeded, text, noise)
 

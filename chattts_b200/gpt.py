@@ -236,8 +236,11 @@ class GPT:
         ``Request`` chooses its mode (``Request.infer_text``); code and text requests share the engine.  ``slots`` may
         be up to the handle's ``max_batch``: engines of 9..64 slots run the wgmma decode step, wider ones the PDL chain.
 
-        Generator of ``(request_index, GenerationOutputs)`` in completion order.  Each request's ids equal, bit for
-        bit, ``generate`` on that request alone with the same arguments and ``manual_seed``.  A seeded request that
+        Generator of ``(request_index, GenerationOutputs)`` in completion order.  A prompt may be up to ``max_context``
+        - ``max_new_token`` tokens.  Up to 1,024 tokens, each request's ids equal, bit for bit, ``generate`` on that
+        request alone with the same arguments and ``manual_seed``.  A longer prompt is prefilled on its own with a tiled
+        attention kernel, while ``generate`` walks such a prompt's columns: the two agree within float rounding, so
+        their ids can differ where the sampler's decision is a near-tie (DESIGN.md §4, "Long prompts").  A seeded request that
         samples EOS first yields empty outputs (``generate`` yields nothing then); an unseeded one with
         ``ensure_non_empty`` runs again.  The handle serves one generator at a time; ``generate`` may be called again
         once it is exhausted.
@@ -312,7 +315,8 @@ class GPT:
         for it; a cancelled job's result is the prefix it had at the poll that stopped it, with ``cancelled=True``.  A
         streaming job iterates ``(GenerationOutputs, last)``, the yields ``generate_continuous_stream`` makes for it
         (copies), and simply ends when cancelled.  ``submit`` checks the request against this handle and
-        ``max_new_cap`` in the caller's thread.  One worker thread owns the handle and its stream; while the engine
+        ``max_new_cap`` in the caller's thread: prompt + ``max_new_token`` within ``max_context``.  A prompt over
+        1,024 tokens is prefilled on its own; the running slots wait for that prefill.  One worker thread owns the handle and its stream; while the engine
         is open ``generate``, ``generate_continuous*`` and another ``open_engine`` raise.  The poll interval is
         ``chunk`` steps (default CTB_DECODE_CHUNK, else 24).  ``slots`` and ``dtype`` as in ``generate_continuous``
         (up to ``max_batch`` slots; a half-precision engine up to 64)."""
@@ -376,9 +380,9 @@ class GPT:
             if not isinstance(r, Request):
                 raise TypeError("requests must be chattts_b200.engine.Request objects")
             T0 = max(MIN_PROMPT_COLS, int(r.emb.shape[0]))
-            if T0 > 1024 or T0 + r.max_new_token > self.max_context:
-                raise ValueError(f"prompt {int(r.emb.shape[0])} + max_new_token {r.max_new_token} exceed this handle "
-                                 f"(max_context={self.max_context}; prompts up to 1024 tokens)")
+            if T0 + r.max_new_token > self.max_context:
+                raise ValueError(f"prompt {int(r.emb.shape[0])} + max_new_token {r.max_new_token} exceed this handle's "
+                                 f"max_context={self.max_context}")
             if r.max_new_token > cap:
                 raise ValueError(f"max_new_token {r.max_new_token} exceeds max_new_cap={cap}")
             check_noise_batch(r, 1 if r.infer_text else self.num_vq, self.max_batch)

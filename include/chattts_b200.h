@@ -181,8 +181,11 @@ int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t 
                             float* hiddens_out_dev, void* stream);
 
 /* Admit n requests into the idle or finished slots slots[0..n) (host array): prefill their prompts (token-parallel,
- * left padded, 8 <= T0 <= 1024: pad shorter prompts with masked columns) into those slots and sample each one's first
- * token; no other slot's state, outputs or KV pages are touched.
+ * left padded, 8 <= T0 <= max_context - 1: pad shorter prompts with masked columns) into those slots and sample each
+ * one's first token; no other slot's state, outputs or KV pages are touched.  Up to T0 = 1024 the prompt's attention is
+ * the one ctb_gpt_begin's prefill runs, bit for bit; a wider admission runs a tiled causal attention (fp32 arithmetic,
+ * results within float rounding of the column walk ctb_gpt_begin uses for such prompts, not bit-equal to it).  Which
+ * one runs depends on T0 alone, and a prompt's results do not depend on the other prompts of its admission.
  *   emb_dev [n, T0, d] fp32, mask_dev [n, T0] uint8 (valid tokens a suffix of each row, as for ctb_gpt_begin)
  *   samplers[n] (host)   sampling parameters of each request (audio codes; penalty_max_ids applies to its own rows
  *                        0..num_vq-1, as in a batch of one)
