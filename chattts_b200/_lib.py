@@ -58,6 +58,10 @@ def engine_flags(dtype) -> int:
     raise ValueError(f"slot engine dtype must be torch.float32 or torch.float16, not {dtype!r}")
 
 
+#: ctb_gpt_engine_prefill_chunk: a chunk's first column, and every chunk but a prompt's last, are multiples of this
+PREFILL_CHUNK_ALIGN = 128
+
+
 #: slot states reported by ctb_gpt_engine_status (CTB_SLOT_* in the header)
 SLOT_IDLE, SLOT_RUNNING, SLOT_FINISHED = 0, 1, 2
 
@@ -78,7 +82,7 @@ EXPORTS = (
     "ctb_abi_version", "ctb_last_error", "ctb_launch_count", "ctb_gpt_layout_query", "ctb_gpt_create",
     "ctb_gpt_destroy", "ctb_gpt_begin", "ctb_gpt_decode", "ctb_gpt_status_query", "ctb_gpt_profile_kernel", "ctb_gpt_debug_trace", "ctb_gpt_embed_prompt", "ctb_sample",
     "ctb_gpt_engine_begin", "ctb_gpt_engine_admit", "ctb_gpt_engine_admit_text", "ctb_gpt_engine_status",
-    "ctb_gpt_engine_cancel", "ctb_gpt_engine_begin_ex",
+    "ctb_gpt_engine_cancel", "ctb_gpt_engine_begin_ex", "ctb_gpt_engine_prefill_chunk",
     "ctb_dvae_blob_floats", "ctb_vocos_blob_floats", "ctb_decoder_create", "ctb_decoder_destroy",
     "ctb_dvae_decode", "ctb_vocos_decode", "ctb_decode_rows",
     "ctb_dvae_encoder_blob_floats", "ctb_dvae_encoder_create", "ctb_dvae_encoder_destroy", "ctb_dvae_encode",
@@ -131,6 +135,8 @@ def load(build_if_missing: bool = True):
         lib.ctb_gpt_engine_admit_text.argtypes = lib.ctb_gpt_engine_admit.argtypes
         lib.ctb_gpt_engine_status.argtypes = [vp, C.POINTER(GptStatus), vp, vp, vp, vp]
         lib.ctb_gpt_engine_cancel.argtypes = [vp, i32, vp, vp]
+        lib.ctb_gpt_engine_prefill_chunk.argtypes = [vp, i32, i32, i32, i32, vp, i32, C.POINTER(SamplerConfig), vp, i32,
+                                                     vp]
         lib.ctb_sample.argtypes = [vp, i32, i32, i32, C.POINTER(SamplerConfig), vp, vp, i32, i32, i32, vp, vp]
         lib.ctb_dvae_blob_floats.argtypes = [C.POINTER(ConvStackConfig)]
         lib.ctb_dvae_blob_floats.restype = i64

@@ -24,7 +24,7 @@ from . import _lib
 from .config import Config
 from .decoder import ENC_NFFT, decode_to_wavs_window, DVAE, Vocos, decode_to_wavs, stream_window
 from .embed import Embed
-from .engine import Job, OpenEngine
+from .engine import Job, OpenEngine, check_prefill_budget
 from .gpt import GPT
 from .norm import Normalizer
 from .processors import gen_logits
@@ -217,7 +217,7 @@ class Chat:
     def infer_continuous(self, texts, params_infer_code=None, use_decoder=True, slots=None, stream=False, lang=None,
                          skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
                          params_refine_text=None, refine_on_engine=False, split_text=False, max_split_batch=1,
-                         dtype=torch.float32):
+                         dtype=torch.float32, prefill_budget: Optional[int] = None):
         """Synthesise many texts with continuous batching: each text is one job on an open slot engine
         (``open_engine``), all queued at once; ``params_infer_code`` is one ``InferCodeParams`` for all texts or a list
         with one per text (speaker, seed, temperature, top-P/K, penalty, token limits).  Generator of ``(index, wav)``
@@ -248,20 +248,25 @@ class Chat:
 
         ``dtype=torch.float16`` runs every request on a half-precision engine (``GPT.generate_continuous``): fp16
         layer weights and KV cache, as the reference's ``use_vllm=True`` serves; the waveforms then follow that model.
-        It serves up to 64 slots.  Path 2 (DVAE / Vocos) is unchanged."""
+        It serves up to 64 slots.  Path 2 (DVAE / Vocos) is unchanged.
+
+        ``prefill_budget`` (prompt columns per poll, at least 128; default None) bounds the prefill the running texts
+        wait for at each poll: a prompt that does not fit, such as one with a long ``spk_smp``, is prefilled in chunks
+        over several polls with the same results (``GPT.generate_continuous``)."""
         _lib.engine_flags(dtype)  # an unsupported dtype raises here, before any device work
+        check_prefill_budget(prefill_budget)
         if stream:
             raise ValueError("infer_continuous: stream=True is not supported; each waveform is yielded when complete "
                              "(infer_continuous_stream streams)")
         texts, params = self._continuous_params(texts, params_infer_code)
         return self._continuous(texts, params, self._refine_params(texts, params_refine_text), False, use_decoder,
                                 slots, lang, skip_refine_text, do_text_normalization, do_homophone_replacement,
-                                refine_on_engine, split_text, max_split_batch, dtype)
+                                refine_on_engine, split_text, max_split_batch, dtype, prefill_budget)
 
     def infer_continuous_stream(self, texts, params_infer_code=None, use_decoder=True, slots=None, lang=None,
                                 skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
                                 params_refine_text=None, refine_on_engine=False, split_text=False, max_split_batch=1,
-                                dtype=torch.float32):
+                                dtype=torch.float32, prefill_budget: Optional[int] = None):
         """Streaming synthesis of many texts with continuous batching on an open slot engine.  Generator of ``(index,
         chunk, last)``, ``chunk`` a ``[1, n]`` float32 array; for each text the chunks are those ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=True)`` yields with that
         text's params (its own ``stream_batch``, ``stream_speed`` and ``pass_first_n_batches``), and ``last`` marks
@@ -270,13 +275,14 @@ class Chat:
         buffers.  Arguments as for ``infer_continuous``; with ``refine_on_engine=True`` the chunks are those of
         ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=False)``.  With ``split_text=True``
         each text is a paragraph, streamed sentence by sentence as ``ChatEngine.submit(split_text=True,
-        stream=True)`` streams it, refined first with ``skip_refine_text=False``.  ``dtype`` as in
-        ``infer_continuous``."""
+        stream=True)`` streams it, refined first with ``skip_refine_text=False``.  ``dtype`` and ``prefill_budget``
+        as in ``infer_continuous``; a budget leaves the chunks as they are."""
         _lib.engine_flags(dtype)
+        check_prefill_budget(prefill_budget)
         texts, params = self._continuous_params(texts, params_infer_code)
         return self._continuous(texts, params, self._refine_params(texts, params_refine_text), True, use_decoder,
                                 slots, lang, skip_refine_text, do_text_normalization, do_homophone_replacement,
-                                refine_on_engine, split_text, max_split_batch, dtype)
+                                refine_on_engine, split_text, max_split_batch, dtype, prefill_budget)
 
     def refine_continuous(self, texts, params_refine_text=None, slots=None, lang=None, do_text_normalization=True,
                           do_homophone_replacement=True, dtype=torch.float32):
@@ -320,7 +326,7 @@ class Chat:
 
     def _continuous(self, texts, params, refine, stream, use_decoder, slots, lang, skip_refine_text,
                     do_text_normalization, do_homophone_replacement, refine_on_engine, split_text, max_split_batch,
-                    dtype):
+                    dtype, prefill_budget=None):
         """``infer_continuous*``: every text one ``ChatEngine`` job on one open engine.  Generator of ``(index, wav)``
         in completion order, or of ``(index, chunk, last)`` as the chunks come.
 
@@ -368,7 +374,7 @@ class Chat:
         out: queue.Queue = queue.Queue()  # (k, (chunk, last)), or (k, None) once text k's job has ended
         with self.gpt._open_slot_engine(ChatEngine, slots, cap, use_decoder, chunk, self, use_decoder,
                                         None if split_text else self.context,
-                                        flags=_lib.engine_flags(dtype)) as eng:
+                                        flags=_lib.engine_flags(dtype), prefill_budget=prefill_budget) as eng:
             subs = [eng._job(t, p, stream, skip_refine_text, r, split_text, max_split_batch, normalize, (out, k))
                     for k, (t, p, r) in enumerate(zip(texts, params, refine))]
             eng._enqueue(subs)
@@ -443,7 +449,7 @@ class Chat:
         return self.tokenizer.decode([ids[ids.less(self.tokenizer.break_0_ids)]])[0]
 
     def open_engine(self, slots: Optional[int] = None, max_new_cap: int = 2048, use_decoder: bool = True,
-                    dtype=torch.float32):
+                    dtype=torch.float32, prefill_budget: Optional[int] = None):
         """A long-lived slot engine (``GPT.open_engine``) that synthesises texts submitted from any thread while it
         decodes: ``engine.submit(text, params_infer_code=None, stream=False, skip_refine_text=True, ...) -> Job``,
         ``Job.cancel()`` for one text, ``close(cancel=False)`` or a ``with`` block to drain it (``close(cancel=True)``
@@ -451,11 +457,15 @@ class Chat:
         for ``dtype=torch.float16``); every stage's ``max_new_token`` must be at most ``max_new_cap``, and its prompt
         plus ``max_new_token`` at most ``max_context`` (prompts over 1,024 tokens as in ``infer_continuous``).  See
         ``ChatEngine.submit``.  ``dtype`` as in
-        ``infer_continuous``: every stage of every job runs on that engine."""
+        ``infer_continuous``: every stage of every job runs on that engine.  ``prefill_budget`` (prompt columns per
+        poll, at least 128; default None) bounds the prefill the running jobs wait for at each poll
+        (``infer_continuous``); a job cancelled while its prompt is in progress frees its slot at the next poll."""
         flags = _lib.engine_flags(dtype)
+        check_prefill_budget(prefill_budget)
         assert self.has_loaded(use_decoder=use_decoder)
         return self.gpt._open_slot_engine(ChatEngine, self.gpt.max_batch if slots is None else slots, max_new_cap,
-                                          use_decoder, None, self, use_decoder, flags=flags)
+                                          use_decoder, None, self, use_decoder, flags=flags,
+                                          prefill_budget=prefill_budget)
 
     def interrupt(self):
         self.context.set(True)
@@ -779,11 +789,11 @@ class ChatEngine(OpenEngine):
     streaming job and the whole sequence of every non-streaming job that completed go into one ``decode_rows`` call."""
 
     def __init__(self, make_device, chunk, check, device, on_close, chat: "Chat", use_decoder: bool, context=None,
-                 max_new_cap: Optional[int] = None):
+                 max_new_cap: Optional[int] = None, prefill_budget: Optional[int] = None):
         self.chat, self.use_decoder = chat, use_decoder
         self.model = chat.decoder if use_decoder else chat.dvae
         self._sampler = _SpeakerSampler(chat, self.model, use_decoder)
-        super().__init__(make_device, chunk, check, device, on_close, max_new_cap, context)
+        super().__init__(make_device, chunk, check, device, on_close, max_new_cap, context, prefill_budget)
 
     def submit(self, text: str, params_infer_code=None, stream=False, skip_refine_text=True, params_refine_text=None,
                lang=None, do_text_normalization=True, do_homophone_replacement=True, split_text=False,

@@ -75,6 +75,7 @@ struct ctb_gpt {
   float *gw_hi, *gw_lo;            // tf32 hi / lo copies of the per-layer weight region of the blob
   float *pf_resid, *pf_xn, *pf_qkv, *pf_q, *pf_attn, *pf_gu, *pf_h, *pf_ones, *pf_zeros;
   int *pf_npre, *pf_nvalid;
+  uint8_t* pf_mask;                // [pf_rows] a prompt chunk's column mask (all ones)
   size_t pf_rows;                  // capacity (B * T0) of the pf_* activation buffers
   bool mega_ok;      // one-kernel decode step (mega.cuh), built for B <= 8
   int mega_max_batch; // batches that use it (default 4; CTB_MEGA_MAX_BATCH overrides)
@@ -108,6 +109,9 @@ struct ctb_gpt {
   int eng_text;
   cudaGraphExec_t graph_exec_text;
   uint64_t graph_kernels_text;
+  // per slot: the prompt being prefilled in chunks (ctb_gpt_engine_prefill_chunk) - its width (0: none) and the columns
+  // already in the slot's pages
+  std::vector<int> chunk_T0, chunk_done;
   // ---- half-precision slot engine (ctb_gpt_engine_begin_ex)
   int prec;                   // CTB_ENGINE_FP16_* bits of the current engine (0 for fp32 engines and generate())
   bool tc_base;               // tensor-core activation scratch, head copies and their tensor maps exist (tc_setup_base)
@@ -476,7 +480,7 @@ extern "C" int ctb_gpt_destroy(ctb_gpt* h) {
                   h->pos, h->counter, h->end_idx, h->idx, h->active, h->finish, h->st, h->tc_wqkv, h->tc_wgu,
                   h->tc_heads_code, h->tc_heads_text, h->x_hi, h->x_lo, h->attn_hi, h->attn_lo, h->h_hi, h->h_lo, h->bar, h->trace, h->flow_arena, h->flow_epoch, h->gw_hi, h->gw_lo, h->pf_resid, h->pf_xn, h->pf_qkv, h->pf_q,
                   h->pf_attn, h->pf_gu, h->pf_h, h->pf_ones, h->pf_zeros, h->pf_npre, h->pf_nvalid,
-                  h->rows, h->cfgs, h->eng_noise, h->eng_slot, h->eng_text_logits, h->eng_text_idx};
+                  h->pf_mask, h->rows, h->cfgs, h->eng_noise, h->eng_slot, h->eng_text_logits, h->eng_text_idx};
   delete[] h->m_wqkv; delete[] h->m_wo; delete[] h->m_wgu; delete[] h->m_wd;
   for (void* p : ptrs) if (p) cudaFree(p);
   fp16_free(h);
@@ -994,6 +998,7 @@ static int prefill_reserve(ctb_gpt* h, size_t rows) {
     for (float** b : bufs) if (*b) { cudaFree(*b); *b = nullptr; }
     if (h->pf_npre) { cudaFree(h->pf_npre); h->pf_npre = nullptr; }
     if (h->pf_nvalid) { cudaFree(h->pf_nvalid); h->pf_nvalid = nullptr; }
+    if (h->pf_mask) { cudaFree(h->pf_mask); h->pf_mask = nullptr; }
     if ((rc = dalloc(&h->pf_resid, rows * d))) return rc;
     if ((rc = dalloc(&h->pf_xn, rows * d))) return rc;
     if ((rc = dalloc(&h->pf_qkv, rows * nqkv))) return rc;
@@ -1002,37 +1007,29 @@ static int prefill_reserve(ctb_gpt* h, size_t rows) {
     if ((rc = dalloc(&h->pf_gu, rows * 2 * I))) return rc;
     if ((rc = dalloc(&h->pf_h, rows * I))) return rc;
     if ((rc = dalloc(&h->pf_npre, rows))) return rc;
-    if ((rc = dalloc(&h->pf_nvalid, (size_t)h->cfg.max_batch))) return rc;
+    if ((rc = dalloc(&h->pf_nvalid, (size_t)std::max(h->cfg.max_batch, 2)))) return rc;
+    if ((rc = dalloc(&h->pf_mask, rows))) return rc;
     h->pf_rows = rows;
   }
   return CTB_OK;
 }
 
-// B left-padded prompts [B, T0] -> decode rows slot[b] (slot == nullptr: rows 0..B-1), then the first token of every
-// row in state h->phase (all h->B rows of a static batch; the admitted slots of a slot engine)
-static int prefill_batched(ctb_gpt* h, int B, int T0, const float* emb, const uint8_t* mask, const int* slot,
-                           cudaStream_t s) {
+// The 20 layers over the B x T0 prompt columns in h->pf_resid (positions, mask and slots in pp), the prompt's K / V
+// appended to the rows' pages.  attn(pp) launches the layer's causal attention.
+template <typename Attn>
+static int prefill_layers(ctb_gpt* h, PrefillP& pp, Attn attn, cudaStream_t s) {
   const ctb_gpt_config& c = h->cfg;
   const ctb_gpt_layout& L = h->lay;
-  const int M = B * T0;
+  const int B = pp.B, T0 = pp.T0, M = B * T0;
   const int d = c.hidden_size, I = c.intermediate_size, nqkv = (c.num_heads + 2 * c.num_kv_heads) * c.head_dim;
   int rc;
-  if ((rc = prefill_reserve(h, (size_t)M))) return rc;
-  CTB_CUDA(cudaMemcpyAsync(h->pf_resid, emb, (size_t)M * d * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  k_prefill_positions<<<B, 32, 0, s>>>(mask, h->pf_npre, h->pf_nvalid, T0);
-  CTB_LAUNCH_CHECK();
-  PrefillP pp{};
-  pp.B = B; pp.T0 = T0; pp.Hq = c.num_heads; pp.Hkv = c.num_kv_heads; pp.hd = c.head_dim; pp.d = d; pp.mask = mask; pp.slot = slot;
+  pp.Hq = c.num_heads; pp.Hkv = c.num_kv_heads; pp.hd = c.head_dim; pp.d = d;
   pp.npre = h->pf_npre; pp.nvalid = h->pf_nvalid; pp.qkv = h->pf_qkv; pp.q = h->pf_q; pp.block_table = h->block_table;
   pp.pages_per_row = h->pages_per_row; pp.rope_cos = h->W + L.rope_cos; pp.rope_sin = h->W + L.rope_sin;
   pp.permute_qk = h->use_tc ? 1 : 0; pp.attn = h->pf_attn; pp.scaling = 1.0f / sqrtf((float)c.head_dim);
   const int rms_blocks = (M + 7) / 8;
   // a half-precision engine: the rounded weights (norms folded in before rounding) with W_lo = 0 and unit norms
   const bool w16 = (h->prec & CTB_ENGINE_FP16_WEIGHTS) != 0, kv16 = (h->prec & CTB_ENGINE_FP16_KV) != 0;
-  if (T0 > PF_ATT_MAX_T0 &&
-      (rc = kv16 ? ensure_smem_attr((const void*)k_prefill_attn_tiled<__half>, PftSmem<__half>::BYTES)
-                 : ensure_smem_attr((const void*)k_prefill_attn_tiled<float>, PftSmem<float>::BYTES)))
-    return rc;
   for (int l = 0; l < c.num_layers; ++l) {
     const int64_t lo = (int64_t)l * L.layer_stride;
     const float* Wl = h->W + L.layer0 + lo;
@@ -1046,15 +1043,7 @@ static int prefill_batched(ctb_gpt* h, int B, int T0, const float* emb, const ui
     if (kv16) k_prefill_rope_kv<__half><<<dim3(T0, B), 256, 0, s>>>(pp);
     else k_prefill_rope_kv<float><<<dim3(T0, B), 256, 0, s>>>(pp);
     CTB_LAUNCH_CHECK();
-    if (T0 > PF_ATT_MAX_T0) {
-      const dim3 tgrid((T0 + PFT_TILE - 1) / PFT_TILE, c.num_heads, B);
-      if (kv16) k_prefill_attn_tiled<__half><<<tgrid, PFT_THREADS, PftSmem<__half>::BYTES, s>>>(pp);
-      else k_prefill_attn_tiled<float><<<tgrid, PFT_THREADS, PftSmem<float>::BYTES, s>>>(pp);
-    } else {
-      const dim3 agrid((T0 + PF_ATT_WARPS - 1) / PF_ATT_WARPS, c.num_heads, B);
-      if (kv16) k_prefill_attn<__half><<<agrid, PF_ATT_WARPS * 32, (size_t)PF_ATT_WARPS * T0 * sizeof(float), s>>>(pp);
-      else k_prefill_attn<float><<<agrid, PF_ATT_WARPS * 32, (size_t)PF_ATT_WARPS * T0 * sizeof(float), s>>>(pp);
-    }
+    attn(pp);
     CTB_LAUNCH_CHECK();
     if ((rc = tc_gemm_launch<GE_SCALE_RES>(s, h->pf_attn, d, B, T0, d, d, 1, d, 1, 0, Whi + L.wo, wlo(L.wo), h->pf_zeros,
                                            h->pf_ones, h->pf_resid, d, h->pf_resid, d))) return rc;
@@ -1067,14 +1056,92 @@ static int prefill_batched(ctb_gpt* h, int B, int T0, const float* emb, const ui
     if ((rc = tc_gemm_launch<GE_SCALE_RES>(s, h->pf_h, I, B, T0, d, I, 1, I, 1, 0, Whi + L.wdown, wlo(L.wdown),
                                            h->pf_zeros, h->pf_ones, h->pf_resid, d, h->pf_resid, d))) return rc;
   }
+  return CTB_OK;
+}
+
+// The last column of each of the B prefilled rows (width T0) becomes its decode row's state (seq_len = nvalid[b]), then
+// heads -> sampler -> finalize give the first token of every row in state h->phase (the i == 0 iteration of gpt.py:394)
+static int prefill_first_token(ctb_gpt* h, int B, int T0, const int* nvalid, const int* slot, cudaStream_t s) {
+  int rc;
   k_prefill_finish<<<B, 256, 0, s>>>(h->pf_resid, h->x, h->use_tc ? h->x_hi : nullptr, h->use_tc ? h->x_lo : nullptr,
-                                     h->pf_nvalid, h->seq_len, h->pos, h->active, T0, d, slot);
+                                     nvalid, h->seq_len, h->pos, h->active, T0, h->cfg.hidden_size, slot);
   CTB_LAUNCH_CHECK();
-  // first token: heads -> sampler -> finalize (the i == 0 iteration of gpt.py:394)
   const StepCtx x = make_ctx(h, 0);
   if ((rc = h->use_tc ? launch_heads_tc(h, s) : launch_heads(h, x, s))) return rc;
   if ((rc = launch_sampler(h, x, s))) return rc;
   return launch_finalize(h, s);
+}
+
+// B left-padded prompts [B, T0] -> decode rows slot[b] (slot == nullptr: rows 0..B-1), then the first token of every
+// row in state h->phase (all h->B rows of a static batch; the admitted slots of a slot engine)
+static int prefill_batched(ctb_gpt* h, int B, int T0, const float* emb, const uint8_t* mask, const int* slot,
+                           cudaStream_t s) {
+  const ctb_gpt_config& c = h->cfg;
+  const int M = B * T0;
+  const int d = c.hidden_size;
+  int rc;
+  if ((rc = prefill_reserve(h, (size_t)M))) return rc;
+  CTB_CUDA(cudaMemcpyAsync(h->pf_resid, emb, (size_t)M * d * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  k_prefill_positions<<<B, 32, 0, s>>>(mask, h->pf_npre, h->pf_nvalid, T0);
+  CTB_LAUNCH_CHECK();
+  PrefillP pp{};
+  pp.B = B; pp.T0 = T0; pp.mask = mask; pp.slot = slot;
+  const bool kv16 = (h->prec & CTB_ENGINE_FP16_KV) != 0;
+  if (T0 > PF_ATT_MAX_T0 &&
+      (rc = kv16 ? ensure_smem_attr((const void*)k_prefill_attn_tiled<__half>, PftSmem<__half>::BYTES)
+                 : ensure_smem_attr((const void*)k_prefill_attn_tiled<float>, PftSmem<float>::BYTES)))
+    return rc;
+  auto attn = [&](const PrefillP& p) {
+    if (T0 > PF_ATT_MAX_T0) {
+      const dim3 tgrid((T0 + PFT_TILE - 1) / PFT_TILE, c.num_heads, B);
+      if (kv16) k_prefill_attn_tiled<__half><<<tgrid, PFT_THREADS, PftSmem<__half>::BYTES, s>>>(p);
+      else k_prefill_attn_tiled<float><<<tgrid, PFT_THREADS, PftSmem<float>::BYTES, s>>>(p);
+    } else {
+      const dim3 agrid((T0 + PF_ATT_WARPS - 1) / PF_ATT_WARPS, c.num_heads, B);
+      if (kv16) k_prefill_attn<__half><<<agrid, PF_ATT_WARPS * 32, (size_t)PF_ATT_WARPS * T0 * sizeof(float), s>>>(p);
+      else k_prefill_attn<float><<<agrid, PF_ATT_WARPS * 32, (size_t)PF_ATT_WARPS * T0 * sizeof(float), s>>>(p);
+    }
+  };
+  if ((rc = prefill_layers(h, pp, attn, s))) return rc;
+  return prefill_first_token(h, B, T0, h->pf_nvalid, slot, s);
+}
+
+// Columns [c0, c0 + n) of a prompt of T0 columns -> slot `slot`, whose pages hold columns [0, c0) from the earlier
+// chunks: the chunk's n rows run the layers of a one-call prefill (B = 1, every column valid, positions c0 + j), and
+// each query attends to keys 0 .. its position read from the pages, with the attention kernel a one-call prefill of T0
+// columns runs (k_prefill_attn up to PF_ATT_MAX_T0, else the tiled one).  The final chunk (c0 + n == T0) then hands
+// its last column to the slot and samples its first token (the slot is RS_PENDING, h->phase too); earlier chunks touch
+// nothing but the pf_* scratch and the slot's pages.
+static int prefill_chunk(ctb_gpt* h, int slot, int T0, int c0, int n, const float* emb, cudaStream_t s) {
+  const ctb_gpt_config& c = h->cfg;
+  int rc;
+  if ((rc = prefill_reserve(h, (size_t)n))) return rc;
+  CTB_CUDA(cudaMemcpyAsync(h->pf_resid, emb, (size_t)n * c.hidden_size * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  k_prefill_chunk_positions<<<(n + 255) / 256, 256, 0, s>>>(h->pf_mask, h->pf_npre, h->pf_nvalid, h->eng_slot, slot,
+                                                            c0, n);
+  CTB_LAUNCH_CHECK();
+  PrefillP pp{};
+  pp.B = 1; pp.T0 = n; pp.mask = h->pf_mask; pp.slot = h->eng_slot;
+  const bool kv16 = (h->prec & CTB_ENGINE_FP16_KV) != 0, tiled = T0 > PF_ATT_MAX_T0;
+  if (tiled &&
+      (rc = kv16 ? ensure_smem_attr((const void*)k_prefill_attn_tiled_chunk<__half>, PftSmem<__half>::BYTES)
+                 : ensure_smem_attr((const void*)k_prefill_attn_tiled_chunk<float>, PftSmem<float>::BYTES)))
+    return rc;
+  auto attn = [&](const PrefillP& p) {
+    if (tiled) {
+      const dim3 tgrid((n + PFT_TILE - 1) / PFT_TILE, c.num_heads, 1);
+      if (kv16) k_prefill_attn_tiled_chunk<__half><<<tgrid, PFT_THREADS, PftSmem<__half>::BYTES, s>>>(p, c0);
+      else k_prefill_attn_tiled_chunk<float><<<tgrid, PFT_THREADS, PftSmem<float>::BYTES, s>>>(p, c0);
+    } else {
+      const dim3 agrid((n + PF_ATT_WARPS - 1) / PF_ATT_WARPS, c.num_heads, 1);
+      const size_t smem = (size_t)PF_ATT_WARPS * (c0 + n) * sizeof(float);
+      if (kv16) k_prefill_attn_chunk<__half><<<agrid, PF_ATT_WARPS * 32, smem, s>>>(p, c0);
+      else k_prefill_attn_chunk<float><<<agrid, PF_ATT_WARPS * 32, smem, s>>>(p, c0);
+    }
+  };
+  if ((rc = prefill_layers(h, pp, attn, s))) return rc;
+  if (c0 + n < T0) return CTB_OK;
+  return prefill_first_token(h, 1, n, h->pf_nvalid + 1, h->eng_slot, s);
 }
 
 // Pages for B rows of up to `tokens` tokens each: grow the pool if needed (page = 16 tokens x K|V x heads x 64 values per
@@ -1279,6 +1346,8 @@ extern "C" int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_ca
     CTB_CUDA(cudaMemsetAsync(h->h_lo, 0, h->tc_rows * I * sizeof(float), s));
   }
   CTB_CUDA(cudaStreamSynchronize(s));  // idle_state is read by the copy engine
+  h->chunk_T0.assign((size_t)S, 0);     // no prompt in progress
+  h->chunk_done.assign((size_t)S, 0);
   h->started = 1;
   h->steps_enqueued = 0;
   return CTB_OK;
@@ -1316,6 +1385,7 @@ static int engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0,
     r.n_gen = 0; r.step = 0; r.state = RS_PENDING; r.max_new = max_new[i]; r.has_noise = q_noise_dev != nullptr;
     r.eos = sc.eos_token; r.text = text;
   }
+  for (int i = 0; i < n; ++i) h->chunk_T0[slots[i]] = 0;  // the slot's prompt in progress, if any, is dropped
   // host arrays are copied before this call returns (synchronised below), so the caller may free them at once
   CTB_CUDA(cudaMemcpyAsync(h->rows, rows.data(), sizeof(RowState) * rows.size(), cudaMemcpyHostToDevice, s));
   CTB_CUDA(cudaMemcpyAsync(h->eng_slot, slots, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
@@ -1348,6 +1418,67 @@ extern "C" int ctb_gpt_engine_admit_text(ctb_gpt* h, int32_t n, const int32_t* s
                                          const uint8_t* mask_dev, const ctb_sampler_config* samplers,
                                          const float* q_noise_dev, const int32_t* max_new, void* stream) {
   return engine_admit(h, n, slots, T0, emb_dev, mask_dev, samplers, q_noise_dev, max_new, 1, stream);
+}
+
+extern "C" int ctb_gpt_engine_prefill_chunk(ctb_gpt* h, int32_t slot, int32_t T0, int32_t c0, int32_t n,
+                                            const float* emb_dev, int32_t text, const ctb_sampler_config* sampler,
+                                            const float* q_noise_dev, int32_t max_new, void* stream) {
+  if (!h || !emb_dev) return set_err(CTB_ERR_ARG, "null argument");
+  if (!h->engine) return set_err(CTB_ERR_STATE, "ctb_gpt_engine_begin has not been called");
+  const ctb_gpt_config& c = h->cfg;
+  const int S = h->B;
+  if (slot < 0 || slot >= S) return set_err(CTB_ERR_ARG, "slot %d outside [0,%d)", slot, S);
+  if (T0 < 8 || T0 > c.max_context - 1)
+    return set_err(CTB_ERR_ARG, "T0=%d outside [8,%d]", T0, c.max_context - 1);
+  if (c0 < 0 || n < 1 || c0 + n > T0) return set_err(CTB_ERR_ARG, "chunk [%d,%d) outside the prompt [0,%d)", c0, c0 + n, T0);
+  const bool final = c0 + n == T0;
+  if (c0 % CTB_PREFILL_CHUNK_ALIGN || (!final && n % CTB_PREFILL_CHUNK_ALIGN))
+    return set_err(CTB_ERR_ARG, "chunk [%d,%d): c0 and a non-final chunk's n must be multiples of %d", c0, c0 + n,
+                   CTB_PREFILL_CHUNK_ALIGN);
+  if (max_new < 1 || max_new > h->max_new || T0 + max_new > c.max_context)
+    return set_err(CTB_ERR_ARG, "max_new=%d (capacity %d) with T0=%d exceeds max_context=%d", max_new, h->max_new, T0,
+                   c.max_context);
+  if (final) {
+    if (!sampler) return set_err(CTB_ERR_ARG, "null sampler on the final chunk");
+    if (sampler->past_window > 31 || sampler->past_window < 0) return set_err(CTB_ERR_ARG, "past_window out of range");
+    if (sampler->min_tokens_to_keep < 1) return set_err(CTB_ERR_ARG, "min_tokens_to_keep must be >= 1");
+  }
+  const int pT0 = h->chunk_T0[slot], pdone = h->chunk_done[slot];
+  if (pT0 == 0 && c0 != 0)
+    return set_err(CTB_ERR_STATE, "slot %d: chunk [%d,%d) but no prompt in progress (a first chunk starts at 0)", slot,
+                   c0, c0 + n);
+  if (pT0 != 0 && (T0 != pT0 || c0 != pdone))
+    return set_err(CTB_ERR_STATE, "slot %d: chunk [%d,%d) of T0=%d does not continue the prompt in progress ([0,%d) of "
+                   "T0=%d done)", slot, c0, c0 + n, T0, pdone, pT0);
+  cudaStream_t s = (cudaStream_t)stream;
+  RowState r;
+  CTB_CUDA(cudaMemcpyAsync(&r, h->rows + slot, sizeof(RowState), cudaMemcpyDeviceToHost, s));
+  CTB_CUDA(cudaStreamSynchronize(s));
+  if (r.state == RS_RUNNING || r.state == RS_PENDING) return set_err(CTB_ERR_STATE, "slot %d is still generating", slot);
+  if (!final) {
+    const int rc = prefill_chunk(h, slot, T0, c0, n, emb_dev, s);
+    if (rc) { h->chunk_T0[slot] = 0; return rc; }
+    h->chunk_T0[slot] = T0; h->chunk_done[slot] = c0 + n;
+    return CTB_OK;
+  }
+  // the final chunk admits the request as ctb_gpt_engine_admit / _admit_text do for one slot
+  r.n_gen = 0; r.step = 0; r.state = RS_PENDING; r.max_new = max_new; r.has_noise = q_noise_dev != nullptr;
+  r.eos = sampler->eos_token; r.text = text ? 1 : 0;
+  CTB_CUDA(cudaMemcpyAsync(h->rows + slot, &r, sizeof(RowState), cudaMemcpyHostToDevice, s));
+  CTB_CUDA(cudaMemcpyAsync(h->cfgs + slot, sampler, sizeof(ctb_sampler_config), cudaMemcpyHostToDevice, s));
+  const size_t nrow = text ? (size_t)c.num_text_tokens : (size_t)c.num_vq * c.num_audio_tokens;
+  if (q_noise_dev)
+    CTB_CUDA(cudaMemcpyAsync(h->eng_noise + slot * noise_stride(h), q_noise_dev, nrow * sizeof(float),
+                             cudaMemcpyDeviceToDevice, s));
+  CTB_CUDA(cudaMemsetAsync(h->finish + slot, 0, 1, s));
+  CTB_CUDA(cudaMemsetAsync(h->end_idx + slot, 0, sizeof(int), s));
+  CTB_CUDA(cudaStreamSynchronize(s));  // r and *sampler are read by the copy engine
+  h->chunk_T0[slot] = 0;
+  if (text) h->eng_text = 1;
+  h->phase = RS_PENDING;
+  const int rc = prefill_chunk(h, slot, T0, c0, n, emb_dev, s);
+  h->phase = RS_RUNNING;
+  return rc;
 }
 
 extern "C" int ctb_gpt_engine_status(ctb_gpt* h, ctb_gpt_status* out, int32_t* state_host, int32_t* end_idx_host,
@@ -1383,6 +1514,7 @@ extern "C" int ctb_gpt_engine_cancel(ctb_gpt* h, int32_t n, const int32_t* slots
       return set_err(CTB_ERR_ARG, "slot %d out of range or repeated", b);
     p.mask[b >> 5] |= 1u << (b & 31);
   }
+  for (int i = 0; i < n; ++i) h->chunk_T0[slots[i]] = 0;  // a prompt in progress there is dropped
   // h->eng_text stays as it is: the next ctb_gpt_engine_status recomputes it from the rows
   k_cancel_rows<<<1, 256, 0, (cudaStream_t)stream>>>(p);
   CTB_LAUNCH_CHECK();

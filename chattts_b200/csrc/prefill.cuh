@@ -9,6 +9,9 @@
 //               -> k_rms_rows -> GEMM([Wgate;Wup]) -> k_silu_mul -> GEMM(Wdown)+residual
 //   then k_prefill_finish hands the last column's residual to the decode-loop state (x, seq_len) and the
 //   regular heads -> sampler -> finalize kernels produce the first token.
+// A slot-engine prompt may also be prefilled in 128-aligned chunks (ctb_gpt_engine_prefill_chunk): the same layers over
+// the chunk's rows (k_prefill_chunk_positions), and the attention of the whole prompt's width with a query offset
+// (k_prefill_attn_chunk, k_prefill_attn_tiled_chunk) reading the earlier chunks' keys from the pages.
 #pragma once
 #include <type_traits>
 
@@ -100,20 +103,25 @@ __global__ void k_prefill_rope_kv(const PrefillP p) {
 // (Round 1 walked the queries of a (row, head) serially in one 128-thread CTA: 12 CTAs on 132 SMs and O(T^2) per CTA -
 // fine for 16-token prompts, hopeless for speaker-prompt prefixes of hundreds of tokens.)
 // KVT: the cache's element type, widened to fp32 as it is read.
+//
+// q0: position of the call's first query (k_prefill_attn_chunk: a chunk of a longer prompt whose columns 0 .. q0 - 1 are
+// already in the row's pages; 0 for a whole prompt).  Query j of the call is prompt position q0 + j and attends to keys
+// 0 .. q0 + j, each with the arithmetic a one-call prefill gives that position.
 constexpr int PF_ATT_WARPS = 8;
 template <typename KVT>
-__global__ void __launch_bounds__(PF_ATT_WARPS * 32) k_prefill_attn(const PrefillP p) {
+__device__ __forceinline__ void prefill_attn_warp(const PrefillP& p, const int q0) {
   constexpr int HD = 64;
   const int h = blockIdx.y, b = blockIdx.z, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = p.nvalid[b];
-  const int t = blockIdx.x * PF_ATT_WARPS + warp;  // query position among the row's valid tokens
-  if (t >= n) return;                              // warp-uniform; the kernel has no block-wide barrier
+  const int j = blockIdx.x * PF_ATT_WARPS + warp;  // query among the call's valid tokens
+  if (j >= n) return;                              // warp-uniform; the kernel has no block-wide barrier
+  const int t = q0 + j;                            // its position in the prompt
   extern __shared__ float pa_smem[];
-  float* s_p = pa_smem + (size_t)warp * p.T0;      // [T0] scores / probabilities of this warp's query
+  float* s_p = pa_smem + (size_t)warp * (q0 + p.T0);  // [q0 + T0] scores / probabilities of this warp's query
   const int hk = h / (p.Hq / p.Hkv);
   const int* bt = p.block_table + (p.slot ? p.slot[b] : b) * p.pages_per_row;
   const int c0 = p.T0 - n;                        // first valid column (left padding)
-  const size_t qrow = ((size_t)b * p.T0 + c0 + t) * p.Hq * HD + h * HD;
+  const size_t qrow = ((size_t)b * p.T0 + c0 + j) * p.Hq * HD + h * HD;
   float4 q[HD / 4];
 #pragma unroll
   for (int i = 0; i < HD / 4; ++i) q[i] = __ldg(reinterpret_cast<const float4*>(p.q + qrow) + i);
@@ -163,6 +171,16 @@ __global__ void __launch_bounds__(PF_ATT_WARPS * 32) k_prefill_attn(const Prefil
     o0 = fmaf(pk, v.x, o0); o1 = fmaf(pk, v.y, o1);
   }
   *reinterpret_cast<float2*>(p.attn + qrow + 2 * lane) = make_float2(o0 / l, o1 / l);  // V (and the output) is never permuted
+}
+
+template <typename KVT>
+__global__ void __launch_bounds__(PF_ATT_WARPS * 32) k_prefill_attn(const PrefillP p) { prefill_attn_warp<KVT>(p, 0); }
+
+// One chunk (B = 1, T0 = the chunk's columns, all valid) of a prompt of at most PF_ATT_MAX_T0 columns whose first q0
+// columns are in the row's pages: shared memory 8 x (q0 + T0) floats
+template <typename KVT>
+__global__ void __launch_bounds__(PF_ATT_WARPS * 32) k_prefill_attn_chunk(const PrefillP p, int q0) {
+  prefill_attn_warp<KVT>(p, q0);
 }
 
 // k_prefill_attn keeps a query's whole score row in shared memory (8 x T0 floats per CTA): prompts wider than this
@@ -218,14 +236,20 @@ __device__ __forceinline__ float4 pft_ld4(const __half* p) {
   return make_float4(f0.x, f0.y, f1.x, f1.y);
 }
 
+//
+// q0 (a multiple of 64) as in prefill_attn_warp: the call's query tile qj is the prompt's tile q0 / 64 + qj, the same 64
+// queries a one-call prefill gives one CTA, and keys past q0 + n - 1 are zero-filled as keys past a whole prompt's last
+// are (the pages there hold an earlier request's values).
 template <typename KVT>
-__global__ void __launch_bounds__(PFT_THREADS) k_prefill_attn_tiled(const PrefillP p) {
+__device__ __forceinline__ void prefill_attn_tiled_cta(const PrefillP& p, const int q0) {
   using SM = PftSmem<KVT>;
   constexpr int HD = 64, T = PFT_TILE;
   const int h = blockIdx.y, b = blockIdx.z, tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-  const int n = p.nvalid[b];
-  const int qt = gridDim.x - 1 - blockIdx.x;  // the longest walks start first
-  if (qt * T >= n) return;                     // CTA-uniform, before any barrier
+  const int n = p.nvalid[b];                   // queries of the call
+  const int kn = q0 + n;                       // keys: positions 0 .. kn - 1
+  const int qj = gridDim.x - 1 - blockIdx.x;  // the longest walks start first
+  if (qj * T >= n) return;                     // CTA-uniform, before any barrier
+  const int qt = q0 / T + qj;                  // query tile of the prompt
   extern __shared__ __align__(16) unsigned char pft_smem[];
   float* sQ = reinterpret_cast<float*>(pft_smem);
   float* sP = sQ + SM::Q_FLOATS;
@@ -238,7 +262,7 @@ __global__ void __launch_bounds__(PFT_THREADS) k_prefill_attn_tiled(const Prefil
 
   // queries qt*64 .. qt*64+63 (zeros past the row's last)
   for (int i = tid; i < T * 16; i += PFT_THREADS) {
-    const int r = i >> 4, c = i & 15, t = qt * T + r;
+    const int r = i >> 4, c = i & 15, t = qj * T + r;
     const float* src = t < n ? p.q + ((row0 + t) * p.Hq + h) * HD + c * 4 : p.q;
     pft_cp16(sQ + r * SM::QS + c * 4, src, t < n);
   }
@@ -248,8 +272,8 @@ __global__ void __launch_bounds__(PFT_THREADS) k_prefill_attn_tiled(const Prefil
     for (int i = tid; i < 2 * T * SM::CH; i += PFT_THREADS) {
       const int which = i / (T * SM::CH), r = (i / SM::CH) % T, c = i % SM::CH, k = kt * T + r;
       constexpr int E = 16 / (int)sizeof(KVT);
-      const KVT* src = k < n ? kv + kv_off(bt[k / kPageTokens], which, hk, k % kPageTokens, p.Hkv, HD) + c * E : kv;
-      pft_cp16(dst + which * SM::KV_ELEMS + r * SM::KS + c * E, src, k < n);
+      const KVT* src = k < kn ? kv + kv_off(bt[k / kPageTokens], which, hk, k % kPageTokens, p.Hkv, HD) + c * E : kv;
+      pft_cp16(dst + which * SM::KV_ELEMS + r * SM::KS + c * E, src, k < kn);
     }
   };
   load_kv(0, 0);
@@ -299,7 +323,7 @@ __global__ void __launch_bounds__(PFT_THREADS) k_prefill_attn_tiled(const Prefil
     // causal mask, online softmax (a query's 64 scores are spread over the 16 lanes tx of its half-warp)
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const int t = min(qt * T + ty * 4 + i, n - 1);  // queries past the row's last see its keys, and are not written
+      const int t = min(q0 + qj * T + ty * 4 + i, kn - 1);  // queries past the row's last see its keys, and are not written
       float mx = -INFINITY;
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
@@ -347,11 +371,21 @@ __global__ void __launch_bounds__(PFT_THREADS) k_prefill_attn_tiled(const Prefil
   }
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    const int t = qt * T + ty * 4 + i;
+    const int t = qj * T + ty * 4 + i;
     if (t < n)  // V (and the output) is never permuted
       *reinterpret_cast<float4*>(p.attn + ((row0 + t) * p.Hq + h) * HD + tx * 4) =
           make_float4(o[i][0] / l[i], o[i][1] / l[i], o[i][2] / l[i], o[i][3] / l[i]);
   }
+}
+
+template <typename KVT>
+__global__ void __launch_bounds__(PFT_THREADS) k_prefill_attn_tiled(const PrefillP p) { prefill_attn_tiled_cta<KVT>(p, 0); }
+
+// One chunk (B = 1, T0 = the chunk's columns, all valid) of a prompt of more than PF_ATT_MAX_T0 columns whose first q0
+// columns (a multiple of PFT_TILE) are in the row's pages
+template <typename KVT>
+__global__ void __launch_bounds__(PFT_THREADS) k_prefill_attn_tiled_chunk(const PrefillP p, int q0) {
+  prefill_attn_tiled_cta<KVT>(p, q0);
 }
 
 // h = silu(gate) * up over [M, 2I] -> [M, I]
@@ -371,6 +405,15 @@ __global__ void k_prefill_positions(const uint8_t* __restrict__ mask, int* __res
     for (int c = 0; c < T0; ++c) { npre[(size_t)b * T0 + c] = n; n += mask[(size_t)b * T0 + c] != 0; }
     nvalid[b] = n;
   }
+}
+
+// a chunk of n columns of one prompt, at positions q0 .. q0 + n - 1, into decode row `slot`: every column valid
+// (k_prefill_rope_kv's mask and positions), nvalid[0] = n (the chunk's queries), nvalid[1] = q0 + n (the row's tokens
+// after it: k_prefill_finish's seq_len on the final chunk), slot_dev[0] = slot
+__global__ void k_prefill_chunk_positions(uint8_t* __restrict__ mask, int* __restrict__ npre, int* __restrict__ nvalid,
+                                          int* __restrict__ slot_dev, int slot, int q0, int n) {
+  for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < n; c += gridDim.x * blockDim.x) { mask[c] = 1; npre[c] = q0 + c; }
+  if (blockIdx.x == 0 && threadIdx.x == 0) { nvalid[0] = n; nvalid[1] = q0 + n; slot_dev[0] = slot; }
 }
 
 // hand the last prompt column's residual to the decode-loop state of decode row slot[b] (slot == nullptr: row b)

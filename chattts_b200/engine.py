@@ -10,6 +10,10 @@ every waiting request when it ends: text refinement followed by the speech codes
 The scheduling policy (``schedule``) is plain Python over a small device interface, so it can be driven by a stub.
 ``stream_schedule`` runs the same policy and reconstructs, per request, the cumulative yields of
 ``GPT.generate(stream=True)`` from the slots' token counts at each poll.
+
+An opt-in prefill budget (``prefill_budget``, prompt columns per poll) bounds the prefill work the running slots wait
+for at each poll: a prompt that does not fit is prefilled in chunks over several polls (``ctb_gpt_engine_prefill_chunk``),
+with the same bits as one admission of it.
 """
 from __future__ import annotations
 
@@ -36,6 +40,9 @@ LONG_PROMPT_COLS = 1024
 #: kept by the handle (3.8 GB for 64 prompts of 1,024 tokens); larger admissions run as consecutive prefills of up to
 #: this many rows, so an engine of 64 slots needs no more of it (1.9 GB) than one of 32 did.
 ADMIT_MAX_ROWS = 32 * 1024
+#: a prompt prefilled in chunks: every chunk starts at a multiple of this many columns, and every chunk but its last
+#: is a multiple of it (``ctb_gpt_engine_prefill_chunk``)
+PREFILL_CHUNK_ALIGN = _lib.PREFILL_CHUNK_ALIGN
 
 
 def admission_chunks(group: list, T0: int) -> List[list]:
@@ -43,6 +50,36 @@ def admission_chunks(group: list, T0: int) -> List[list]:
     ``ADMIT_MAX_ROWS // T0`` prompts."""
     n = max(1, ADMIT_MAX_ROWS // T0)
     return [group[i: i + n] for i in range(0, len(group), n)]
+
+
+def admission_prefills(batch: list, requests: Sequence["Request"], max_context: int) -> List[Tuple[list, int, bool, bool]]:
+    """The prefill calls ``EngineDevice.admit(batch)`` makes, in order: ``[(pairs, T0, seeded, text)]``.  Seeded
+    requests bring their Exp(1) rows, unseeded ones sample with device Philox, and code and text requests are
+    admitted by separate calls; each kind is split by ``admission_groups`` and ``admission_chunks``."""
+    out = []
+    for seeded, text in ((True, False), (True, True), (False, False), (False, True)):
+        group = [(s, i) for s, i in batch if (requests[i].manual_seed is not None) == seeded
+                 and bool(requests[i].infer_text) == text]
+        if not group:
+            continue
+        for part, T0 in admission_groups(group, requests, max_context):
+            for chunk in admission_chunks(part, T0):  # each prompt's results do not depend on its batch
+                out.append((chunk, T0, seeded, text))
+    return out
+
+
+def admission_cols(batch: list, requests: Sequence["Request"], max_context: int) -> int:
+    """Padded prompt columns ``EngineDevice.admit(batch)`` prefills: prompts x ``T0`` of each of its calls."""
+    return sum(len(pairs) * T0 for pairs, T0, _, _ in admission_prefills(batch, requests, max_context))
+
+
+def check_prefill_budget(budget: Optional[int]) -> Optional[int]:
+    """``budget`` as an int of at least ``PREFILL_CHUNK_ALIGN`` (128) prompt columns, or None; ValueError otherwise."""
+    if budget is None:
+        return None
+    if int(budget) != budget or int(budget) < PREFILL_CHUNK_ALIGN:
+        raise ValueError(f"prefill_budget={budget!r}: an int of at least {PREFILL_CHUNK_ALIGN} prompt columns, or None")
+    return int(budget)
 
 
 def admission_groups(group: list, requests: Sequence["Request"], max_context: int) -> List[Tuple[list, int]]:
@@ -184,6 +221,10 @@ class ScheduleStats:
     children: Dict[int, int] = field(default_factory=dict)  # request index -> index of the follow-up it returned
     fanout: Dict[int, List[int]] = field(default_factory=dict)  # request index -> indices of the list ``then`` returned
     cancelled: Set[int] = field(default_factory=set)  # request indices stopped by an ``Arrivals.cancel``
+    # with a prefill budget: the prompt columns prefilled in each poll (the admissions and chunks between two decode
+    # chunks), and the number of prompt chunks issued
+    prefill_cols: List[int] = field(default_factory=list)
+    chunks: int = 0
     keys: Dict[int, object] = field(default_factory=dict)  # open source: index of a submitted request -> its key
     failed: Dict[int, BaseException] = field(default_factory=dict)  # open source: request index -> its follow-up's error
 
@@ -288,8 +329,8 @@ def _follow_up(requests: List[Request], i: int, slot: Optional[int], n: int, dev
 
 
 def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: Optional[ScheduleStats] = None,
-                 check: Optional[Callable[[Request], None]] = None, source: Optional[Arrivals] = None
-                 ) -> Iterator[Tuple[SlotStatus, List[Optional[int]], list]]:
+                 check: Optional[Callable[[Request], None]] = None, source: Optional[Arrivals] = None,
+                 prefill_budget: Optional[int] = None) -> Iterator[Tuple[SlotStatus, List[Optional[int]], list]]:
     """The scheduling policy of ``schedule``: yields once per poll ``(status, owner, ended)`` - the slots' status, the
     request each slot held when it was read, and the requests that ended at this poll as ``(request_index, slot or
     None, n_tokens, eos)``.  The slots of the ended requests are refilled only after the generator is resumed.
@@ -305,8 +346,44 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
     finished is finished); neither calls its ``then``, and cancelling a request whose follow-up was already made
     cancels the follow-up.  A submission's live stages are all cancelled together (a fan-out runs several).  Cancelled
     requests are listed in ``stats.cancelled``.  With nothing running and nothing
-    waiting the loop blocks in ``source.take`` instead of decoding, and it ends once the source is closed and drained."""
+    waiting the loop blocks in ``source.take`` instead of decoding, and it ends once the source is closed and drained.
+
+    ``prefill_budget`` (prompt columns, at least 128; None: no bound) bounds the prefill of each poll - the admissions
+    and chunks between two decode chunks - with ``dev.prefill_chunk(slot, index, c0, n)`` and ``dev.max_context``:
+
+    1. A prompt in progress (at most one) first advances by ``min(remaining, budget left rounded down to 128)``
+       columns; its final chunk admits the request.
+    2. With no prompt in progress, waiting requests then enter free slots in order, lowest slot first, while the
+       padded columns of the poll's admission (``admission_cols``) stay within the budget left.
+    3. The first request that does not fit takes a free slot and becomes the prompt in progress, starting with the
+       budget left over (rounded down to 128) if that is at least 128 columns, else at the next poll; the requests
+       behind it wait.
+    4. Its slot is reserved: not refilled, and its status is not read for it until its final chunk.  A cancel frees
+       the slot at the next poll (``dev.cancel`` drops the prompt in progress; the request ends empty, without a
+       follow-up); an interrupt drops it as it drops the waiting requests.
+
+    ``stats.prefill_cols`` records each poll's prefilled columns, ``stats.chunks`` the chunks."""
     stats = stats if stats is not None else ScheduleStats()
+    budget = prefill_budget
+    prog: Optional[List[int]] = None  # the prompt in progress: [slot, request index, columns done]
+    left = budget  # prompt columns this poll may still prefill
+
+    def advance() -> None:  # the prompt in progress by one chunk of the budget left
+        nonlocal prog, left
+        s, i, c0 = prog
+        T = int(requests[i].emb.shape[0])
+        n = min(T - c0, left // PREFILL_CHUNK_ALIGN * PREFILL_CHUNK_ALIGN)
+        if n <= 0:
+            return
+        dev.prefill_chunk(s, i, c0, n)
+        stats.chunks += 1
+        left -= max(MIN_PROMPT_COLS, n) if c0 == 0 and n == T else n  # a whole prompt is padded as an admission
+        if c0 + n == T:
+            prog = None
+            stats.admitted += 1
+        else:
+            prog[2] = c0 + n
+
     waiting = deque(range(len(requests)))
     owner: List[Optional[int]] = [None] * dev.slots
     live: Dict[object, Set[int]] = {}  # open source: submission key -> indices of its live stages
@@ -341,23 +418,48 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
                         retire(i)
                         stats.cancelled.add(i)
                         taken.append((i, None, 0, False))
+                    elif prog is not None and prog[1] == i:  # mid-prefill: no final chunk, the slot is free again
+                        dev.cancel([prog[0]])
+                        owner[prog[0]] = None
+                        prog = None
+                        retire(i)
+                        stats.cancelled.add(i)
+                        taken.append((i, None, 0, False))
                     else:
                         doomed.add(i)
             if idle and closed and not new and not taken:
                 return
         free = [s for s in range(dev.slots) if owner[s] is None]
         batch = []
-        while free and waiting:
-            s, i = free.pop(0), waiting.popleft()
-            owner[s] = i
-            batch.append((s, i))
+        created = False
+        if budget is None:
+            while free and waiting:
+                s, i = free.pop(0), waiting.popleft()
+                owner[s] = i
+                batch.append((s, i))
+        else:
+            if prog is not None:
+                advance()
+            room = left
+            while free and waiting and prog is None:  # the requests behind a prompt in progress wait for it
+                s, i = free.pop(0), waiting.popleft()
+                owner[s] = i
+                if admission_cols(batch + [(s, i)], requests, dev.max_context) > room:
+                    prog, created = [s, i, 0], True  # the first request that does not fit
+                    break
+                batch.append((s, i))
+            left = room - admission_cols(batch, requests, dev.max_context)
         if batch:
             dev.admit(batch)
             stats.admissions += 1
             stats.admitted += len(batch)
+        if created:  # its first chunk, from the budget left over
+            advance()
         st = dev.status()
         stats.decode_steps = st.steps_done
         polled = list(owner)
+        if prog is not None:  # reserved: the slot's status is not its request's yet
+            polled[prog[0]] = None
         ended = taken
         follow: List[int] = []
         done = []  # (index, slot, n_tokens, cancelled at this read) of the requests that may have a follow-up
@@ -366,7 +468,7 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
         if stop:
             dev.cancel(stop)
         for s in range(dev.slots):
-            i = owner[s]
+            i = polled[s]
             if i is None or (st.state[s] != _lib.SLOT_FINISHED and s not in stop):
                 continue
             owner[s] = None
@@ -410,22 +512,26 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
         if freed and waiting:
             yield st, polled, ended
             continue  # refill the freed slots before the next chunk
-        running = [s for s in range(dev.slots) if owner[s] is not None]
-        interrupted = bool(running) and context is not None and context.get()
+        running = [s for s in range(dev.slots) if owner[s] is not None and (prog is None or s != prog[0])]
+        interrupted = (bool(running) or prog is not None) and context is not None and context.get()
         if interrupted:
             stats.interrupted = True
             for s in running:
                 stats.tokens += st.end_idx[s]
                 ended.append((owner[s], s, st.end_idx[s], False))
         yield st, polled, ended
-        if interrupted or (not running and source is None):
+        if budget is not None:  # the poll ends here: the next one has the whole budget
+            stats.prefill_cols.append(budget - left)
+            left = budget
+        if interrupted or (not running and source is None and prog is None):
             return
         if running:
             dev.decode(chunk)
 
 
 def schedule(requests: List[Request], dev, chunk: int, context=None, stats: Optional[ScheduleStats] = None,
-             check: Optional[Callable[[Request], None]] = None) -> Iterator[Tuple[int, Optional[int], int]]:
+             check: Optional[Callable[[Request], None]] = None, prefill_budget: Optional[int] = None
+             ) -> Iterator[Tuple[int, Optional[int], int]]:
     """Drive ``dev`` (``slots``, ``admit([(slot, request_index)])``, ``decode(n)``, ``status() -> SlotStatus``) until
     every request has finished; yields ``(request_index, slot, n_tokens)`` as each one completes - the caller harvests
     the slot's first ``n_tokens`` outputs before resuming the generator - or ``(request_index, None, 0)`` for a seeded
@@ -434,16 +540,17 @@ def schedule(requests: List[Request], dev, chunk: int, context=None, stats: Opti
 
     Waiting requests enter free slots in order, lowest slot first, at every poll (every ``chunk`` decode steps).  On a
     ``context`` interrupt the running requests are yielded with what they have so far and the waiting ones are dropped.
-    Follow-ups (``Request.then``) need ``dev.harvest(slot, n)`` and ``dev.empty(request_index)``; see ``_poll_cycles``.
+    Follow-ups (``Request.then``) need ``dev.harvest(slot, n)`` and ``dev.empty(request_index)``; see ``_poll_cycles``,
+    which also describes the policy of a ``prefill_budget`` (``dev.prefill_chunk``, ``dev.max_context``).
     """
-    for _, _, ended in _poll_cycles(requests, dev, chunk, context, stats, check):
+    for _, _, ended in _poll_cycles(requests, dev, chunk, context, stats, check, None, prefill_budget):
         for i, s, n, _ in ended:
             yield i, s, n
 
 
 def stream_schedule(requests: List[Request], dev, chunk: int, context=None, stats: Optional[ScheduleStats] = None,
-                    check: Optional[Callable[[Request], None]] = None, source: Optional[Arrivals] = None
-                    ) -> Iterator[List[Tuple[int, Optional[int], int, bool]]]:
+                    check: Optional[Callable[[Request], None]] = None, source: Optional[Arrivals] = None,
+                    prefill_budget: Optional[int] = None) -> Iterator[List[Tuple[int, Optional[int], int, bool]]]:
     """``schedule``'s policy, yielding once per poll the list of ``(request_index, slot, n_tokens, last)``: for each
     request, the yields ``GPT.generate(stream=True, stream_batch=r.stream_batch)`` makes for it alone, in its order,
     as cumulative token counts (the slot's first ``n_tokens`` outputs; slot None: a seeded request that ended empty).
@@ -455,9 +562,10 @@ def stream_schedule(requests: List[Request], dev, chunk: int, context=None, stat
     the yields do not depend on ``chunk``.  The slots' outputs stay in place until the generator is resumed.
 
     With an open ``source`` (see ``_poll_cycles``) a cancelled request gets a final yield of what it has, and
-    ``stats.cancelled`` tells it apart."""
+    ``stats.cancelled`` tells it apart.  A request yields nothing before its first token, so a ``prefill_budget``
+    leaves every request's yields as they are."""
     sent: Dict[int, int] = {}  # last boundary yielded per request
-    for st, owner, ended in _poll_cycles(requests, dev, chunk, context, stats, check, source):
+    for st, owner, ended in _poll_cycles(requests, dev, chunk, context, stats, check, source, prefill_budget):
         out = []
         for s, i in enumerate(owner):
             if i is None:
@@ -486,6 +594,7 @@ class EngineDevice:
     def __init__(self, gpt, requests: Sequence[Request], slots: int, max_new_cap: int, return_hidden: bool = True,
                  flags: int = 0):
         self.gpt, self.requests, self.slots = gpt, requests, slots
+        self.max_context = gpt.max_context
         self.lib = _lib.load()
         dev = gpt.device_gpt
         self.dev = dev
@@ -502,17 +611,41 @@ class EngineDevice:
         self._text = [False] * slots  # mode of the request each slot was last given
 
     def admit(self, batch: List[Tuple[int, int]]) -> None:
-        # one prefill per kind: seeded requests bring their Exp(1) rows, unseeded ones sample with device Philox; code
-        # and text requests are admitted by separate calls
         noise: Dict[tuple, torch.Tensor] = {}  # one static batch's noise per (B, rows, cols, seed) in this admission
-        for seeded, text in ((True, False), (True, True), (False, False), (False, True)):
-            group = [(s, i) for s, i in batch if (self.requests[i].manual_seed is not None) == seeded
-                     and bool(self.requests[i].infer_text) == text]
-            if not group:
-                continue
-            for part, T0 in admission_groups(group, self.requests, self.gpt.max_context):
-                for chunk in admission_chunks(part, T0):  # each prompt's results do not depend on its batch
-                    self._admit(chunk, seeded, text, noise)
+        for chunk, _, seeded, text in admission_prefills(batch, self.requests, self.gpt.max_context):
+            self._admit(chunk, seeded, text, noise)
+
+    def prefill_chunk(self, slot: int, index: int, c0: int, n: int) -> None:
+        """Prompt columns ``[c0, c0 + n)`` of request ``index`` into ``slot`` (ctb_gpt_engine_prefill_chunk); the
+        final chunk admits the request.  A whole prompt (``c0 == 0``, ``n`` its length) is one ordinary admission."""
+        r = self.requests[index]
+        T, seeded, text = int(r.emb.shape[0]), r.manual_seed is not None, bool(r.infer_text)
+        if c0 == 0 and n == T:
+            self._admit([(slot, index)], seeded, text, {})
+            return
+        emb = r.emb[c0: c0 + n].to(self.dev, torch.float32).contiguous()
+        cfg, noise = None, None
+        if c0 + n == T:
+            cfgs, noise = self._sampling([r], seeded, text, {})
+            cfg = C.byref(cfgs[0])
+            self._text[slot] = text
+        _lib.check(self.lib.ctb_gpt_engine_prefill_chunk(
+            self.gpt._handle, slot, T, c0, n, C.c_void_p(emb.data_ptr()), int(text), cfg,
+            C.c_void_p(noise.data_ptr()) if noise is not None else None, r.max_new_token, self.stream))
+
+    def _sampling(self, reqs: List[Request], seeded: bool, text: bool, cache: Dict[tuple, torch.Tensor]):
+        """The sampler configs (host array) and seeded Exp(1) rows (device, or None) of an admission of ``reqs``."""
+        gpt, n = self.gpt, len(reqs)
+        cfgs = (_lib.SamplerConfig * n)()
+        for k, r in enumerate(reqs):
+            temps = [float(t) for t in torch.as_tensor(r.temperature).flatten().tolist()]
+            philox = 0 if seeded else int(torch.randint(0, 2 ** 62, (1,)).item())
+            cfgs[k] = build_sampler_config(r.logits_processors, temps, int(r.eos_token), r.min_new_token, philox)
+        noise = None
+        if seeded:  # the rows GPT.generate draws for this request's row of its batch (noise_batch) with this seed
+            rows, cols = (1, gpt.num_text_tokens) if text else (gpt.num_vq, gpt.num_audio_tokens)
+            noise = noise_rows(reqs, rows, cols, cache).to(self.dev)
+        return cfgs, noise
 
     def _admit(self, group, seeded: bool, text: bool, cache: Dict[tuple, torch.Tensor]) -> None:
         gpt, n = self.gpt, len(group)
@@ -525,15 +658,7 @@ class EngineDevice:
             T = int(r.emb.shape[0])
             emb[k, T0 - T:] = r.emb.to(self.dev, torch.float32)
             mask[k, T0 - T:] = 1
-        cfgs = (_lib.SamplerConfig * n)()
-        for k, r in enumerate(reqs):
-            temps = [float(t) for t in torch.as_tensor(r.temperature).flatten().tolist()]
-            philox = 0 if seeded else int(torch.randint(0, 2 ** 62, (1,)).item())
-            cfgs[k] = build_sampler_config(r.logits_processors, temps, int(r.eos_token), r.min_new_token, philox)
-        noise = None
-        if seeded:  # the rows GPT.generate draws for this request's row of its batch (noise_batch) with this seed
-            rows, cols = (1, gpt.num_text_tokens) if text else (gpt.num_vq, gpt.num_audio_tokens)
-            noise = noise_rows(reqs, rows, cols, cache).to(self.dev)
+        cfgs, noise = self._sampling(reqs, seeded, text, cache)
         slots = (C.c_int32 * n)(*[s for s, _ in group])
         max_new = (C.c_int32 * n)(*[r.max_new_token for r in reqs])
         for s, _ in group:
@@ -687,12 +812,14 @@ class OpenEngine:
     every pending job with it, stops the engine and is raised again by ``close``.  With a ``context`` (``GPT.Context``)
     an interrupt is ``schedule``'s: at the first poll that sees it the running requests end with what they have, the
     engine stops, and every job that has not ended by then is cancelled.  Subclasses turn each poll's yields into job
-    results (``_serve``)."""
+    results (``_serve``).  ``prefill_budget``: ``_poll_cycles``' bound on each poll's prompt columns (None: none)."""
 
     def __init__(self, make_device: Callable[[List[Request]], object], chunk: int,
                  check: Optional[Callable[[Request], None]] = None, device=None,
-                 on_close: Optional[Callable[[], None]] = None, max_new_cap: Optional[int] = None, context=None):
+                 on_close: Optional[Callable[[], None]] = None, max_new_cap: Optional[int] = None, context=None,
+                 prefill_budget: Optional[int] = None):
         self._make_device, self.chunk, self._check, self._on_close = make_device, int(chunk), check, on_close
+        self.prefill_budget = check_prefill_budget(prefill_budget)
         self.device, self.max_new_cap, self._context = device, max_new_cap, context
         cuda = device is not None and torch.device(device).type == "cuda"
         self._stream = torch.cuda.Stream(device) if cuda else None
@@ -795,7 +922,8 @@ class OpenEngine:
 
     def _loop(self, requests: _RequestTable) -> None:
         dev = self._make_device(requests)
-        for batch in stream_schedule(requests, dev, self.chunk, self._context, self.stats, self._check, self._source):
+        for batch in stream_schedule(requests, dev, self.chunk, self._context, self.stats, self._check, self._source,
+                                     self.prefill_budget):
             jobs = []
             for i, s, n, last in batch:
                 job = self._job_at.get(i)

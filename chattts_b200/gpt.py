@@ -229,7 +229,8 @@ class GPT:
     @torch.no_grad()
     def generate_continuous(self, requests, slots: Optional[int] = None, return_hidden=True, infer_text=False,
                             stream=False, return_attn=False, context=None, chunk: Optional[int] = None,
-                            max_new_cap: Optional[int] = None, dtype=torch.float32):
+                            max_new_cap: Optional[int] = None, dtype=torch.float32,
+                            prefill_budget: Optional[int] = None):
         """Generate audio codes or text for many utterances on a slot engine (chattts_b200.engine): up to ``slots``
         requests (default: ``max_batch``, at most the number of requests) decode together, and a waiting request takes
         the place of a finished one at the next poll (every ``chunk`` steps, default CTB_DECODE_CHUNK or 32).  Each
@@ -253,10 +254,16 @@ class GPT:
         ``dtype=torch.float16`` runs a half-precision engine (ctb_gpt_engine_begin_ex): the four matrices of every
         layer and the KV cache in fp16, everything else fp32 (the model the reference serves with
         ``Chat.load(use_vllm=True)``).  Its ids then follow that model, not ``generate``'s fp32 one.  It serves up to
-        64 slots (``CtbError`` above)."""
-        from .engine import ScheduleStats, schedule
+        64 slots (``CtbError`` above).
+
+        ``prefill_budget`` (prompt columns per poll, at least 128; default None: every admission is prefilled whole)
+        bounds the prefill the running slots wait for at each poll: a prompt that does not fit is prefilled in chunks
+        of multiples of 128 columns over the next polls (``engine._poll_cycles``), and its outputs are bit for bit
+        those of its admission in one call.  The yields are the same; a long prompt's first token comes later."""
+        from .engine import ScheduleStats, check_prefill_budget, schedule
 
         flags = _lib.engine_flags(dtype)
+        prefill_budget = check_prefill_budget(prefill_budget)
 
         if stream:
             raise ValueError("generate_continuous: stream=True is not supported; results are yielded per request "
@@ -268,7 +275,7 @@ class GPT:
         with torch.cuda.device(self.device_gpt):
             dev = self._engine_device(requests, S, cap, return_hidden, flags)
             self.last_schedule_stats = stats = ScheduleStats()  # admissions, decode steps (tools/bench_continuous.py)
-            for i, slot, n in schedule(requests, dev, chunk, context, stats, check):
+            for i, slot, n in schedule(requests, dev, chunk, context, stats, check, prefill_budget):
                 yield i, (dev.empty(i) if slot is None else dev.harvest(slot, n))
             if stats.interrupted:
                 self.logger.warning("generation is interrupted")
@@ -276,7 +283,8 @@ class GPT:
     @torch.no_grad()
     def generate_continuous_stream(self, requests, slots: Optional[int] = None, return_hidden=True, context=None,
                                    chunk: Optional[int] = None, infer_text=False, return_attn=False,
-                                   max_new_cap: Optional[int] = None, dtype=torch.float32):
+                                   max_new_cap: Optional[int] = None, dtype=torch.float32,
+                                   prefill_budget: Optional[int] = None):
         """Streaming form of ``generate_continuous``: generator of ``(request_index, GenerationOutputs, last)``.
 
         For each request the yields are exactly those ``generate(stream=True, stream_batch=r.stream_batch)`` makes for
@@ -288,11 +296,12 @@ class GPT:
         served as in ``generate_continuous``.
 
         ``ids`` are copies.  ``hiddens`` are views into the engine's buffer, like the narrowed views ``generate``
-        hands out: they stay valid until this generator is resumed (copy them to keep them).  ``dtype`` as in
-        ``generate_continuous``."""
-        from .engine import ScheduleStats, stream_schedule
+        hands out: they stay valid until this generator is resumed (copy them to keep them).  ``dtype`` and
+        ``prefill_budget`` as in ``generate_continuous``: a budget leaves every request's yields as they are."""
+        from .engine import ScheduleStats, check_prefill_budget, stream_schedule
 
         flags = _lib.engine_flags(dtype)
+        prefill_budget = check_prefill_budget(prefill_budget)
         requests, S, chunk, context, cap, check = self._engine_args(
             "generate_continuous_stream", requests, slots, infer_text, return_attn, context, chunk, None, max_new_cap)
         if not requests:
@@ -300,14 +309,14 @@ class GPT:
         with torch.cuda.device(self.device_gpt):
             dev = self._engine_device(requests, S, cap, return_hidden, flags)
             self.last_schedule_stats = stats = ScheduleStats()
-            for batch in stream_schedule(requests, dev, chunk, context, stats, check):
+            for batch in stream_schedule(requests, dev, chunk, context, stats, check, prefill_budget=prefill_budget):
                 for i, slot, n, last in batch:
                     yield i, (dev.empty(i) if slot is None else dev.harvest(slot, n, copy=False)), last
             if stats.interrupted:
                 self.logger.warning("generation is interrupted")
 
     def open_engine(self, slots: int, max_new_cap: int, return_hidden=True, chunk: Optional[int] = None,
-                    dtype=torch.float32):
+                    dtype=torch.float32, prefill_budget: Optional[int] = None):
         """A slot engine that takes requests while it decodes: ``submit(request, stream=False) -> engine.Job`` from
         any thread, ``Job.cancel()`` for one request, ``close(cancel=False)`` (or a ``with`` block) to drain it.
 
@@ -316,22 +325,28 @@ class GPT:
         streaming job iterates ``(GenerationOutputs, last)``, the yields ``generate_continuous_stream`` makes for it
         (copies), and simply ends when cancelled.  ``submit`` checks the request against this handle and
         ``max_new_cap`` in the caller's thread: prompt + ``max_new_token`` within ``max_context``.  A prompt over
-        1,024 tokens is prefilled on its own; the running slots wait for that prefill.  One worker thread owns the handle and its stream; while the engine
+        1,024 tokens is prefilled on its own; the running slots wait for that prefill, unless ``prefill_budget``
+        bounds each poll's prefill (``generate_continuous``; a job cancelled while its prompt is in progress frees its
+        slot at the next poll).  One worker thread owns the handle and its stream; while the engine
         is open ``generate``, ``generate_continuous*`` and another ``open_engine`` raise.  The poll interval is
         ``chunk`` steps (default CTB_DECODE_CHUNK, else 24).  ``slots`` and ``dtype`` as in ``generate_continuous``
         (up to ``max_batch`` slots; a half-precision engine up to 64)."""
         from .engine import GptEngine
 
         return self._open_slot_engine(GptEngine, slots, max_new_cap, return_hidden, chunk,
-                                      flags=_lib.engine_flags(dtype))
+                                      flags=_lib.engine_flags(dtype), prefill_budget=prefill_budget)
 
-    def _open_slot_engine(self, cls, slots, max_new_cap, return_hidden, chunk, *args, flags=0):
+    def _open_slot_engine(self, cls, slots, max_new_cap, return_hidden, chunk, *args, flags=0, prefill_budget=None):
         """An ``engine.OpenEngine`` subclass ``cls`` that owns this handle until it is closed (``flags``: the
-        ctb_gpt_engine_begin_ex precision flags)."""
+        ctb_gpt_engine_begin_ex precision flags; ``prefill_budget``: the engine's bound on each poll's prefill)."""
+        from .engine import check_prefill_budget
+
+        prefill_budget = check_prefill_budget(prefill_budget)
         _, S, chunk, _, cap, check = self._engine_args("open_engine", [], slots, False, False, None, chunk, None,
                                                        max_new_cap)
+        kw = {} if prefill_budget is None else {"prefill_budget": prefill_budget}
         engine = cls(lambda requests: self._engine_device(requests, S, cap, return_hidden, flags), chunk, check,
-                     self.device_gpt, self._close_engine, *args, max_new_cap=cap)
+                     self.device_gpt, self._close_engine, *args, max_new_cap=cap, **kw)
         self._open = engine
         return engine
 

@@ -207,6 +207,34 @@ int ctb_gpt_engine_admit_text(ctb_gpt* h, int32_t n, const int32_t* slots, int32
                               const uint8_t* mask_dev, const ctb_sampler_config* samplers, const float* q_noise_dev,
                               const int32_t* max_new, void* stream);
 
+/* Prefill columns [c0, c0 + n) of a prompt of T0 columns (8 <= T0 <= max_context - 1, every column valid, no padding)
+ * into the idle or finished slot `slot`, whose KV pages hold columns [0, c0) from the earlier chunks of the same
+ * prompt.  A prompt prefilled in chunks gives the same bits - KV pages, first token, and every later token and hidden
+ * state - as the same prompt admitted by one ctb_gpt_engine_admit / _admit_text call: each chunk row runs the layers
+ * as that call runs it, and its attention is the kernel that call would choose for T0 (not for n), over keys 0 .. its
+ * position read from the pages.  c0, and n unless the chunk is the final one (c0 + n == T0), are multiples of
+ * CTB_PREFILL_CHUNK_ALIGN, which keeps every row's GEMM tile and every query's attention tile where one call puts them.
+ *   emb_dev [n, d] fp32  the chunk's prompt embeddings (columns c0 .. c0 + n - 1)
+ *   text                 0: an audio-code request (ctb_gpt_engine_admit), 1: a text request (_admit_text)
+ *   sampler (host), q_noise_dev ([num_vq, num_audio] or [1, num_text] fp32, or NULL), max_new: one request's, as for
+ *                        those calls; read on the final chunk only (sampler may be NULL before it)
+ * A chunk before the final one touches nothing but the slot's pages: the slot keeps its state (idle or finished), and
+ * decode steps in between neither read nor append its pages.  The final chunk admits the request as those calls do:
+ * the slot becomes pending and its first token is sampled.  The handle records each slot's prompt in progress (T0,
+ * columns done); ctb_gpt_engine_admit / _admit_text / _cancel on the slot and ctb_gpt_engine_begin* drop it.
+ * Enqueued on `stream` after one synchronisation (two on the final chunk); the host arguments may be released on return.
+ * Errors leave the handle usable and the prompt in progress as it was:
+ *   CTB_ERR_STATE  outside engine mode; a chunk that does not continue the slot's prompt in progress (other c0 or T0),
+ *                  a first chunk with c0 != 0, or a slot that is running or pending
+ *   CTB_ERR_ARG    a null argument; slot out of range; T0 outside [8, max_context - 1]; [c0, c0 + n) not inside
+ *                  [0, T0); c0, or a non-final n, not a multiple of CTB_PREFILL_CHUNK_ALIGN; max_new outside
+ *                  [1, max_new_cap] or T0 + max_new > max_context; on the final chunk, a sampler ctb_gpt_engine_admit
+ *                  refuses */
+#define CTB_PREFILL_CHUNK_ALIGN 128
+int ctb_gpt_engine_prefill_chunk(ctb_gpt* h, int32_t slot, int32_t T0, int32_t c0, int32_t n, const float* emb_dev,
+                                 int32_t text, const ctb_sampler_config* sampler, const float* q_noise_dev,
+                                 int32_t max_new, void* stream);
+
 /* Synchronises `stream`, then reports per-slot results (each array [S], any may be NULL): state_host CTB_SLOT_*,
  * end_idx_host tokens of the slot's request, finish_host 1 if it ended at EOS.  A finished slot with end_idx 0 and
  * finish 1 sampled EOS as its first token (gpt.py:527: the request ends empty).  out->steps_done counts decode steps
