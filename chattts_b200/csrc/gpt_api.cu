@@ -230,9 +230,15 @@ static int encode_map_2d(CUtensorMap* m, const void* base, uint64_t rows, uint64
   return CTB_OK;
 }
 
-template <int EPI, int NPAD, int CS, int PREC = 0>
+// the shared-memory attribute of k_tc_dec<EPI, NPAD, CS, PREC> for the 16-, 32- and 64-row tiles
+template <int EPI, int CS, int PREC = 0>
 static int set_tc_attr() {
-  return ensure_smem_attr((const void*)k_tc_dec<EPI, NPAD, CS, PREC>, TdCfg<NPAD, (PREC & TD_W16) != 0>::SMEM_BYTES);
+  constexpr bool w16 = (PREC & TD_W16) != 0;
+  int rc;
+  if ((rc = ensure_smem_attr((const void*)k_tc_dec<EPI, 16, CS, PREC>, TdCfg<16, w16>::SMEM_BYTES)) ||
+      (rc = ensure_smem_attr((const void*)k_tc_dec<EPI, 32, CS, PREC>, TdCfg<32, w16>::SMEM_BYTES)))
+    return rc;
+  return ensure_smem_attr((const void*)k_tc_dec<EPI, 64, CS, PREC>, TdCfg<64, w16>::SMEM_BYTES);
 }
 
 // cluster sizes of the split-K (K slices per 128-row tile)
@@ -265,11 +271,10 @@ static int tc_setup(ctb_gpt* h) {
     if ((rc = encode_map_2d(&h->m_wd[l], Wl + L.wdown, d, I, 128))) return rc;
   }
   CTB_CUDA(cudaDeviceSynchronize());
-#define TCATTR(E, C) if ((rc = set_tc_attr<E, 16, C>())) return rc; if ((rc = set_tc_attr<E, 32, C>())) return rc; \
-  if ((rc = set_tc_attr<E, 64, C>())) return rc;
-  TCATTR(DE_QKV, CS_QKV) TCATTR(DE_OPROJ, CS_O) TCATTR(DE_GATEUP, CS_GU) TCATTR(DE_DOWN, CS_DOWN)
-#undef TCATTR
-  return CTB_OK;
+  if ((rc = set_tc_attr<DE_QKV, CS_QKV>()) || (rc = set_tc_attr<DE_OPROJ, CS_O>()) ||
+      (rc = set_tc_attr<DE_GATEUP, CS_GU>()))
+    return rc;
+  return set_tc_attr<DE_DOWN, CS_DOWN>();
 }
 
 // what every wgmma step shares: the tf32-split activation scratch (32 rows; 64 on a handle whose max_batch exceeds 32,
@@ -306,9 +311,7 @@ static int tc_setup_base(ctb_gpt* h) {
     if ((rc = encode_map_2d(&h->m_h[n][0], h->h_hi, R, I, npad))) return rc;
     if ((rc = encode_map_2d(&h->m_h[n][1], h->h_lo, R, I, npad))) return rc;
   }
-  if ((rc = set_tc_attr<DE_HEADS, 16, CS_HEADS>())) return rc;
-  if ((rc = set_tc_attr<DE_HEADS, 32, CS_HEADS>())) return rc;
-  if ((rc = set_tc_attr<DE_HEADS, 64, CS_HEADS>())) return rc;
+  if ((rc = set_tc_attr<DE_HEADS, CS_HEADS>())) return rc;
   h->tc_base = true;
   return CTB_OK;
 }
@@ -378,12 +381,10 @@ static int fp16_setup(ctb_gpt* h) {
       return rc;
     }
   }
-#define TCATTR(E, C, P) if ((rc = set_tc_attr<E, 16, C, P>())) return rc; if ((rc = set_tc_attr<E, 32, C, P>())) return rc; \
-  if ((rc = set_tc_attr<E, 64, C, P>())) return rc;
-  TCATTR(DE_QKV, CS_QKV, 1) TCATTR(DE_QKV, CS_QKV, 3) TCATTR(DE_OPROJ, CS_O, 1) TCATTR(DE_GATEUP, CS_GU, 1)
-  TCATTR(DE_DOWN, CS_DOWN, 1)
-#undef TCATTR
-  return CTB_OK;
+  if ((rc = set_tc_attr<DE_QKV, CS_QKV, 1>()) || (rc = set_tc_attr<DE_QKV, CS_QKV, 3>()) ||
+      (rc = set_tc_attr<DE_OPROJ, CS_O, 1>()) || (rc = set_tc_attr<DE_GATEUP, CS_GU, 1>()))
+    return rc;
+  return set_tc_attr<DE_DOWN, CS_DOWN, 1>();
 }
 
 extern "C" int ctb_gpt_create(const ctb_gpt_config* c, const float* weights_dev, ctb_gpt** out) {
@@ -1072,76 +1073,49 @@ static int prefill_first_token(ctb_gpt* h, int B, int T0, const int* nvalid, con
   return launch_finalize(h, s);
 }
 
-// B left-padded prompts [B, T0] -> decode rows slot[b] (slot == nullptr: rows 0..B-1), then the first token of every
-// row in state h->phase (all h->B rows of a static batch; the admitted slots of a slot engine)
-static int prefill_batched(ctb_gpt* h, int B, int T0, const float* emb, const uint8_t* mask, const int* slot,
-                           cudaStream_t s) {
+// Columns [q0, q0 + n) of B prompts of T columns -> decode rows slots[b] (slots: host array, copied to h->eng_slot by
+// the admission or written there by k_prefill_chunk_positions; nullptr: rows 0..B-1), whose pages hold columns [0, q0).
+//   whole prompts (q0 = 0, n = T): left padded, the positions counted from `mask` [B, T] (device)
+//   a chunk (mask == nullptr, B = 1): every column valid, positions q0 + j; q0, and n unless the chunk is the last, are
+//     multiples of CTB_PREFILL_CHUNK_ALIGN, so each row and query is computed as in the one-call prefill of T columns
+// Each query attends to keys 0 .. its position, read from the pages, with the kernel chosen by T: k_prefill_attn up to
+// PF_ATT_MAX_T0, else k_prefill_attn_tiled.  The call that ends the prompts (q0 + n == T) then hands each row's last
+// column to its decode row and samples the first token of every row in state h->phase (all h->B rows of a static batch;
+// the admitted slots of a slot engine); an earlier chunk touches nothing but the pf_* scratch and the slot's pages.
+static int prefill(ctb_gpt* h, int B, int T, int q0, int n, const float* emb, const uint8_t* mask,
+                   const int32_t* slots, cudaStream_t s) {
   const ctb_gpt_config& c = h->cfg;
-  const int M = B * T0;
-  const int d = c.hidden_size;
+  const int M = B * n;
   int rc;
   if ((rc = prefill_reserve(h, (size_t)M))) return rc;
-  CTB_CUDA(cudaMemcpyAsync(h->pf_resid, emb, (size_t)M * d * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  k_prefill_positions<<<B, 32, 0, s>>>(mask, h->pf_npre, h->pf_nvalid, T0);
+  CTB_CUDA(cudaMemcpyAsync(h->pf_resid, emb, (size_t)M * c.hidden_size * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  if (mask) k_prefill_positions<<<B, 32, 0, s>>>(mask, h->pf_npre, h->pf_nvalid, T);
+  else k_prefill_chunk_positions<<<(n + 255) / 256, 256, 0, s>>>(h->pf_mask, h->pf_npre, h->pf_nvalid, h->eng_slot,
+                                                                 slots[0], q0, n);
   CTB_LAUNCH_CHECK();
   PrefillP pp{};
-  pp.B = B; pp.T0 = T0; pp.mask = mask; pp.slot = slot;
-  const bool kv16 = (h->prec & CTB_ENGINE_FP16_KV) != 0;
-  if (T0 > PF_ATT_MAX_T0 &&
+  pp.B = B; pp.T0 = n; pp.mask = mask ? mask : h->pf_mask; pp.slot = slots ? h->eng_slot : nullptr;
+  const bool kv16 = (h->prec & CTB_ENGINE_FP16_KV) != 0, tiled = T > PF_ATT_MAX_T0;
+  if (tiled &&
       (rc = kv16 ? ensure_smem_attr((const void*)k_prefill_attn_tiled<__half>, PftSmem<__half>::BYTES)
                  : ensure_smem_attr((const void*)k_prefill_attn_tiled<float>, PftSmem<float>::BYTES)))
     return rc;
   auto attn = [&](const PrefillP& p) {
-    if (T0 > PF_ATT_MAX_T0) {
-      const dim3 tgrid((T0 + PFT_TILE - 1) / PFT_TILE, c.num_heads, B);
-      if (kv16) k_prefill_attn_tiled<__half><<<tgrid, PFT_THREADS, PftSmem<__half>::BYTES, s>>>(p);
-      else k_prefill_attn_tiled<float><<<tgrid, PFT_THREADS, PftSmem<float>::BYTES, s>>>(p);
-    } else {
-      const dim3 agrid((T0 + PF_ATT_WARPS - 1) / PF_ATT_WARPS, c.num_heads, B);
-      if (kv16) k_prefill_attn<__half><<<agrid, PF_ATT_WARPS * 32, (size_t)PF_ATT_WARPS * T0 * sizeof(float), s>>>(p);
-      else k_prefill_attn<float><<<agrid, PF_ATT_WARPS * 32, (size_t)PF_ATT_WARPS * T0 * sizeof(float), s>>>(p);
-    }
-  };
-  if ((rc = prefill_layers(h, pp, attn, s))) return rc;
-  return prefill_first_token(h, B, T0, h->pf_nvalid, slot, s);
-}
-
-// Columns [c0, c0 + n) of a prompt of T0 columns -> slot `slot`, whose pages hold columns [0, c0) from the earlier
-// chunks: the chunk's n rows run the layers of a one-call prefill (B = 1, every column valid, positions c0 + j), and
-// each query attends to keys 0 .. its position read from the pages, with the attention kernel a one-call prefill of T0
-// columns runs (k_prefill_attn up to PF_ATT_MAX_T0, else the tiled one).  The final chunk (c0 + n == T0) then hands
-// its last column to the slot and samples its first token (the slot is RS_PENDING, h->phase too); earlier chunks touch
-// nothing but the pf_* scratch and the slot's pages.
-static int prefill_chunk(ctb_gpt* h, int slot, int T0, int c0, int n, const float* emb, cudaStream_t s) {
-  const ctb_gpt_config& c = h->cfg;
-  int rc;
-  if ((rc = prefill_reserve(h, (size_t)n))) return rc;
-  CTB_CUDA(cudaMemcpyAsync(h->pf_resid, emb, (size_t)n * c.hidden_size * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  k_prefill_chunk_positions<<<(n + 255) / 256, 256, 0, s>>>(h->pf_mask, h->pf_npre, h->pf_nvalid, h->eng_slot, slot,
-                                                            c0, n);
-  CTB_LAUNCH_CHECK();
-  PrefillP pp{};
-  pp.B = 1; pp.T0 = n; pp.mask = h->pf_mask; pp.slot = h->eng_slot;
-  const bool kv16 = (h->prec & CTB_ENGINE_FP16_KV) != 0, tiled = T0 > PF_ATT_MAX_T0;
-  if (tiled &&
-      (rc = kv16 ? ensure_smem_attr((const void*)k_prefill_attn_tiled_chunk<__half>, PftSmem<__half>::BYTES)
-                 : ensure_smem_attr((const void*)k_prefill_attn_tiled_chunk<float>, PftSmem<float>::BYTES)))
-    return rc;
-  auto attn = [&](const PrefillP& p) {
     if (tiled) {
-      const dim3 tgrid((n + PFT_TILE - 1) / PFT_TILE, c.num_heads, 1);
-      if (kv16) k_prefill_attn_tiled_chunk<__half><<<tgrid, PFT_THREADS, PftSmem<__half>::BYTES, s>>>(p, c0);
-      else k_prefill_attn_tiled_chunk<float><<<tgrid, PFT_THREADS, PftSmem<float>::BYTES, s>>>(p, c0);
+      const dim3 tgrid((n + PFT_TILE - 1) / PFT_TILE, c.num_heads, B);
+      if (kv16) k_prefill_attn_tiled<__half><<<tgrid, PFT_THREADS, PftSmem<__half>::BYTES, s>>>(p, q0);
+      else k_prefill_attn_tiled<float><<<tgrid, PFT_THREADS, PftSmem<float>::BYTES, s>>>(p, q0);
     } else {
-      const dim3 agrid((n + PF_ATT_WARPS - 1) / PF_ATT_WARPS, c.num_heads, 1);
-      const size_t smem = (size_t)PF_ATT_WARPS * (c0 + n) * sizeof(float);
-      if (kv16) k_prefill_attn_chunk<__half><<<agrid, PF_ATT_WARPS * 32, smem, s>>>(p, c0);
-      else k_prefill_attn_chunk<float><<<agrid, PF_ATT_WARPS * 32, smem, s>>>(p, c0);
+      const dim3 agrid((n + PF_ATT_WARPS - 1) / PF_ATT_WARPS, c.num_heads, B);
+      const size_t smem = (size_t)PF_ATT_WARPS * (q0 + n) * sizeof(float);
+      if (kv16) k_prefill_attn<__half><<<agrid, PF_ATT_WARPS * 32, smem, s>>>(p, q0);
+      else k_prefill_attn<float><<<agrid, PF_ATT_WARPS * 32, smem, s>>>(p, q0);
     }
   };
   if ((rc = prefill_layers(h, pp, attn, s))) return rc;
-  if (c0 + n < T0) return CTB_OK;
-  return prefill_first_token(h, 1, n, h->pf_nvalid + 1, h->eng_slot, s);
+  if (q0 + n < T) return CTB_OK;
+  // a chunk's k_prefill_chunk_positions puts the row's token count q0 + n in nvalid[1]
+  return prefill_first_token(h, B, n, mask ? h->pf_nvalid : h->pf_nvalid + 1, pp.slot, s);
 }
 
 // Pages for B rows of up to `tokens` tokens each: grow the pool if needed (page = 16 tokens x K|V x heads x 64 values per
@@ -1177,6 +1151,27 @@ static int kv_reserve(ctb_gpt* h, int B, int tokens, cudaStream_t s) {
   return CTB_OK;
 }
 
+static int check_sampler(const ctb_sampler_config& sc) {
+  if (sc.past_window > 31 || sc.past_window < 0) return set_err(CTB_ERR_ARG, "past_window out of range");
+  if (sc.min_tokens_to_keep < 1) return set_err(CTB_ERR_ARG, "min_tokens_to_keep must be >= 1");
+  return CTB_OK;
+}
+
+// A new static batch or slot engine: the captured decode graphs were built for the old one, and the wgmma step's
+// activation scratch starts from zeros (h->use_tc already chosen)
+static int restart_decode(ctb_gpt* h, cudaStream_t s) {
+  if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
+  if (h->graph_exec_text) { cudaGraphExecDestroy(h->graph_exec_text); h->graph_exec_text = nullptr; }
+  if (h->use_tc) {
+    const size_t d = h->cfg.hidden_size, I = h->cfg.intermediate_size;
+    float* z768[] = {h->x_hi, h->x_lo, h->attn_hi, h->attn_lo};
+    for (float* zp : z768) CTB_CUDA(cudaMemsetAsync(zp, 0, h->tc_rows * d * sizeof(float), s));
+    CTB_CUDA(cudaMemsetAsync(h->h_hi, 0, h->tc_rows * I * sizeof(float), s));
+    CTB_CUDA(cudaMemsetAsync(h->h_lo, 0, h->tc_rows * I * sizeof(float), s));
+  }
+  return CTB_OK;
+}
+
 extern "C" int ctb_gpt_begin(ctb_gpt* h, int32_t B, int32_t T0, const float* emb_dev, const uint8_t* mask_dev,
                              const ctb_sampler_config* sampler, const float* q_noise_dev, int32_t max_new_token,
                              int32_t infer_text, int32_t* ids_out_dev, float* hiddens_out_dev, void* stream) {
@@ -1184,17 +1179,15 @@ extern "C" int ctb_gpt_begin(ctb_gpt* h, int32_t B, int32_t T0, const float* emb
   if (B < 1 || B > h->cfg.max_batch) return set_err(CTB_ERR_ARG, "B=%d outside [1,%d]", B, h->cfg.max_batch);
   if (T0 < 1 || max_new_token < 1 || T0 + max_new_token > h->cfg.max_context)
     return set_err(CTB_ERR_ARG, "T0=%d + max_new=%d exceeds max_context=%d", T0, max_new_token, h->cfg.max_context);
-  if (sampler->past_window > 31 || sampler->past_window < 0) return set_err(CTB_ERR_ARG, "past_window out of range");
-  if (sampler->min_tokens_to_keep < 1) return set_err(CTB_ERR_ARG, "min_tokens_to_keep must be >= 1");
+  int rc;
+  if ((rc = check_sampler(*sampler))) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   h->B = B; h->T0 = T0; h->max_new = max_new_token; h->infer_text = infer_text ? 1 : 0;
   h->engine = 0; h->phase = RS_RUNNING; h->prec = 0;
   h->use_tc = h->tc_ready && B >= h->tc_min_batch;
   h->sampler = *sampler; h->q_noise = q_noise_dev; h->emb = emb_dev; h->mask = mask_dev;
   h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev;
-  if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
-  if (h->graph_exec_text) { cudaGraphExecDestroy(h->graph_exec_text); h->graph_exec_text = nullptr; }
-  { int rc0 = kv_reserve(h, B, T0 + max_new_token, s); if (rc0) return rc0; }
+  if ((rc = restart_decode(h, s)) || (rc = kv_reserve(h, B, T0 + max_new_token, s))) return rc;
   CTB_CUDA(cudaMemsetAsync(h->st, 0, sizeof(LoopState), s));
   CTB_CUDA(cudaMemsetAsync(h->seq_len, 0, sizeof(int) * h->bpad_max, s));
   CTB_CUDA(cudaMemsetAsync(h->finish, 0, h->bpad_max, s));
@@ -1206,19 +1199,9 @@ extern "C" int ctb_gpt_begin(ctb_gpt* h, int32_t B, int32_t T0, const float* emb
     CTB_CUDA(cudaMemcpyAsync(h->flow_epoch, &e0, sizeof(e0), cudaMemcpyHostToDevice, s));
     CTB_CUDA(cudaMemsetAsync(h->flow_arena, 0, FL_ARENA_WORDS * sizeof(unsigned long long), s));
   }
-  if (h->use_tc) {
-    const size_t d = h->cfg.hidden_size, I = h->cfg.intermediate_size;
-    float* z768[] = {h->x_hi, h->x_lo, h->attn_hi, h->attn_lo};
-    for (float* zp : z768) CTB_CUDA(cudaMemsetAsync(zp, 0, h->tc_rows * d * sizeof(float), s));
-    CTB_CUDA(cudaMemsetAsync(h->h_hi, 0, h->tc_rows * I * sizeof(float), s));
-    CTB_CUDA(cudaMemsetAsync(h->h_lo, 0, h->tc_rows * I * sizeof(float), s));
-  }
-  int rc;
-  // prefill: the prompt is walked column by column through the decode kernels (left padding
-  // keeps every row's last prompt token in the last column, like the reference's batches)
   if (h->pf_enabled && T0 >= 8 && T0 <= 1024) {
     // whole prompt as token-parallel wgmma GEMMs (prefill.cuh)
-    if ((rc = prefill_batched(h, B, T0, emb_dev, mask_dev, nullptr, s))) return rc;
+    if ((rc = prefill(h, B, T0, 0, T0, emb_dev, mask_dev, nullptr, s))) return rc;
   } else {
     // short prompts: walk the columns through the decode kernels (left padding keeps every row's last prompt
     // token in the last column, like the reference's batches)
@@ -1303,11 +1286,9 @@ extern "C" int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_ca
   if (use_tc) {
     // build what this handle lacks (a handle whose max_batch is below 9 or above 32 has no tensor-core state yet)
     if ((flags & CTB_ENGINE_FP16_WEIGHTS) ? (rc = fp16_setup(h)) : (!h->tc_wqkv && (rc = tc_setup(h)))) return rc;
-    if ((flags & CTB_ENGINE_FP16_KV) && !(flags & CTB_ENGINE_FP16_WEIGHTS)) {
-      if ((rc = set_tc_attr<DE_QKV, 16, CS_QKV, CTB_ENGINE_FP16_KV>())) return rc;
-      if ((rc = set_tc_attr<DE_QKV, 32, CS_QKV, CTB_ENGINE_FP16_KV>())) return rc;
-      if ((rc = set_tc_attr<DE_QKV, 64, CS_QKV, CTB_ENGINE_FP16_KV>())) return rc;
-    }
+    if ((flags & CTB_ENGINE_FP16_KV) && !(flags & CTB_ENGINE_FP16_WEIGHTS) &&
+        (rc = set_tc_attr<DE_QKV, CS_QKV, CTB_ENGINE_FP16_KV>()))
+      return rc;
   }
   if (!h->rows) {
     if ((rc = dalloc(&h->rows, (size_t)h->bpad_max))) return rc;
@@ -1325,9 +1306,7 @@ extern "C" int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_ca
   h->use_tc = use_tc;
   h->q_noise = h->eng_noise; h->emb = nullptr; h->mask = nullptr;
   h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev; h->eng_text = 0;
-  if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
-  if (h->graph_exec_text) { cudaGraphExecDestroy(h->graph_exec_text); h->graph_exec_text = nullptr; }
-  if ((rc = kv_reserve(h, S, c.max_context, s))) return rc;
+  if ((rc = restart_decode(h, s)) || (rc = kv_reserve(h, S, c.max_context, s))) return rc;
   static const LoopState idle_state = {0, 1, 0, 0, 0};  // no running slot: decode steps are no-ops
   CTB_CUDA(cudaMemcpyAsync(h->st, &idle_state, sizeof(LoopState), cudaMemcpyHostToDevice, s));
   CTB_CUDA(cudaMemsetAsync(h->rows, 0, sizeof(RowState) * h->bpad_max, s));  // every slot RS_IDLE
@@ -1338,13 +1317,6 @@ extern "C" int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_ca
   CTB_CUDA(cudaMemsetAsync(h->end_idx, 0, sizeof(int) * h->bpad_max, s));
   CTB_CUDA(cudaMemsetAsync(h->counter, 0, sizeof(int) * c.max_batch * c.num_heads, s));
   CTB_CUDA(cudaMemsetAsync(h->x, 0, sizeof(float) * h->bpad_max * c.hidden_size, s));
-  if (h->use_tc) {
-    const size_t d = c.hidden_size, I = c.intermediate_size;
-    float* z768[] = {h->x_hi, h->x_lo, h->attn_hi, h->attn_lo};
-    for (float* zp : z768) CTB_CUDA(cudaMemsetAsync(zp, 0, h->tc_rows * d * sizeof(float), s));
-    CTB_CUDA(cudaMemsetAsync(h->h_hi, 0, h->tc_rows * I * sizeof(float), s));
-    CTB_CUDA(cudaMemsetAsync(h->h_lo, 0, h->tc_rows * I * sizeof(float), s));
-  }
   CTB_CUDA(cudaStreamSynchronize(s));  // idle_state is read by the copy engine
   h->chunk_T0.assign((size_t)S, 0);     // no prompt in progress
   h->chunk_done.assign((size_t)S, 0);
@@ -1353,18 +1325,16 @@ extern "C" int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_ca
   return CTB_OK;
 }
 
-static int engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0, const float* emb_dev,
-                        const uint8_t* mask_dev, const ctb_sampler_config* samplers, const float* q_noise_dev,
-                        const int32_t* max_new, int text, void* stream) {
-  if (!h || !slots || !emb_dev || !mask_dev || !samplers || !max_new) return set_err(CTB_ERR_ARG, "null argument");
-  if (!h->engine) return set_err(CTB_ERR_STATE, "ctb_gpt_engine_begin has not been called");
+// Admit n requests into `slots` (host): prefill columns [q0, T0) of their prompts - whole prompts (q0 = 0) with
+// `mask`, or the final chunk of one slot's prompt (mask == nullptr) - and sample their first tokens.  Every slot is
+// validated before anything is written, so a refused call leaves the handle as it was; the host arrays are copied
+// before the call returns (synchronised), so the caller may free them at once.
+static int admit(ctb_gpt* h, int n, const int32_t* slots, int T0, int q0, const float* emb_dev, const uint8_t* mask_dev,
+                 const ctb_sampler_config* samplers, const float* q_noise_dev, const int32_t* max_new, int text,
+                 cudaStream_t s) {
   const ctb_gpt_config& c = h->cfg;
   const int S = h->B;
-  if (n < 1 || n > S) return set_err(CTB_ERR_ARG, "n=%d outside [1,%d]", n, S);
-  // prompts over 1,024 columns take the tiled prefill attention; every slot owns max_context tokens of pages
-  if (T0 < 8 || T0 > c.max_context - 1)
-    return set_err(CTB_ERR_ARG, "T0=%d outside [8,%d]: left-pad shorter prompts to 8", T0, c.max_context - 1);
-  cudaStream_t s = (cudaStream_t)stream;
+  int rc;
   std::vector<RowState> rows((size_t)h->bpad_max);
   CTB_CUDA(cudaMemcpyAsync(rows.data(), h->rows, sizeof(RowState) * rows.size(), cudaMemcpyDeviceToHost, s));
   CTB_CUDA(cudaStreamSynchronize(s));
@@ -1379,14 +1349,12 @@ static int engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0,
     if (max_new[i] < 1 || max_new[i] > h->max_new || T0 + max_new[i] > c.max_context)
       return set_err(CTB_ERR_ARG, "slot %d: max_new=%d (capacity %d) with T0=%d exceeds max_context=%d", b, max_new[i],
                      h->max_new, T0, c.max_context);
-    if (sc.past_window > 31 || sc.past_window < 0) return set_err(CTB_ERR_ARG, "past_window out of range");
-    if (sc.min_tokens_to_keep < 1) return set_err(CTB_ERR_ARG, "min_tokens_to_keep must be >= 1");
+    if ((rc = check_sampler(sc))) return rc;
     RowState& r = rows[b];
     r.n_gen = 0; r.step = 0; r.state = RS_PENDING; r.max_new = max_new[i]; r.has_noise = q_noise_dev != nullptr;
     r.eos = sc.eos_token; r.text = text;
   }
   for (int i = 0; i < n; ++i) h->chunk_T0[slots[i]] = 0;  // the slot's prompt in progress, if any, is dropped
-  // host arrays are copied before this call returns (synchronised below), so the caller may free them at once
   CTB_CUDA(cudaMemcpyAsync(h->rows, rows.data(), sizeof(RowState) * rows.size(), cudaMemcpyHostToDevice, s));
   CTB_CUDA(cudaMemcpyAsync(h->eng_slot, slots, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
   const size_t nrow = text ? (size_t)c.num_text_tokens : (size_t)c.num_vq * c.num_audio_tokens;
@@ -1403,9 +1371,22 @@ static int engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0,
   // prompts -> their slots' pages, then heads / sampler / finalize for the RS_PENDING rows only
   if (text) h->eng_text = 1;
   h->phase = RS_PENDING;
-  const int rc = prefill_batched(h, n, T0, emb_dev, mask_dev, h->eng_slot, s);
+  rc = prefill(h, n, T0, q0, T0 - q0, emb_dev, mask_dev, slots, s);
   h->phase = RS_RUNNING;
   return rc;
+}
+
+static int engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0, const float* emb_dev,
+                        const uint8_t* mask_dev, const ctb_sampler_config* samplers, const float* q_noise_dev,
+                        const int32_t* max_new, int text, void* stream) {
+  if (!h || !slots || !emb_dev || !mask_dev || !samplers || !max_new) return set_err(CTB_ERR_ARG, "null argument");
+  if (!h->engine) return set_err(CTB_ERR_STATE, "ctb_gpt_engine_begin has not been called");
+  const ctb_gpt_config& c = h->cfg;
+  if (n < 1 || n > h->B) return set_err(CTB_ERR_ARG, "n=%d outside [1,%d]", n, h->B);
+  // prompts over 1,024 columns take the tiled prefill attention; every slot owns max_context tokens of pages
+  if (T0 < 8 || T0 > c.max_context - 1)
+    return set_err(CTB_ERR_ARG, "T0=%d outside [8,%d]: left-pad shorter prompts to 8", T0, c.max_context - 1);
+  return admit(h, n, slots, T0, 0, emb_dev, mask_dev, samplers, q_noise_dev, max_new, text, (cudaStream_t)stream);
 }
 
 extern "C" int ctb_gpt_engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0, const float* emb_dev,
@@ -1438,10 +1419,10 @@ extern "C" int ctb_gpt_engine_prefill_chunk(ctb_gpt* h, int32_t slot, int32_t T0
   if (max_new < 1 || max_new > h->max_new || T0 + max_new > c.max_context)
     return set_err(CTB_ERR_ARG, "max_new=%d (capacity %d) with T0=%d exceeds max_context=%d", max_new, h->max_new, T0,
                    c.max_context);
+  int rc;
   if (final) {
     if (!sampler) return set_err(CTB_ERR_ARG, "null sampler on the final chunk");
-    if (sampler->past_window > 31 || sampler->past_window < 0) return set_err(CTB_ERR_ARG, "past_window out of range");
-    if (sampler->min_tokens_to_keep < 1) return set_err(CTB_ERR_ARG, "min_tokens_to_keep must be >= 1");
+    if ((rc = check_sampler(*sampler))) return rc;
   }
   const int pT0 = h->chunk_T0[slot], pdone = h->chunk_done[slot];
   if (pT0 == 0 && c0 != 0)
@@ -1451,34 +1432,15 @@ extern "C" int ctb_gpt_engine_prefill_chunk(ctb_gpt* h, int32_t slot, int32_t T0
     return set_err(CTB_ERR_STATE, "slot %d: chunk [%d,%d) of T0=%d does not continue the prompt in progress ([0,%d) of "
                    "T0=%d done)", slot, c0, c0 + n, T0, pdone, pT0);
   cudaStream_t s = (cudaStream_t)stream;
+  // the final chunk admits the request as ctb_gpt_engine_admit / _admit_text do for one slot
+  if (final) return admit(h, 1, &slot, T0, c0, emb_dev, nullptr, sampler, q_noise_dev, &max_new, text ? 1 : 0, s);
   RowState r;
   CTB_CUDA(cudaMemcpyAsync(&r, h->rows + slot, sizeof(RowState), cudaMemcpyDeviceToHost, s));
   CTB_CUDA(cudaStreamSynchronize(s));
   if (r.state == RS_RUNNING || r.state == RS_PENDING) return set_err(CTB_ERR_STATE, "slot %d is still generating", slot);
-  if (!final) {
-    const int rc = prefill_chunk(h, slot, T0, c0, n, emb_dev, s);
-    if (rc) { h->chunk_T0[slot] = 0; return rc; }
-    h->chunk_T0[slot] = T0; h->chunk_done[slot] = c0 + n;
-    return CTB_OK;
-  }
-  // the final chunk admits the request as ctb_gpt_engine_admit / _admit_text do for one slot
-  r.n_gen = 0; r.step = 0; r.state = RS_PENDING; r.max_new = max_new; r.has_noise = q_noise_dev != nullptr;
-  r.eos = sampler->eos_token; r.text = text ? 1 : 0;
-  CTB_CUDA(cudaMemcpyAsync(h->rows + slot, &r, sizeof(RowState), cudaMemcpyHostToDevice, s));
-  CTB_CUDA(cudaMemcpyAsync(h->cfgs + slot, sampler, sizeof(ctb_sampler_config), cudaMemcpyHostToDevice, s));
-  const size_t nrow = text ? (size_t)c.num_text_tokens : (size_t)c.num_vq * c.num_audio_tokens;
-  if (q_noise_dev)
-    CTB_CUDA(cudaMemcpyAsync(h->eng_noise + slot * noise_stride(h), q_noise_dev, nrow * sizeof(float),
-                             cudaMemcpyDeviceToDevice, s));
-  CTB_CUDA(cudaMemsetAsync(h->finish + slot, 0, 1, s));
-  CTB_CUDA(cudaMemsetAsync(h->end_idx + slot, 0, sizeof(int), s));
-  CTB_CUDA(cudaStreamSynchronize(s));  // r and *sampler are read by the copy engine
-  h->chunk_T0[slot] = 0;
-  if (text) h->eng_text = 1;
-  h->phase = RS_PENDING;
-  const int rc = prefill_chunk(h, slot, T0, c0, n, emb_dev, s);
-  h->phase = RS_RUNNING;
-  return rc;
+  if ((rc = prefill(h, 1, T0, c0, n, emb_dev, nullptr, &slot, s))) { h->chunk_T0[slot] = 0; return rc; }
+  h->chunk_T0[slot] = T0; h->chunk_done[slot] = c0 + n;
+  return CTB_OK;
 }
 
 extern "C" int ctb_gpt_engine_status(ctb_gpt* h, ctb_gpt_status* out, int32_t* state_host, int32_t* end_idx_host,
@@ -1589,8 +1551,7 @@ extern "C" int ctb_sample(const float* logits_dev, int32_t rows, int32_t V, int3
   if (rows < 1 || V < 1 || rows_per_item < 1 || rows % rows_per_item) return set_err(CTB_ERR_ARG, "bad shape");
   if ((size_t)V * 4 + 8192 > 200 * 1024) return set_err(CTB_ERR_ARG, "V=%d too large for the sampler", V);
   if (sampler->penalty_on && n_gen > 0 && !gen_ids_dev) return set_err(CTB_ERR_ARG, "gen_ids required");
-  if (sampler->past_window > 31 || sampler->past_window < 0) return set_err(CTB_ERR_ARG, "past_window out of range");
-  if (sampler->min_tokens_to_keep < 1) return set_err(CTB_ERR_ARG, "min_tokens_to_keep must be >= 1");
+  if (int rc = check_sampler(*sampler)) return rc;
   SampleP sp{};
   sp.st = nullptr; sp.check_finished = 0; sp.logits = logits_dev; sp.rows = rows; sp.V = V;
   sp.rows_per_item = rows_per_item; sp.cfg = *sampler; sp.q_noise = q_noise_dev; sp.gen_ids = gen_ids_dev;

@@ -10,8 +10,9 @@
 //   then k_prefill_finish hands the last column's residual to the decode-loop state (x, seq_len) and the
 //   regular heads -> sampler -> finalize kernels produce the first token.
 // A slot-engine prompt may also be prefilled in 128-aligned chunks (ctb_gpt_engine_prefill_chunk): the same layers over
-// the chunk's rows (k_prefill_chunk_positions), and the attention of the whole prompt's width with a query offset
-// (k_prefill_attn_chunk, k_prefill_attn_tiled_chunk) reading the earlier chunks' keys from the pages.
+// the chunk's rows (k_prefill_chunk_positions), and the attention kernel of the whole prompt's width with the chunk's
+// first position as its query offset q0, reading the earlier chunks' keys from the pages.  A whole prompt is the chunk
+// with q0 = 0.
 #pragma once
 #include <type_traits>
 
@@ -104,12 +105,13 @@ __global__ void k_prefill_rope_kv(const PrefillP p) {
 // fine for 16-token prompts, hopeless for speaker-prompt prefixes of hundreds of tokens.)
 // KVT: the cache's element type, widened to fp32 as it is read.
 //
-// q0: position of the call's first query (k_prefill_attn_chunk: a chunk of a longer prompt whose columns 0 .. q0 - 1 are
-// already in the row's pages; 0 for a whole prompt).  Query j of the call is prompt position q0 + j and attends to keys
-// 0 .. q0 + j, each with the arithmetic a one-call prefill gives that position.
+// q0: position of the call's first query (a chunk of a longer prompt whose columns 0 .. q0 - 1 are already in the row's
+// pages, with B = 1 and T0 = the chunk's columns, all valid; 0 for a whole prompt).  Query j of the call is prompt
+// position q0 + j and attends to keys 0 .. q0 + j, each with the arithmetic a one-call prefill gives that position.
+// Shared memory: 8 x (q0 + T0) floats.
 constexpr int PF_ATT_WARPS = 8;
 template <typename KVT>
-__device__ __forceinline__ void prefill_attn_warp(const PrefillP& p, const int q0) {
+__global__ void __launch_bounds__(PF_ATT_WARPS * 32) k_prefill_attn(const PrefillP p, int q0) {
   constexpr int HD = 64;
   const int h = blockIdx.y, b = blockIdx.z, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = p.nvalid[b];
@@ -173,16 +175,6 @@ __device__ __forceinline__ void prefill_attn_warp(const PrefillP& p, const int q
   *reinterpret_cast<float2*>(p.attn + qrow + 2 * lane) = make_float2(o0 / l, o1 / l);  // V (and the output) is never permuted
 }
 
-template <typename KVT>
-__global__ void __launch_bounds__(PF_ATT_WARPS * 32) k_prefill_attn(const PrefillP p) { prefill_attn_warp<KVT>(p, 0); }
-
-// One chunk (B = 1, T0 = the chunk's columns, all valid) of a prompt of at most PF_ATT_MAX_T0 columns whose first q0
-// columns are in the row's pages: shared memory 8 x (q0 + T0) floats
-template <typename KVT>
-__global__ void __launch_bounds__(PF_ATT_WARPS * 32) k_prefill_attn_chunk(const PrefillP p, int q0) {
-  prefill_attn_warp<KVT>(p, q0);
-}
-
 // k_prefill_attn keeps a query's whole score row in shared memory (8 x T0 floats per CTA): prompts wider than this
 // take k_prefill_attn_tiled.  The choice depends on T0 alone, so a prompt of up to 1,024 columns is computed as before.
 constexpr int PF_ATT_MAX_T0 = 1024;
@@ -237,11 +229,11 @@ __device__ __forceinline__ float4 pft_ld4(const __half* p) {
 }
 
 //
-// q0 (a multiple of 64) as in prefill_attn_warp: the call's query tile qj is the prompt's tile q0 / 64 + qj, the same 64
+// q0 (a multiple of 64) as in k_prefill_attn: the call's query tile qj is the prompt's tile q0 / 64 + qj, the same 64
 // queries a one-call prefill gives one CTA, and keys past q0 + n - 1 are zero-filled as keys past a whole prompt's last
 // are (the pages there hold an earlier request's values).
 template <typename KVT>
-__device__ __forceinline__ void prefill_attn_tiled_cta(const PrefillP& p, const int q0) {
+__global__ void __launch_bounds__(PFT_THREADS) k_prefill_attn_tiled(const PrefillP p, int q0) {
   using SM = PftSmem<KVT>;
   constexpr int HD = 64, T = PFT_TILE;
   const int h = blockIdx.y, b = blockIdx.z, tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
@@ -376,16 +368,6 @@ __device__ __forceinline__ void prefill_attn_tiled_cta(const PrefillP& p, const 
       *reinterpret_cast<float4*>(p.attn + ((row0 + t) * p.Hq + h) * HD + tx * 4) =
           make_float4(o[i][0] / l[i], o[i][1] / l[i], o[i][2] / l[i], o[i][3] / l[i]);
   }
-}
-
-template <typename KVT>
-__global__ void __launch_bounds__(PFT_THREADS) k_prefill_attn_tiled(const PrefillP p) { prefill_attn_tiled_cta<KVT>(p, 0); }
-
-// One chunk (B = 1, T0 = the chunk's columns, all valid) of a prompt of more than PF_ATT_MAX_T0 columns whose first q0
-// columns (a multiple of PFT_TILE) are in the row's pages
-template <typename KVT>
-__global__ void __launch_bounds__(PFT_THREADS) k_prefill_attn_tiled_chunk(const PrefillP p, int q0) {
-  prefill_attn_tiled_cta<KVT>(p, q0);
 }
 
 // h = silu(gate) * up over [M, 2I] -> [M, I]

@@ -432,23 +432,18 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
         free = [s for s in range(dev.slots) if owner[s] is None]
         batch = []
         created = False
-        if budget is None:
-            while free and waiting:
-                s, i = free.pop(0), waiting.popleft()
-                owner[s] = i
-                batch.append((s, i))
-        else:
-            if prog is not None:
-                advance()
-            room = left
-            while free and waiting and prog is None:  # the requests behind a prompt in progress wait for it
-                s, i = free.pop(0), waiting.popleft()
-                owner[s] = i
-                if admission_cols(batch + [(s, i)], requests, dev.max_context) > room:
-                    prog, created = [s, i, 0], True  # the first request that does not fit
-                    break
-                batch.append((s, i))
-            left = room - admission_cols(batch, requests, dev.max_context)
+        if prog is not None:
+            advance()
+        while free and waiting and prog is None:  # the requests behind a prompt in progress wait for it
+            s, i = free.pop(0), waiting.popleft()
+            owner[s] = i
+            # no budget, no bound: admission_cols (quadratic in the admission's size) is not evaluated
+            if budget is not None and admission_cols(batch + [(s, i)], requests, dev.max_context) > left:
+                prog, created = [s, i, 0], True  # the first request that does not fit
+                break
+            batch.append((s, i))
+        if budget is not None:
+            left -= admission_cols(batch, requests, dev.max_context)
         if batch:
             dev.admit(batch)
             stats.admissions += 1
