@@ -65,6 +65,20 @@ PREFILL_CHUNK_ALIGN = 128
 #: slot states reported by ctb_gpt_engine_status (CTB_SLOT_* in the header)
 SLOT_IDLE, SLOT_RUNNING, SLOT_FINISHED = 0, 1, 2
 
+#: ctb_gpt_engine_reserve: the KV pool's free pages cannot cover the call (CTB_ERR_POOL)
+ERR_POOL = -5
+#: tokens per KV page
+PAGE_TOKENS = 16
+
+
+class SlotImage(C.Structure):
+    """The header of a suspended slot's image (ctb_slot_image)."""
+    _fields_ = [("magic", C.c_uint32)] + [(n, C.c_int32) for n in (
+        "prec", "seq_len", "pos", "end_idx", "finish", "n_gen", "npages", "page_bytes", "num_vq", "hidden_size",
+        "noise_floats", "has_hidden")] + [
+        ("row", C.c_int32 * 8), ("reserved", C.c_int32 * 3), ("sampler", SamplerConfig)] + [
+        (n, C.c_uint64) for n in ("off_noise", "off_ids", "off_hiddens", "off_kv", "bytes")]
+
 
 class ConvStackConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
@@ -83,6 +97,8 @@ EXPORTS = (
     "ctb_gpt_destroy", "ctb_gpt_begin", "ctb_gpt_decode", "ctb_gpt_status_query", "ctb_gpt_profile_kernel", "ctb_gpt_debug_trace", "ctb_gpt_embed_prompt", "ctb_sample",
     "ctb_gpt_engine_begin", "ctb_gpt_engine_admit", "ctb_gpt_engine_admit_text", "ctb_gpt_engine_status",
     "ctb_gpt_engine_cancel", "ctb_gpt_engine_begin_ex", "ctb_gpt_engine_prefill_chunk",
+    "ctb_gpt_engine_begin_paged", "ctb_gpt_engine_reserve", "ctb_gpt_engine_release", "ctb_gpt_engine_suspend_bytes",
+    "ctb_gpt_engine_suspend", "ctb_gpt_engine_resume",
     "ctb_dvae_blob_floats", "ctb_vocos_blob_floats", "ctb_decoder_create", "ctb_decoder_destroy",
     "ctb_dvae_decode", "ctb_vocos_decode", "ctb_decode_rows",
     "ctb_dvae_encoder_blob_floats", "ctb_dvae_encoder_create", "ctb_dvae_encoder_destroy", "ctb_dvae_encode",
@@ -137,6 +153,12 @@ def load(build_if_missing: bool = True):
         lib.ctb_gpt_engine_cancel.argtypes = [vp, i32, vp, vp]
         lib.ctb_gpt_engine_prefill_chunk.argtypes = [vp, i32, i32, i32, i32, vp, i32, C.POINTER(SamplerConfig), vp, i32,
                                                      vp]
+        lib.ctb_gpt_engine_begin_paged.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp]
+        lib.ctb_gpt_engine_reserve.argtypes = [vp, i32, vp, vp, vp]
+        lib.ctb_gpt_engine_release.argtypes = [vp, i32, vp, vp]
+        lib.ctb_gpt_engine_suspend_bytes.argtypes = [vp, i32, C.POINTER(C.c_uint64), vp]
+        lib.ctb_gpt_engine_suspend.argtypes = [vp, i32, vp, C.c_uint64, vp]
+        lib.ctb_gpt_engine_resume.argtypes = [vp, i32, vp, C.c_uint64, vp]
         lib.ctb_sample.argtypes = [vp, i32, i32, i32, C.POINTER(SamplerConfig), vp, vp, i32, i32, i32, vp, vp]
         lib.ctb_dvae_blob_floats.argtypes = [C.POINTER(ConvStackConfig)]
         lib.ctb_dvae_blob_floats.restype = i64

@@ -24,7 +24,7 @@ from . import _lib
 from .config import Config
 from .decoder import ENC_NFFT, decode_to_wavs_window, DVAE, Vocos, decode_to_wavs, stream_window
 from .embed import Embed
-from .engine import Job, OpenEngine, check_prefill_budget
+from .engine import Job, OpenEngine, SlotImage, check_prefill_budget
 from .gpt import GPT
 from .norm import Normalizer
 from .processors import gen_logits
@@ -217,7 +217,8 @@ class Chat:
     def infer_continuous(self, texts, params_infer_code=None, use_decoder=True, slots=None, stream=False, lang=None,
                          skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
                          params_refine_text=None, refine_on_engine=False, split_text=False, max_split_batch=1,
-                         dtype=torch.float32, prefill_budget: Optional[int] = None):
+                         dtype=torch.float32, prefill_budget: Optional[int] = None,
+                         kv_pool_bytes: Optional[int] = None):
         """Synthesise many texts with continuous batching: each text is one job on an open slot engine
         (``open_engine``), all queued at once; ``params_infer_code`` is one ``InferCodeParams`` for all texts or a list
         with one per text (speaker, seed, temperature, top-P/K, penalty, token limits).  Generator of ``(index, wav)``
@@ -252,7 +253,11 @@ class Chat:
 
         ``prefill_budget`` (prompt columns per poll, at least 128; default None) bounds the prefill the running texts
         wait for at each poll: a prompt that does not fit, such as one with a long ``spk_smp``, is prefilled in chunks
-        over several polls with the same results (``GPT.generate_continuous``)."""
+        over several polls with the same results (``GPT.generate_continuous``).
+
+        ``kv_pool_bytes`` (default None) bounds the engine's KV memory: slots take pages from a pool of that many bytes
+        as they grow, and a running request the pool cannot cover is suspended to host memory and resumed later with
+        the same results (``GPT.generate_continuous``)."""
         _lib.engine_flags(dtype)  # an unsupported dtype raises here, before any device work
         check_prefill_budget(prefill_budget)
         if stream:
@@ -261,12 +266,13 @@ class Chat:
         texts, params = self._continuous_params(texts, params_infer_code)
         return self._continuous(texts, params, self._refine_params(texts, params_refine_text), False, use_decoder,
                                 slots, lang, skip_refine_text, do_text_normalization, do_homophone_replacement,
-                                refine_on_engine, split_text, max_split_batch, dtype, prefill_budget)
+                                refine_on_engine, split_text, max_split_batch, dtype, prefill_budget, kv_pool_bytes)
 
     def infer_continuous_stream(self, texts, params_infer_code=None, use_decoder=True, slots=None, lang=None,
                                 skip_refine_text=True, do_text_normalization=True, do_homophone_replacement=True,
                                 params_refine_text=None, refine_on_engine=False, split_text=False, max_split_batch=1,
-                                dtype=torch.float32, prefill_budget: Optional[int] = None):
+                                dtype=torch.float32, prefill_budget: Optional[int] = None,
+                                kv_pool_bytes: Optional[int] = None):
         """Streaming synthesis of many texts with continuous batching on an open slot engine.  Generator of ``(index,
         chunk, last)``, ``chunk`` a ``[1, n]`` float32 array; for each text the chunks are those ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=True)`` yields with that
         text's params (its own ``stream_batch``, ``stream_speed`` and ``pass_first_n_batches``), and ``last`` marks
@@ -275,21 +281,21 @@ class Chat:
         buffers.  Arguments as for ``infer_continuous``; with ``refine_on_engine=True`` the chunks are those of
         ``infer([texts[index]], stream=True, split_text=False, skip_refine_text=False)``.  With ``split_text=True``
         each text is a paragraph, streamed sentence by sentence as ``ChatEngine.submit(split_text=True,
-        stream=True)`` streams it, refined first with ``skip_refine_text=False``.  ``dtype`` and ``prefill_budget``
-        as in ``infer_continuous``; a budget leaves the chunks as they are."""
+        stream=True)`` streams it, refined first with ``skip_refine_text=False``.  ``dtype``, ``prefill_budget`` and
+        ``kv_pool_bytes`` as in ``infer_continuous``; neither of the last two changes the chunks."""
         _lib.engine_flags(dtype)
         check_prefill_budget(prefill_budget)
         texts, params = self._continuous_params(texts, params_infer_code)
         return self._continuous(texts, params, self._refine_params(texts, params_refine_text), True, use_decoder,
                                 slots, lang, skip_refine_text, do_text_normalization, do_homophone_replacement,
-                                refine_on_engine, split_text, max_split_batch, dtype, prefill_budget)
+                                refine_on_engine, split_text, max_split_batch, dtype, prefill_budget, kv_pool_bytes)
 
     def refine_continuous(self, texts, params_refine_text=None, slots=None, lang=None, do_text_normalization=True,
-                          do_homophone_replacement=True, dtype=torch.float32):
+                          do_homophone_replacement=True, dtype=torch.float32, kv_pool_bytes: Optional[int] = None):
         """Refine many texts on the slot engine, each as a request of its own: generator of ``(index, refined_text)``
         in completion order.  ``refined_text`` is what ``infer([texts[index]], refine_text_only=True,
         split_text=False, params_refine_text=...)[0]`` returns for that text; ``params_refine_text`` is one
-        ``RefineTextParams`` or one per text.  ``dtype`` as in ``infer_continuous``."""
+        ``RefineTextParams`` or one per text.  ``dtype`` and ``kv_pool_bytes`` as in ``infer_continuous``."""
         _lib.engine_flags(dtype)
         if isinstance(texts, str):
             texts = [texts]
@@ -302,7 +308,7 @@ class Chat:
         texts = [self.normalizer(t, do_text_normalization, do_homophone_replacement, lang) for t in texts]
         requests = [self._refine_request(t, r) for t, r in zip(texts, refine)]
         for i, out in self.gpt.generate_continuous(requests, slots=slots, return_hidden=False, context=self.context,
-                                                   dtype=dtype):
+                                                   dtype=dtype, kv_pool_bytes=kv_pool_bytes):
             yield i, self._refined_text(out)
 
     @staticmethod
@@ -326,7 +332,7 @@ class Chat:
 
     def _continuous(self, texts, params, refine, stream, use_decoder, slots, lang, skip_refine_text,
                     do_text_normalization, do_homophone_replacement, refine_on_engine, split_text, max_split_batch,
-                    dtype, prefill_budget=None):
+                    dtype, prefill_budget=None, kv_pool_bytes=None):
         """``infer_continuous*``: every text one ``ChatEngine`` job on one open engine.  Generator of ``(index, wav)``
         in completion order, or of ``(index, chunk, last)`` as the chunks come.
 
@@ -374,7 +380,8 @@ class Chat:
         out: queue.Queue = queue.Queue()  # (k, (chunk, last)), or (k, None) once text k's job has ended
         with self.gpt._open_slot_engine(ChatEngine, slots, cap, use_decoder, chunk, self, use_decoder,
                                         None if split_text else self.context,
-                                        flags=_lib.engine_flags(dtype), prefill_budget=prefill_budget) as eng:
+                                        flags=_lib.engine_flags(dtype), prefill_budget=prefill_budget,
+                                        kv_pool_bytes=kv_pool_bytes) as eng:
             subs = [eng._job(t, p, stream, skip_refine_text, r, split_text, max_split_batch, normalize, (out, k))
                     for k, (t, p, r) in enumerate(zip(texts, params, refine))]
             eng._enqueue(subs)
@@ -449,7 +456,7 @@ class Chat:
         return self.tokenizer.decode([ids[ids.less(self.tokenizer.break_0_ids)]])[0]
 
     def open_engine(self, slots: Optional[int] = None, max_new_cap: int = 2048, use_decoder: bool = True,
-                    dtype=torch.float32, prefill_budget: Optional[int] = None):
+                    dtype=torch.float32, prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None):
         """A long-lived slot engine (``GPT.open_engine``) that synthesises texts submitted from any thread while it
         decodes: ``engine.submit(text, params_infer_code=None, stream=False, skip_refine_text=True, ...) -> Job``,
         ``Job.cancel()`` for one text, ``close(cancel=False)`` or a ``with`` block to drain it (``close(cancel=True)``
@@ -459,13 +466,15 @@ class Chat:
         ``ChatEngine.submit``.  ``dtype`` as in
         ``infer_continuous``: every stage of every job runs on that engine.  ``prefill_budget`` (prompt columns per
         poll, at least 128; default None) bounds the prefill the running jobs wait for at each poll
-        (``infer_continuous``); a job cancelled while its prompt is in progress frees its slot at the next poll."""
+        (``infer_continuous``); a job cancelled while its prompt is in progress frees its slot at the next poll.
+        ``kv_pool_bytes`` (default None) bounds the engine's KV memory as in ``infer_continuous``; ``submit`` refuses
+        a stage that does not fit in the pool alone."""
         flags = _lib.engine_flags(dtype)
         check_prefill_budget(prefill_budget)
         assert self.has_loaded(use_decoder=use_decoder)
         return self.gpt._open_slot_engine(ChatEngine, self.gpt.max_batch if slots is None else slots, max_new_cap,
                                           use_decoder, None, self, use_decoder, flags=flags,
-                                          prefill_budget=prefill_budget)
+                                          prefill_budget=prefill_budget, kv_pool_bytes=kv_pool_bytes)
 
     def interrupt(self):
         self.context.set(True)
@@ -636,7 +645,8 @@ def _decode_windows(dev, jobs, model: DVAE, use_decoder: bool):
         for k in due:
             _, s, n, a, b = jobs[k][:5]
             a, b, t0, t1 = stream_window(n, a, b)
-            rows.append(buf[s, t0:t1])
+            # an interrupted request that was suspended: its image holds its tokens
+            rows.append((s.row(use_decoder) if isinstance(s, SlotImage) else buf[s])[t0:t1])
             cuts.append((a - 512 * t0, b - 512 * t0))
         wavs = model.engine.decode_rows(rows, 1 if use_decoder else 2)
         flat = torch.cat([w[c0:c1] for w, (c0, c1) in zip(wavs, cuts)]).cpu().numpy()

@@ -14,6 +14,7 @@
 #include "flow.cuh"
 #include "prefill.cuh"
 #include "tc_gemm.cuh"
+#include "kv_pool.cuh"
 
 namespace ctb {
 
@@ -119,6 +120,15 @@ struct ctb_gpt {
   CUtensorMap *m16_wqkv, *m16_wo, *m16_wgu, *m16_wd;
   float* gw16;                // the same rounded values as fp32 in the blob's layer layout: prefill W_hi
   float* pf_wzero;            // prefill W_lo of the rounded weights (exactly zero), as large as the largest matrix
+  // ---- on-demand KV pages (ctb_gpt_engine_begin_paged); pg_pages == 0: the fixed page ranges of kv_reserve
+  int pg_pages;               // pages in the pool, page 0 the zero page
+  bool pg_poison;             // CTB_KV_POISON=1 at begin: free pages hold quiet-NaN bits
+  std::vector<int> pg_free;   // free pages, taken from the back
+  std::vector<int> pg_bt;     // [S][pages_per_row] host copy of the block table
+  // per slot: pages mapped, and the tokens its request may hold after the steps enqueued so far (pg_hi, 0: none) and
+  // at most (pg_cap: prompt + max_new - 1)
+  std::vector<int> pg_map, pg_hi, pg_cap;
+  char* pg_stage;             // KV_STAGE_BYTES of device staging for suspend / resume (allocated by the first one)
 };
 
 static size_t kv_elem_bytes(const ctb_gpt* h) { return (h->prec & CTB_ENGINE_FP16_KV) ? 2 : 4; }
@@ -481,7 +491,8 @@ extern "C" int ctb_gpt_destroy(ctb_gpt* h) {
                   h->pos, h->counter, h->end_idx, h->idx, h->active, h->finish, h->st, h->tc_wqkv, h->tc_wgu,
                   h->tc_heads_code, h->tc_heads_text, h->x_hi, h->x_lo, h->attn_hi, h->attn_lo, h->h_hi, h->h_lo, h->bar, h->trace, h->flow_arena, h->flow_epoch, h->gw_hi, h->gw_lo, h->pf_resid, h->pf_xn, h->pf_qkv, h->pf_q,
                   h->pf_attn, h->pf_gu, h->pf_h, h->pf_ones, h->pf_zeros, h->pf_npre, h->pf_nvalid,
-                  h->pf_mask, h->rows, h->cfgs, h->eng_noise, h->eng_slot, h->eng_text_logits, h->eng_text_idx};
+                  h->pf_mask, h->rows, h->cfgs, h->eng_noise, h->eng_slot, h->eng_text_logits, h->eng_text_idx,
+                  h->pg_stage};
   delete[] h->m_wqkv; delete[] h->m_wo; delete[] h->m_wgu; delete[] h->m_wd;
   for (void* p : ptrs) if (p) cudaFree(p);
   fp16_free(h);
@@ -1183,7 +1194,7 @@ extern "C" int ctb_gpt_begin(ctb_gpt* h, int32_t B, int32_t T0, const float* emb
   if ((rc = check_sampler(*sampler))) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   h->B = B; h->T0 = T0; h->max_new = max_new_token; h->infer_text = infer_text ? 1 : 0;
-  h->engine = 0; h->phase = RS_RUNNING; h->prec = 0;
+  h->engine = 0; h->phase = RS_RUNNING; h->prec = 0; h->pg_pages = 0;
   h->use_tc = h->tc_ready && B >= h->tc_min_batch;
   h->sampler = *sampler; h->q_noise = q_noise_dev; h->emb = emb_dev; h->mask = mask_dev;
   h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev;
@@ -1221,6 +1232,14 @@ extern "C" int ctb_gpt_decode(ctb_gpt* h, int32_t n_steps, void* stream) {
   // (a slot engine's rows stop at their own max_new, checked against both at admission)
   if (!h->engine) n_steps = std::min(n_steps, h->max_new - h->steps_enqueued);
   if (n_steps <= 0) return CTB_OK;
+  if (h->pg_pages) {  // a paged engine: every slot that may run must hold the positions these steps append
+    for (int b = 0; b < h->B; ++b)
+      if (h->pg_hi[b] && h->pg_map[b] * kPageTokens < std::min(h->pg_hi[b] + n_steps, h->pg_cap[b]))
+        return set_err(CTB_ERR_STATE, "slot %d: its pages hold %d positions, %d decode steps may need %d", b,
+                       h->pg_map[b] * kPageTokens, n_steps, std::min(h->pg_hi[b] + n_steps, h->pg_cap[b]));
+    for (int b = 0; b < h->B; ++b)
+      if (h->pg_hi[b]) h->pg_hi[b] = std::min(h->pg_hi[b] + n_steps, h->pg_cap[b]);
+  }
   h->steps_enqueued += n_steps;
   if (flow_ink(h)) {
     // the whole loop body (step, sampling tail, finish bookkeeping) is inside k_flow: many iterations per launch
@@ -1267,8 +1286,11 @@ extern "C" int ctb_gpt_engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, 
 
 static_assert((int)TD_W16 == CTB_ENGINE_FP16_WEIGHTS && (int)TD_KV16 == CTB_ENGINE_FP16_KV, "precision bits");
 
-extern "C" int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t flags, int32_t* ids_out_dev,
-                                       float* hiddens_out_dev, void* stream) {
+static int kv_pool_paged(ctb_gpt* h, int S, int pool_pages, cudaStream_t s);
+
+// ctb_gpt_engine_begin_ex (pool_pages == 0) and ctb_gpt_engine_begin_paged
+static int engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t flags, int32_t pool_pages,
+                        int32_t* ids_out_dev, float* hiddens_out_dev, void* stream) {
   if (!h || !ids_out_dev) return set_err(CTB_ERR_ARG, "null argument");
   const ctb_gpt_config& c = h->cfg;
   if (S < 2 || S > c.max_batch) return set_err(CTB_ERR_ARG, "S=%d outside [2,%d]", S, c.max_batch);
@@ -1305,8 +1327,10 @@ extern "C" int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_ca
   h->B = S; h->T0 = 0; h->max_new = max_new_cap; h->infer_text = 0;
   h->use_tc = use_tc;
   h->q_noise = h->eng_noise; h->emb = nullptr; h->mask = nullptr;
-  h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev; h->eng_text = 0;
-  if ((rc = restart_decode(h, s)) || (rc = kv_reserve(h, S, c.max_context, s))) return rc;
+  h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev; h->eng_text = 0; h->pg_pages = 0;
+  if ((rc = restart_decode(h, s)) ||
+      (rc = pool_pages ? kv_pool_paged(h, S, pool_pages, s) : kv_reserve(h, S, c.max_context, s)))
+    return rc;
   static const LoopState idle_state = {0, 1, 0, 0, 0};  // no running slot: decode steps are no-ops
   CTB_CUDA(cudaMemcpyAsync(h->st, &idle_state, sizeof(LoopState), cudaMemcpyHostToDevice, s));
   CTB_CUDA(cudaMemsetAsync(h->rows, 0, sizeof(RowState) * h->bpad_max, s));  // every slot RS_IDLE
@@ -1325,6 +1349,11 @@ extern "C" int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_ca
   return CTB_OK;
 }
 
+extern "C" int ctb_gpt_engine_begin_ex(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t flags, int32_t* ids_out_dev,
+                                       float* hiddens_out_dev, void* stream) {
+  return engine_begin(h, S, max_new_cap, flags, 0, ids_out_dev, hiddens_out_dev, stream);
+}
+
 // Admit n requests into `slots` (host): prefill columns [q0, T0) of their prompts - whole prompts (q0 = 0) with
 // `mask`, or the final chunk of one slot's prompt (mask == nullptr) - and sample their first tokens.  Every slot is
 // validated before anything is written, so a refused call leaves the handle as it was; the host arrays are copied
@@ -1337,7 +1366,14 @@ static int admit(ctb_gpt* h, int n, const int32_t* slots, int T0, int q0, const 
   int rc;
   std::vector<RowState> rows((size_t)h->bpad_max);
   CTB_CUDA(cudaMemcpyAsync(rows.data(), h->rows, sizeof(RowState) * rows.size(), cudaMemcpyDeviceToHost, s));
+  std::vector<uint8_t> mask_h;  // a paged engine counts the positions each whole prompt writes
+  if (h->pg_pages && mask_dev) {
+    mask_h.resize((size_t)n * T0);
+    CTB_CUDA(cudaMemcpyAsync(mask_h.data(), mask_dev, mask_h.size(), cudaMemcpyDeviceToHost, s));
+  }
   CTB_CUDA(cudaStreamSynchronize(s));
+  std::vector<int> held((size_t)n, T0);  // positions [0, held[i]) of slot slots[i] after the prefill
+  for (size_t j = 0; j < mask_h.size(); ++j) held[j / T0] -= mask_h[j] == 0;
   std::vector<char> taken((size_t)S, 0);
   for (int i = 0; i < n; ++i) {
     const int b = slots[i];
@@ -1350,11 +1386,16 @@ static int admit(ctb_gpt* h, int n, const int32_t* slots, int T0, int q0, const 
       return set_err(CTB_ERR_ARG, "slot %d: max_new=%d (capacity %d) with T0=%d exceeds max_context=%d", b, max_new[i],
                      h->max_new, T0, c.max_context);
     if ((rc = check_sampler(sc))) return rc;
+    if (h->pg_pages && h->pg_map[b] * kPageTokens < held[i])
+      return set_err(CTB_ERR_STATE, "slot %d: its pages hold %d positions, the prompt writes %d", b,
+                     h->pg_map[b] * kPageTokens, held[i]);
     RowState& r = rows[b];
     r.n_gen = 0; r.step = 0; r.state = RS_PENDING; r.max_new = max_new[i]; r.has_noise = q_noise_dev != nullptr;
     r.eos = sc.eos_token; r.text = text;
   }
   for (int i = 0; i < n; ++i) h->chunk_T0[slots[i]] = 0;  // the slot's prompt in progress, if any, is dropped
+  if (h->pg_pages)
+    for (int i = 0; i < n; ++i) { h->pg_hi[slots[i]] = held[i]; h->pg_cap[slots[i]] = held[i] + max_new[i] - 1; }
   CTB_CUDA(cudaMemcpyAsync(h->rows, rows.data(), sizeof(RowState) * rows.size(), cudaMemcpyHostToDevice, s));
   CTB_CUDA(cudaMemcpyAsync(h->eng_slot, slots, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
   const size_t nrow = text ? (size_t)c.num_text_tokens : (size_t)c.num_vq * c.num_audio_tokens;
@@ -1438,6 +1479,9 @@ extern "C" int ctb_gpt_engine_prefill_chunk(ctb_gpt* h, int32_t slot, int32_t T0
   CTB_CUDA(cudaMemcpyAsync(&r, h->rows + slot, sizeof(RowState), cudaMemcpyDeviceToHost, s));
   CTB_CUDA(cudaStreamSynchronize(s));
   if (r.state == RS_RUNNING || r.state == RS_PENDING) return set_err(CTB_ERR_STATE, "slot %d is still generating", slot);
+  if (h->pg_pages && h->pg_map[slot] * kPageTokens < c0 + n)
+    return set_err(CTB_ERR_STATE, "slot %d: its pages hold %d positions, the chunk writes up to %d", slot,
+                   h->pg_map[slot] * kPageTokens, c0 + n);
   if ((rc = prefill(h, 1, T0, c0, n, emb_dev, nullptr, &slot, s))) { h->chunk_T0[slot] = 0; return rc; }
   h->chunk_T0[slot] = T0; h->chunk_done[slot] = c0 + n;
   return CTB_OK;
@@ -1454,6 +1498,9 @@ extern "C" int ctb_gpt_engine_status(ctb_gpt* h, ctb_gpt_status* out, int32_t* s
   if (rc) return rc;
   if (state_host)
     for (int b = 0; b < h->B; ++b) state_host[b] = rows[b].state;
+  if (h->pg_pages)  // a slot seen idle or finished appends nothing until its next admission
+    for (int b = 0; b < h->B; ++b)
+      if (rows[b].state != RS_RUNNING && rows[b].state != RS_PENDING) h->pg_hi[b] = 0;
   if (h->eng_text) {  // the stream is synchronised: the rows are current
     h->eng_text = 0;
     for (int b = 0; b < h->B; ++b)
@@ -1480,6 +1527,348 @@ extern "C" int ctb_gpt_engine_cancel(ctb_gpt* h, int32_t n, const int32_t* slots
   // h->eng_text stays as it is: the next ctb_gpt_engine_status recomputes it from the rows
   k_cancel_rows<<<1, 256, 0, (cudaStream_t)stream>>>(p);
   CTB_LAUNCH_CHECK();
+  return CTB_OK;
+}
+
+// ------------------------------------------------------------------ KV pages on demand (ctb_gpt_engine_begin_paged)
+static_assert(sizeof(RowState) == 8 * sizeof(int32_t), "ctb_slot_image.row");
+
+static size_t page_elems(const ctb_gpt* h) { return (size_t)2 * h->cfg.num_kv_heads * kPageTokens * h->cfg.head_dim; }
+static size_t page_bytes(const ctb_gpt* h) { return page_elems(h) * kv_elem_bytes(h); }  // one page of one layer
+static unsigned move_blocks(size_t words) { return (unsigned)std::min<size_t>((words + 255) / 256, (size_t)g_num_sms * 8); }
+
+// the poison pattern (quiet NaN of the cache's element type) into n pages of every layer: list[0..n), or p0 .. p0 + n - 1
+static int kv_poison(ctb_gpt* h, const int* list, int p0, int n, cudaStream_t s) {
+  KvFillP p{};
+  p.kv = reinterpret_cast<char*>(h->kv); p.layer_bytes = h->kv_layer_elems * kv_elem_bytes(h);
+  p.page_bytes = page_bytes(h); p.layers = h->cfg.num_layers; p.p0 = p0; p.use_list = list != nullptr;
+  p.word = (h->prec & CTB_ENGINE_FP16_KV) ? 0x7e007e00u : 0x7fc00000u;
+  for (int k = 0; k < n; k += KV_BT_MAX) {
+    p.n = std::min(KV_BT_MAX, n - k);
+    if (list) std::copy(list + k, list + k + p.n, p.list);
+    else p.p0 = p0 + k;
+    k_kv_fill<<<move_blocks((size_t)p.layers * p.n * p.page_bytes / 16), 256, 0, s>>>(p);
+    CTB_LAUNCH_CHECK();
+  }
+  return CTB_OK;
+}
+
+// block-table entries (index into [S][pages_per_row], page), KV_BT_MAX per launch
+static int bt_write(ctb_gpt* h, const std::vector<std::pair<int, int>>& e, cudaStream_t s) {
+  BtWriteP p{};
+  p.bt = h->block_table;
+  for (size_t k = 0; k < e.size(); k += KV_BT_MAX) {
+    p.n = (int)std::min<size_t>(KV_BT_MAX, e.size() - k);
+    for (int j = 0; j < p.n; ++j) { p.idx[j] = e[k + j].first; p.page[j] = e[k + j].second; }
+    k_bt_write<<<1, 256, 0, s>>>(p);
+    CTB_LAUNCH_CHECK();
+  }
+  return CTB_OK;
+}
+
+// A pool of exactly pool_pages pages, zeroed (poisoned past the zero page with CTB_KV_POISON=1), every entry of the S
+// slots' block table on the zero page and every other page free
+static int kv_pool_paged(ctb_gpt* h, int S, int pool_pages, cudaStream_t s) {
+  const ctb_gpt_config& c = h->cfg;
+  const size_t bytes = (size_t)pool_pages * page_bytes(h) * c.num_layers;
+  if (bytes != h->kv_bytes) {
+    CTB_CUDA(cudaStreamSynchronize(s));
+    if (h->kv) { cudaFree(h->kv); h->kv = nullptr; h->kv_bytes = 0; }
+    if (cudaMalloc(reinterpret_cast<void**>(&h->kv), bytes) != cudaSuccess) {
+      cudaGetLastError();
+      return set_err(CTB_ERR_NOMEM, "KV pool: %d pages x %d layers (%.2f GB) do not fit", pool_pages, c.num_layers,
+                     (double)bytes / 1e9);
+    }
+    h->kv_bytes = bytes;
+  }
+  h->kv_layer_elems = (size_t)pool_pages * page_elems(h);
+  h->bt_B = 0;  // kv_reserve uploads its table again
+  CTB_CUDA(cudaMemsetAsync(h->kv, 0, bytes, s));
+  const char* poison = getenv("CTB_KV_POISON");
+  h->pg_poison = poison != nullptr && atoi(poison) == 1;
+  int rc;
+  if (h->pg_poison && (rc = kv_poison(h, nullptr, 1, pool_pages - 1, s))) return rc;
+  CTB_CUDA(cudaMemsetAsync(h->block_table, 0, sizeof(int) * (size_t)S * h->pages_per_row, s));
+  h->pg_free.clear();
+  for (int p = pool_pages - 1; p >= 1; --p) h->pg_free.push_back(p);
+  h->pg_bt.assign((size_t)S * h->pages_per_row, 0);
+  h->pg_map.assign((size_t)S, 0); h->pg_hi.assign((size_t)S, 0); h->pg_cap.assign((size_t)S, 0);
+  h->pg_pages = pool_pages;
+  return CTB_OK;
+}
+
+extern "C" int ctb_gpt_engine_begin_paged(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t flags, int32_t pool_pages,
+                                          int32_t* ids_out_dev, float* hiddens_out_dev, void* stream) {
+  if (!h) return set_err(CTB_ERR_ARG, "null argument");
+  if (pool_pages < 2) return set_err(CTB_ERR_ARG, "pool_pages=%d: the zero page and at least one more", pool_pages);
+  if (h->pages_per_row > KV_MOVE_MAX_PAGES)
+    return set_err(CTB_ERR_ARG, "max_context=%d: a paged engine serves up to %d tokens per slot", h->cfg.max_context,
+                   KV_MOVE_MAX_PAGES * kPageTokens);
+  return engine_begin(h, S, max_new_cap, flags, pool_pages, ids_out_dev, hiddens_out_dev, stream);
+}
+
+static int check_paged(const ctb_gpt* h) {
+  if (!h->engine || !h->pg_pages) return set_err(CTB_ERR_STATE, "not a paged slot engine (ctb_gpt_engine_begin_paged)");
+  return CTB_OK;
+}
+
+static int check_slot_list(const ctb_gpt* h, int n, const int32_t* slots) {
+  if (n < 1 || n > h->B) return set_err(CTB_ERR_ARG, "n=%d outside [1,%d]", n, h->B);
+  std::vector<char> seen((size_t)h->B, 0);
+  for (int i = 0; i < n; ++i) {
+    if (slots[i] < 0 || slots[i] >= h->B || seen[slots[i]])
+      return set_err(CTB_ERR_ARG, "slot %d out of range or repeated", slots[i]);
+    seen[slots[i]] = 1;
+  }
+  return CTB_OK;
+}
+
+extern "C" int ctb_gpt_engine_reserve(ctb_gpt* h, int32_t n, const int32_t* slots, const int32_t* tokens, void* stream) {
+  if (!h || !slots || !tokens) return set_err(CTB_ERR_ARG, "null argument");
+  int rc;
+  if ((rc = check_paged(h)) || (rc = check_slot_list(h, n, slots))) return rc;
+  size_t need = 0;
+  for (int i = 0; i < n; ++i) {
+    if (tokens[i] < 0 || tokens[i] > h->cfg.max_context)
+      return set_err(CTB_ERR_ARG, "slot %d: tokens=%d outside [0,%d]", slots[i], tokens[i], h->cfg.max_context);
+    need += (size_t)std::max(0, (tokens[i] + kPageTokens - 1) / kPageTokens - h->pg_map[slots[i]]);
+  }
+  if (need > h->pg_free.size())
+    return set_err(CTB_ERR_POOL, "KV pool: %zu more pages needed, %zu of %d free", need, h->pg_free.size(),
+                   h->pg_pages - 1);
+  std::vector<std::pair<int, int>> e;
+  for (int i = 0; i < n; ++i) {
+    const int b = slots[i], want = (tokens[i] + kPageTokens - 1) / kPageTokens;
+    for (int k = h->pg_map[b]; k < want; ++k) {
+      const int idx = b * h->pages_per_row + k, page = h->pg_free.back();
+      h->pg_free.pop_back();
+      h->pg_bt[idx] = page;
+      e.emplace_back(idx, page);
+    }
+    h->pg_map[b] = std::max(h->pg_map[b], want);
+  }
+  return bt_write(h, e, (cudaStream_t)stream);
+}
+
+// slot b's pages back to the free list (taken again in the order they had), its entries on the zero page
+static int release_pages(ctb_gpt* h, int b, cudaStream_t s) {
+  std::vector<std::pair<int, int>> e;
+  std::vector<int> freed;
+  for (int k = 0; k < h->pg_map[b]; ++k) {
+    const int idx = b * h->pages_per_row + k;
+    freed.push_back(h->pg_bt[idx]);
+    h->pg_bt[idx] = 0;
+    e.emplace_back(idx, 0);
+  }
+  h->pg_free.insert(h->pg_free.end(), freed.rbegin(), freed.rend());
+  h->pg_map[b] = h->pg_hi[b] = h->pg_cap[b] = 0;
+  int rc;
+  if ((rc = bt_write(h, e, s))) return rc;
+  return h->pg_poison ? kv_poison(h, freed.data(), 0, (int)freed.size(), s) : CTB_OK;
+}
+
+extern "C" int ctb_gpt_engine_release(ctb_gpt* h, int32_t n, const int32_t* slots, void* stream) {
+  if (!h || !slots) return set_err(CTB_ERR_ARG, "null argument");
+  int rc;
+  if ((rc = check_paged(h)) || (rc = check_slot_list(h, n, slots))) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  std::vector<RowState> rows((size_t)h->B);
+  CTB_CUDA(cudaMemcpyAsync(rows.data(), h->rows, sizeof(RowState) * h->B, cudaMemcpyDeviceToHost, s));
+  CTB_CUDA(cudaStreamSynchronize(s));
+  for (int i = 0; i < n; ++i) {
+    const int b = slots[i];
+    if (rows[b].state == RS_RUNNING || rows[b].state == RS_PENDING)
+      return set_err(CTB_ERR_STATE, "slot %d is still generating: its pages stay", b);
+    if (h->chunk_T0[b]) return set_err(CTB_ERR_STATE, "slot %d has a prompt in progress: its pages stay", b);
+  }
+  for (int i = 0; i < n; ++i)
+    if ((rc = release_pages(h, slots[i], s))) return rc;
+  return CTB_OK;
+}
+
+// the sections of an image of n_gen tokens and seq_len positions on this engine, each 256-byte aligned
+static void image_layout(const ctb_gpt* h, int n_gen, int seq_len, ctb_slot_image* img) {
+  const ctb_gpt_config& c = h->cfg;
+  auto up = [](uint64_t x) { return (x + 255) & ~(uint64_t)255; };
+  img->magic = CTB_SLOT_IMAGE_MAGIC; img->prec = h->prec; img->n_gen = n_gen; img->seq_len = seq_len;
+  img->npages = (seq_len + kPageTokens - 1) / kPageTokens; img->page_bytes = (int32_t)page_bytes(h);
+  img->num_vq = c.num_vq; img->hidden_size = c.hidden_size; img->noise_floats = (int32_t)noise_stride(h);
+  img->has_hidden = h->hiddens_out != nullptr;
+  img->off_noise = up(sizeof(ctb_slot_image));
+  img->off_ids = up(img->off_noise + (uint64_t)img->noise_floats * sizeof(float));
+  img->off_hiddens = up(img->off_ids + (uint64_t)n_gen * c.num_vq * sizeof(int32_t));
+  img->off_kv = up(img->off_hiddens + (img->has_hidden ? (uint64_t)n_gen * c.hidden_size * sizeof(float) : 0));
+  img->bytes = img->off_kv + (uint64_t)c.num_layers * img->npages * img->page_bytes;
+}
+
+// slot's loop state and counters (synchronises s)
+static int read_slot(ctb_gpt* h, int slot, ctb_slot_image* img, cudaStream_t s) {
+  uint8_t fin = 0;
+  CTB_CUDA(cudaMemcpyAsync(img->row, h->rows + slot, sizeof(RowState), cudaMemcpyDeviceToHost, s));
+  CTB_CUDA(cudaMemcpyAsync(&img->seq_len, h->seq_len + slot, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CTB_CUDA(cudaMemcpyAsync(&img->pos, h->pos + slot, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CTB_CUDA(cudaMemcpyAsync(&img->end_idx, h->end_idx + slot, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CTB_CUDA(cudaMemcpyAsync(&fin, h->finish + slot, 1, cudaMemcpyDeviceToHost, s));
+  CTB_CUDA(cudaStreamSynchronize(s));
+  img->finish = fin;
+  return CTB_OK;
+}
+
+// CTB_ERR_ARG unless host_buf is pinned host memory (the copies through it are asynchronous)
+static int check_pinned(const void* host_buf) {
+  void* p = nullptr;
+  if (cudaHostGetDevicePointer(&p, const_cast<void*>(host_buf), 0) != cudaSuccess) {
+    cudaGetLastError();
+    return set_err(CTB_ERR_ARG, "the image buffer is not pinned host memory");
+  }
+  return CTB_OK;
+}
+
+static int check_slot(const ctb_gpt* h, int slot) {
+  if (slot < 0 || slot >= h->B) return set_err(CTB_ERR_ARG, "slot %d outside [0,%d)", slot, h->B);
+  if (h->chunk_T0[slot]) return set_err(CTB_ERR_STATE, "slot %d has a prompt in progress", slot);
+  return CTB_OK;
+}
+
+static int launch_set_row(ctb_gpt* h, int slot, const RowState& r, cudaStream_t s) {
+  SetRowP p{};
+  p.st = h->st; p.rows = h->rows; p.B = h->B; p.b = slot; p.row = r;
+  k_set_row<<<1, 256, 0, s>>>(p);
+  CTB_LAUNCH_CHECK();
+  return CTB_OK;
+}
+
+// A slot's KV pages <-> the image's KV section in pinned host memory, through the device staging buffer: as many
+// image pages as it holds at a time, k_kv_pack into it and one cudaMemcpyAsync out (or one copy in and k_kv_unpack).
+// Measured on an H100 (DESIGN.md §4): resumes this way took 25-30 % less time than k_kv_unpack reading mapped pinned
+// memory directly, and one copy out of the staging buffer runs at about 40 GB/s.
+static int kv_move(ctb_gpt* h, int slot, char* img, int npages, bool pack, cudaStream_t s) {
+  if (npages == 0) return CTB_OK;
+  int rc;
+  if (!h->pg_stage && (rc = dalloc(&h->pg_stage, KV_STAGE_BYTES))) return rc;
+  KvMoveP p{};
+  p.kv = reinterpret_cast<char*>(h->kv); p.img = reinterpret_cast<uint4*>(h->pg_stage);
+  p.layer_bytes = h->kv_layer_elems * kv_elem_bytes(h); p.page_words = (int)(page_bytes(h) / 16);
+  p.layers = h->cfg.num_layers; p.npages = npages;
+  for (int i = 0; i < npages; ++i) p.pages[i] = h->pg_bt[(size_t)slot * h->pages_per_row + i];
+  const size_t pb = page_bytes(h);
+  const int per = (int)(KV_STAGE_BYTES / pb), total = p.layers * npages;
+  for (p.pg0 = 0; p.pg0 < total; p.pg0 = p.pg1) {
+    p.pg1 = std::min(total, p.pg0 + per);
+    const size_t bytes = (size_t)(p.pg1 - p.pg0) * pb;
+    char* hp = img + (size_t)p.pg0 * pb;
+    const unsigned grid = (unsigned)std::min(p.pg1 - p.pg0, g_num_sms * 4);
+    if (pack) {
+      k_kv_pack<<<grid, 256, 0, s>>>(p);
+      CTB_LAUNCH_CHECK();
+      CTB_CUDA(cudaMemcpyAsync(hp, h->pg_stage, bytes, cudaMemcpyDeviceToHost, s));
+    } else {
+      CTB_CUDA(cudaMemcpyAsync(h->pg_stage, hp, bytes, cudaMemcpyHostToDevice, s));
+      k_kv_unpack<<<grid, 256, 0, s>>>(p);
+      CTB_LAUNCH_CHECK();
+    }
+  }
+  return CTB_OK;
+}
+
+// the running slot's state (synchronises s) and its image's layout
+static int running_image(ctb_gpt* h, int slot, ctb_slot_image* img, cudaStream_t s) {
+  int rc;
+  if ((rc = check_paged(h)) || (rc = check_slot(h, slot)) || (rc = read_slot(h, slot, img, s))) return rc;
+  RowState r;
+  memcpy(&r, img->row, sizeof(r));
+  if (r.state != RS_RUNNING) return set_err(CTB_ERR_STATE, "slot %d is not running (state %d)", slot, r.state);
+  image_layout(h, r.n_gen, img->seq_len, img);
+  if (img->npages > h->pg_map[slot])
+    return set_err(CTB_ERR_STATE, "slot %d holds %d positions on %d pages", slot, img->seq_len, h->pg_map[slot]);
+  return CTB_OK;
+}
+
+extern "C" int ctb_gpt_engine_suspend_bytes(ctb_gpt* h, int32_t slot, uint64_t* bytes, void* stream) {
+  if (!h || !bytes) return set_err(CTB_ERR_ARG, "null argument");
+  ctb_slot_image img{};
+  int rc;
+  if ((rc = running_image(h, slot, &img, (cudaStream_t)stream))) return rc;
+  *bytes = img.bytes;
+  return CTB_OK;
+}
+
+extern "C" int ctb_gpt_engine_suspend(ctb_gpt* h, int32_t slot, void* host_buf, uint64_t host_bytes, void* stream) {
+  if (!h || !host_buf) return set_err(CTB_ERR_ARG, "null argument");
+  cudaStream_t s = (cudaStream_t)stream;
+  const ctb_gpt_config& c = h->cfg;
+  ctb_slot_image img{};
+  int rc;
+  if ((rc = running_image(h, slot, &img, s)) || (rc = check_pinned(host_buf))) return rc;
+  if (host_bytes < img.bytes)
+    return set_err(CTB_ERR_ARG, "image buffer of %llu bytes, slot %d needs %llu", (unsigned long long)host_bytes, slot,
+                   (unsigned long long)img.bytes);
+  char* hb = static_cast<char*>(host_buf);
+  memcpy(hb, &img, sizeof(img));  // the header; the device fills in the sampler and the sections
+  const int n_gen = img.n_gen;
+  CTB_CUDA(cudaMemcpyAsync(hb + offsetof(ctb_slot_image, sampler), h->cfgs + slot, sizeof(ctb_sampler_config),
+                           cudaMemcpyDeviceToHost, s));
+  CTB_CUDA(cudaMemcpyAsync(hb + img.off_noise, h->eng_noise + slot * noise_stride(h), img.noise_floats * sizeof(float),
+                           cudaMemcpyDeviceToHost, s));
+  CTB_CUDA(cudaMemcpyAsync(hb + img.off_ids, h->ids_out + (size_t)slot * h->max_new * c.num_vq,
+                           (size_t)n_gen * c.num_vq * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  if (img.has_hidden)
+    CTB_CUDA(cudaMemcpyAsync(hb + img.off_hiddens, h->hiddens_out + (size_t)slot * h->max_new * c.hidden_size,
+                             (size_t)n_gen * c.hidden_size * sizeof(float), cudaMemcpyDeviceToHost, s));
+  if ((rc = kv_move(h, slot, hb + img.off_kv, img.npages, true, s)) || (rc = release_pages(h, slot, s)))
+    return rc;
+  return launch_set_row(h, slot, RowState{}, s);  // RS_IDLE
+}
+
+extern "C" int ctb_gpt_engine_resume(ctb_gpt* h, int32_t slot, const void* host_buf, uint64_t host_bytes, void* stream) {
+  if (!h || !host_buf) return set_err(CTB_ERR_ARG, "null argument");
+  cudaStream_t s = (cudaStream_t)stream;
+  const ctb_gpt_config& c = h->cfg;
+  int rc;
+  if ((rc = check_paged(h)) || (rc = check_slot(h, slot)) || (rc = check_pinned(host_buf))) return rc;
+  if (host_bytes < sizeof(ctb_slot_image)) return set_err(CTB_ERR_ARG, "image buffer of %llu bytes", (unsigned long long)host_bytes);
+  const ctb_slot_image* img = static_cast<const ctb_slot_image*>(host_buf);
+  RowState r;
+  memcpy(&r, img->row, sizeof(r));
+  ctb_slot_image want{};
+  image_layout(h, img->n_gen, img->seq_len, &want);
+  if (img->magic != want.magic || img->prec != want.prec || img->page_bytes != want.page_bytes ||
+      img->num_vq != want.num_vq || img->hidden_size != want.hidden_size || img->noise_floats != want.noise_floats ||
+      img->has_hidden != want.has_hidden || img->npages != want.npages || img->off_noise != want.off_noise ||
+      img->off_ids != want.off_ids || img->off_hiddens != want.off_hiddens || img->off_kv != want.off_kv ||
+      img->bytes != want.bytes || img->n_gen < 1 || img->seq_len < 1 || r.state != RS_RUNNING ||
+      r.n_gen != img->n_gen || r.max_new > h->max_new)
+    return set_err(CTB_ERR_ARG, "the buffer holds no slot image of this engine");
+  if (host_bytes < img->bytes)
+    return set_err(CTB_ERR_ARG, "image buffer of %llu bytes, the image has %llu", (unsigned long long)host_bytes,
+                   (unsigned long long)img->bytes);
+  if (img->npages > h->pg_map[slot])
+    return set_err(CTB_ERR_STATE, "slot %d: its pages hold %d positions, the image %d", slot,
+                   h->pg_map[slot] * kPageTokens, img->seq_len);
+  RowState cur;
+  CTB_CUDA(cudaMemcpyAsync(&cur, h->rows + slot, sizeof(RowState), cudaMemcpyDeviceToHost, s));
+  CTB_CUDA(cudaStreamSynchronize(s));
+  if (cur.state == RS_RUNNING || cur.state == RS_PENDING) return set_err(CTB_ERR_STATE, "slot %d is still generating", slot);
+  const char* hb = static_cast<const char*>(host_buf);
+  const int n_gen = img->n_gen;
+  CTB_CUDA(cudaMemcpyAsync(h->cfgs + slot, &img->sampler, sizeof(ctb_sampler_config), cudaMemcpyHostToDevice, s));
+  CTB_CUDA(cudaMemcpyAsync(h->eng_noise + slot * noise_stride(h), hb + img->off_noise, img->noise_floats * sizeof(float),
+                           cudaMemcpyHostToDevice, s));
+  CTB_CUDA(cudaMemcpyAsync(h->ids_out + (size_t)slot * h->max_new * c.num_vq, hb + img->off_ids,
+                           (size_t)n_gen * c.num_vq * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  if (img->has_hidden)
+    CTB_CUDA(cudaMemcpyAsync(h->hiddens_out + (size_t)slot * h->max_new * c.hidden_size, hb + img->off_hiddens,
+                             (size_t)n_gen * c.hidden_size * sizeof(float), cudaMemcpyHostToDevice, s));
+  CTB_CUDA(cudaMemcpyAsync(h->seq_len + slot, &img->seq_len, sizeof(int), cudaMemcpyHostToDevice, s));
+  CTB_CUDA(cudaMemcpyAsync(h->pos + slot, &img->pos, sizeof(int), cudaMemcpyHostToDevice, s));
+  CTB_CUDA(cudaMemcpyAsync(h->end_idx + slot, &img->end_idx, sizeof(int), cudaMemcpyHostToDevice, s));
+  CTB_CUDA(cudaMemsetAsync(h->finish + slot, img->finish ? 1 : 0, 1, s));
+  if ((rc = kv_move(h, slot, const_cast<char*>(hb) + img->off_kv, img->npages, false, s)) ||
+      (rc = launch_set_row(h, slot, r, s)))
+    return rc;
+  h->pg_hi[slot] = img->seq_len;
+  h->pg_cap[slot] = img->seq_len + r.max_new - r.n_gen;
+  if (r.text) h->eng_text = 1;
   return CTB_OK;
 }
 

@@ -14,13 +14,19 @@ The scheduling policy (``schedule``) is plain Python over a small device interfa
 An opt-in prefill budget (``prefill_budget``, prompt columns per poll) bounds the prefill work the running slots wait
 for at each poll: a prompt that does not fit is prefilled in chunks over several polls (``ctb_gpt_engine_prefill_chunk``),
 with the same bits as one admission of it.
+
+An opt-in KV pool (``kv_pool_bytes``) bounds the engine's KV memory: slots take 16-token pages from a shared pool as
+they grow, and when the pool runs short a running request is suspended to host memory and later resumed, in any
+slot, bit for bit as if it had never moved (``_poll_cycles`` has the policy).
 """
 from __future__ import annotations
 
 import ctypes as C
+import itertools
 import logging
 import queue
 import threading
+import weakref
 from collections import deque
 from concurrent.futures import Future
 from dataclasses import dataclass, field
@@ -80,6 +86,26 @@ def check_prefill_budget(budget: Optional[int]) -> Optional[int]:
     if int(budget) != budget or int(budget) < PREFILL_CHUNK_ALIGN:
         raise ValueError(f"prefill_budget={budget!r}: an int of at least {PREFILL_CHUNK_ALIGN} prompt columns, or None")
     return int(budget)
+
+
+def kv_pool_pages(gpt_config, kv_pool_bytes: Optional[int], flags: int) -> Optional[int]:
+    """The pages (16 tokens of K and V of every layer; page 0 is the zero page) a pool of ``kv_pool_bytes`` holds on an
+    engine of precision ``flags``, or None for None.  ValueError when it holds fewer than two."""
+    if kv_pool_bytes is None:
+        return None
+    c = gpt_config
+    elem = 2 if flags & _lib.ENGINE_FP16_KV else 4
+    page = 2 * c.num_key_value_heads * _lib.PAGE_TOKENS * c.head_dim * elem
+    pages = int(kv_pool_bytes) // (page * c.num_hidden_layers)
+    if int(kv_pool_bytes) != kv_pool_bytes or pages < 2:
+        raise ValueError(f"kv_pool_bytes={kv_pool_bytes!r}: an int of at least two pages "
+                         f"({2 * page * c.num_hidden_layers} bytes), or None")
+    return pages
+
+
+def pool_pages_needed(r: "Request") -> int:
+    """Pages request ``r`` holds at most on a paged engine: its prompt plus ``max_new_token`` positions."""
+    return -(-(int(r.emb.shape[0]) + r.max_new_token) // _lib.PAGE_TOKENS)
 
 
 def admission_groups(group: list, requests: Sequence["Request"], max_context: int) -> List[Tuple[list, int]]:
@@ -225,6 +251,13 @@ class ScheduleStats:
     # chunks), and the number of prompt chunks issued
     prefill_cols: List[int] = field(default_factory=list)
     chunks: int = 0
+    # with a KV pool: pages mapped at each poll (as its decode chunk starts), their peak, requests suspended and
+    # resumed, and host bytes their images held at each poll
+    pages: List[int] = field(default_factory=list)
+    peak_pages: int = 0
+    suspensions: int = 0
+    resumes: int = 0
+    host_bytes: List[int] = field(default_factory=list)
     keys: Dict[int, object] = field(default_factory=dict)  # open source: index of a submitted request -> its key
     failed: Dict[int, BaseException] = field(default_factory=dict)  # open source: request index -> its follow-up's error
 
@@ -362,8 +395,55 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
        the slot at the next poll (``dev.cancel`` drops the prompt in progress; the request ends empty, without a
        follow-up); an interrupt drops it as it drops the waiting requests.
 
-    ``stats.prefill_cols`` records each poll's prefilled columns, ``stats.chunks`` the chunks."""
+    ``stats.prefill_cols`` records each poll's prefilled columns, ``stats.chunks`` the chunks.
+
+    A device with a KV pool (``dev.pool_pages`` not None: ``dev.reserve(slots, tokens) -> bool``, ``dev.release(slots)``,
+    ``dev.suspend(slot) -> image``, ``dev.resume(slot, image)``, ``dev.pages_in_use``, ``dev.host_bytes``) maps pages
+    as the slots grow.  A request of prompt ``T`` never holds more than ``T + max_new_token`` positions, and every
+    mapping below is capped there:
+
+    1. Before an admission, or a chunk ending at column ``c``, the slot is mapped up to ``T`` (``c``) plus ``chunk``
+       positions.  When the pool cannot cover it, the request waits at the head of the queue (a chunk waits for the
+       next poll).
+    2. Before each decode chunk every running slot is mapped up to ``seq_len + chunk + 1`` positions (``T`` plus its
+       tokens plus ``chunk``), all in one call.  When the pool cannot cover them all, the running request admitted
+       last is suspended (``dev.suspend``: its state and KV go to host memory, its slot and pages are freed) and the
+       call is repeated, until the rest fit.  A prompt in progress is never suspended.
+    3. Suspended requests are served before the waiting queue: at each poll, in admission order, each takes the
+       lowest free slot as soon as its tokens plus ``chunk`` fit together with one more chunk for every running slot
+       (mapped in the same call, so the decode that follows cannot suspend it again at once), and no waiting request
+       is admitted while one is suspended.  A resumed request continues bit for bit as if it had not moved.
+    4. Pages are released when a slot's request ends (harvest, cancel, requeue) or its prompt in progress is dropped.
+    5. A cancelled suspended request ends with the tokens it had (its image becomes the ``slot`` of its ``ended``
+       entry: ``dev.harvest`` reads it); an interrupt ends suspended requests as it ends running ones.
+
+    ``stats`` records the pages mapped at each poll and their peak, the suspensions, the resumes and the host bytes
+    held by images.  Without a pool none of these calls are made."""
     stats = stats if stats is not None else ScheduleStats()
+    pool = getattr(dev, "pool_pages", None)
+    admitted_at: Dict[int, int] = {}  # request index -> admission number (suspension victims: the highest)
+    suspended: List[list] = []  # [request index, image, tokens], in admission order
+
+    mapped: Dict[int, int] = {}  # slot -> positions its pages hold
+
+    def reserve(slots: List[int], tokens: List[int]) -> bool:
+        if not dev.reserve(slots, tokens):
+            return False
+        for s, t in zip(slots, tokens):
+            mapped[s] = max(mapped.get(s, 0), t)
+        return True
+
+    def limit(i: int, n: int) -> int:  # n positions plus one chunk, capped at what request i can ever hold
+        r = requests[i]
+        return min(n + chunk, int(r.emb.shape[0]) + r.max_new_token)
+
+    def held(i: int, n: int) -> int:  # positions request i holds with n tokens generated (and one more appended)
+        return int(requests[i].emb.shape[0]) + n
+
+    admission_no = itertools.count()
+
+    def note_admitted(i: int) -> None:
+        admitted_at[i] = next(admission_no)
     budget = prefill_budget
     prog: Optional[List[int]] = None  # the prompt in progress: [slot, request index, columns done]
     left = budget  # prompt columns this poll may still prefill
@@ -373,7 +453,7 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
         s, i, c0 = prog
         T = int(requests[i].emb.shape[0])
         n = min(T - c0, left // PREFILL_CHUNK_ALIGN * PREFILL_CHUNK_ALIGN)
-        if n <= 0:
+        if n <= 0 or (pool is not None and not reserve([s], [limit(i, c0 + n)])):
             return
         dev.prefill_chunk(s, i, c0, n)
         stats.chunks += 1
@@ -381,6 +461,8 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
         if c0 + n == T:
             prog = None
             stats.admitted += 1
+            if pool is not None:
+                note_admitted(i)
         else:
             prog[2] = c0 + n
 
@@ -401,7 +483,7 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
     while True:
         taken: list = []
         if source is not None:
-            idle = not waiting and all(o is None for o in owner)
+            idle = not waiting and not suspended and all(o is None for o in owner)
             new, cancels, closed = source.take(block=idle)
             for key, r in new:
                 stages = live.setdefault(key, set())
@@ -420,27 +502,53 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
                         taken.append((i, None, 0, False))
                     elif prog is not None and prog[1] == i:  # mid-prefill: no final chunk, the slot is free again
                         dev.cancel([prog[0]])
+                        if pool is not None:
+                            dev.release([prog[0]])
+                            mapped.pop(prog[0], None)
                         owner[prog[0]] = None
                         prog = None
                         retire(i)
                         stats.cancelled.add(i)
                         taken.append((i, None, 0, False))
+                    elif any(e[0] == i for e in suspended):  # its image ends it with the tokens it had
+                        e = next(e for e in suspended if e[0] == i)
+                        suspended.remove(e)
+                        retire(i)
+                        stats.cancelled.add(i)
+                        stats.tokens += e[2]
+                        taken.append((i, e[1], e[2], False))
                     else:
                         doomed.add(i)
             if idle and closed and not new and not taken:
                 return
         free = [s for s in range(dev.slots) if owner[s] is None]
+        # a suspended request resumes only if the running slots' pages for their next chunk fit beside it, so the
+        # decode that follows does not suspend it again before it has moved
+        ahead = [s for s in range(dev.slots) if owner[s] is not None and (prog is None or s != prog[0])]
+        while suspended and free and reserve([free[0]] + ahead, [limit(suspended[0][0], held(*suspended[0][::2]))] +
+                                             [limit(owner[s], mapped.get(s, 0)) for s in ahead]):
+            i, image, _ = suspended.pop(0)
+            s = free.pop(0)
+            dev.resume(s, image)
+            owner[s] = i
+            ahead.append(s)
+            stats.resumes += 1
         batch = []
         created = False
         if prog is not None:
             advance()
-        while free and waiting and prog is None:  # the requests behind a prompt in progress wait for it
+        # the requests behind a prompt in progress, or behind a suspended request, wait for it
+        while free and waiting and prog is None and not suspended:
             s, i = free.pop(0), waiting.popleft()
-            owner[s] = i
             # no budget, no bound: admission_cols (quadratic in the admission's size) is not evaluated
             if budget is not None and admission_cols(batch + [(s, i)], requests, dev.max_context) > left:
+                owner[s] = i
                 prog, created = [s, i, 0], True  # the first request that does not fit
                 break
+            if pool is not None and not reserve([s], [limit(i, int(requests[i].emb.shape[0]))]):
+                waiting.appendleft(i)  # the pool is short: it waits for pages at the head of the queue
+                break
+            owner[s] = i
             batch.append((s, i))
         if budget is not None:
             left -= admission_cols(batch, requests, dev.max_context)
@@ -448,6 +556,9 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
             dev.admit(batch)
             stats.admissions += 1
             stats.admitted += len(batch)
+            if pool is not None:
+                for _, i in batch:
+                    note_admitted(i)
         if created:  # its first chunk, from the budget left over
             advance()
         st = dev.status()
@@ -459,6 +570,7 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
         follow: List[int] = []
         done = []  # (index, slot, n_tokens, cancelled at this read) of the requests that may have a follow-up
         freed = False
+        released: List[int] = []
         stop = [s for s in range(dev.slots) if owner[s] in doomed and st.state[s] != _lib.SLOT_FINISHED]
         if stop:
             dev.cancel(stop)
@@ -468,6 +580,8 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
                 continue
             owner[s] = None
             freed = True
+            released.append(s)
+            admitted_at.pop(i, None)
             was_doomed = i in doomed
             doomed.discard(i)
             if s in stop:  # no follow-up after a cancel
@@ -488,6 +602,10 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
                 stats.tokens += st.end_idx[s]
                 ended.append((i, s, st.end_idx[s], bool(st.finish[s])))
                 done.append((i, s, st.end_idx[s], was_doomed))
+        if pool is not None and released:
+            dev.release(released)
+            for s in released:
+                mapped.pop(s, None)
         _prepare(requests, done, dev, stats, source)
         for i, s, n, was_doomed in done:
             kids = _follow_up(requests, i, s, n, dev, check, stats, source)
@@ -508,18 +626,36 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
             yield st, polled, ended
             continue  # refill the freed slots before the next chunk
         running = [s for s in range(dev.slots) if owner[s] is not None and (prog is None or s != prog[0])]
-        interrupted = (bool(running) or prog is not None) and context is not None and context.get()
+        interrupted = (bool(running) or prog is not None or bool(suspended)) and context is not None and context.get()
         if interrupted:
             stats.interrupted = True
             for s in running:
                 stats.tokens += st.end_idx[s]
                 ended.append((owner[s], s, st.end_idx[s], False))
+            for i, image, n in suspended:
+                stats.tokens += n
+                ended.append((i, image, n, False))
         yield st, polled, ended
         if budget is not None:  # the poll ends here: the next one has the whole budget
             stats.prefill_cols.append(budget - left)
             left = budget
-        if interrupted or (not running and source is None and prog is None):
+        if interrupted or (not running and source is None and prog is None and not suspended):
             return
+        while pool is not None and running:  # map every running slot for the chunk, suspending the last admitted
+            if reserve(running, [limit(owner[s], held(owner[s], st.end_idx[s])) for s in running]):
+                break
+            s = max(running, key=lambda s: admitted_at[owner[s]])
+            i = owner[s]
+            suspended.append([i, dev.suspend(s), st.end_idx[s]])
+            mapped.pop(s, None)
+            suspended.sort(key=lambda e: admitted_at[e[0]])
+            owner[s] = None
+            running.remove(s)
+            stats.suspensions += 1
+        if pool is not None:
+            stats.pages.append(dev.pages_in_use)
+            stats.peak_pages = max(stats.peak_pages, dev.pages_in_use)
+            stats.host_bytes.append(dev.host_bytes)
         if running:
             dev.decode(chunk)
 
@@ -583,23 +719,72 @@ def stream_schedule(requests: List[Request], dev, chunk: int, context=None, stat
             yield out
 
 
+class SlotImage:
+    """A suspended request (``EngineDevice.suspend``): its slot's image in pinned host memory (ctb_slot_image), until
+    ``EngineDevice.resume`` restores it into a slot.  ``row(hidden)`` and ``outputs(n)`` read its first tokens' ids and
+    hidden states, as the slot held them, once the copies that filled it are complete (``ready``)."""
+
+    def __init__(self, buf: torch.Tensor, text: bool, device, num_vq: int, hidden_size: int, stream):
+        self.buf, self.text, self.device, self.num_vq, self.hidden_size = buf, text, device, num_vq, hidden_size
+        self.ready = torch.cuda.Event()
+        self.ready.record(stream)  # after the copies that fill the image
+        self.header = _lib.SlotImage.from_address(buf.data_ptr())
+
+    @property
+    def nbytes(self) -> int:
+        return int(self.buf.numel())
+
+    def row(self, hidden: bool) -> torch.Tensor:
+        """The slot's hidden states [n_gen, d] (fp32) or ids [n_gen, num_vq] (int32), on the device."""
+        self.ready.synchronize()
+        h = self.header
+        if hidden:
+            off, n = h.off_hiddens, h.n_gen * self.hidden_size
+            return self.buf[off: off + 4 * n].view(torch.float32).view(h.n_gen, self.hidden_size).to(self.device)
+        off, n = h.off_ids, h.n_gen * self.num_vq
+        return self.buf[off: off + 4 * n].view(torch.int32).view(h.n_gen, self.num_vq).to(self.device)
+
+    def outputs(self, n: int, return_hidden: bool):
+        """GenerationOutputs of the first ``n`` tokens, as ``EngineDevice.harvest`` gives them for a slot."""
+        from .gpt import GPT
+
+        ids = self.row(False)[:n].to(torch.int64)
+        if self.text:
+            return GPT.GenerationOutputs(ids=[ids[:, 0].contiguous()], attentions=[], hiddens=[])
+        hid = [self.row(True)[:n]] if return_hidden else []
+        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid)
+
+
 class EngineDevice:
-    """The device layer of ``schedule`` on a GPT handle (ctb_gpt_engine_begin / _admit / _status, ctb_gpt_decode)."""
+    """The device layer of ``schedule`` on a GPT handle (ctb_gpt_engine_begin / _admit / _status, ctb_gpt_decode).
+    ``kv_pool_pages`` (``kv_pool_pages()``) makes a paged engine (ctb_gpt_engine_begin_paged) with the pool interface
+    ``_poll_cycles`` describes; None keeps every slot's fixed pages."""
 
     def __init__(self, gpt, requests: Sequence[Request], slots: int, max_new_cap: int, return_hidden: bool = True,
-                 flags: int = 0):
+                 flags: int = 0, kv_pool_pages: Optional[int] = None):
         self.gpt, self.requests, self.slots = gpt, requests, slots
         self.max_context = gpt.max_context
         self.lib = _lib.load()
         dev = gpt.device_gpt
         self.dev = dev
-        self.stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        self._torch_stream = torch.cuda.current_stream(dev)  # every device call of this engine is enqueued on it
+        self.stream = C.c_void_p(self._torch_stream.cuda_stream)
         self.ids_out = torch.zeros(slots, max_new_cap, gpt.num_vq, dtype=torch.int32, device=dev)
         self.hid_out = (torch.zeros(slots, max_new_cap, gpt.config.hidden_size, dtype=torch.float32, device=dev)
                         if return_hidden else None)
-        _lib.check(self.lib.ctb_gpt_engine_begin_ex(
-            gpt._handle, slots, max_new_cap, flags, C.c_void_p(self.ids_out.data_ptr()),
-            C.c_void_p(self.hid_out.data_ptr()) if self.hid_out is not None else None, self.stream))
+        hid = C.c_void_p(self.hid_out.data_ptr()) if self.hid_out is not None else None
+        self.pool_pages = kv_pool_pages
+        if kv_pool_pages is None:
+            _lib.check(self.lib.ctb_gpt_engine_begin_ex(
+                gpt._handle, slots, max_new_cap, flags, C.c_void_p(self.ids_out.data_ptr()), hid, self.stream))
+        else:
+            _lib.check(self.lib.ctb_gpt_engine_begin_paged(
+                gpt._handle, slots, max_new_cap, flags, kv_pool_pages, C.c_void_p(self.ids_out.data_ptr()), hid,
+                self.stream))
+        self._mapped = [0] * slots  # pages of each slot
+        # the images of suspended requests, by id, while anything holds them (a cancelled one's ends with its outputs)
+        self._images: "weakref.WeakValueDictionary[int, SlotImage]" = weakref.WeakValueDictionary()
+        self._resumed: List[SlotImage] = []  # read by the device until the next status read
         self._state = (C.c_int32 * slots)()
         self._end = torch.zeros(slots, dtype=torch.int32)
         self._fin = torch.zeros(slots, dtype=torch.uint8)
@@ -666,6 +851,60 @@ class EngineDevice:
     def decode(self, n: int) -> None:
         _lib.check(self.lib.ctb_gpt_decode(self.gpt._handle, n, self.stream))
 
+    # ---------------------------------------------------------------- KV pool (paged engines)
+    @property
+    def pages_in_use(self) -> int:
+        return sum(self._mapped)
+
+    @property
+    def host_bytes(self) -> int:
+        """Bytes of the images of suspended requests.  They live in pinned blocks of torch's caching host allocator,
+        which rounds each block up to a power of two and keeps freed blocks for reuse: the process can hold up to about
+        twice the peak of this figure pinned until it exits."""
+        return sum(im.nbytes for im in self._images.values())
+
+    def reserve(self, slots: List[int], tokens: List[int]) -> bool:
+        """Map pages so that each slot holds positions [0, tokens[i]) (ctb_gpt_engine_reserve); False, with nothing
+        mapped, when the pool cannot cover them all."""
+        n = len(slots)
+        rc = self.lib.ctb_gpt_engine_reserve(self.gpt._handle, n, (C.c_int32 * n)(*slots), (C.c_int32 * n)(*tokens),
+                                             self.stream)
+        if rc == _lib.ERR_POOL:
+            return False
+        _lib.check(rc)
+        for s, t in zip(slots, tokens):
+            self._mapped[s] = max(self._mapped[s], -(-t // _lib.PAGE_TOKENS))
+        return True
+
+    def release(self, slots: List[int]) -> None:
+        """Return the pages of idle or finished slots to the pool (ctb_gpt_engine_release)."""
+        _lib.check(self.lib.ctb_gpt_engine_release(self.gpt._handle, len(slots), (C.c_int32 * len(slots))(*slots),
+                                                   self.stream))
+        for s in slots:
+            self._mapped[s] = 0
+
+    def suspend(self, slot: int) -> SlotImage:
+        """Move the running request in ``slot`` to a pinned host image (ctb_gpt_engine_suspend); the slot and its pages
+        are free afterwards."""
+        nbytes = C.c_uint64()
+        _lib.check(self.lib.ctb_gpt_engine_suspend_bytes(self.gpt._handle, slot, C.byref(nbytes), self.stream))
+        buf = torch.empty(nbytes.value, dtype=torch.uint8, pin_memory=True)
+        _lib.check(self.lib.ctb_gpt_engine_suspend(self.gpt._handle, slot, C.c_void_p(buf.data_ptr()), nbytes.value,
+                                                   self.stream))
+        self._mapped[slot] = 0
+        image = SlotImage(buf, self._text[slot], self.dev, self.gpt.num_vq, self.gpt.config.hidden_size,
+                          self._torch_stream)
+        self._images[id(image)] = image
+        return image
+
+    def resume(self, slot: int, image: SlotImage) -> None:
+        """Restore a suspended request into ``slot``, whose pages already cover it (ctb_gpt_engine_resume)."""
+        _lib.check(self.lib.ctb_gpt_engine_resume(self.gpt._handle, slot, C.c_void_p(image.buf.data_ptr()),
+                                                  image.nbytes, self.stream))
+        self._text[slot] = image.text
+        self._images.pop(id(image), None)
+        self._resumed.append(image)  # the copies read it until the stream passes them
+
     def cancel(self, slots: List[int]) -> None:
         """Stop the requests in ``slots`` (ctb_gpt_engine_cancel): each keeps the tokens it has."""
         _lib.check(self.lib.ctb_gpt_engine_cancel(self.gpt._handle, len(slots), (C.c_int32 * len(slots))(*slots),
@@ -676,6 +915,7 @@ class EngineDevice:
         _lib.check(self.lib.ctb_gpt_engine_status(self.gpt._handle, C.byref(st), self._state,
                                                   C.c_void_p(self._end.data_ptr()), C.c_void_p(self._fin.data_ptr()),
                                                   self.stream))
+        self._resumed.clear()  # the status read synchronised the stream
         return SlotStatus(list(self._state), self._end.tolist(), self._fin.tolist(), int(st.steps_done))
 
     def harvest(self, slot: int, n: int, copy: bool = True):
@@ -684,6 +924,9 @@ class EngineDevice:
         request's ids are 1-D and it has no hidden states, as ``GPT.generate(infer_text=True)`` returns them."""
         from .gpt import GPT
 
+        if isinstance(slot, SlotImage):  # a suspended request that was cancelled or interrupted
+            self._images.pop(id(slot), None)
+            return slot.outputs(n, self.hid_out is not None)
         if self._text[slot]:
             return GPT.GenerationOutputs(ids=[self.ids_out[slot, :n, 0].to(torch.int64)], attentions=[], hiddens=[])
         ids = self.ids_out[slot, :n].to(torch.int64)

@@ -230,7 +230,7 @@ class GPT:
     def generate_continuous(self, requests, slots: Optional[int] = None, return_hidden=True, infer_text=False,
                             stream=False, return_attn=False, context=None, chunk: Optional[int] = None,
                             max_new_cap: Optional[int] = None, dtype=torch.float32,
-                            prefill_budget: Optional[int] = None):
+                            prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None):
         """Generate audio codes or text for many utterances on a slot engine (chattts_b200.engine): up to ``slots``
         requests (default: ``max_batch``, at most the number of requests) decode together, and a waiting request takes
         the place of a finished one at the next poll (every ``chunk`` steps, default CTB_DECODE_CHUNK or 32).  Each
@@ -259,21 +259,28 @@ class GPT:
         ``prefill_budget`` (prompt columns per poll, at least 128; default None: every admission is prefilled whole)
         bounds the prefill the running slots wait for at each poll: a prompt that does not fit is prefilled in chunks
         of multiples of 128 columns over the next polls (``engine._poll_cycles``), and its outputs are bit for bit
-        those of its admission in one call.  The yields are the same; a long prompt's first token comes later."""
-        from .engine import ScheduleStats, check_prefill_budget, schedule
+        those of its admission in one call.  The yields are the same; a long prompt's first token comes later.
+
+        ``kv_pool_bytes`` (default None: every slot owns ``max_context`` tokens of KV pages from the start) bounds the
+        engine's KV memory: slots take 16-token pages from a pool of that many bytes as they grow, and when it runs
+        short the running request admitted last is suspended to pinned host memory and resumed later, in any slot, bit
+        for bit as if it had not moved (``engine._poll_cycles``).  A request whose prompt + ``max_new_token`` does not
+        fit in the pool alone is refused.  ``last_schedule_stats`` records pages, suspensions and resumes."""
+        from .engine import ScheduleStats, check_prefill_budget, kv_pool_pages, schedule
 
         flags = _lib.engine_flags(dtype)
         prefill_budget = check_prefill_budget(prefill_budget)
+        pool = kv_pool_pages(self.config, kv_pool_bytes, flags)
 
         if stream:
             raise ValueError("generate_continuous: stream=True is not supported; results are yielded per request "
                              "(generate_continuous_stream streams)")
         requests, S, chunk, context, cap, check = self._engine_args(
-            "generate_continuous", requests, slots, infer_text, return_attn, context, chunk, 32, max_new_cap)
+            "generate_continuous", requests, slots, infer_text, return_attn, context, chunk, 32, max_new_cap, pool)
         if not requests:
             return
         with torch.cuda.device(self.device_gpt):
-            dev = self._engine_device(requests, S, cap, return_hidden, flags)
+            dev = self._engine_device(requests, S, cap, return_hidden, flags, pool)
             self.last_schedule_stats = stats = ScheduleStats()  # admissions, decode steps (tools/bench_continuous.py)
             for i, slot, n in schedule(requests, dev, chunk, context, stats, check, prefill_budget):
                 yield i, (dev.empty(i) if slot is None else dev.harvest(slot, n))
@@ -284,7 +291,7 @@ class GPT:
     def generate_continuous_stream(self, requests, slots: Optional[int] = None, return_hidden=True, context=None,
                                    chunk: Optional[int] = None, infer_text=False, return_attn=False,
                                    max_new_cap: Optional[int] = None, dtype=torch.float32,
-                                   prefill_budget: Optional[int] = None):
+                                   prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None):
         """Streaming form of ``generate_continuous``: generator of ``(request_index, GenerationOutputs, last)``.
 
         For each request the yields are exactly those ``generate(stream=True, stream_batch=r.stream_batch)`` makes for
@@ -297,17 +304,19 @@ class GPT:
 
         ``ids`` are copies.  ``hiddens`` are views into the engine's buffer, like the narrowed views ``generate``
         hands out: they stay valid until this generator is resumed (copy them to keep them).  ``dtype`` and
-        ``prefill_budget`` as in ``generate_continuous``: a budget leaves every request's yields as they are."""
-        from .engine import ScheduleStats, check_prefill_budget, stream_schedule
+        ``prefill_budget`` and ``kv_pool_bytes`` as in ``generate_continuous``: neither changes a request's yields."""
+        from .engine import ScheduleStats, check_prefill_budget, kv_pool_pages, stream_schedule
 
         flags = _lib.engine_flags(dtype)
         prefill_budget = check_prefill_budget(prefill_budget)
+        pool = kv_pool_pages(self.config, kv_pool_bytes, flags)
         requests, S, chunk, context, cap, check = self._engine_args(
-            "generate_continuous_stream", requests, slots, infer_text, return_attn, context, chunk, None, max_new_cap)
+            "generate_continuous_stream", requests, slots, infer_text, return_attn, context, chunk, None, max_new_cap,
+            pool)
         if not requests:
             return
         with torch.cuda.device(self.device_gpt):
-            dev = self._engine_device(requests, S, cap, return_hidden, flags)
+            dev = self._engine_device(requests, S, cap, return_hidden, flags, pool)
             self.last_schedule_stats = stats = ScheduleStats()
             for batch in stream_schedule(requests, dev, chunk, context, stats, check, prefill_budget=prefill_budget):
                 for i, slot, n, last in batch:
@@ -316,7 +325,7 @@ class GPT:
                 self.logger.warning("generation is interrupted")
 
     def open_engine(self, slots: int, max_new_cap: int, return_hidden=True, chunk: Optional[int] = None,
-                    dtype=torch.float32, prefill_budget: Optional[int] = None):
+                    dtype=torch.float32, prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None):
         """A slot engine that takes requests while it decodes: ``submit(request, stream=False) -> engine.Job`` from
         any thread, ``Job.cancel()`` for one request, ``close(cancel=False)`` (or a ``with`` block) to drain it.
 
@@ -330,31 +339,39 @@ class GPT:
         slot at the next poll).  One worker thread owns the handle and its stream; while the engine
         is open ``generate``, ``generate_continuous*`` and another ``open_engine`` raise.  The poll interval is
         ``chunk`` steps (default CTB_DECODE_CHUNK, else 24).  ``slots`` and ``dtype`` as in ``generate_continuous``
-        (up to ``max_batch`` slots; a half-precision engine up to 64)."""
+        (up to ``max_batch`` slots; a half-precision engine up to 64).  ``kv_pool_bytes`` as in
+        ``generate_continuous``: ``submit`` refuses a request that does not fit in the pool alone, and a job cancelled
+        while suspended ends with the tokens it had."""
         from .engine import GptEngine
 
         return self._open_slot_engine(GptEngine, slots, max_new_cap, return_hidden, chunk,
-                                      flags=_lib.engine_flags(dtype), prefill_budget=prefill_budget)
+                                      flags=_lib.engine_flags(dtype), prefill_budget=prefill_budget,
+                                      kv_pool_bytes=kv_pool_bytes)
 
-    def _open_slot_engine(self, cls, slots, max_new_cap, return_hidden, chunk, *args, flags=0, prefill_budget=None):
+    def _open_slot_engine(self, cls, slots, max_new_cap, return_hidden, chunk, *args, flags=0, prefill_budget=None,
+                          kv_pool_bytes=None):
         """An ``engine.OpenEngine`` subclass ``cls`` that owns this handle until it is closed (``flags``: the
-        ctb_gpt_engine_begin_ex precision flags; ``prefill_budget``: the engine's bound on each poll's prefill)."""
-        from .engine import check_prefill_budget
+        ctb_gpt_engine_begin_ex precision flags; ``prefill_budget``: the engine's bound on each poll's prefill;
+        ``kv_pool_bytes``: its KV pool, None for fixed pages)."""
+        from .engine import check_prefill_budget, kv_pool_pages
 
         prefill_budget = check_prefill_budget(prefill_budget)
+        pool = kv_pool_pages(self.config, kv_pool_bytes, flags)
         _, S, chunk, _, cap, check = self._engine_args("open_engine", [], slots, False, False, None, chunk, None,
-                                                       max_new_cap)
+                                                       max_new_cap, pool)
         kw = {} if prefill_budget is None else {"prefill_budget": prefill_budget}
-        engine = cls(lambda requests: self._engine_device(requests, S, cap, return_hidden, flags), chunk, check,
+        engine = cls(lambda requests: self._engine_device(requests, S, cap, return_hidden, flags, pool), chunk, check,
                      self.device_gpt, self._close_engine, *args, max_new_cap=cap, **kw)
         self._open = engine
         return engine
 
-    def _engine_device(self, requests, S, cap, return_hidden, flags):
-        """The ``engine.EngineDevice`` of one slot engine; an fp32 engine gets the five-argument form that stand-in
-        devices implement."""
+    def _engine_device(self, requests, S, cap, return_hidden, flags, pool_pages=None):
+        """The ``engine.EngineDevice`` of one slot engine; an fp32 engine with fixed pages gets the five-argument form
+        that stand-in devices implement."""
         from . import engine
 
+        if pool_pages is not None:
+            return engine.EngineDevice(self, requests, S, cap, return_hidden, flags=flags, kv_pool_pages=pool_pages)
         if flags:
             return engine.EngineDevice(self, requests, S, cap, return_hidden, flags=flags)
         return engine.EngineDevice(self, requests, S, cap, return_hidden)
@@ -367,11 +384,12 @@ class GPT:
             raise RuntimeError(f"{name}: an open engine owns this handle; close it first")
 
     def _engine_args(self, name, requests, slots, infer_text, return_attn, context, chunk, default_chunk,
-                     max_new_cap=None):
+                     max_new_cap=None, pool_pages=None):
         """Checks shared by the slot-engine generators -> (requests, slots, chunk, context, max_new_cap, check), where
-        ``check`` validates a follow-up request as the up-front ones are.  The poll interval is `chunk`, else
-        CTB_DECODE_CHUNK, else `default_chunk` (None: the smallest ``stream_batch``)."""
-        from .engine import MIN_PROMPT_COLS, Request, check_noise_batch
+        ``check`` validates a follow-up request as the up-front ones are (with a KV pool of ``pool_pages`` pages, also
+        that it fits in the pool alone).  The poll interval is `chunk`, else CTB_DECODE_CHUNK, else `default_chunk`
+        (None: the smallest ``stream_batch``)."""
+        from .engine import MIN_PROMPT_COLS, Request, check_noise_batch, pool_pages_needed
 
         self._check_free(name)
         if infer_text:
@@ -400,6 +418,9 @@ class GPT:
                                  f"max_context={self.max_context}")
             if r.max_new_token > cap:
                 raise ValueError(f"max_new_token {r.max_new_token} exceeds max_new_cap={cap}")
+            if pool_pages is not None and pool_pages_needed(r) > pool_pages - 1:
+                raise ValueError(f"prompt {int(r.emb.shape[0])} + max_new_token {r.max_new_token} need "
+                                 f"{pool_pages_needed(r)} KV pages; the pool has {pool_pages - 1} (kv_pool_bytes)")
             check_noise_batch(r, 1 if r.infer_text else self.num_vq, self.max_batch)
 
         for r in requests:

@@ -254,6 +254,80 @@ int ctb_gpt_engine_status(ctb_gpt* h, ctb_gpt_status* out, int32_t* state_host, 
  * or repeated, or an engine of more than 1024 slots. */
 int ctb_gpt_engine_cancel(ctb_gpt* h, int32_t n, const int32_t* slots, void* stream);
 
+/* ---- KV pages on demand: a slot engine whose KV memory is a bounded pool shared by its slots.
+ * ctb_gpt_engine_begin_ex with two differences: the pool holds pool_pages pages of every layer (one page: 16 tokens
+ * of K and V, 2 x num_kv_heads x 16 x head_dim values per layer, fp32 or fp16 by CTB_ENGINE_FP16_KV), and no slot
+ * owns any page.  Page 0 is the zero page: never handed out, always zero, and every block-table entry that maps no
+ * page points at it, so a read of a position a slot does not own sees zeros.  The handle keeps the free list.
+ * A request's results do not depend on which pages hold its KV: ctb_gpt_engine_admit / _admit_text /
+ * _prefill_chunk / _cancel and ctb_gpt_decode keep their contracts, and the first three, and ctb_gpt_decode, refuse
+ * (CTB_ERR_STATE, nothing enqueued) a slot whose pages do not cover the positions they are about to write.
+ * With CTB_KV_POISON=1 in the environment at this call, the pool (all but the zero page) and every released page
+ * are filled with quiet-NaN bits instead of zeros, so a read of a page a request does not own shows in its outputs.
+ * Errors: those of ctb_gpt_engine_begin_ex; CTB_ERR_ARG for pool_pages < 2 or max_context over 8,192 tokens;
+ * CTB_ERR_NOMEM if the pool does not fit. */
+#define CTB_ERR_POOL (-5)
+int ctb_gpt_engine_begin_paged(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t flags, int32_t pool_pages,
+                               int32_t* ids_out_dev, float* hiddens_out_dev, void* stream);
+
+/* Map pages so that each slot slots[i] (host array of n distinct slots) holds positions [0, tokens[i]) (0 <= tokens[i]
+ * <= max_context; a slot that holds them already is left as it is).  All or nothing: when the free list cannot cover
+ * the whole call it returns CTB_ERR_POOL and the handle is unchanged.  Enqueued on `stream` (the new block-table
+ * entries travel by value), no synchronisation.
+ * Errors: CTB_ERR_STATE outside a paged engine; CTB_ERR_ARG for a null argument, n outside [1, S], a slot out of
+ * range or repeated, or tokens outside [0, max_context]. */
+int ctb_gpt_engine_reserve(ctb_gpt* h, int32_t n, const int32_t* slots, const int32_t* tokens, void* stream);
+
+/* Return the pages of the idle or finished slots slots[0..n) to the free list and point their entries back at the
+ * zero page (CTB_KV_POISON=1: the pages are filled with quiet-NaN bits).  Synchronises `stream` once to read the
+ * slots' states.  Errors: CTB_ERR_STATE outside a paged engine, or for a slot that is running, pending or has a
+ * prompt in progress (nothing is released); CTB_ERR_ARG as for ctb_gpt_engine_reserve. */
+int ctb_gpt_engine_release(ctb_gpt* h, int32_t n, const int32_t* slots, void* stream);
+
+/* A suspended slot's image in a pinned host buffer: this header, then the sections at the offsets it records. */
+#define CTB_SLOT_IMAGE_MAGIC 0x4b565031u
+typedef struct ctb_slot_image {
+  uint32_t magic;
+  int32_t prec;            /* the engine's CTB_ENGINE_FP16_* flags */
+  int32_t seq_len, pos, end_idx, finish;
+  int32_t n_gen;           /* tokens in the ids / hiddens sections */
+  int32_t npages;          /* KV pages: positions [0, 16 * npages) of every layer */
+  int32_t page_bytes;      /* one page of one layer */
+  int32_t num_vq, hidden_size, noise_floats;
+  int32_t has_hidden;      /* the hiddens section exists */
+  int32_t row[8];          /* the slot's loop state (n_gen, step, state, max_new, has_noise, eos, text, -) */
+  int32_t reserved[3];
+  ctb_sampler_config sampler;
+  uint64_t off_noise;      /* float[noise_floats]: the slot's Exp(1) rows */
+  uint64_t off_ids;        /* int32[n_gen][num_vq] */
+  uint64_t off_hiddens;    /* float[n_gen][hidden_size], if has_hidden */
+  uint64_t off_kv;         /* [layer][npages] pages as the pool stores them */
+  uint64_t bytes;          /* the whole image */
+} ctb_slot_image;
+
+/* Bytes of the image ctb_gpt_engine_suspend would write for the running slot `slot` now.  Synchronises `stream`.
+ * Errors: CTB_ERR_STATE outside a paged engine or for a slot that is not running; CTB_ERR_ARG for a null argument
+ * or a slot out of range. */
+int ctb_gpt_engine_suspend_bytes(ctb_gpt* h, int32_t slot, uint64_t* bytes, void* stream);
+
+/* Move the running slot `slot` out of the engine into host_buf (pinned host memory of host_bytes bytes, at least
+ * ctb_gpt_engine_suspend_bytes): its KV for positions [0, seq_len) of every layer (k_kv_pack: one launch, 16-byte
+ * stores straight into the mapped buffer), its loop state, sampler, noise row, seq_len / pos / finish / end_idx, and
+ * its ids_out / hiddens_out rows 0 .. n_gen-1.  Its pages are then released and the slot becomes idle.  The header is
+ * written before the call returns; the rest is enqueued on `stream` (synchronise it before reading them on the host).
+ * Errors (the handle as it was): CTB_ERR_STATE outside a paged engine, for a slot that is not running or has a prompt
+ * in progress; CTB_ERR_ARG for a null argument, a slot out of range, a buffer that is not pinned or too small. */
+int ctb_gpt_engine_suspend(ctb_gpt* h, int32_t slot, void* host_buf, uint64_t host_bytes, void* stream);
+
+/* Restore the image in host_buf into `slot` - any idle or finished slot whose pages already hold the image's
+ * positions [0, seq_len) - and set it running (k_kv_unpack scatters the pages).  The request then continues exactly
+ * as it would have without the move.  Enqueued on `stream` after one synchronisation; host_buf must stay alive until
+ * the stream has passed this call.  Errors (the handle as it was): CTB_ERR_STATE outside a paged engine, for a slot
+ * that is running, pending or has a prompt in progress, or whose pages do not cover the image; CTB_ERR_ARG for a null
+ * argument, a slot out of range, a buffer that is not pinned or smaller than the image, or an image of another
+ * engine shape (magic, precision, page, noise or hidden-state layout, max_new_cap). */
+int ctb_gpt_engine_resume(ctb_gpt* h, int32_t slot, const void* host_buf, uint64_t host_bytes, void* stream);
+
 /* Measurement hook for bench.py's roofline: launches ONE kernel kind once per layer on the
  * state left by the last generate call (kind 0 qkv, 1 attention, 2 o-proj, 3 gate/up, 4 down;
  * 5 = heads, 6 = sampler, 7 = one decode step as ONE kernel launch (k_flow / k_step), 8 = 16 decode steps in one
