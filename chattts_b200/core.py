@@ -14,7 +14,7 @@ import logging
 import os
 import queue
 import re
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
 from typing import Dict, List, Optional, Union
 
 import numpy as np
@@ -668,8 +668,8 @@ class _Paragraph:
     stage, which request speaks which sentence, and the in-order assembly of the sentences' audio (``add``).  ``sink`` =
     (queue, key): the chunks and the end of the job are also posted there, for ``Chat.infer_continuous*``."""
 
-    def __init__(self, n: int, stream_params, sink=None):
-        self.n, self.sink = n, sink
+    def __init__(self, n: int, stream_params, sink=None, takes: bool = False):
+        self.n, self.sink, self.takes = n, sink, takes
         self.windows = ([StreamWindows(stream_params.stream_speed, stream_params.pass_first_n_batches)
                          for _ in range(n)] if stream_params is not None else None)
         self.ref = None
@@ -702,6 +702,8 @@ class _Paragraph:
                     self.sink[0].put((self.sink[1], item))
             if done:
                 job._finish(None)
+        elif done and self.takes:  # n takes of one sentence: one waveform each
+            job._finish([np.concatenate([c[0] for c in part]) for part in self.parts])
         elif done:
             job._finish(np.concatenate([c[0] for part in self.parts for c in part]))
         if done:
@@ -799,15 +801,15 @@ class ChatEngine(OpenEngine):
     streaming job and the whole sequence of every non-streaming job that completed go into one ``decode_rows`` call."""
 
     def __init__(self, make_device, chunk, check, device, on_close, chat: "Chat", use_decoder: bool, context=None,
-                 max_new_cap: Optional[int] = None, prefill_budget: Optional[int] = None):
+                 max_new_cap: Optional[int] = None, prefill_budget: Optional[int] = None, slots: Optional[int] = None):
         self.chat, self.use_decoder = chat, use_decoder
         self.model = chat.decoder if use_decoder else chat.dvae
         self._sampler = _SpeakerSampler(chat, self.model, use_decoder)
-        super().__init__(make_device, chunk, check, device, on_close, max_new_cap, context, prefill_budget)
+        super().__init__(make_device, chunk, check, device, on_close, max_new_cap, context, prefill_budget, slots)
 
     def submit(self, text: str, params_infer_code=None, stream=False, skip_refine_text=True, params_refine_text=None,
                lang=None, do_text_normalization=True, do_homophone_replacement=True, split_text=False,
-               max_split_batch=1) -> Job:
+               max_split_batch=1, takes: int = 1) -> Job:
         """Queue one text -> ``Job``: ``result()`` is the waveform ``infer_continuous`` yields for it, or with
         ``stream=True`` the job iterates the ``(chunk, last)`` pairs ``infer_continuous_stream`` yields for it.
         ``skip_refine_text=False`` refines the text on the engine first (``refine_on_engine=True``).  A cancelled
@@ -841,15 +843,53 @@ class ChatEngine(OpenEngine):
         ``result()`` is then what ``infer(text, use_decoder=False, max_split_batch=m, params_refine_text=...)[0]``
         returns, bit for bit on the code path when seeded (with the default arguments and m = 4: ``infer(text)``).
         A refinement that ends empty fails the job, as it makes ``infer`` raise.  Without ``split_text`` the text is
-        a paragraph of one sentence, and a refinement that ends empty goes on to speak the empty refined text."""
+        a paragraph of one sentence, and a refinement that ends empty goes on to speak the empty refined text.
+
+        ``takes`` = n > 1: n takes of the text, to keep the best (ChatTTS output varies from seed to seed).
+        ``result()`` is the list of their n waveforms, each what a one-sentence job gives; ``Job.cancel()`` cancels
+        every take.  The takes are n code requests of one ``Request.prompt_key``: once one of them runs, the others
+        share its prompt's KV and prefill only the last chunk of at most 128 columns, with the same results.  With
+        ``manual_seed`` set, take k samples as row k of ``infer([text] * n)``'s code batch (``noise_batch`` = (n, k));
+        without it, each take draws its own seed.  It takes ``stream=False``, ``split_text=False`` and
+        ``skip_refine_text=True``, and n at most the engine's slots and the handle's ``max_batch``."""
 
         def normalize(t):
             return self.chat.normalizer(t, do_text_normalization, do_homophone_replacement, lang)
+
+        if takes != 1:
+            job, requests = self._takes_job(text, params_infer_code or Chat.InferCodeParams(), takes, stream,
+                                            skip_refine_text, split_text, normalize)
+            self._enqueue([(job, requests)])
+            return job
 
         job, requests = self._job(text, params_infer_code or Chat.InferCodeParams(), stream, skip_refine_text,
                                   params_refine_text or Chat.RefineTextParams(), split_text, max_split_batch, normalize)
         self._enqueue([(job, requests)])
         return job
+
+    def _takes_job(self, text, params, takes, stream, skip_refine_text, split_text, normalize):
+        """``submit``'s job of ``takes`` takes of ``text`` and its requests -> ``(Job, requests)``."""
+        n = int(takes)
+        if n != takes or n < 1:
+            raise ValueError(f"takes={takes!r}: a positive int")
+        if stream or split_text or not skip_refine_text:
+            raise ValueError("takes > 1 needs stream=False, split_text=False and skip_refine_text=True")
+        limit = min(self.chat.gpt.max_batch, self.slots or self.chat.gpt.max_batch)
+        if n > limit:
+            raise ValueError(f"takes={n} exceed this engine's slots and the handle's max_batch ({limit})")
+        if self.max_new_cap is not None and params.max_new_token > self.max_new_cap:
+            raise ValueError(f"max_new_token {params.max_new_token} exceeds max_new_cap={self.max_new_cap}")
+        first = self.chat._code_request(normalize(text), params)
+        key = object()  # this job's takes, and nothing else, share a prompt
+        seeded = params.manual_seed is not None
+        para = _Paragraph(n, None, takes=True)
+        reqs = []
+        for k in range(n):
+            r = replace(first, noise_batch=(n, k) if seeded else None, prompt_key=key)
+            para.order[r] = k
+            reqs.append(r)
+        para.job = self._new_job(reqs, False, para)
+        return para.job, reqs
 
     def _job(self, text, params, stream, skip_refine_text, refine, split_text, max_split_batch, normalize, sink=None):
         """``submit``'s job, not queued yet, and its first requests -> ``(Job, requests)``; ``normalize`` maps each

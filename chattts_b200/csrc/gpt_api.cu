@@ -113,6 +113,9 @@ struct ctb_gpt {
   // per slot: the prompt being prefilled in chunks (ctb_gpt_engine_prefill_chunk) - its width (0: none) and the columns
   // already in the slot's pages
   std::vector<int> chunk_T0, chunk_done;
+  // per slot: the admitted prompt whose KV its pages hold (ctb_gpt_engine_share_prompt's source) - its positions
+  // (pr_len, 0: none) and the width whose attention kernel prefilled it (pr_W)
+  std::vector<int> pr_len, pr_W;
   // ---- half-precision slot engine (ctb_gpt_engine_begin_ex)
   int prec;                   // CTB_ENGINE_FP16_* bits of the current engine (0 for fp32 engines and generate())
   bool tc_base;               // tensor-core activation scratch, head copies and their tensor maps exist (tc_setup_base)
@@ -128,6 +131,7 @@ struct ctb_gpt {
   // per slot: pages mapped, and the tokens its request may hold after the steps enqueued so far (pg_hi, 0: none) and
   // at most (pg_cap: prompt + max_new - 1)
   std::vector<int> pg_map, pg_hi, pg_cap;
+  std::vector<int> pg_ref;    // [pool_pages] block-table entries that map each page (above 1: a shared prompt's)
   char* pg_stage;             // KV_STAGE_BYTES of device staging for suspend / resume (allocated by the first one)
 };
 
@@ -140,6 +144,16 @@ static float* kv_layer(const ctb_gpt* h, int l) {
 // floats of one slot's noise in the engine's buffer: room for a code request's or a text request's rows
 static size_t noise_stride(const ctb_gpt* h) {
   return std::max((size_t)h->cfg.num_vq * h->cfg.num_audio_tokens, (size_t)h->cfg.num_text_tokens);
+}
+
+// A paged engine's kernels write only pages that a single block-table entry maps: CTB_ERR_STATE if slot b's pages
+// for positions [lo, hi) include one it shares with another slot (ctb_gpt_engine_share_prompt)
+static int check_private(const ctb_gpt* h, int b, int lo, int hi) {
+  if (!h->pg_pages) return CTB_OK;
+  for (int k = lo / kPageTokens; k * kPageTokens < hi && k < h->pg_map[b]; ++k)
+    if (h->pg_ref[h->pg_bt[(size_t)b * h->pages_per_row + k]] > 1)
+      return set_err(CTB_ERR_STATE, "slot %d: positions [%d,%d) reach page entry %d, which is shared", b, lo, hi, k);
+  return CTB_OK;
 }
 
 extern "C" int ctb_abi_version(void) { return CTB_ABI_VERSION; }
@@ -1238,6 +1252,9 @@ extern "C" int ctb_gpt_decode(ctb_gpt* h, int32_t n_steps, void* stream) {
         return set_err(CTB_ERR_STATE, "slot %d: its pages hold %d positions, %d decode steps may need %d", b,
                        h->pg_map[b] * kPageTokens, n_steps, std::min(h->pg_hi[b] + n_steps, h->pg_cap[b]));
     for (int b = 0; b < h->B; ++b)
+      if (h->pg_hi[b] && (rc = check_private(h, b, h->pg_hi[b], std::min(h->pg_hi[b] + n_steps, h->pg_cap[b]))))
+        return rc;
+    for (int b = 0; b < h->B; ++b)
       if (h->pg_hi[b]) h->pg_hi[b] = std::min(h->pg_hi[b] + n_steps, h->pg_cap[b]);
   }
   h->steps_enqueued += n_steps;
@@ -1344,6 +1361,8 @@ static int engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t flag
   CTB_CUDA(cudaStreamSynchronize(s));  // idle_state is read by the copy engine
   h->chunk_T0.assign((size_t)S, 0);     // no prompt in progress
   h->chunk_done.assign((size_t)S, 0);
+  h->pr_len.assign((size_t)S, 0);       // no prompt to share
+  h->pr_W.assign((size_t)S, 0);
   h->started = 1;
   h->steps_enqueued = 0;
   return CTB_OK;
@@ -1366,8 +1385,8 @@ static int admit(ctb_gpt* h, int n, const int32_t* slots, int T0, int q0, const 
   int rc;
   std::vector<RowState> rows((size_t)h->bpad_max);
   CTB_CUDA(cudaMemcpyAsync(rows.data(), h->rows, sizeof(RowState) * rows.size(), cudaMemcpyDeviceToHost, s));
-  std::vector<uint8_t> mask_h;  // a paged engine counts the positions each whole prompt writes
-  if (h->pg_pages && mask_dev) {
+  std::vector<uint8_t> mask_h;  // the positions each whole prompt writes (its pages, and the prompt it can share)
+  if (mask_dev) {
     mask_h.resize((size_t)n * T0);
     CTB_CUDA(cudaMemcpyAsync(mask_h.data(), mask_dev, mask_h.size(), cudaMemcpyDeviceToHost, s));
   }
@@ -1389,11 +1408,15 @@ static int admit(ctb_gpt* h, int n, const int32_t* slots, int T0, int q0, const 
     if (h->pg_pages && h->pg_map[b] * kPageTokens < held[i])
       return set_err(CTB_ERR_STATE, "slot %d: its pages hold %d positions, the prompt writes %d", b,
                      h->pg_map[b] * kPageTokens, held[i]);
+    if ((rc = check_private(h, b, q0, held[i]))) return rc;
     RowState& r = rows[b];
     r.n_gen = 0; r.step = 0; r.state = RS_PENDING; r.max_new = max_new[i]; r.has_noise = q_noise_dev != nullptr;
     r.eos = sc.eos_token; r.text = text;
   }
-  for (int i = 0; i < n; ++i) h->chunk_T0[slots[i]] = 0;  // the slot's prompt in progress, if any, is dropped
+  for (int i = 0; i < n; ++i) {
+    h->chunk_T0[slots[i]] = 0;  // the slot's prompt in progress, if any, is dropped
+    h->pr_len[slots[i]] = held[i]; h->pr_W[slots[i]] = T0;
+  }
   if (h->pg_pages)
     for (int i = 0; i < n; ++i) { h->pg_hi[slots[i]] = held[i]; h->pg_cap[slots[i]] = held[i] + max_new[i] - 1; }
   CTB_CUDA(cudaMemcpyAsync(h->rows, rows.data(), sizeof(RowState) * rows.size(), cudaMemcpyHostToDevice, s));
@@ -1482,6 +1505,8 @@ extern "C" int ctb_gpt_engine_prefill_chunk(ctb_gpt* h, int32_t slot, int32_t T0
   if (h->pg_pages && h->pg_map[slot] * kPageTokens < c0 + n)
     return set_err(CTB_ERR_STATE, "slot %d: its pages hold %d positions, the chunk writes up to %d", slot,
                    h->pg_map[slot] * kPageTokens, c0 + n);
+  if ((rc = check_private(h, slot, c0, c0 + n))) return rc;
+  h->pr_len[slot] = 0;  // its pages now hold part of a prompt
   if ((rc = prefill(h, 1, T0, c0, n, emb_dev, nullptr, &slot, s))) { h->chunk_T0[slot] = 0; return rc; }
   h->chunk_T0[slot] = T0; h->chunk_done[slot] = c0 + n;
   return CTB_OK;
@@ -1593,6 +1618,7 @@ static int kv_pool_paged(ctb_gpt* h, int S, int pool_pages, cudaStream_t s) {
   for (int p = pool_pages - 1; p >= 1; --p) h->pg_free.push_back(p);
   h->pg_bt.assign((size_t)S * h->pages_per_row, 0);
   h->pg_map.assign((size_t)S, 0); h->pg_hi.assign((size_t)S, 0); h->pg_cap.assign((size_t)S, 0);
+  h->pg_ref.assign((size_t)pool_pages, 0);
   h->pg_pages = pool_pages;
   return CTB_OK;
 }
@@ -1643,6 +1669,7 @@ extern "C" int ctb_gpt_engine_reserve(ctb_gpt* h, int32_t n, const int32_t* slot
       const int idx = b * h->pages_per_row + k, page = h->pg_free.back();
       h->pg_free.pop_back();
       h->pg_bt[idx] = page;
+      h->pg_ref[page] = 1;
       e.emplace_back(idx, page);
     }
     h->pg_map[b] = std::max(h->pg_map[b], want);
@@ -1650,18 +1677,20 @@ extern "C" int ctb_gpt_engine_reserve(ctb_gpt* h, int32_t n, const int32_t* slot
   return bt_write(h, e, (cudaStream_t)stream);
 }
 
-// slot b's pages back to the free list (taken again in the order they had), its entries on the zero page
+// slot b's entries on the zero page; each page no other entry maps goes back to the free list (taken again in the
+// order they had)
 static int release_pages(ctb_gpt* h, int b, cudaStream_t s) {
   std::vector<std::pair<int, int>> e;
   std::vector<int> freed;
   for (int k = 0; k < h->pg_map[b]; ++k) {
     const int idx = b * h->pages_per_row + k;
-    freed.push_back(h->pg_bt[idx]);
+    if (--h->pg_ref[h->pg_bt[idx]] == 0) freed.push_back(h->pg_bt[idx]);
     h->pg_bt[idx] = 0;
     e.emplace_back(idx, 0);
   }
   h->pg_free.insert(h->pg_free.end(), freed.rbegin(), freed.rend());
   h->pg_map[b] = h->pg_hi[b] = h->pg_cap[b] = 0;
+  h->pr_len[b] = 0;
   int rc;
   if ((rc = bt_write(h, e, s))) return rc;
   return h->pg_poison ? kv_poison(h, freed.data(), 0, (int)freed.size(), s) : CTB_OK;
@@ -1849,6 +1878,8 @@ extern "C" int ctb_gpt_engine_resume(ctb_gpt* h, int32_t slot, const void* host_
   CTB_CUDA(cudaMemcpyAsync(&cur, h->rows + slot, sizeof(RowState), cudaMemcpyDeviceToHost, s));
   CTB_CUDA(cudaStreamSynchronize(s));
   if (cur.state == RS_RUNNING || cur.state == RS_PENDING) return set_err(CTB_ERR_STATE, "slot %d is still generating", slot);
+  if ((rc = check_private(h, slot, 0, img->seq_len))) return rc;
+  h->pr_len[slot] = 0;  // the image does not record its prompt: a resumed request is no source to share from
   const char* hb = static_cast<const char*>(host_buf);
   const int n_gen = img->n_gen;
   CTB_CUDA(cudaMemcpyAsync(h->cfgs + slot, &img->sampler, sizeof(ctb_sampler_config), cudaMemcpyHostToDevice, s));
@@ -1869,6 +1900,69 @@ extern "C" int ctb_gpt_engine_resume(ctb_gpt* h, int32_t slot, const void* host_
   h->pg_hi[slot] = img->seq_len;
   h->pg_cap[slot] = img->seq_len + r.max_new - r.n_gen;
   if (r.text) h->eng_text = 1;
+  return CTB_OK;
+}
+
+// ------------------------------------------------------------------ shared prompts (ctb_gpt_engine_share_prompt)
+extern "C" int ctb_gpt_engine_share_prompt(ctb_gpt* h, int32_t src, int32_t dst, int32_t T0, int32_t c0, void* stream) {
+  if (!h) return set_err(CTB_ERR_ARG, "null argument");
+  if (!h->engine) return set_err(CTB_ERR_STATE, "ctb_gpt_engine_begin has not been called");
+  const int S = h->B;
+  if (src < 0 || src >= S || dst < 0 || dst >= S || src == dst)
+    return set_err(CTB_ERR_ARG, "slots %d -> %d: two distinct slots of [0,%d)", src, dst, S);
+  if (T0 < 8 || T0 > h->cfg.max_context - 1) return set_err(CTB_ERR_ARG, "T0=%d outside [8,%d]", T0, h->cfg.max_context - 1);
+  if (c0 < CTB_PREFILL_CHUNK_ALIGN || c0 % CTB_PREFILL_CHUNK_ALIGN || c0 >= T0)
+    return set_err(CTB_ERR_ARG, "c0=%d: a positive multiple of %d below T0=%d", c0, CTB_PREFILL_CHUNK_ALIGN, T0);
+  cudaStream_t s = (cudaStream_t)stream;
+  RowState rs, rd;
+  CTB_CUDA(cudaMemcpyAsync(&rs, h->rows + src, sizeof(RowState), cudaMemcpyDeviceToHost, s));
+  CTB_CUDA(cudaMemcpyAsync(&rd, h->rows + dst, sizeof(RowState), cudaMemcpyDeviceToHost, s));
+  CTB_CUDA(cudaStreamSynchronize(s));
+  // a finished source still holds its KV until the slot is released or admitted again (pr_len is then 0)
+  if ((rs.state != RS_RUNNING && rs.state != RS_FINISHED) || h->pr_len[src] == 0)
+    return set_err(CTB_ERR_STATE, "slot %d holds no admitted prompt (state %d)", src, rs.state);
+  if (rd.state == RS_RUNNING || rd.state == RS_PENDING) return set_err(CTB_ERR_STATE, "slot %d is still generating", dst);
+  if (h->chunk_T0[dst]) return set_err(CTB_ERR_STATE, "slot %d has a prompt in progress", dst);
+  if (h->pg_pages && h->pg_map[dst]) return set_err(CTB_ERR_STATE, "slot %d has pages mapped", dst);
+  if (h->pr_len[src] < c0)
+    return set_err(CTB_ERR_STATE, "slot %d holds a prompt of %d positions, fewer than c0=%d", src, h->pr_len[src], c0);
+  if ((T0 > PF_ATT_MAX_T0) != (h->pr_W[src] > PF_ATT_MAX_T0))
+    return set_err(CTB_ERR_ARG, "T0=%d and slot %d's prompt width %d take different prefill attention kernels", T0, src,
+                   h->pr_W[src]);
+  const int shared = c0 / kPageTokens;
+  int rc;
+  if (h->pg_pages) {  // dst's entries [0, shared) map src's pages; [shared, ceil(T0 / 16)) map pages of its own
+    const int own = (T0 + kPageTokens - 1) / kPageTokens - shared;
+    if ((size_t)own > h->pg_free.size())
+      return set_err(CTB_ERR_POOL, "KV pool: %d more pages needed, %zu of %d free", own, h->pg_free.size(),
+                     h->pg_pages - 1);
+    std::vector<std::pair<int, int>> e;
+    for (int k = 0; k < shared + own; ++k) {
+      int page;
+      if (k < shared) {
+        page = h->pg_bt[(size_t)src * h->pages_per_row + k];
+        ++h->pg_ref[page];
+      } else {
+        page = h->pg_free.back();
+        h->pg_free.pop_back();
+        h->pg_ref[page] = 1;
+      }
+      const int idx = dst * h->pages_per_row + k;
+      h->pg_bt[idx] = page;
+      e.emplace_back(idx, page);
+    }
+    h->pg_map[dst] = shared + own;
+    if ((rc = bt_write(h, e, s))) return rc;
+  } else {  // a fixed engine: row b owns pages [b * bt_per_row, (b + 1) * bt_per_row)
+    KvCopyP p{};
+    p.kv = reinterpret_cast<char*>(h->kv); p.layer_bytes = h->kv_layer_elems * kv_elem_bytes(h);
+    p.page_words = (int)(page_bytes(h) / 16); p.layers = h->cfg.num_layers; p.npages = shared;
+    p.src0 = src * (int)h->bt_per_row; p.dst0 = dst * (int)h->bt_per_row;
+    k_kv_copy<<<(unsigned)std::min(p.layers * shared, g_num_sms * 8), 256, 0, s>>>(p);
+    CTB_LAUNCH_CHECK();
+  }
+  h->chunk_T0[dst] = T0; h->chunk_done[dst] = c0;  // the final chunk [c0, T0) admits the request
+  h->pr_len[dst] = 0;
   return CTB_OK;
 }
 

@@ -1,5 +1,6 @@
 // On-demand KV pages of a slot engine (ctb_gpt_engine_begin_paged): block-table writes, page fills, one slot's loop
-// state, and the gather / scatter of one slot's pages between the pool and a host image (k_kv_pack / k_kv_unpack).
+// state, and the gather / scatter of one slot's pages between the pool and a host image (k_kv_pack / k_kv_unpack);
+// and the copy of a shared prompt's pages between two rows of a fixed engine (k_kv_copy).
 // The decode, prefill and attention kernels are not involved: they reach the pool only through the block table.
 #pragma once
 #include "gpt_kernels.cuh"
@@ -37,6 +38,14 @@ struct KvMoveP {
   int page_words;       // 16-byte words of one page of one layer
   int layers, npages;
   int pages[KV_MOVE_MAX_PAGES];
+};
+
+// pages [0, npages) of every layer of one fixed-engine row (pages src0 + i) to another's (dst0 + i)
+struct KvCopyP {
+  char* kv;             // the pool
+  size_t layer_bytes;   // one layer's share of the pool
+  int page_words;       // 16-byte words of one page of one layer
+  int layers, npages, src0, dst0;
 };
 
 struct SetRowP {
@@ -77,6 +86,26 @@ __device__ __forceinline__ void kv_move(const KvMoveP& p) {
 }
 __global__ void k_kv_pack(const __grid_constant__ KvMoveP p) { kv_move<true>(p); }
 __global__ void k_kv_unpack(const __grid_constant__ KvMoveP p) { kv_move<false>(p); }
+
+// A shared prompt's KV on a fixed engine (ctb_gpt_engine_share_prompt): a CTA per (layer, page) pair in turn, its
+// threads over the page's 16-byte words, four loads in flight per thread before their stores
+__global__ void k_kv_copy(const __grid_constant__ KvCopyP p) {
+  constexpr int U = 4;
+  for (int pg = blockIdx.x; pg < p.layers * p.npages; pg += gridDim.x) {
+    const int l = pg / p.npages, i = pg - l * p.npages;
+    const uint4* __restrict__ s = reinterpret_cast<const uint4*>(p.kv + l * p.layer_bytes) + (size_t)(p.src0 + i) * p.page_words;
+    uint4* __restrict__ d = reinterpret_cast<uint4*>(p.kv + l * p.layer_bytes) + (size_t)(p.dst0 + i) * p.page_words;
+    for (int w = threadIdx.x; w < p.page_words; w += U * blockDim.x) {
+      uint4 v[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u)
+        if (w + u * (int)blockDim.x < p.page_words) v[u] = s[w + u * blockDim.x];
+#pragma unroll
+      for (int u = 0; u < U; ++u)
+        if (w + u * (int)blockDim.x < p.page_words) d[w + u * blockDim.x] = v[u];
+    }
+  }
+}
 
 // slot b's RowState <- row (outside the captured graphs, between decode chunks); all_finished = no running row, as
 // k_cancel_rows leaves it

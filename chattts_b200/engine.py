@@ -154,7 +154,14 @@ class Request:
     with the same seed: it draws rows ``b * rows ... (b + 1) * rows - 1`` of that batch's Exp(1) noise (``rows``: 1
     for text, ``num_vq`` for codes) instead of the rows of a batch of one.  Nothing else the sampler computes depends
     on the row, as long as the repetition penalty covers the row (``check_noise_batch``).  ``None`` and ``(1, 0)`` are
-    a batch of one; an unseeded request ignores it."""
+    a batch of one; an unseeded request ignores it.
+
+    ``prompt_key``: any hashable (default None: none).  Requests with equal keys promise the same ``emb`` and
+    ``infer_text`` (checked against the first live request of the key when they are submitted): several takes of one
+    utterance.  When one of them is running in a slot, a waiting one is admitted by sharing that slot's KV for prompt
+    columns ``[0, c0)``, ``c0 = 128 * floor((T - 1) / 128)`` (``shared_prompt_cols``), and prefilling only ``[c0, T)``
+    (``ctb_gpt_engine_share_prompt`` and the final prefill chunk); its outputs are bit for bit those of its normal
+    admission.  Prompts of 128 tokens or fewer are admitted as usual."""
 
     emb: torch.Tensor
     temperature: Sequence[float]
@@ -169,6 +176,7 @@ class Request:
     then: Optional[Callable[[object], object]] = None
     prepare: Optional[Callable[[object, list], None]] = None
     noise_batch: Optional[Tuple[int, int]] = None
+    prompt_key: object = None
 
     def __post_init__(self):
         if self.emb.dim() == 3:
@@ -187,6 +195,27 @@ class Request:
             B, b = (int(x) for x in self.noise_batch)
             self.noise_batch = (B, b)
             check_noise_batch(self, 1 if self.infer_text else None)
+
+
+def shared_prompt_cols(T: int) -> int:
+    """Columns of a prompt of ``T`` tokens that a request sharing another slot's prompt takes from it: the last chunk
+    boundary (a multiple of ``PREFILL_CHUNK_ALIGN``) before its last column, 0 for prompts of up to 128 tokens."""
+    return (T - 1) // PREFILL_CHUNK_ALIGN * PREFILL_CHUNK_ALIGN
+
+
+def check_prompt_key(r: Request, first: "weakref.WeakValueDictionary") -> None:
+    """Raise ``ValueError`` unless ``r`` has the prompt (``emb``, ``infer_text``) of ``first[r.prompt_key]``, the first
+    request of its key still alive; ``r`` becomes that one when there is none."""
+    if r.prompt_key is None:
+        return
+    f = first.get(r.prompt_key)
+    if f is None:
+        first[r.prompt_key] = r
+        return
+    if (f.emb.shape != r.emb.shape or bool(f.infer_text) != bool(r.infer_text)
+            or not torch.equal(f.emb, r.emb.to(f.emb.device, f.emb.dtype))):
+        raise ValueError(f"prompt_key {r.prompt_key!r}: the request's prompt differs from that of the key's first "
+                         f"request (same emb and infer_text required)")
 
 
 def check_noise_batch(r: Request, rows: Optional[int], max_batch: Optional[int] = None) -> None:
@@ -258,6 +287,11 @@ class ScheduleStats:
     suspensions: int = 0
     resumes: int = 0
     host_bytes: List[int] = field(default_factory=list)
+    # shared prompts (Request.prompt_key): requests admitted by sharing another slot's prompt, the prompt columns they
+    # did not prefill, and (KV pool) the peak of pages mapped by more than one slot
+    shares: int = 0
+    shared_cols: int = 0
+    peak_shared_pages: int = 0
     keys: Dict[int, object] = field(default_factory=dict)  # open source: index of a submitted request -> its key
     failed: Dict[int, BaseException] = field(default_factory=dict)  # open source: request index -> its follow-up's error
 
@@ -418,7 +452,20 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
        entry: ``dev.harvest`` reads it); an interrupt ends suspended requests as it ends running ones.
 
     ``stats`` records the pages mapped at each poll and their peak, the suspensions, the resumes and the host bytes
-    held by images.  Without a pool none of these calls are made."""
+    held by images.  Without a pool none of these calls are made.
+
+    Shared prompts (``Request.prompt_key``; ``dev.share(src, dst, index, c0) -> bool``, ``dev.shared_pages``): a
+    holder of a key is a running slot (not suspended, not resumed) whose request has the key and whose prompt was
+    prefilled there, wholly or by chunks, or shared.  A waiting keyed request of ``T > 128`` tokens whose key has a
+    holder takes its place in the queue as usual, but is admitted by ``dev.share(holder, slot, index, c0)`` (``c0 =
+    shared_prompt_cols(T)``) and the final chunk ``dev.prefill_chunk(slot, index, c0, T - c0)``.  Several members
+    waiting at one poll with no holder: the first is admitted normally and the others share from it at the same poll.
+    The shares of a poll follow its admission call on the same stream.  A member that finds no holder is an
+    ordinary request.  A share's final chunk costs ``T - c0`` columns of the prefill budget; when they do not fit, the
+    member waits at the head of the queue for the next poll.  With a KV pool, a share needs pages for positions
+    ``[c0, T + chunk)`` only: when the pool (counted in physical pages) cannot cover them, it waits at the head of the
+    queue.  A suspended member resumes into pages of its own, and a resumed request is no holder.  ``stats`` records
+    the shares, the prompt columns they did not prefill, and the peak of shared pages."""
     stats = stats if stats is not None else ScheduleStats()
     pool = getattr(dev, "pool_pages", None)
     admitted_at: Dict[int, int] = {}  # request index -> admission number (suspension victims: the highest)
@@ -444,6 +491,14 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
 
     def note_admitted(i: int) -> None:
         admitted_at[i] = next(admission_no)
+
+    holders: Dict[int, Tuple[object, int]] = {}  # slot -> (prompt key, request index) of a request admitted there
+
+    def holder(key) -> Optional[int]:
+        for s, (k, i) in holders.items():
+            if k == key and owner[s] == i:
+                return s
+        return None
     budget = prefill_budget
     prog: Optional[List[int]] = None  # the prompt in progress: [slot, request index, columns done]
     left = budget  # prompt columns this poll may still prefill
@@ -461,6 +516,8 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
         if c0 + n == T:
             prog = None
             stats.admitted += 1
+            if requests[i].prompt_key is not None:
+                holders[s] = (requests[i].prompt_key, i)
             if pool is not None:
                 note_admitted(i)
         else:
@@ -534,31 +591,69 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
             ahead.append(s)
             stats.resumes += 1
         batch = []
+        shares = []  # (slot, request index, source slot, c0): after the admission of `batch`
+        share_cols = share_pages = 0  # the shares' final chunks' columns, and the pages they will map
         created = False
         if prog is not None:
             advance()
         # the requests behind a prompt in progress, or behind a suspended request, wait for it
         while free and waiting and prog is None and not suspended:
             s, i = free.pop(0), waiting.popleft()
+            r = requests[i]
+            T = int(r.emb.shape[0])
+            if r.prompt_key is not None and shared_prompt_cols(T) > 0:
+                src = holder(r.prompt_key)
+                if src is None:  # a member admitted at this poll
+                    src = next((t for t, j in batch if requests[j].prompt_key == r.prompt_key), None)
+                if src is not None:
+                    c0 = shared_prompt_cols(T)
+                    need = -(-limit(i, T) // _lib.PAGE_TOKENS) - c0 // _lib.PAGE_TOKENS
+                    if ((budget is not None
+                         and admission_cols(batch, requests, dev.max_context) + share_cols + T - c0 > left)
+                            or (pool is not None and dev.pages_in_use + share_pages + need > pool - 1)):
+                        waiting.appendleft(i)  # the budget or the pool is short: it waits at the head of the queue
+                        break
+                    owner[s] = i
+                    shares.append((s, i, src, c0))
+                    share_cols += T - c0
+                    share_pages += need
+                    continue
             # no budget, no bound: admission_cols (quadratic in the admission's size) is not evaluated
-            if budget is not None and admission_cols(batch + [(s, i)], requests, dev.max_context) > left:
+            if budget is not None and admission_cols(batch + [(s, i)], requests, dev.max_context) + share_cols > left:
                 owner[s] = i
                 prog, created = [s, i, 0], True  # the first request that does not fit
                 break
-            if pool is not None and not reserve([s], [limit(i, int(requests[i].emb.shape[0]))]):
+            if pool is not None and share_pages and (
+                    dev.pages_in_use + share_pages + -(-limit(i, T) // _lib.PAGE_TOKENS) > pool - 1):
+                waiting.appendleft(i)  # the pages the shares ahead of it need come first
+                break
+            if pool is not None and not reserve([s], [limit(i, T)]):
                 waiting.appendleft(i)  # the pool is short: it waits for pages at the head of the queue
                 break
             owner[s] = i
             batch.append((s, i))
         if budget is not None:
-            left -= admission_cols(batch, requests, dev.max_context)
+            left -= admission_cols(batch, requests, dev.max_context) + share_cols
         if batch:
             dev.admit(batch)
             stats.admissions += 1
             stats.admitted += len(batch)
-            if pool is not None:
-                for _, i in batch:
+            for s, i in batch:
+                if pool is not None:
                     note_admitted(i)
+                if requests[i].prompt_key is not None:
+                    holders[s] = (requests[i].prompt_key, i)
+        for s, i, src, c0 in shares:
+            T = int(requests[i].emb.shape[0])
+            if not dev.share(src, s, i, c0) or (pool is not None and not reserve([s], [limit(i, T)])):
+                raise RuntimeError("a shared prompt's pages were counted and did not fit")  # share_pages covers them
+            if pool is not None:
+                note_admitted(i)
+            dev.prefill_chunk(s, i, c0, T - c0)
+            holders[s] = (requests[i].prompt_key, i)
+            stats.shares += 1
+            stats.shared_cols += c0
+            stats.admitted += 1
         if created:  # its first chunk, from the budget left over
             advance()
         st = dev.status()
@@ -648,6 +743,7 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
             i = owner[s]
             suspended.append([i, dev.suspend(s), st.end_idx[s]])
             mapped.pop(s, None)
+            holders.pop(s, None)
             suspended.sort(key=lambda e: admitted_at[e[0]])
             owner[s] = None
             running.remove(s)
@@ -656,6 +752,7 @@ def _poll_cycles(requests: List[Request], dev, chunk: int, context=None, stats: 
             stats.pages.append(dev.pages_in_use)
             stats.peak_pages = max(stats.peak_pages, dev.pages_in_use)
             stats.host_bytes.append(dev.host_bytes)
+            stats.peak_shared_pages = max(stats.peak_shared_pages, getattr(dev, "shared_pages", 0))
         if running:
             dev.decode(chunk)
 
@@ -781,7 +878,11 @@ class EngineDevice:
             _lib.check(self.lib.ctb_gpt_engine_begin_paged(
                 gpt._handle, slots, max_new_cap, flags, kv_pool_pages, C.c_void_p(self.ids_out.data_ptr()), hid,
                 self.stream))
-        self._mapped = [0] * slots  # pages of each slot
+        # the pool's pages as the block table maps them: each slot's entries (page numbers of this mirror, not the
+        # device's) and the entries that map each page, so shared pages count once
+        self._pages: List[List[int]] = [[] for _ in range(slots)]
+        self._refs: Dict[int, int] = {}
+        self._page_ids = itertools.count()
         # the images of suspended requests, by id, while anything holds them (a cancelled one's ends with its outputs)
         self._images: "weakref.WeakValueDictionary[int, SlotImage]" = weakref.WeakValueDictionary()
         self._resumed: List[SlotImage] = []  # read by the device until the next status read
@@ -854,7 +955,25 @@ class EngineDevice:
     # ---------------------------------------------------------------- KV pool (paged engines)
     @property
     def pages_in_use(self) -> int:
-        return sum(self._mapped)
+        """Pages mapped, each counted once however many slots share it."""
+        return len(self._refs)
+
+    @property
+    def shared_pages(self) -> int:
+        """Pages more than one slot maps (shared prompts)."""
+        return sum(1 for n in self._refs.values() if n > 1)
+
+    def _map(self, slot: int, pages: List[int]) -> None:
+        for p in pages:
+            self._refs[p] = self._refs.get(p, 0) + 1
+        self._pages[slot] += pages
+
+    def _unmap(self, slot: int) -> None:
+        for p in self._pages[slot]:
+            self._refs[p] -= 1
+            if not self._refs[p]:
+                del self._refs[p]
+        self._pages[slot] = []
 
     @property
     def host_bytes(self) -> int:
@@ -873,7 +992,8 @@ class EngineDevice:
             return False
         _lib.check(rc)
         for s, t in zip(slots, tokens):
-            self._mapped[s] = max(self._mapped[s], -(-t // _lib.PAGE_TOKENS))
+            new = -(-t // _lib.PAGE_TOKENS) - len(self._pages[s])
+            self._map(s, [next(self._page_ids) for _ in range(max(0, new))])
         return True
 
     def release(self, slots: List[int]) -> None:
@@ -881,7 +1001,7 @@ class EngineDevice:
         _lib.check(self.lib.ctb_gpt_engine_release(self.gpt._handle, len(slots), (C.c_int32 * len(slots))(*slots),
                                                    self.stream))
         for s in slots:
-            self._mapped[s] = 0
+            self._unmap(s)
 
     def suspend(self, slot: int) -> SlotImage:
         """Move the running request in ``slot`` to a pinned host image (ctb_gpt_engine_suspend); the slot and its pages
@@ -891,7 +1011,7 @@ class EngineDevice:
         buf = torch.empty(nbytes.value, dtype=torch.uint8, pin_memory=True)
         _lib.check(self.lib.ctb_gpt_engine_suspend(self.gpt._handle, slot, C.c_void_p(buf.data_ptr()), nbytes.value,
                                                    self.stream))
-        self._mapped[slot] = 0
+        self._unmap(slot)
         image = SlotImage(buf, self._text[slot], self.dev, self.gpt.num_vq, self.gpt.config.hidden_size,
                           self._torch_stream)
         self._images[id(image)] = image
@@ -904,6 +1024,22 @@ class EngineDevice:
         self._text[slot] = image.text
         self._images.pop(id(image), None)
         self._resumed.append(image)  # the copies read it until the stream passes them
+
+    def share(self, src: int, dst: int, index: int, c0: int) -> bool:
+        """Set up ``dst`` for request ``index`` with prompt columns ``[0, c0)`` taken from the prompt of the request in
+        ``src`` (ctb_gpt_engine_share_prompt); ``prefill_chunk(dst, index, c0, T - c0)`` then admits it.  A paged
+        engine maps ``src``'s pages for them, and pages of ``dst``'s own up to the prompt's end: False, with nothing
+        changed, when the pool cannot cover those."""
+        T = int(self.requests[index].emb.shape[0])
+        rc = self.lib.ctb_gpt_engine_share_prompt(self.gpt._handle, src, dst, T, c0, self.stream)
+        if rc == _lib.ERR_POOL:
+            return False
+        _lib.check(rc)
+        if self.pool_pages is not None:
+            shared = c0 // _lib.PAGE_TOKENS
+            self._map(dst, self._pages[src][:shared])
+            self._map(dst, [next(self._page_ids) for _ in range(-(-T // _lib.PAGE_TOKENS) - shared)])
+        return True
 
     def cancel(self, slots: List[int]) -> None:
         """Stop the requests in ``slots`` (ctb_gpt_engine_cancel): each keeps the tokens it has."""
@@ -1050,13 +1186,15 @@ class OpenEngine:
     every pending job with it, stops the engine and is raised again by ``close``.  With a ``context`` (``GPT.Context``)
     an interrupt is ``schedule``'s: at the first poll that sees it the running requests end with what they have, the
     engine stops, and every job that has not ended by then is cancelled.  Subclasses turn each poll's yields into job
-    results (``_serve``).  ``prefill_budget``: ``_poll_cycles``' bound on each poll's prompt columns (None: none)."""
+    results (``_serve``).  ``prefill_budget``: ``_poll_cycles``' bound on each poll's prompt columns (None: none).
+    ``slots``: the device's slot count, when known."""
 
     def __init__(self, make_device: Callable[[List[Request]], object], chunk: int,
                  check: Optional[Callable[[Request], None]] = None, device=None,
                  on_close: Optional[Callable[[], None]] = None, max_new_cap: Optional[int] = None, context=None,
-                 prefill_budget: Optional[int] = None):
+                 prefill_budget: Optional[int] = None, slots: Optional[int] = None):
         self._make_device, self.chunk, self._check, self._on_close = make_device, int(chunk), check, on_close
+        self.slots = slots
         self.prefill_budget = check_prefill_budget(prefill_budget)
         self.device, self.max_new_cap, self._context = device, max_new_cap, context
         cuda = device is not None and torch.device(device).type == "cuda"

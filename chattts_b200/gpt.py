@@ -11,6 +11,7 @@ from __future__ import annotations
 import ctypes as C
 import logging
 import os
+import weakref
 from dataclasses import dataclass, field
 from typing import Callable, Dict, List, Optional, Tuple, Union
 
@@ -265,7 +266,12 @@ class GPT:
         engine's KV memory: slots take 16-token pages from a pool of that many bytes as they grow, and when it runs
         short the running request admitted last is suspended to pinned host memory and resumed later, in any slot, bit
         for bit as if it had not moved (``engine._poll_cycles``).  A request whose prompt + ``max_new_token`` does not
-        fit in the pool alone is refused.  ``last_schedule_stats`` records pages, suspensions and resumes."""
+        fit in the pool alone is refused.  ``last_schedule_stats`` records pages, suspensions and resumes.
+
+        Requests with equal ``Request.prompt_key`` (several takes of one utterance) must have equal prompts
+        (``ValueError`` otherwise).  While one of them runs, another is admitted by taking that slot's KV for all but
+        the last chunk of at most 128 prompt columns and prefilling only that chunk (``engine._poll_cycles``), with
+        the same outputs; a paged engine shares the pages themselves.  ``last_schedule_stats`` records the shares."""
         from .engine import ScheduleStats, check_prefill_budget, kv_pool_pages, schedule
 
         flags = _lib.engine_flags(dtype)
@@ -359,7 +365,7 @@ class GPT:
         pool = kv_pool_pages(self.config, kv_pool_bytes, flags)
         _, S, chunk, _, cap, check = self._engine_args("open_engine", [], slots, False, False, None, chunk, None,
                                                        max_new_cap, pool)
-        kw = {} if prefill_budget is None else {"prefill_budget": prefill_budget}
+        kw = {"slots": S} if prefill_budget is None else {"prefill_budget": prefill_budget, "slots": S}
         engine = cls(lambda requests: self._engine_device(requests, S, cap, return_hidden, flags, pool), chunk, check,
                      self.device_gpt, self._close_engine, *args, max_new_cap=cap, **kw)
         self._open = engine
@@ -387,9 +393,10 @@ class GPT:
                      max_new_cap=None, pool_pages=None):
         """Checks shared by the slot-engine generators -> (requests, slots, chunk, context, max_new_cap, check), where
         ``check`` validates a follow-up request as the up-front ones are (with a KV pool of ``pool_pages`` pages, also
-        that it fits in the pool alone).  The poll interval is `chunk`, else CTB_DECODE_CHUNK, else `default_chunk`
+        that it fits in the pool alone; with a ``prompt_key``, that its prompt is that of the key's first live
+        request).  The poll interval is `chunk`, else CTB_DECODE_CHUNK, else `default_chunk`
         (None: the smallest ``stream_batch``)."""
-        from .engine import MIN_PROMPT_COLS, Request, check_noise_batch, pool_pages_needed
+        from .engine import MIN_PROMPT_COLS, Request, check_noise_batch, check_prompt_key, pool_pages_needed
 
         self._check_free(name)
         if infer_text:
@@ -408,6 +415,7 @@ class GPT:
         cap = max((r.max_new_token for r in requests), default=1) if max_new_cap is None else int(max_new_cap)
         if cap < 1 or cap >= self.max_context:
             raise ValueError(f"max_new_cap={cap} outside [1, max_context={self.max_context})")
+        keyed = weakref.WeakValueDictionary()  # prompt key -> the first of its requests still alive
 
         def check(r):
             if not isinstance(r, Request):
@@ -422,6 +430,7 @@ class GPT:
                 raise ValueError(f"prompt {int(r.emb.shape[0])} + max_new_token {r.max_new_token} need "
                                  f"{pool_pages_needed(r)} KV pages; the pool has {pool_pages - 1} (kv_pool_bytes)")
             check_noise_batch(r, 1 if r.infer_text else self.num_vq, self.max_batch)
+            check_prompt_key(r, keyed)
 
         for r in requests:
             check(r)

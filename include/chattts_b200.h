@@ -328,6 +328,28 @@ int ctb_gpt_engine_suspend(ctb_gpt* h, int32_t slot, void* host_buf, uint64_t ho
  * engine shape (magic, precision, page, noise or hidden-state layout, max_new_cap). */
 int ctb_gpt_engine_resume(ctb_gpt* h, int32_t slot, const void* host_buf, uint64_t host_bytes, void* stream);
 
+/* ---- Shared prompts: a request whose prompt equals the one slot `src` was admitted with takes that slot's KV for
+ * prompt columns [0, c0) instead of prefilling them.  Sets up slot `dst` as a prompt of T0 columns in progress with
+ * [0, c0) done; the next call for it must be its final chunk, ctb_gpt_engine_prefill_chunk(dst, T0, c0, T0 - c0, ...),
+ * which samples its first token with its own sampler and noise.  Its results are then bit for bit those of admitting
+ * the request normally, provided the two prompts are equal: the handle cannot check that, and c0 being a chunk
+ * boundary (CTB_PREFILL_CHUNK_ALIGN) is what makes the final chunk after [0, c0) equal a one-call admission.
+ *   A fixed engine copies positions [0, c0) of every layer from src's pages to dst's (k_kv_copy, enqueued on
+ *   `stream`).  A paged engine copies nothing: dst's block-table entries [0, c0 / 16) map src's pages, whose
+ *   reference counts rise, and entries [c0 / 16, ceil(T0 / 16)) map pages of dst's own.  A page returns to the free
+ *   list (and is poisoned under CTB_KV_POISON=1) when its last entry is released; ctb_gpt_engine_suspend releases the
+ *   suspended slot's entries, so a resumed request holds private pages only.  No call writes a page that more than one
+ *   entry maps: admissions, chunks, decode steps and resumes that would are refused with CTB_ERR_STATE.
+ * `src` is a slot whose admitted prompt's KV is still in place: running, or finished and neither released nor given
+ * another prompt, prefill or image since (a resumed request is no source).  Synchronises `stream` once to read both
+ * slots' states.
+ * Errors (the handle as it was): CTB_ERR_STATE outside a slot engine, when src holds no admitted prompt or one of fewer
+ * than c0 positions, or when dst is running, pending, has a prompt in progress or (paged) has pages mapped;
+ * CTB_ERR_ARG for src == dst, a slot out of range, T0 outside [8, max_context - 1], c0 that is not a positive
+ * multiple of CTB_PREFILL_CHUNK_ALIGN below T0, or T0 and src's prompt width on different sides of 1,024 columns
+ * (different prefill attention kernels); CTB_ERR_POOL (paged) when the free list cannot map dst's own pages. */
+int ctb_gpt_engine_share_prompt(ctb_gpt* h, int32_t src, int32_t dst, int32_t T0, int32_t c0, void* stream);
+
 /* Measurement hook for bench.py's roofline: launches ONE kernel kind once per layer on the
  * state left by the last generate call (kind 0 qkv, 1 attention, 2 o-proj, 3 gate/up, 4 down;
  * 5 = heads, 6 = sampler, 7 = one decode step as ONE kernel launch (k_flow / k_step), 8 = 16 decode steps in one
