@@ -97,7 +97,8 @@ EXPORTS = (
     "ctb_gpt_destroy", "ctb_gpt_begin", "ctb_gpt_decode", "ctb_gpt_status_query", "ctb_gpt_profile_kernel", "ctb_gpt_debug_trace", "ctb_gpt_embed_prompt", "ctb_sample",
     "ctb_gpt_engine_begin", "ctb_gpt_engine_admit", "ctb_gpt_engine_admit_text", "ctb_gpt_engine_status",
     "ctb_gpt_engine_cancel", "ctb_gpt_engine_begin_ex", "ctb_gpt_engine_prefill_chunk",
-    "ctb_gpt_engine_begin_paged", "ctb_gpt_engine_reserve", "ctb_gpt_engine_release", "ctb_gpt_engine_suspend_bytes",
+    "ctb_gpt_engine_begin_paged", "ctb_gpt_engine_reserve", "ctb_gpt_engine_release", "ctb_gpt_engine_pages",
+    "ctb_gpt_engine_suspend_bytes",
     "ctb_gpt_engine_suspend", "ctb_gpt_engine_resume", "ctb_gpt_engine_share_prompt",
     "ctb_dvae_blob_floats", "ctb_vocos_blob_floats", "ctb_decoder_create", "ctb_decoder_destroy",
     "ctb_dvae_decode", "ctb_vocos_decode", "ctb_decode_rows",
@@ -156,6 +157,7 @@ def load(build_if_missing: bool = True):
         lib.ctb_gpt_engine_begin_paged.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp]
         lib.ctb_gpt_engine_reserve.argtypes = [vp, i32, vp, vp, vp]
         lib.ctb_gpt_engine_release.argtypes = [vp, i32, vp, vp]
+        lib.ctb_gpt_engine_pages.argtypes = [vp, C.POINTER(i32), C.POINTER(i32)]
         lib.ctb_gpt_engine_suspend_bytes.argtypes = [vp, i32, C.POINTER(C.c_uint64), vp]
         lib.ctb_gpt_engine_suspend.argtypes = [vp, i32, vp, C.c_uint64, vp]
         lib.ctb_gpt_engine_resume.argtypes = [vp, i32, vp, C.c_uint64, vp]

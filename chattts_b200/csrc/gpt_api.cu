@@ -43,6 +43,15 @@ static int bt_for(int B) {
 using namespace ctb;
 using ctb::g_num_sms;
 
+// What the host knows of one slot of a slot engine (ctb_gpt::slot); all zero when ctb_gpt_engine_begin* starts it
+struct SlotRecord {
+  int chunk_T0, chunk_done;  // prompt being prefilled in chunks: its width (0: none), the columns in the slot's pages
+  int pr_len, pr_W;  // admitted prompt its pages hold (a share's source): its positions (0: none), the kernels' width
+  int pages;         // block-table entries mapped (paged engines)
+  int hi;            // positions its request may hold after the steps enqueued so far (0: none)
+  int cap;           // and at most: prompt + max_new - 1
+};
+
 struct ctb_gpt {
   ctb_gpt_config cfg;
   ctb_gpt_layout lay;
@@ -110,12 +119,7 @@ struct ctb_gpt {
   int eng_text;
   cudaGraphExec_t graph_exec_text;
   uint64_t graph_kernels_text;
-  // per slot: the prompt being prefilled in chunks (ctb_gpt_engine_prefill_chunk) - its width (0: none) and the columns
-  // already in the slot's pages
-  std::vector<int> chunk_T0, chunk_done;
-  // per slot: the admitted prompt whose KV its pages hold (ctb_gpt_engine_share_prompt's source) - its positions
-  // (pr_len, 0: none) and the width whose attention kernel prefilled it (pr_W)
-  std::vector<int> pr_len, pr_W;
+  std::vector<SlotRecord> slot;  // [S] host-side record of each slot
   // ---- half-precision slot engine (ctb_gpt_engine_begin_ex)
   int prec;                   // CTB_ENGINE_FP16_* bits of the current engine (0 for fp32 engines and generate())
   bool tc_base;               // tensor-core activation scratch, head copies and their tensor maps exist (tc_setup_base)
@@ -128,10 +132,8 @@ struct ctb_gpt {
   bool pg_poison;             // CTB_KV_POISON=1 at begin: free pages hold quiet-NaN bits
   std::vector<int> pg_free;   // free pages, taken from the back
   std::vector<int> pg_bt;     // [S][pages_per_row] host copy of the block table
-  // per slot: pages mapped, and the tokens its request may hold after the steps enqueued so far (pg_hi, 0: none) and
-  // at most (pg_cap: prompt + max_new - 1)
-  std::vector<int> pg_map, pg_hi, pg_cap;
   std::vector<int> pg_ref;    // [pool_pages] block-table entries that map each page (above 1: a shared prompt's)
+  int pg_shared;              // pages whose count is above 1
   char* pg_stage;             // KV_STAGE_BYTES of device staging for suspend / resume (allocated by the first one)
 };
 
@@ -140,17 +142,81 @@ static size_t kv_elem_bytes(const ctb_gpt* h) { return (h->prec & CTB_ENGINE_FP1
 static float* kv_layer(const ctb_gpt* h, int l) {
   return reinterpret_cast<float*>(reinterpret_cast<char*>(h->kv) + (size_t)l * h->kv_layer_elems * kv_elem_bytes(h));
 }
+static size_t page_elems(const ctb_gpt* h) { return (size_t)2 * h->cfg.num_kv_heads * kPageTokens * h->cfg.head_dim; }
+static size_t page_bytes(const ctb_gpt* h) { return page_elems(h) * kv_elem_bytes(h); }  // one page of one layer
 
 // floats of one slot's noise in the engine's buffer: room for a code request's or a text request's rows
 static size_t noise_stride(const ctb_gpt* h) {
   return std::max((size_t)h->cfg.num_vq * h->cfg.num_audio_tokens, (size_t)h->cfg.num_text_tokens);
 }
 
-// A paged engine's kernels write only pages that a single block-table entry maps: CTB_ERR_STATE if slot b's pages
-// for positions [lo, hi) include one it shares with another slot (ctb_gpt_engine_share_prompt)
-static int check_private(const ctb_gpt* h, int b, int lo, int hi) {
+static int check_engine(const ctb_gpt* h) {
+  return h->engine ? CTB_OK : set_err(CTB_ERR_STATE, "ctb_gpt_engine_begin has not been called");
+}
+
+static int check_paged(const ctb_gpt* h) {
+  if (!h->engine || !h->pg_pages) return set_err(CTB_ERR_STATE, "not a paged slot engine (ctb_gpt_engine_begin_paged)");
+  return CTB_OK;
+}
+
+static int check_slot_list(const ctb_gpt* h, int n, const int32_t* slots) {
+  if (n < 1 || n > h->B) return set_err(CTB_ERR_ARG, "n=%d outside [1,%d]", n, h->B);
+  std::vector<char> seen((size_t)h->B, 0);
+  for (int i = 0; i < n; ++i) {
+    if (slots[i] < 0 || slots[i] >= h->B || seen[slots[i]])
+      return set_err(CTB_ERR_ARG, "slot %d out of range or repeated", slots[i]);
+    seen[slots[i]] = 1;
+  }
+  return CTB_OK;
+}
+
+static int check_slot(const ctb_gpt* h, int slot) {
+  if (slot < 0 || slot >= h->B) return set_err(CTB_ERR_ARG, "slot %d outside [0,%d)", slot, h->B);
+  if (h->slot[slot].chunk_T0) return set_err(CTB_ERR_STATE, "slot %d has a prompt in progress", slot);
+  return CTB_OK;
+}
+
+// prompts over 1,024 columns take the tiled prefill attention; every slot owns max_context tokens of pages
+static int check_T0(const ctb_gpt* h, int T0) {
+  if (T0 < 8 || T0 > h->cfg.max_context - 1)
+    return set_err(CTB_ERR_ARG, "T0=%d outside [8,%d]: left-pad shorter prompts to 8", T0, h->cfg.max_context - 1);
+  return CTB_OK;
+}
+
+static int check_max_new(const ctb_gpt* h, int b, int T0, int max_new) {
+  if (max_new < 1 || max_new > h->max_new || T0 + max_new > h->cfg.max_context)
+    return set_err(CTB_ERR_ARG, "slot %d: max_new=%d (capacity %d) with T0=%d exceeds max_context=%d", b, max_new,
+                   h->max_new, T0, h->cfg.max_context);
+  return CTB_OK;
+}
+
+// every slot's RowState (bpad_max: an admission writes them all back); synchronises s and the caller's copies on it
+static int read_rows(ctb_gpt* h, std::vector<RowState>& rows, cudaStream_t s) {
+  rows.resize((size_t)h->bpad_max);
+  CTB_CUDA(cudaMemcpyAsync(rows.data(), h->rows, sizeof(RowState) * rows.size(), cudaMemcpyDeviceToHost, s));
+  CTB_CUDA(cudaStreamSynchronize(s));
+  return CTB_OK;
+}
+
+static int check_not_generating(const RowState& r, int b) {
+  if (r.state == RS_RUNNING || r.state == RS_PENDING) return set_err(CTB_ERR_STATE, "slot %d is still generating", b);
+  return CTB_OK;
+}
+
+// CTB_ERR_STATE unless a paged engine's slot b has pages for positions [0, hi)
+static int check_covers(const ctb_gpt* h, int b, int hi) {
+  const int held = h->slot[b].pages * kPageTokens;
+  if (h->pg_pages && held < hi)
+    return set_err(CTB_ERR_STATE, "slot %d: its pages hold %d positions, the call writes up to %d", b, held, hi);
+  return CTB_OK;
+}
+
+// CTB_ERR_STATE unless a paged engine's slot b has pages for the positions [lo, hi) a call writes, none of them mapped
+// by another entry too (kernels never write a shared prompt's pages, ctb_gpt_engine_share_prompt)
+static int check_writes(const ctb_gpt* h, int b, int lo, int hi) {
   if (!h->pg_pages) return CTB_OK;
-  for (int k = lo / kPageTokens; k * kPageTokens < hi && k < h->pg_map[b]; ++k)
+  if (int rc = check_covers(h, b, hi)) return rc;
+  for (int k = lo / kPageTokens; k * kPageTokens < hi && k < h->slot[b].pages; ++k)
     if (h->pg_ref[h->pg_bt[(size_t)b * h->pages_per_row + k]] > 1)
       return set_err(CTB_ERR_STATE, "slot %d: positions [%d,%d) reach page entry %d, which is shared", b, lo, hi, k);
   return CTB_OK;
@@ -1146,26 +1212,31 @@ static int prefill(ctb_gpt* h, int B, int T, int q0, int n, const float* emb, co
 // Pages for B rows of up to `tokens` tokens each: grow the pool if needed (page = 16 tokens x K|V x heads x 64 values per
 // layer, fp32 or fp16 by the call's CTB_ENGINE_FP16_KV bit; the pool is sized in bytes, so calls of either type reuse
 // it) and assign row b the pages [b * need, (b + 1) * need) - kernels only ever see the block table.
+static size_t pool_bytes(const ctb_gpt* h, size_t pages) { return pages * page_bytes(h) * h->cfg.num_layers; }
+
+// A pool of `pages` pages of every layer in place of the current one, which kernels on s may still read (CTB_ERR_NOMEM,
+// and no pool, when it does not fit); the callers keep a pool that serves them
+static int kv_alloc(ctb_gpt* h, size_t pages, cudaStream_t s) {
+  CTB_CUDA(cudaStreamSynchronize(s));
+  if (h->kv) { cudaFree(h->kv); h->kv = nullptr; h->kv_bytes = 0; }
+  if (cudaMalloc(reinterpret_cast<void**>(&h->kv), pool_bytes(h, pages)) != cudaSuccess) {
+    cudaGetLastError();
+    return set_err(CTB_ERR_NOMEM, "KV pool: %zu pages x %d layers (%.2f GB) do not fit", pages, h->cfg.num_layers,
+                   (double)pool_bytes(h, pages) / 1e9);
+  }
+  h->kv_bytes = pool_bytes(h, pages);
+  return CTB_OK;
+}
+
 static int kv_reserve(ctb_gpt* h, int B, int tokens, cudaStream_t s) {
-  const ctb_gpt_config& c = h->cfg;
   const size_t per_row = ((size_t)tokens + kPageTokens - 1) / kPageTokens;
   const size_t need = per_row * (size_t)B;
-  const size_t page_elems = (size_t)2 * c.num_kv_heads * kPageTokens * c.head_dim;
-  const size_t page_bytes = page_elems * kv_elem_bytes(h) * c.num_layers;  // one page of every layer
-  if (need * page_bytes > h->kv_bytes) {
-    CTB_CUDA(cudaStreamSynchronize(s));
-    if (h->kv) { cudaFree(h->kv); h->kv = nullptr; h->kv_bytes = 0; }
-    const size_t pages = need + need / 8;  // a little head-room against re-allocation on slightly longer calls
-    if (cudaMalloc(reinterpret_cast<void**>(&h->kv), pages * page_bytes) != cudaSuccess) {
-      cudaGetLastError();
-      return set_err(CTB_ERR_NOMEM, "KV pool: %zu pages x %d layers (%.1f GB) do not fit", pages, c.num_layers,
-                     (double)(pages * page_bytes) / 1e9);
-    }
-    CTB_CUDA(cudaMemsetAsync(h->kv, 0, pages * page_bytes, s));
-    h->kv_bytes = pages * page_bytes;
+  if (pool_bytes(h, need) > h->kv_bytes) {
+    if (int rc = kv_alloc(h, need + need / 8, s)) return rc;  // head-room against re-allocation on slightly longer calls
+    CTB_CUDA(cudaMemsetAsync(h->kv, 0, h->kv_bytes, s));
     h->bt_B = 0;
   }
-  h->kv_layer_elems = h->kv_bytes / page_bytes * page_elems;
+  h->kv_layer_elems = h->kv_bytes / pool_bytes(h, 1) * page_elems(h);
   if (h->bt_B == B && h->bt_per_row == per_row) return CTB_OK;  // table already describes this shape: nothing to upload
   std::vector<int> bt((size_t)B * h->pages_per_row, 0);
   for (int b = 0; b < B; ++b)
@@ -1248,14 +1319,10 @@ extern "C" int ctb_gpt_decode(ctb_gpt* h, int32_t n_steps, void* stream) {
   if (n_steps <= 0) return CTB_OK;
   if (h->pg_pages) {  // a paged engine: every slot that may run must hold the positions these steps append
     for (int b = 0; b < h->B; ++b)
-      if (h->pg_hi[b] && h->pg_map[b] * kPageTokens < std::min(h->pg_hi[b] + n_steps, h->pg_cap[b]))
-        return set_err(CTB_ERR_STATE, "slot %d: its pages hold %d positions, %d decode steps may need %d", b,
-                       h->pg_map[b] * kPageTokens, n_steps, std::min(h->pg_hi[b] + n_steps, h->pg_cap[b]));
-    for (int b = 0; b < h->B; ++b)
-      if (h->pg_hi[b] && (rc = check_private(h, b, h->pg_hi[b], std::min(h->pg_hi[b] + n_steps, h->pg_cap[b]))))
+      if (h->slot[b].hi && (rc = check_writes(h, b, h->slot[b].hi, std::min(h->slot[b].hi + n_steps, h->slot[b].cap))))
         return rc;
-    for (int b = 0; b < h->B; ++b)
-      if (h->pg_hi[b]) h->pg_hi[b] = std::min(h->pg_hi[b] + n_steps, h->pg_cap[b]);
+    for (SlotRecord& r : h->slot)
+      if (r.hi) r.hi = std::min(r.hi + n_steps, r.cap);
   }
   h->steps_enqueued += n_steps;
   if (flow_ink(h)) {
@@ -1359,10 +1426,7 @@ static int engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t flag
   CTB_CUDA(cudaMemsetAsync(h->counter, 0, sizeof(int) * c.max_batch * c.num_heads, s));
   CTB_CUDA(cudaMemsetAsync(h->x, 0, sizeof(float) * h->bpad_max * c.hidden_size, s));
   CTB_CUDA(cudaStreamSynchronize(s));  // idle_state is read by the copy engine
-  h->chunk_T0.assign((size_t)S, 0);     // no prompt in progress
-  h->chunk_done.assign((size_t)S, 0);
-  h->pr_len.assign((size_t)S, 0);       // no prompt to share
-  h->pr_W.assign((size_t)S, 0);
+  h->slot.assign((size_t)S, SlotRecord{});
   h->started = 1;
   h->steps_enqueued = 0;
   return CTB_OK;
@@ -1383,14 +1447,13 @@ static int admit(ctb_gpt* h, int n, const int32_t* slots, int T0, int q0, const 
   const ctb_gpt_config& c = h->cfg;
   const int S = h->B;
   int rc;
-  std::vector<RowState> rows((size_t)h->bpad_max);
-  CTB_CUDA(cudaMemcpyAsync(rows.data(), h->rows, sizeof(RowState) * rows.size(), cudaMemcpyDeviceToHost, s));
   std::vector<uint8_t> mask_h;  // the positions each whole prompt writes (its pages, and the prompt it can share)
   if (mask_dev) {
     mask_h.resize((size_t)n * T0);
     CTB_CUDA(cudaMemcpyAsync(mask_h.data(), mask_dev, mask_h.size(), cudaMemcpyDeviceToHost, s));
   }
-  CTB_CUDA(cudaStreamSynchronize(s));
+  std::vector<RowState> rows;
+  if ((rc = read_rows(h, rows, s))) return rc;
   std::vector<int> held((size_t)n, T0);  // positions [0, held[i]) of slot slots[i] after the prefill
   for (size_t j = 0; j < mask_h.size(); ++j) held[j / T0] -= mask_h[j] == 0;
   std::vector<char> taken((size_t)S, 0);
@@ -1399,26 +1462,19 @@ static int admit(ctb_gpt* h, int n, const int32_t* slots, int T0, int q0, const 
     const ctb_sampler_config& sc = samplers[i];
     if (b < 0 || b >= S || taken[b]) return set_err(CTB_ERR_ARG, "slot %d out of range or repeated", b);
     taken[b] = 1;
-    if (rows[b].state == RS_RUNNING || rows[b].state == RS_PENDING)
-      return set_err(CTB_ERR_STATE, "slot %d is still generating", b);
-    if (max_new[i] < 1 || max_new[i] > h->max_new || T0 + max_new[i] > c.max_context)
-      return set_err(CTB_ERR_ARG, "slot %d: max_new=%d (capacity %d) with T0=%d exceeds max_context=%d", b, max_new[i],
-                     h->max_new, T0, c.max_context);
-    if ((rc = check_sampler(sc))) return rc;
-    if (h->pg_pages && h->pg_map[b] * kPageTokens < held[i])
-      return set_err(CTB_ERR_STATE, "slot %d: its pages hold %d positions, the prompt writes %d", b,
-                     h->pg_map[b] * kPageTokens, held[i]);
-    if ((rc = check_private(h, b, q0, held[i]))) return rc;
+    if ((rc = check_not_generating(rows[b], b)) || (rc = check_max_new(h, b, T0, max_new[i])) ||
+        (rc = check_sampler(sc)) || (rc = check_writes(h, b, q0, held[i])))
+      return rc;
     RowState& r = rows[b];
     r.n_gen = 0; r.step = 0; r.state = RS_PENDING; r.max_new = max_new[i]; r.has_noise = q_noise_dev != nullptr;
     r.eos = sc.eos_token; r.text = text;
   }
   for (int i = 0; i < n; ++i) {
-    h->chunk_T0[slots[i]] = 0;  // the slot's prompt in progress, if any, is dropped
-    h->pr_len[slots[i]] = held[i]; h->pr_W[slots[i]] = T0;
+    SlotRecord& r = h->slot[slots[i]];
+    r.chunk_T0 = 0;  // the slot's prompt in progress, if any, is dropped
+    r.pr_len = held[i]; r.pr_W = T0;
+    r.hi = held[i]; r.cap = held[i] + max_new[i] - 1;
   }
-  if (h->pg_pages)
-    for (int i = 0; i < n; ++i) { h->pg_hi[slots[i]] = held[i]; h->pg_cap[slots[i]] = held[i] + max_new[i] - 1; }
   CTB_CUDA(cudaMemcpyAsync(h->rows, rows.data(), sizeof(RowState) * rows.size(), cudaMemcpyHostToDevice, s));
   CTB_CUDA(cudaMemcpyAsync(h->eng_slot, slots, sizeof(int32_t) * n, cudaMemcpyHostToDevice, s));
   const size_t nrow = text ? (size_t)c.num_text_tokens : (size_t)c.num_vq * c.num_audio_tokens;
@@ -1444,12 +1500,9 @@ static int engine_admit(ctb_gpt* h, int32_t n, const int32_t* slots, int32_t T0,
                         const uint8_t* mask_dev, const ctb_sampler_config* samplers, const float* q_noise_dev,
                         const int32_t* max_new, int text, void* stream) {
   if (!h || !slots || !emb_dev || !mask_dev || !samplers || !max_new) return set_err(CTB_ERR_ARG, "null argument");
-  if (!h->engine) return set_err(CTB_ERR_STATE, "ctb_gpt_engine_begin has not been called");
-  const ctb_gpt_config& c = h->cfg;
+  if (int rc = check_engine(h)) return rc;
   if (n < 1 || n > h->B) return set_err(CTB_ERR_ARG, "n=%d outside [1,%d]", n, h->B);
-  // prompts over 1,024 columns take the tiled prefill attention; every slot owns max_context tokens of pages
-  if (T0 < 8 || T0 > c.max_context - 1)
-    return set_err(CTB_ERR_ARG, "T0=%d outside [8,%d]: left-pad shorter prompts to 8", T0, c.max_context - 1);
+  if (int rc = check_T0(h, T0)) return rc;
   return admit(h, n, slots, T0, 0, emb_dev, mask_dev, samplers, q_noise_dev, max_new, text, (cudaStream_t)stream);
 }
 
@@ -1469,26 +1522,22 @@ extern "C" int ctb_gpt_engine_prefill_chunk(ctb_gpt* h, int32_t slot, int32_t T0
                                             const float* emb_dev, int32_t text, const ctb_sampler_config* sampler,
                                             const float* q_noise_dev, int32_t max_new, void* stream) {
   if (!h || !emb_dev) return set_err(CTB_ERR_ARG, "null argument");
-  if (!h->engine) return set_err(CTB_ERR_STATE, "ctb_gpt_engine_begin has not been called");
-  const ctb_gpt_config& c = h->cfg;
-  const int S = h->B;
-  if (slot < 0 || slot >= S) return set_err(CTB_ERR_ARG, "slot %d outside [0,%d)", slot, S);
-  if (T0 < 8 || T0 > c.max_context - 1)
-    return set_err(CTB_ERR_ARG, "T0=%d outside [8,%d]", T0, c.max_context - 1);
+  int rc;
+  if ((rc = check_engine(h))) return rc;
+  if (slot < 0 || slot >= h->B) return set_err(CTB_ERR_ARG, "slot %d outside [0,%d)", slot, h->B);
+  if ((rc = check_T0(h, T0))) return rc;
   if (c0 < 0 || n < 1 || c0 + n > T0) return set_err(CTB_ERR_ARG, "chunk [%d,%d) outside the prompt [0,%d)", c0, c0 + n, T0);
   const bool final = c0 + n == T0;
   if (c0 % CTB_PREFILL_CHUNK_ALIGN || (!final && n % CTB_PREFILL_CHUNK_ALIGN))
     return set_err(CTB_ERR_ARG, "chunk [%d,%d): c0 and a non-final chunk's n must be multiples of %d", c0, c0 + n,
                    CTB_PREFILL_CHUNK_ALIGN);
-  if (max_new < 1 || max_new > h->max_new || T0 + max_new > c.max_context)
-    return set_err(CTB_ERR_ARG, "max_new=%d (capacity %d) with T0=%d exceeds max_context=%d", max_new, h->max_new, T0,
-                   c.max_context);
-  int rc;
+  if ((rc = check_max_new(h, slot, T0, max_new))) return rc;
   if (final) {
     if (!sampler) return set_err(CTB_ERR_ARG, "null sampler on the final chunk");
     if ((rc = check_sampler(*sampler))) return rc;
   }
-  const int pT0 = h->chunk_T0[slot], pdone = h->chunk_done[slot];
+  SlotRecord& rec = h->slot[slot];
+  const int pT0 = rec.chunk_T0, pdone = rec.chunk_done;
   if (pT0 == 0 && c0 != 0)
     return set_err(CTB_ERR_STATE, "slot %d: chunk [%d,%d) but no prompt in progress (a first chunk starts at 0)", slot,
                    c0, c0 + n);
@@ -1498,34 +1547,28 @@ extern "C" int ctb_gpt_engine_prefill_chunk(ctb_gpt* h, int32_t slot, int32_t T0
   cudaStream_t s = (cudaStream_t)stream;
   // the final chunk admits the request as ctb_gpt_engine_admit / _admit_text do for one slot
   if (final) return admit(h, 1, &slot, T0, c0, emb_dev, nullptr, sampler, q_noise_dev, &max_new, text ? 1 : 0, s);
-  RowState r;
-  CTB_CUDA(cudaMemcpyAsync(&r, h->rows + slot, sizeof(RowState), cudaMemcpyDeviceToHost, s));
-  CTB_CUDA(cudaStreamSynchronize(s));
-  if (r.state == RS_RUNNING || r.state == RS_PENDING) return set_err(CTB_ERR_STATE, "slot %d is still generating", slot);
-  if (h->pg_pages && h->pg_map[slot] * kPageTokens < c0 + n)
-    return set_err(CTB_ERR_STATE, "slot %d: its pages hold %d positions, the chunk writes up to %d", slot,
-                   h->pg_map[slot] * kPageTokens, c0 + n);
-  if ((rc = check_private(h, slot, c0, c0 + n))) return rc;
-  h->pr_len[slot] = 0;  // its pages now hold part of a prompt
-  if ((rc = prefill(h, 1, T0, c0, n, emb_dev, nullptr, &slot, s))) { h->chunk_T0[slot] = 0; return rc; }
-  h->chunk_T0[slot] = T0; h->chunk_done[slot] = c0 + n;
+  std::vector<RowState> rows;
+  if ((rc = read_rows(h, rows, s)) || (rc = check_not_generating(rows[slot], slot)) ||
+      (rc = check_writes(h, slot, c0, c0 + n)))
+    return rc;
+  rec.pr_len = 0;  // its pages now hold part of a prompt
+  if ((rc = prefill(h, 1, T0, c0, n, emb_dev, nullptr, &slot, s))) { rec.chunk_T0 = 0; return rc; }
+  rec.chunk_T0 = T0; rec.chunk_done = c0 + n;
   return CTB_OK;
 }
 
 extern "C" int ctb_gpt_engine_status(ctb_gpt* h, ctb_gpt_status* out, int32_t* state_host, int32_t* end_idx_host,
                                      uint8_t* finish_host, void* stream) {
   if (!h || !out) return set_err(CTB_ERR_ARG, "null argument");
-  if (!h->engine) return set_err(CTB_ERR_STATE, "ctb_gpt_engine_begin has not been called");
+  if (int rc = check_engine(h)) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   std::vector<RowState> rows((size_t)h->B);
   CTB_CUDA(cudaMemcpyAsync(rows.data(), h->rows, sizeof(RowState) * h->B, cudaMemcpyDeviceToHost, s));
-  int rc = ctb_gpt_status_query(h, out, end_idx_host, finish_host, stream);  // synchronises `stream`
-  if (rc) return rc;
+  if (int rc = ctb_gpt_status_query(h, out, end_idx_host, finish_host, stream)) return rc;  // synchronises `stream`
   if (state_host)
     for (int b = 0; b < h->B; ++b) state_host[b] = rows[b].state;
-  if (h->pg_pages)  // a slot seen idle or finished appends nothing until its next admission
-    for (int b = 0; b < h->B; ++b)
-      if (rows[b].state != RS_RUNNING && rows[b].state != RS_PENDING) h->pg_hi[b] = 0;
+  for (int b = 0; b < h->B; ++b)  // a slot seen idle or finished appends nothing until its next admission
+    if (rows[b].state != RS_RUNNING && rows[b].state != RS_PENDING) h->slot[b].hi = 0;
   if (h->eng_text) {  // the stream is synchronised: the rows are current
     h->eng_text = 0;
     for (int b = 0; b < h->B; ++b)
@@ -1536,19 +1579,16 @@ extern "C" int ctb_gpt_engine_status(ctb_gpt* h, ctb_gpt_status* out, int32_t* s
 
 extern "C" int ctb_gpt_engine_cancel(ctb_gpt* h, int32_t n, const int32_t* slots, void* stream) {
   if (!h || !slots) return set_err(CTB_ERR_ARG, "null argument");
-  if (!h->engine) return set_err(CTB_ERR_STATE, "ctb_gpt_engine_begin has not been called");
+  int rc;
+  if ((rc = check_engine(h)) || (rc = check_slot_list(h, n, slots))) return rc;
   const int S = h->B;
-  if (n < 1 || n > S) return set_err(CTB_ERR_ARG, "n=%d outside [1,%d]", n, S);
   if (S > CANCEL_MAX_SLOTS) return set_err(CTB_ERR_ARG, "S=%d: cancellation serves up to %d slots", S, CANCEL_MAX_SLOTS);
   CancelP p{};
   p.st = h->st; p.rows = h->rows; p.finish = h->finish; p.B = S;
   for (int i = 0; i < n; ++i) {
-    const int b = slots[i];
-    if (b < 0 || b >= S || (p.mask[b >> 5] >> (b & 31) & 1u))
-      return set_err(CTB_ERR_ARG, "slot %d out of range or repeated", b);
-    p.mask[b >> 5] |= 1u << (b & 31);
+    p.mask[slots[i] >> 5] |= 1u << (slots[i] & 31);
+    h->slot[slots[i]].chunk_T0 = 0;  // a prompt in progress there is dropped
   }
-  for (int i = 0; i < n; ++i) h->chunk_T0[slots[i]] = 0;  // a prompt in progress there is dropped
   // h->eng_text stays as it is: the next ctb_gpt_engine_status recomputes it from the rows
   k_cancel_rows<<<1, 256, 0, (cudaStream_t)stream>>>(p);
   CTB_LAUNCH_CHECK();
@@ -1558,8 +1598,6 @@ extern "C" int ctb_gpt_engine_cancel(ctb_gpt* h, int32_t n, const int32_t* slots
 // ------------------------------------------------------------------ KV pages on demand (ctb_gpt_engine_begin_paged)
 static_assert(sizeof(RowState) == 8 * sizeof(int32_t), "ctb_slot_image.row");
 
-static size_t page_elems(const ctb_gpt* h) { return (size_t)2 * h->cfg.num_kv_heads * kPageTokens * h->cfg.head_dim; }
-static size_t page_bytes(const ctb_gpt* h) { return page_elems(h) * kv_elem_bytes(h); }  // one page of one layer
 static unsigned move_blocks(size_t words) { return (unsigned)std::min<size_t>((words + 255) / 256, (size_t)g_num_sms * 8); }
 
 // the poison pattern (quiet NaN of the cache's element type) into n pages of every layer: list[0..n), or p0 .. p0 + n - 1
@@ -1591,35 +1629,50 @@ static int bt_write(ctb_gpt* h, const std::vector<std::pair<int, int>>& e, cudaS
   return CTB_OK;
 }
 
+// Slot b's next block-table entry onto `page` (another entry's) or, for page < 0, the back of the free list: the page's
+// count goes up and the entry joins e, for bt_write.  With unmap_slot, the only writer of pg_free, pg_bt and pg_ref.
+static void map_page(ctb_gpt* h, int b, int page, std::vector<std::pair<int, int>>& e) {
+  if (page < 0) { page = h->pg_free.back(); h->pg_free.pop_back(); }
+  if (++h->pg_ref[page] == 2) ++h->pg_shared;
+  const int idx = b * h->pages_per_row + h->slot[b].pages++;
+  h->pg_bt[idx] = page;
+  e.emplace_back(idx, page);
+}
+
+// Every entry of slot b onto the zero page (joining e, for bt_write): each page's count goes down, and a page no entry
+// maps any more returns to the free list, to be taken again in the order it had.  Returns those pages.
+static std::vector<int> unmap_slot(ctb_gpt* h, int b, std::vector<std::pair<int, int>>& e) {
+  std::vector<int> freed;
+  for (int k = 0; k < h->slot[b].pages; ++k) {
+    const int idx = b * h->pages_per_row + k;
+    const int page = h->pg_bt[idx];
+    if (--h->pg_ref[page] == 0) freed.push_back(page);
+    else if (h->pg_ref[page] == 1) --h->pg_shared;
+    h->pg_bt[idx] = 0;
+    e.emplace_back(idx, 0);
+  }
+  h->pg_free.insert(h->pg_free.end(), freed.rbegin(), freed.rend());
+  h->slot[b].pages = 0;
+  return freed;
+}
+
 // A pool of exactly pool_pages pages, zeroed (poisoned past the zero page with CTB_KV_POISON=1), every entry of the S
 // slots' block table on the zero page and every other page free
 static int kv_pool_paged(ctb_gpt* h, int S, int pool_pages, cudaStream_t s) {
-  const ctb_gpt_config& c = h->cfg;
-  const size_t bytes = (size_t)pool_pages * page_bytes(h) * c.num_layers;
-  if (bytes != h->kv_bytes) {
-    CTB_CUDA(cudaStreamSynchronize(s));
-    if (h->kv) { cudaFree(h->kv); h->kv = nullptr; h->kv_bytes = 0; }
-    if (cudaMalloc(reinterpret_cast<void**>(&h->kv), bytes) != cudaSuccess) {
-      cudaGetLastError();
-      return set_err(CTB_ERR_NOMEM, "KV pool: %d pages x %d layers (%.2f GB) do not fit", pool_pages, c.num_layers,
-                     (double)bytes / 1e9);
-    }
-    h->kv_bytes = bytes;
-  }
+  int rc;
+  if (pool_bytes(h, pool_pages) != h->kv_bytes && (rc = kv_alloc(h, pool_pages, s))) return rc;
   h->kv_layer_elems = (size_t)pool_pages * page_elems(h);
   h->bt_B = 0;  // kv_reserve uploads its table again
-  CTB_CUDA(cudaMemsetAsync(h->kv, 0, bytes, s));
+  CTB_CUDA(cudaMemsetAsync(h->kv, 0, h->kv_bytes, s));
   const char* poison = getenv("CTB_KV_POISON");
   h->pg_poison = poison != nullptr && atoi(poison) == 1;
-  int rc;
   if (h->pg_poison && (rc = kv_poison(h, nullptr, 1, pool_pages - 1, s))) return rc;
   CTB_CUDA(cudaMemsetAsync(h->block_table, 0, sizeof(int) * (size_t)S * h->pages_per_row, s));
   h->pg_free.clear();
   for (int p = pool_pages - 1; p >= 1; --p) h->pg_free.push_back(p);
   h->pg_bt.assign((size_t)S * h->pages_per_row, 0);
-  h->pg_map.assign((size_t)S, 0); h->pg_hi.assign((size_t)S, 0); h->pg_cap.assign((size_t)S, 0);
   h->pg_ref.assign((size_t)pool_pages, 0);
-  h->pg_pages = pool_pages;
+  h->pg_pages = pool_pages; h->pg_shared = 0;
   return CTB_OK;
 }
 
@@ -1633,22 +1686,6 @@ extern "C" int ctb_gpt_engine_begin_paged(ctb_gpt* h, int32_t S, int32_t max_new
   return engine_begin(h, S, max_new_cap, flags, pool_pages, ids_out_dev, hiddens_out_dev, stream);
 }
 
-static int check_paged(const ctb_gpt* h) {
-  if (!h->engine || !h->pg_pages) return set_err(CTB_ERR_STATE, "not a paged slot engine (ctb_gpt_engine_begin_paged)");
-  return CTB_OK;
-}
-
-static int check_slot_list(const ctb_gpt* h, int n, const int32_t* slots) {
-  if (n < 1 || n > h->B) return set_err(CTB_ERR_ARG, "n=%d outside [1,%d]", n, h->B);
-  std::vector<char> seen((size_t)h->B, 0);
-  for (int i = 0; i < n; ++i) {
-    if (slots[i] < 0 || slots[i] >= h->B || seen[slots[i]])
-      return set_err(CTB_ERR_ARG, "slot %d out of range or repeated", slots[i]);
-    seen[slots[i]] = 1;
-  }
-  return CTB_OK;
-}
-
 extern "C" int ctb_gpt_engine_reserve(ctb_gpt* h, int32_t n, const int32_t* slots, const int32_t* tokens, void* stream) {
   if (!h || !slots || !tokens) return set_err(CTB_ERR_ARG, "null argument");
   int rc;
@@ -1657,40 +1694,23 @@ extern "C" int ctb_gpt_engine_reserve(ctb_gpt* h, int32_t n, const int32_t* slot
   for (int i = 0; i < n; ++i) {
     if (tokens[i] < 0 || tokens[i] > h->cfg.max_context)
       return set_err(CTB_ERR_ARG, "slot %d: tokens=%d outside [0,%d]", slots[i], tokens[i], h->cfg.max_context);
-    need += (size_t)std::max(0, (tokens[i] + kPageTokens - 1) / kPageTokens - h->pg_map[slots[i]]);
+    need += (size_t)std::max(0, (tokens[i] + kPageTokens - 1) / kPageTokens - h->slot[slots[i]].pages);
   }
   if (need > h->pg_free.size())
     return set_err(CTB_ERR_POOL, "KV pool: %zu more pages needed, %zu of %d free", need, h->pg_free.size(),
                    h->pg_pages - 1);
   std::vector<std::pair<int, int>> e;
-  for (int i = 0; i < n; ++i) {
-    const int b = slots[i], want = (tokens[i] + kPageTokens - 1) / kPageTokens;
-    for (int k = h->pg_map[b]; k < want; ++k) {
-      const int idx = b * h->pages_per_row + k, page = h->pg_free.back();
-      h->pg_free.pop_back();
-      h->pg_bt[idx] = page;
-      h->pg_ref[page] = 1;
-      e.emplace_back(idx, page);
-    }
-    h->pg_map[b] = std::max(h->pg_map[b], want);
-  }
+  for (int i = 0; i < n; ++i)
+    while (h->slot[slots[i]].pages * kPageTokens < tokens[i]) map_page(h, slots[i], -1, e);
   return bt_write(h, e, (cudaStream_t)stream);
 }
 
-// slot b's entries on the zero page; each page no other entry maps goes back to the free list (taken again in the
-// order they had)
+// slot b's pages and the positions they hold released, its prompt no longer shareable (neither caller leaves a prompt
+// in progress there)
 static int release_pages(ctb_gpt* h, int b, cudaStream_t s) {
   std::vector<std::pair<int, int>> e;
-  std::vector<int> freed;
-  for (int k = 0; k < h->pg_map[b]; ++k) {
-    const int idx = b * h->pages_per_row + k;
-    if (--h->pg_ref[h->pg_bt[idx]] == 0) freed.push_back(h->pg_bt[idx]);
-    h->pg_bt[idx] = 0;
-    e.emplace_back(idx, 0);
-  }
-  h->pg_free.insert(h->pg_free.end(), freed.rbegin(), freed.rend());
-  h->pg_map[b] = h->pg_hi[b] = h->pg_cap[b] = 0;
-  h->pr_len[b] = 0;
+  const std::vector<int> freed = unmap_slot(h, b, e);
+  h->slot[b] = SlotRecord{};
   int rc;
   if ((rc = bt_write(h, e, s))) return rc;
   return h->pg_poison ? kv_poison(h, freed.data(), 0, (int)freed.size(), s) : CTB_OK;
@@ -1701,17 +1721,21 @@ extern "C" int ctb_gpt_engine_release(ctb_gpt* h, int32_t n, const int32_t* slot
   int rc;
   if ((rc = check_paged(h)) || (rc = check_slot_list(h, n, slots))) return rc;
   cudaStream_t s = (cudaStream_t)stream;
-  std::vector<RowState> rows((size_t)h->B);
-  CTB_CUDA(cudaMemcpyAsync(rows.data(), h->rows, sizeof(RowState) * h->B, cudaMemcpyDeviceToHost, s));
-  CTB_CUDA(cudaStreamSynchronize(s));
+  std::vector<RowState> rows;
+  if ((rc = read_rows(h, rows, s))) return rc;
   for (int i = 0; i < n; ++i) {
-    const int b = slots[i];
-    if (rows[b].state == RS_RUNNING || rows[b].state == RS_PENDING)
-      return set_err(CTB_ERR_STATE, "slot %d is still generating: its pages stay", b);
-    if (h->chunk_T0[b]) return set_err(CTB_ERR_STATE, "slot %d has a prompt in progress: its pages stay", b);
+    if ((rc = check_not_generating(rows[slots[i]], slots[i])) || (rc = check_slot(h, slots[i]))) return rc;
   }
   for (int i = 0; i < n; ++i)
     if ((rc = release_pages(h, slots[i], s))) return rc;
+  return CTB_OK;
+}
+
+extern "C" int ctb_gpt_engine_pages(ctb_gpt* h, int32_t* in_use, int32_t* shared) {
+  if (!h || !in_use || !shared) return set_err(CTB_ERR_ARG, "null argument");
+  if (int rc = check_paged(h)) return rc;
+  *in_use = h->pg_pages - 1 - (int32_t)h->pg_free.size();  // every page but the zero page is mapped or free
+  *shared = h->pg_shared;
   return CTB_OK;
 }
 
@@ -1750,12 +1774,6 @@ static int check_pinned(const void* host_buf) {
     cudaGetLastError();
     return set_err(CTB_ERR_ARG, "the image buffer is not pinned host memory");
   }
-  return CTB_OK;
-}
-
-static int check_slot(const ctb_gpt* h, int slot) {
-  if (slot < 0 || slot >= h->B) return set_err(CTB_ERR_ARG, "slot %d outside [0,%d)", slot, h->B);
-  if (h->chunk_T0[slot]) return set_err(CTB_ERR_STATE, "slot %d has a prompt in progress", slot);
   return CTB_OK;
 }
 
@@ -1808,9 +1826,7 @@ static int running_image(ctb_gpt* h, int slot, ctb_slot_image* img, cudaStream_t
   memcpy(&r, img->row, sizeof(r));
   if (r.state != RS_RUNNING) return set_err(CTB_ERR_STATE, "slot %d is not running (state %d)", slot, r.state);
   image_layout(h, r.n_gen, img->seq_len, img);
-  if (img->npages > h->pg_map[slot])
-    return set_err(CTB_ERR_STATE, "slot %d holds %d positions on %d pages", slot, img->seq_len, h->pg_map[slot]);
-  return CTB_OK;
+  return check_covers(h, slot, img->seq_len);
 }
 
 extern "C" int ctb_gpt_engine_suspend_bytes(ctb_gpt* h, int32_t slot, uint64_t* bytes, void* stream) {
@@ -1871,15 +1887,11 @@ extern "C" int ctb_gpt_engine_resume(ctb_gpt* h, int32_t slot, const void* host_
   if (host_bytes < img->bytes)
     return set_err(CTB_ERR_ARG, "image buffer of %llu bytes, the image has %llu", (unsigned long long)host_bytes,
                    (unsigned long long)img->bytes);
-  if (img->npages > h->pg_map[slot])
-    return set_err(CTB_ERR_STATE, "slot %d: its pages hold %d positions, the image %d", slot,
-                   h->pg_map[slot] * kPageTokens, img->seq_len);
-  RowState cur;
-  CTB_CUDA(cudaMemcpyAsync(&cur, h->rows + slot, sizeof(RowState), cudaMemcpyDeviceToHost, s));
-  CTB_CUDA(cudaStreamSynchronize(s));
-  if (cur.state == RS_RUNNING || cur.state == RS_PENDING) return set_err(CTB_ERR_STATE, "slot %d is still generating", slot);
-  if ((rc = check_private(h, slot, 0, img->seq_len))) return rc;
-  h->pr_len[slot] = 0;  // the image does not record its prompt: a resumed request is no source to share from
+  std::vector<RowState> rows;
+  if ((rc = check_writes(h, slot, 0, img->seq_len)) || (rc = read_rows(h, rows, s)) ||
+      (rc = check_not_generating(rows[slot], slot)))
+    return rc;
+  h->slot[slot].pr_len = 0;  // the image does not record its prompt: a resumed request is no source to share from
   const char* hb = static_cast<const char*>(host_buf);
   const int n_gen = img->n_gen;
   CTB_CUDA(cudaMemcpyAsync(h->cfgs + slot, &img->sampler, sizeof(ctb_sampler_config), cudaMemcpyHostToDevice, s));
@@ -1897,8 +1909,8 @@ extern "C" int ctb_gpt_engine_resume(ctb_gpt* h, int32_t slot, const void* host_
   if ((rc = kv_move(h, slot, const_cast<char*>(hb) + img->off_kv, img->npages, false, s)) ||
       (rc = launch_set_row(h, slot, r, s)))
     return rc;
-  h->pg_hi[slot] = img->seq_len;
-  h->pg_cap[slot] = img->seq_len + r.max_new - r.n_gen;
+  h->slot[slot].hi = img->seq_len;
+  h->slot[slot].cap = img->seq_len + r.max_new - r.n_gen;
   if (r.text) h->eng_text = 1;
   return CTB_OK;
 }
@@ -1906,52 +1918,38 @@ extern "C" int ctb_gpt_engine_resume(ctb_gpt* h, int32_t slot, const void* host_
 // ------------------------------------------------------------------ shared prompts (ctb_gpt_engine_share_prompt)
 extern "C" int ctb_gpt_engine_share_prompt(ctb_gpt* h, int32_t src, int32_t dst, int32_t T0, int32_t c0, void* stream) {
   if (!h) return set_err(CTB_ERR_ARG, "null argument");
-  if (!h->engine) return set_err(CTB_ERR_STATE, "ctb_gpt_engine_begin has not been called");
+  int rc;
+  if ((rc = check_engine(h))) return rc;
   const int S = h->B;
   if (src < 0 || src >= S || dst < 0 || dst >= S || src == dst)
     return set_err(CTB_ERR_ARG, "slots %d -> %d: two distinct slots of [0,%d)", src, dst, S);
-  if (T0 < 8 || T0 > h->cfg.max_context - 1) return set_err(CTB_ERR_ARG, "T0=%d outside [8,%d]", T0, h->cfg.max_context - 1);
+  if ((rc = check_T0(h, T0))) return rc;
   if (c0 < CTB_PREFILL_CHUNK_ALIGN || c0 % CTB_PREFILL_CHUNK_ALIGN || c0 >= T0)
     return set_err(CTB_ERR_ARG, "c0=%d: a positive multiple of %d below T0=%d", c0, CTB_PREFILL_CHUNK_ALIGN, T0);
   cudaStream_t s = (cudaStream_t)stream;
-  RowState rs, rd;
-  CTB_CUDA(cudaMemcpyAsync(&rs, h->rows + src, sizeof(RowState), cudaMemcpyDeviceToHost, s));
-  CTB_CUDA(cudaMemcpyAsync(&rd, h->rows + dst, sizeof(RowState), cudaMemcpyDeviceToHost, s));
-  CTB_CUDA(cudaStreamSynchronize(s));
+  std::vector<RowState> rows;
+  if ((rc = read_rows(h, rows, s))) return rc;
+  const SlotRecord& from = h->slot[src];
+  SlotRecord& to = h->slot[dst];
   // a finished source still holds its KV until the slot is released or admitted again (pr_len is then 0)
-  if ((rs.state != RS_RUNNING && rs.state != RS_FINISHED) || h->pr_len[src] == 0)
-    return set_err(CTB_ERR_STATE, "slot %d holds no admitted prompt (state %d)", src, rs.state);
-  if (rd.state == RS_RUNNING || rd.state == RS_PENDING) return set_err(CTB_ERR_STATE, "slot %d is still generating", dst);
-  if (h->chunk_T0[dst]) return set_err(CTB_ERR_STATE, "slot %d has a prompt in progress", dst);
-  if (h->pg_pages && h->pg_map[dst]) return set_err(CTB_ERR_STATE, "slot %d has pages mapped", dst);
-  if (h->pr_len[src] < c0)
-    return set_err(CTB_ERR_STATE, "slot %d holds a prompt of %d positions, fewer than c0=%d", src, h->pr_len[src], c0);
-  if ((T0 > PF_ATT_MAX_T0) != (h->pr_W[src] > PF_ATT_MAX_T0))
+  if ((rows[src].state != RS_RUNNING && rows[src].state != RS_FINISHED) || from.pr_len == 0)
+    return set_err(CTB_ERR_STATE, "slot %d holds no admitted prompt (state %d)", src, rows[src].state);
+  if ((rc = check_not_generating(rows[dst], dst)) || (rc = check_slot(h, dst))) return rc;
+  if (h->pg_pages && to.pages) return set_err(CTB_ERR_STATE, "slot %d has pages mapped", dst);
+  if (from.pr_len < c0)
+    return set_err(CTB_ERR_STATE, "slot %d holds a prompt of %d positions, fewer than c0=%d", src, from.pr_len, c0);
+  if ((T0 > PF_ATT_MAX_T0) != (from.pr_W > PF_ATT_MAX_T0))
     return set_err(CTB_ERR_ARG, "T0=%d and slot %d's prompt width %d take different prefill attention kernels", T0, src,
-                   h->pr_W[src]);
+                   from.pr_W);
   const int shared = c0 / kPageTokens;
-  int rc;
   if (h->pg_pages) {  // dst's entries [0, shared) map src's pages; [shared, ceil(T0 / 16)) map pages of its own
     const int own = (T0 + kPageTokens - 1) / kPageTokens - shared;
     if ((size_t)own > h->pg_free.size())
       return set_err(CTB_ERR_POOL, "KV pool: %d more pages needed, %zu of %d free", own, h->pg_free.size(),
                      h->pg_pages - 1);
     std::vector<std::pair<int, int>> e;
-    for (int k = 0; k < shared + own; ++k) {
-      int page;
-      if (k < shared) {
-        page = h->pg_bt[(size_t)src * h->pages_per_row + k];
-        ++h->pg_ref[page];
-      } else {
-        page = h->pg_free.back();
-        h->pg_free.pop_back();
-        h->pg_ref[page] = 1;
-      }
-      const int idx = dst * h->pages_per_row + k;
-      h->pg_bt[idx] = page;
-      e.emplace_back(idx, page);
-    }
-    h->pg_map[dst] = shared + own;
+    for (int k = 0; k < shared + own; ++k)
+      map_page(h, dst, k < shared ? h->pg_bt[(size_t)src * h->pages_per_row + k] : -1, e);
     if ((rc = bt_write(h, e, s))) return rc;
   } else {  // a fixed engine: row b owns pages [b * bt_per_row, (b + 1) * bt_per_row)
     KvCopyP p{};
@@ -1961,8 +1959,8 @@ extern "C" int ctb_gpt_engine_share_prompt(ctb_gpt* h, int32_t src, int32_t dst,
     k_kv_copy<<<(unsigned)std::min(p.layers * shared, g_num_sms * 8), 256, 0, s>>>(p);
     CTB_LAUNCH_CHECK();
   }
-  h->chunk_T0[dst] = T0; h->chunk_done[dst] = c0;  // the final chunk [c0, T0) admits the request
-  h->pr_len[dst] = 0;
+  to.chunk_T0 = T0; to.chunk_done = c0;  // the final chunk [c0, T0) admits the request
+  to.pr_len = 0;
   return CTB_OK;
 }
 

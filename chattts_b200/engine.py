@@ -878,11 +878,6 @@ class EngineDevice:
             _lib.check(self.lib.ctb_gpt_engine_begin_paged(
                 gpt._handle, slots, max_new_cap, flags, kv_pool_pages, C.c_void_p(self.ids_out.data_ptr()), hid,
                 self.stream))
-        # the pool's pages as the block table maps them: each slot's entries (page numbers of this mirror, not the
-        # device's) and the entries that map each page, so shared pages count once
-        self._pages: List[List[int]] = [[] for _ in range(slots)]
-        self._refs: Dict[int, int] = {}
-        self._page_ids = itertools.count()
         # the images of suspended requests, by id, while anything holds them (a cancelled one's ends with its outputs)
         self._images: "weakref.WeakValueDictionary[int, SlotImage]" = weakref.WeakValueDictionary()
         self._resumed: List[SlotImage] = []  # read by the device until the next status read
@@ -953,27 +948,20 @@ class EngineDevice:
         _lib.check(self.lib.ctb_gpt_decode(self.gpt._handle, n, self.stream))
 
     # ---------------------------------------------------------------- KV pool (paged engines)
+    def _page_counts(self) -> Tuple[int, int]:
+        used, shared = C.c_int32(), C.c_int32()
+        _lib.check(self.lib.ctb_gpt_engine_pages(self.gpt._handle, C.byref(used), C.byref(shared)))
+        return used.value, shared.value
+
     @property
     def pages_in_use(self) -> int:
-        """Pages mapped, each counted once however many slots share it."""
-        return len(self._refs)
+        """Pages mapped, each counted once however many slots share it (ctb_gpt_engine_pages)."""
+        return self._page_counts()[0]
 
     @property
     def shared_pages(self) -> int:
         """Pages more than one slot maps (shared prompts)."""
-        return sum(1 for n in self._refs.values() if n > 1)
-
-    def _map(self, slot: int, pages: List[int]) -> None:
-        for p in pages:
-            self._refs[p] = self._refs.get(p, 0) + 1
-        self._pages[slot] += pages
-
-    def _unmap(self, slot: int) -> None:
-        for p in self._pages[slot]:
-            self._refs[p] -= 1
-            if not self._refs[p]:
-                del self._refs[p]
-        self._pages[slot] = []
+        return self._page_counts()[1]
 
     @property
     def host_bytes(self) -> int:
@@ -991,17 +979,12 @@ class EngineDevice:
         if rc == _lib.ERR_POOL:
             return False
         _lib.check(rc)
-        for s, t in zip(slots, tokens):
-            new = -(-t // _lib.PAGE_TOKENS) - len(self._pages[s])
-            self._map(s, [next(self._page_ids) for _ in range(max(0, new))])
         return True
 
     def release(self, slots: List[int]) -> None:
         """Return the pages of idle or finished slots to the pool (ctb_gpt_engine_release)."""
         _lib.check(self.lib.ctb_gpt_engine_release(self.gpt._handle, len(slots), (C.c_int32 * len(slots))(*slots),
                                                    self.stream))
-        for s in slots:
-            self._unmap(s)
 
     def suspend(self, slot: int) -> SlotImage:
         """Move the running request in ``slot`` to a pinned host image (ctb_gpt_engine_suspend); the slot and its pages
@@ -1011,7 +994,6 @@ class EngineDevice:
         buf = torch.empty(nbytes.value, dtype=torch.uint8, pin_memory=True)
         _lib.check(self.lib.ctb_gpt_engine_suspend(self.gpt._handle, slot, C.c_void_p(buf.data_ptr()), nbytes.value,
                                                    self.stream))
-        self._unmap(slot)
         image = SlotImage(buf, self._text[slot], self.dev, self.gpt.num_vq, self.gpt.config.hidden_size,
                           self._torch_stream)
         self._images[id(image)] = image
@@ -1035,10 +1017,6 @@ class EngineDevice:
         if rc == _lib.ERR_POOL:
             return False
         _lib.check(rc)
-        if self.pool_pages is not None:
-            shared = c0 // _lib.PAGE_TOKENS
-            self._map(dst, self._pages[src][:shared])
-            self._map(dst, [next(self._page_ids) for _ in range(-(-T // _lib.PAGE_TOKENS) - shared)])
         return True
 
     def cancel(self, slots: List[int]) -> None:

@@ -284,6 +284,12 @@ int ctb_gpt_engine_reserve(ctb_gpt* h, int32_t n, const int32_t* slots, const in
  * prompt in progress (nothing is released); CTB_ERR_ARG as for ctb_gpt_engine_reserve. */
 int ctb_gpt_engine_release(ctb_gpt* h, int32_t n, const int32_t* slots, void* stream);
 
+/* The pool's pages as the block table maps them now: *in_use physical pages mapped, each counted once however many
+ * slots map it, and *shared of them mapped by more than one block-table entry (shared prompts).  Host bookkeeping
+ * only: no device work, no synchronisation.  Errors: CTB_ERR_STATE outside a paged engine; CTB_ERR_ARG for a null
+ * argument. */
+int ctb_gpt_engine_pages(ctb_gpt* h, int32_t* in_use, int32_t* shared);
+
 /* A suspended slot's image in a pinned host buffer: this header, then the sections at the offsets it records. */
 #define CTB_SLOT_IMAGE_MAGIC 0x4b565031u
 typedef struct ctb_slot_image {
