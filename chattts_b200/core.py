@@ -456,7 +456,8 @@ class Chat:
         return self.tokenizer.decode([ids[ids.less(self.tokenizer.break_0_ids)]])[0]
 
     def open_engine(self, slots: Optional[int] = None, max_new_cap: int = 2048, use_decoder: bool = True,
-                    dtype=torch.float32, prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None):
+                    dtype=torch.float32, prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None,
+                    logprobs: bool = False):
         """A long-lived slot engine (``GPT.open_engine``) that synthesises texts submitted from any thread while it
         decodes: ``engine.submit(text, params_infer_code=None, stream=False, skip_refine_text=True, ...) -> Job``,
         ``Job.cancel()`` for one text, ``close(cancel=False)`` or a ``with`` block to drain it (``close(cancel=True)``
@@ -468,13 +469,20 @@ class Chat:
         poll, at least 128; default None) bounds the prefill the running jobs wait for at each poll
         (``infer_continuous``); a job cancelled while its prompt is in progress frees its slot at the next poll.
         ``kv_pool_bytes`` (default None) bounds the engine's KV memory as in ``infer_continuous``; ``submit`` refuses
-        a stage that does not fit in the pool alone."""
+        a stage that does not fit in the pool alone.
+
+        ``logprobs=True``: every finished job has ``Job.logprobs`` (CPU fp32), the log-probability of each speech
+        token under the model's head logits at temperature 1 (``GPT.generate_continuous(logprobs=True)``): the
+        ``[n, num_vq]`` tensor of its code request for a one-sentence job, a list of such tensors in take order with
+        ``takes``, and in sentence order with ``split_text=True`` (neither the reference stage nor refinements are
+        included).  The waveforms are the same as without it.  None on an engine opened without it."""
         flags = _lib.engine_flags(dtype)
         check_prefill_budget(prefill_budget)
         assert self.has_loaded(use_decoder=use_decoder)
         return self.gpt._open_slot_engine(ChatEngine, self.gpt.max_batch if slots is None else slots, max_new_cap,
                                           use_decoder, None, self, use_decoder, flags=flags,
-                                          prefill_budget=prefill_budget, kv_pool_bytes=kv_pool_bytes)
+                                          prefill_budget=prefill_budget, kv_pool_bytes=kv_pool_bytes,
+                                          logprobs=logprobs)
 
     def interrupt(self):
         self.context.set(True)
@@ -666,10 +674,12 @@ def _decode_windows(dev, jobs, model: DVAE, use_decoder: bool):
 class _Paragraph:
     """A job's state on ``ChatEngine`` (a text without ``split_text`` is a paragraph of one sentence): its reference
     stage, which request speaks which sentence, and the in-order assembly of the sentences' audio (``add``).  ``sink`` =
-    (queue, key): the chunks and the end of the job are also posted there, for ``Chat.infer_continuous*``."""
+    (queue, key): the chunks and the end of the job are also posted there, for ``Chat.infer_continuous*``.  ``split``:
+    the job was submitted with ``split_text=True``."""
 
-    def __init__(self, n: int, stream_params, sink=None, takes: bool = False):
-        self.n, self.sink, self.takes = n, sink, takes
+    def __init__(self, n: int, stream_params, sink=None, takes: bool = False, split: bool = False):
+        self.n, self.sink, self.takes, self.split = n, sink, takes, split
+        self.logprobs: Optional[list] = None  # an engine with logprobs: each sentence's, once its code request ends
         self.windows = ([StreamWindows(stream_params.stream_speed, stream_params.pass_first_n_batches)
                          for _ in range(n)] if stream_params is not None else None)
         self.ref = None
@@ -694,6 +704,8 @@ class _Paragraph:
             self.next += 1
         done = self.next == self.n
         job = self.job
+        if done and self.logprobs is not None:
+            job.logprobs = self.logprobs if self.takes or self.split else self.logprobs[0]
         if self.windows is not None:
             for j, c in enumerate(out):
                 item = (c, done and j == len(out) - 1)
@@ -911,7 +923,7 @@ class ChatEngine(OpenEngine):
         if min(m, n) > chat.gpt.max_batch:
             raise ValueError(f"max_split_batch={m}: a batch of {min(m, n)} sentences exceeds this handle's "
                              f"max_batch={chat.gpt.max_batch}")
-        para = _Paragraph(n, params if stream else None, sink)
+        para = _Paragraph(n, params if stream else None, sink, split=split_text)
         spk_stage = n > 1 and params.spk_smp is None
         if spk_stage and chat.dvae.audio_encoder is None:
             raise RuntimeError("this DVAE checkpoint carries no encoder / VQ weights: cannot sample a speaker")
@@ -975,6 +987,11 @@ class ChatEngine(OpenEngine):
                 continue  # a refinement, or the reference stage, whose audio only becomes the speaker sample
             else:
                 k = para.order[requests[i]]
+                if last and getattr(dev, "lp_out", None) is not None:  # an engine opened with logprobs
+                    if para.logprobs is None:
+                        para.logprobs = [None] * para.n
+                    out = dev.empty(i) if s is None else dev.harvest(s, n, copy=False)
+                    para.logprobs[k] = out.logprobs[0].cpu()
                 if para.windows is not None:
                     ws = para.windows[k].windows(n, last)
                     wjobs += [((para, k), s, n, a, b, flush, last and j == len(ws) - 1) for j, (a, b, flush) in

@@ -119,6 +119,8 @@ struct ctb_gpt {
   int eng_text;
   cudaGraphExec_t graph_exec_text;
   uint64_t graph_kernels_text;
+  float* eng_logprobs;        // [S, max_new, num_vq] token log-probabilities (ctb_gpt_engine_logprobs), or nullptr
+  int eng_served;             // 1 once the engine has admitted, chunked or resumed a request
   std::vector<SlotRecord> slot;  // [S] host-side record of each slot
   // ---- half-precision slot engine (ctb_gpt_engine_begin_ex)
   int prec;                   // CTB_ENGINE_FP16_* bits of the current engine (0 for fp32 engines and generate())
@@ -770,6 +772,17 @@ static int launch_heads(ctb_gpt* h, const StepCtx& x, cudaStream_t s) {
   return launch_gemv<EPI_HEADS>(x.bt, hp, x.ntiles, s);
 }
 
+// the log-probabilities of the ids the k_sample<true> launch `sp` just wrote, at the index k_finalize_rows writes them
+static int launch_logprob(ctb_gpt* h, const SampleP& sp, cudaStream_t s) {
+  LogprobP lp{};
+  lp.st = sp.st; lp.check_finished = sp.check_finished; lp.logits = sp.logits; lp.V = sp.V;
+  lp.rows_per_item = sp.rows_per_item; lp.idx = sp.out_idx; lp.rstate = sp.rstate; lp.want = sp.want;
+  lp.out = h->eng_logprobs; lp.max_new = h->max_new; lp.num_vq = h->cfg.num_vq;
+  CTB_CUDA(launch_pdl(k_token_logprob, dim3(sp.rows), dim3(LOGPROB_THREADS), 0, s, lp));
+  CTB_LAUNCH_CHECK();
+  return CTB_OK;
+}
+
 static int launch_sampler(ctb_gpt* h, const StepCtx& x, cudaStream_t s) {
   const ctb_gpt_config& c = h->cfg;
   const int rpi = h->infer_text ? 1 : c.num_vq;
@@ -781,12 +794,14 @@ static int launch_sampler(ctb_gpt* h, const StepCtx& x, cudaStream_t s) {
   if (!h->engine) return launch_sample(sp, s);
   sp.rstate = h->rows; sp.cfgs = h->cfgs; sp.want = h->phase; sp.q_noise = h->eng_noise;
   sp.noise_stride = (int)noise_stride(h);
-  const int rc = launch_sample(sp, s);
+  int rc = launch_sample(sp, s);
+  if (!rc && h->eng_logprobs) rc = launch_logprob(h, sp, s);
   if (rc || !h->eng_text) return rc;
   // text rows: one row per slot over the text head's logits, as a batch of one samples them
   sp.logits = h->eng_text_logits; sp.rows = h->B; sp.V = c.num_text_tokens; sp.rows_per_item = 1;
   sp.out_idx = h->eng_text_idx; sp.want = h->phase | WANT_TEXT;
-  return launch_sample(sp, s);
+  if ((rc = launch_sample(sp, s)) || !h->eng_logprobs) return rc;
+  return launch_logprob(h, sp, s);
 }
 
 // npad 16 for B <= 16, 32 for B <= 32, 64 for B <= 64 (a 64-row scratch only: tc_rows == 64)
@@ -1412,6 +1427,7 @@ static int engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t flag
   h->use_tc = use_tc;
   h->q_noise = h->eng_noise; h->emb = nullptr; h->mask = nullptr;
   h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev; h->eng_text = 0; h->pg_pages = 0;
+  h->eng_logprobs = nullptr; h->eng_served = 0;
   if ((rc = restart_decode(h, s)) ||
       (rc = pool_pages ? kv_pool_paged(h, S, pool_pages, s) : kv_reserve(h, S, c.max_context, s)))
     return rc;
@@ -1490,6 +1506,7 @@ static int admit(ctb_gpt* h, int n, const int32_t* slots, int T0, int q0, const 
   CTB_CUDA(cudaStreamSynchronize(s));
   // prompts -> their slots' pages, then heads / sampler / finalize for the RS_PENDING rows only
   if (text) h->eng_text = 1;
+  h->eng_served = 1;
   h->phase = RS_PENDING;
   rc = prefill(h, n, T0, q0, T0 - q0, emb_dev, mask_dev, slots, s);
   h->phase = RS_RUNNING;
@@ -1552,8 +1569,23 @@ extern "C" int ctb_gpt_engine_prefill_chunk(ctb_gpt* h, int32_t slot, int32_t T0
       (rc = check_writes(h, slot, c0, c0 + n)))
     return rc;
   rec.pr_len = 0;  // its pages now hold part of a prompt
+  h->eng_served = 1;
   if ((rc = prefill(h, 1, T0, c0, n, emb_dev, nullptr, &slot, s))) { rec.chunk_T0 = 0; return rc; }
   rec.chunk_T0 = T0; rec.chunk_done = c0 + n;
+  return CTB_OK;
+}
+
+extern "C" int ctb_gpt_engine_logprobs(ctb_gpt* h, float* logprobs_out_dev, void* stream) {
+  if (!h || !logprobs_out_dev) return set_err(CTB_ERR_ARG, "null argument");
+  if (int rc = check_engine(h)) return rc;
+  if (h->eng_served)
+    return set_err(CTB_ERR_STATE, "the engine has served a request: attach the log-probability buffer right after begin");
+  CTB_CUDA(cudaMemsetAsync(logprobs_out_dev, 0, (size_t)h->B * h->max_new * h->cfg.num_vq * sizeof(float),
+                           (cudaStream_t)stream));
+  h->eng_logprobs = logprobs_out_dev;
+  // decode graphs captured so far (steps of the idle engine) lack the k_token_logprob nodes
+  if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
+  if (h->graph_exec_text) { cudaGraphExecDestroy(h->graph_exec_text); h->graph_exec_text = nullptr; }
   return CTB_OK;
 }
 
@@ -1892,6 +1924,7 @@ extern "C" int ctb_gpt_engine_resume(ctb_gpt* h, int32_t slot, const void* host_
       (rc = check_not_generating(rows[slot], slot)))
     return rc;
   h->slot[slot].pr_len = 0;  // the image does not record its prompt: a resumed request is no source to share from
+  h->eng_served = 1;
   const char* hb = static_cast<const char*>(host_buf);
   const int n_gen = img->n_gen;
   CTB_CUDA(cudaMemcpyAsync(h->cfgs + slot, &img->sampler, sizeof(ctb_sampler_config), cudaMemcpyHostToDevice, s));
@@ -2038,4 +2071,15 @@ extern "C" int ctb_sample(const float* logits_dev, int32_t rows, int32_t V, int3
   sp.rows_per_item = rows_per_item; sp.cfg = *sampler; sp.q_noise = q_noise_dev; sp.gen_ids = gen_ids_dev;
   sp.gen_stride = gen_stride; sp.gen_inner = rows_per_item; sp.n_gen_fixed = n_gen; sp.step_fixed = step; sp.out_idx = out_idx_dev;
   return launch_sample(sp, (cudaStream_t)stream);
+}
+
+extern "C" int ctb_token_logprobs(const float* logits_dev, int32_t rows, int32_t V, const int32_t* ids_dev, float* out_dev,
+                                  void* stream) {
+  if (!logits_dev || !ids_dev || !out_dev) return set_err(CTB_ERR_ARG, "null argument");
+  if (rows < 1 || V < 1) return set_err(CTB_ERR_ARG, "bad shape");
+  LogprobP lp{};
+  lp.logits = logits_dev; lp.V = V; lp.rows_per_item = 1; lp.idx = ids_dev; lp.out = out_dev;
+  CTB_CUDA(launch_pdl(k_token_logprob, dim3(rows), dim3(LOGPROB_THREADS), 0, (cudaStream_t)stream, lp));
+  CTB_LAUNCH_CHECK();
+  return CTB_OK;
 }

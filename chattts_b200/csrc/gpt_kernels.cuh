@@ -744,6 +744,23 @@ constexpr int SAMPLE_THREADS = 1024;
 template <bool ENGINE>
 __global__ void k_sample(const SampleP p);
 
+// k_token_logprob: log softmax(logits row)[id] of the id a sampler just chose, at temperature 1 and before any logits
+// processing.  Its launch mirrors the k_sample<true> it follows (same rows, rows_per_item, want and st), and each served
+// row r of item b, codebook q = r % rows_per_item writes out[(b * max_new + n_gen(b)) * num_vq + q], the index
+// k_finalize_rows then writes the id at.  rstate == nullptr (ctb_token_logprobs): every row, out[r], ids from idx[r].
+struct LogprobP {
+  const LoopState* st; int check_finished;
+  const float* logits;   // [rows, V]
+  int V, rows_per_item;
+  const int32_t* idx;    // [rows] the sampled ids
+  const RowState* rstate;
+  int want;
+  float* out;            // slot engine: [B, max_new, num_vq]; stand-alone: [rows]
+  int max_new, num_vq;
+};
+constexpr int LOGPROB_THREADS = 256;
+__global__ void k_token_logprob(const LogprobP p);
+
 struct FinalP {
   LoopState* st;
   int B, rows_per_item, num_vq, max_new, eos;

@@ -6,6 +6,7 @@ namespace ctb {
 
 namespace {
 
+template <int NT = SAMPLE_THREADS>
 __device__ __forceinline__ double block_sum_d(double v, double* s_red) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   v = warp_sum_d(v);
@@ -14,7 +15,7 @@ __device__ __forceinline__ double block_sum_d(double v, double* s_red) {
   __syncthreads();
   double t = 0.0;
 #pragma unroll 8
-  for (int w = 0; w < SAMPLE_THREADS / 32; ++w) t += s_red[w];  // fixed order => deterministic
+  for (int w = 0; w < NT / 32; ++w) t += s_red[w];  // fixed order => deterministic
   return t;
 }
 
@@ -30,6 +31,7 @@ __device__ __forceinline__ int block_sum_i(int v, int* s_red) {
   return t;
 }
 
+template <int NT = SAMPLE_THREADS>
 __device__ __forceinline__ float block_max_f(float v, float* s_red) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   v = warp_max(v);
@@ -38,7 +40,7 @@ __device__ __forceinline__ float block_max_f(float v, float* s_red) {
   __syncthreads();
   float t = -INFINITY;
 #pragma unroll 8
-  for (int w = 0; w < SAMPLE_THREADS / 32; ++w) t = fmaxf(t, s_red[w]);
+  for (int w = 0; w < NT / 32; ++w) t = fmaxf(t, s_red[w]);
   return t;
 }
 
@@ -363,6 +365,37 @@ __global__ void k_cancel_rows(const CancelP p) {
   }
   __syncthreads();
   if (threadIdx.x == 0) p.st->all_finished = s_running ? 0 : 1;
+}
+
+// Token log-probability (ctb_gpt_engine_logprobs, ctb_token_logprobs): one CTA per logits row.  The row max in fp32,
+// den = sum exp(z_v - max) summed in double in a fixed order (per thread over v, then warps, then the CTA's warps in
+// order, as k_sample sums its denominators), lp = (double)(z_id - max) - log(den) rounded once to fp32: the same
+// logits give the same bits.  An id outside [0, V) (stand-alone calls only; k_sample never writes one) gives NaN.
+__global__ void __launch_bounds__(LOGPROB_THREADS) k_token_logprob(const LogprobP p) {
+  pdl_trigger();
+  pdl_wait();
+  if (p.check_finished && ldg_cg(&p.st->all_finished)) return;
+  const int row = blockIdx.x, V = p.V;
+  const int item = row / p.rows_per_item, q = row % p.rows_per_item;
+  if (p.rstate != nullptr && !row_wanted(p.rstate + item, p.want)) return;  // CTA-uniform: the rows k_sample served
+  __shared__ double s_redd[LOGPROB_THREADS / 32];
+  __shared__ float s_redf[LOGPROB_THREADS / 32];
+  const float* lg = p.logits + (size_t)row * V;
+  float mx = -INFINITY;
+  for (int v = threadIdx.x; v < V; v += LOGPROB_THREADS) mx = fmaxf(mx, ldg_cg(&lg[v]));
+  mx = block_max_f<LOGPROB_THREADS>(mx, s_redf);
+  double den = 0.0;
+  for (int v = threadIdx.x; v < V; v += LOGPROB_THREADS) den += (double)expf(ldg_cg(&lg[v]) - mx);
+  den = block_sum_d<LOGPROB_THREADS>(den, s_redd);
+  if (threadIdx.x != 0) return;
+  const int id = ldg_cg(&p.idx[row]);
+  const float lp = (id >= 0 && id < V) ? (float)((double)(ldg_cg(&lg[id]) - mx) - log(den)) : __int_as_float(0x7fc00000);
+  if (p.rstate == nullptr) {
+    p.out[row] = lp;
+  } else {
+    const int n_gen = ldg_cg(&p.rstate[item].n_gen);
+    p.out[((size_t)item * p.max_new + n_gen) * p.num_vq + q] = lp;
+  }
 }
 
 template __global__ void k_sample<false>(const SampleP p);

@@ -819,10 +819,14 @@ def stream_schedule(requests: List[Request], dev, chunk: int, context=None, stat
 class SlotImage:
     """A suspended request (``EngineDevice.suspend``): its slot's image in pinned host memory (ctb_slot_image), until
     ``EngineDevice.resume`` restores it into a slot.  ``row(hidden)`` and ``outputs(n)`` read its first tokens' ids and
-    hidden states, as the slot held them, once the copies that filled it are complete (``ready``)."""
+    hidden states, as the slot held them, once the copies that filled it are complete (``ready``).  ``logprobs``: the
+    slot's log-probabilities [n_gen, num_vq] in pinned host memory (an engine with logprobs; they are not part of the
+    device image), else None."""
 
-    def __init__(self, buf: torch.Tensor, text: bool, device, num_vq: int, hidden_size: int, stream):
+    def __init__(self, buf: torch.Tensor, text: bool, device, num_vq: int, hidden_size: int, stream,
+                 logprobs: Optional[torch.Tensor] = None):
         self.buf, self.text, self.device, self.num_vq, self.hidden_size = buf, text, device, num_vq, hidden_size
+        self.logprobs = logprobs
         self.ready = torch.cuda.Event()
         self.ready.record(stream)  # after the copies that fill the image
         self.header = _lib.SlotImage.from_address(buf.data_ptr())
@@ -846,19 +850,23 @@ class SlotImage:
         from .gpt import GPT
 
         ids = self.row(False)[:n].to(torch.int64)
+        lp = [] if self.logprobs is None else [self.logprobs[:n, 0] if self.text else self.logprobs[:n]]
+        lp = [t.to(self.device) for t in lp]
         if self.text:
-            return GPT.GenerationOutputs(ids=[ids[:, 0].contiguous()], attentions=[], hiddens=[])
+            return GPT.GenerationOutputs(ids=[ids[:, 0].contiguous()], attentions=[], hiddens=[], logprobs=lp)
         hid = [self.row(True)[:n]] if return_hidden else []
-        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid)
+        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid, logprobs=lp)
 
 
 class EngineDevice:
     """The device layer of ``schedule`` on a GPT handle (ctb_gpt_engine_begin / _admit / _status, ctb_gpt_decode).
     ``kv_pool_pages`` (``kv_pool_pages()``) makes a paged engine (ctb_gpt_engine_begin_paged) with the pool interface
-    ``_poll_cycles`` describes; None keeps every slot's fixed pages."""
+    ``_poll_cycles`` describes; None keeps every slot's fixed pages.  ``logprobs`` attaches a buffer of token
+    log-probabilities (ctb_gpt_engine_logprobs) beside ``ids_out``: outputs then carry them (``GenerationOutputs
+    .logprobs``), and suspended requests take theirs along in their ``SlotImage``."""
 
     def __init__(self, gpt, requests: Sequence[Request], slots: int, max_new_cap: int, return_hidden: bool = True,
-                 flags: int = 0, kv_pool_pages: Optional[int] = None):
+                 flags: int = 0, kv_pool_pages: Optional[int] = None, logprobs: bool = False):
         self.gpt, self.requests, self.slots = gpt, requests, slots
         self.max_context = gpt.max_context
         self.lib = _lib.load()
@@ -869,6 +877,8 @@ class EngineDevice:
         self.ids_out = torch.zeros(slots, max_new_cap, gpt.num_vq, dtype=torch.int32, device=dev)
         self.hid_out = (torch.zeros(slots, max_new_cap, gpt.config.hidden_size, dtype=torch.float32, device=dev)
                         if return_hidden else None)
+        self.lp_out = (torch.zeros(slots, max_new_cap, gpt.num_vq, dtype=torch.float32, device=dev) if logprobs
+                       else None)
         hid = C.c_void_p(self.hid_out.data_ptr()) if self.hid_out is not None else None
         self.pool_pages = kv_pool_pages
         if kv_pool_pages is None:
@@ -878,6 +888,8 @@ class EngineDevice:
             _lib.check(self.lib.ctb_gpt_engine_begin_paged(
                 gpt._handle, slots, max_new_cap, flags, kv_pool_pages, C.c_void_p(self.ids_out.data_ptr()), hid,
                 self.stream))
+        if self.lp_out is not None:
+            _lib.check(self.lib.ctb_gpt_engine_logprobs(gpt._handle, C.c_void_p(self.lp_out.data_ptr()), self.stream))
         # the images of suspended requests, by id, while anything holds them (a cancelled one's ends with its outputs)
         self._images: "weakref.WeakValueDictionary[int, SlotImage]" = weakref.WeakValueDictionary()
         self._resumed: List[SlotImage] = []  # read by the device until the next status read
@@ -994,8 +1006,14 @@ class EngineDevice:
         buf = torch.empty(nbytes.value, dtype=torch.uint8, pin_memory=True)
         _lib.check(self.lib.ctb_gpt_engine_suspend(self.gpt._handle, slot, C.c_void_p(buf.data_ptr()), nbytes.value,
                                                    self.stream))
+        lp = None
+        if self.lp_out is not None:  # the header is written: n_gen is known on the host
+            n = _lib.SlotImage.from_address(buf.data_ptr()).n_gen
+            lp = torch.empty(n, self.gpt.num_vq, dtype=torch.float32, pin_memory=True)
+            with torch.cuda.stream(self._torch_stream):
+                lp.copy_(self.lp_out[slot, :n], non_blocking=True)
         image = SlotImage(buf, self._text[slot], self.dev, self.gpt.num_vq, self.gpt.config.hidden_size,
-                          self._torch_stream)
+                          self._torch_stream, lp)
         self._images[id(image)] = image
         return image
 
@@ -1003,6 +1021,9 @@ class EngineDevice:
         """Restore a suspended request into ``slot``, whose pages already cover it (ctb_gpt_engine_resume)."""
         _lib.check(self.lib.ctb_gpt_engine_resume(self.gpt._handle, slot, C.c_void_p(image.buf.data_ptr()),
                                                   image.nbytes, self.stream))
+        if self.lp_out is not None:
+            with torch.cuda.stream(self._torch_stream):
+                self.lp_out[slot, :image.logprobs.shape[0]].copy_(image.logprobs, non_blocking=True)
         self._text[slot] = image.text
         self._images.pop(id(image), None)
         self._resumed.append(image)  # the copies read it until the stream passes them
@@ -1041,25 +1062,31 @@ class EngineDevice:
         if isinstance(slot, SlotImage):  # a suspended request that was cancelled or interrupted
             self._images.pop(id(slot), None)
             return slot.outputs(n, self.hid_out is not None)
-        if self._text[slot]:
-            return GPT.GenerationOutputs(ids=[self.ids_out[slot, :n, 0].to(torch.int64)], attentions=[], hiddens=[])
+        text = self._text[slot]
+        lp = [] if self.lp_out is None else [(self.lp_out[slot, :n, 0] if text else self.lp_out[slot, :n]).clone()]
+        if text:
+            return GPT.GenerationOutputs(ids=[self.ids_out[slot, :n, 0].to(torch.int64)], attentions=[], hiddens=[],
+                                         logprobs=lp)
         ids = self.ids_out[slot, :n].to(torch.int64)
         hid = ([self.hid_out[slot, :n].clone() if copy else self.hid_out[slot, :n]] if self.hid_out is not None
                else [])
-        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid)
+        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid, logprobs=lp)
 
     def empty(self, index: Optional[int] = None):
         """The outputs of request ``index`` (default: a code request) when it ended empty (a seeded request whose
         first token was EOS)."""
         from .gpt import GPT
 
-        if index is not None and self.requests[index].infer_text:
+        text = index is not None and self.requests[index].infer_text
+        lp = ([] if self.lp_out is None else
+              [torch.zeros((0,) if text else (0, self.gpt.num_vq), dtype=torch.float32, device=self.dev)])
+        if text:
             return GPT.GenerationOutputs(ids=[torch.zeros(0, dtype=torch.int64, device=self.dev)], attentions=[],
-                                         hiddens=[])
+                                         hiddens=[], logprobs=lp)
         ids = torch.zeros(0, self.gpt.num_vq, dtype=torch.int64, device=self.dev)
         hid = ([torch.zeros(0, self.gpt.config.hidden_size, dtype=torch.float32, device=self.dev)]
                if self.hid_out is not None else [])
-        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid)
+        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid, logprobs=lp)
 
 
 _END = object()  # closes a streaming job's iterator
@@ -1107,6 +1134,7 @@ class Job:
         self.state = None
         self.spk_smp: Optional[str] = None  # Chat.open_engine paragraphs: the speaker sampled from sentence 0
         self.refined: Optional[List[Optional[str]]] = None  # refined paragraphs: each sentence's text once refined
+        self.logprobs = None  # Chat.open_engine(logprobs=True): the speech tokens' log-probabilities once it has ended
 
     def cancel(self) -> None:
         self._engine._source.cancel(self)
@@ -1321,7 +1349,7 @@ class GptEngine(OpenEngine):
             out = value[0] if isinstance(value, tuple) else value
             cur = torch.cuda.current_stream(self.device)
             cur.wait_event(event)
-            for t in [*out.ids, *out.hiddens]:
+            for t in [*out.ids, *out.hiddens, *out.logprobs]:
                 t.record_stream(cur)
         return value
 

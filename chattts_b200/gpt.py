@@ -60,11 +60,15 @@ class GPT:
         attentions: List[Optional[Tuple[torch.FloatTensor, ...]]]
         hiddens: List[torch.Tensor]
         cancelled: bool = False  # an open engine's job that was cancelled: the outputs are the prefix it had
+        # a slot engine opened with logprobs=True: per item, log p of each returned id under the model's logits at
+        # temperature 1 ([n, num_vq] fp32 for codes, [n] for text), aligned with ``ids``; otherwise empty
+        logprobs: List[torch.Tensor] = field(default_factory=list)
 
         def destroy(self):
             _del_all(self.ids)
             _del_all(self.attentions)
             _del_all(self.hiddens)
+            _del_all(self.logprobs)
 
     def __init__(self, gpt_config: Union[dict, GPTConfig], embed: Embed, use_flash_attn=False, use_vllm=False,
                  device=torch.device("cuda"), device_gpt=torch.device("cuda"),
@@ -231,7 +235,8 @@ class GPT:
     def generate_continuous(self, requests, slots: Optional[int] = None, return_hidden=True, infer_text=False,
                             stream=False, return_attn=False, context=None, chunk: Optional[int] = None,
                             max_new_cap: Optional[int] = None, dtype=torch.float32,
-                            prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None):
+                            prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None,
+                            logprobs: bool = False):
         """Generate audio codes or text for many utterances on a slot engine (chattts_b200.engine): up to ``slots``
         requests (default: ``max_batch``, at most the number of requests) decode together, and a waiting request takes
         the place of a finished one at the next poll (every ``chunk`` steps, default CTB_DECODE_CHUNK or 32).  Each
@@ -271,7 +276,11 @@ class GPT:
         Requests with equal ``Request.prompt_key`` (several takes of one utterance) must have equal prompts
         (``ValueError`` otherwise).  While one of them runs, another is admitted by taking that slot's KV for all but
         the last chunk of at most 128 prompt columns and prefilling only that chunk (``engine._poll_cycles``), with
-        the same outputs; a paged engine shares the pages themselves.  ``last_schedule_stats`` records the shares."""
+        the same outputs; a paged engine shares the pages themselves.  ``last_schedule_stats`` records the shares.
+
+        ``logprobs=True`` fills ``GenerationOutputs.logprobs``: for each returned id, its log-probability under the
+        head logits the sampler read, at temperature 1 and before the repetition penalty, top-P, top-K and the EOS ban
+        (ctb_gpt_engine_logprobs).  Ids and hidden states are the same with or without it."""
         from .engine import ScheduleStats, check_prefill_budget, kv_pool_pages, schedule
 
         flags = _lib.engine_flags(dtype)
@@ -286,7 +295,7 @@ class GPT:
         if not requests:
             return
         with torch.cuda.device(self.device_gpt):
-            dev = self._engine_device(requests, S, cap, return_hidden, flags, pool)
+            dev = self._engine_device(requests, S, cap, return_hidden, flags, pool, logprobs)
             self.last_schedule_stats = stats = ScheduleStats()  # admissions, decode steps (tools/bench_continuous.py)
             for i, slot, n in schedule(requests, dev, chunk, context, stats, check, prefill_budget):
                 yield i, (dev.empty(i) if slot is None else dev.harvest(slot, n))
@@ -297,7 +306,8 @@ class GPT:
     def generate_continuous_stream(self, requests, slots: Optional[int] = None, return_hidden=True, context=None,
                                    chunk: Optional[int] = None, infer_text=False, return_attn=False,
                                    max_new_cap: Optional[int] = None, dtype=torch.float32,
-                                   prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None):
+                                   prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None,
+                                   logprobs: bool = False):
         """Streaming form of ``generate_continuous``: generator of ``(request_index, GenerationOutputs, last)``.
 
         For each request the yields are exactly those ``generate(stream=True, stream_batch=r.stream_batch)`` makes for
@@ -309,8 +319,9 @@ class GPT:
         served as in ``generate_continuous``.
 
         ``ids`` are copies.  ``hiddens`` are views into the engine's buffer, like the narrowed views ``generate``
-        hands out: they stay valid until this generator is resumed (copy them to keep them).  ``dtype`` and
-        ``prefill_budget`` and ``kv_pool_bytes`` as in ``generate_continuous``: neither changes a request's yields."""
+        hands out: they stay valid until this generator is resumed (copy them to keep them).  ``dtype``,
+        ``prefill_budget`` and ``kv_pool_bytes`` as in ``generate_continuous``: none changes a request's yields.
+        ``logprobs`` as there: each yield carries copies of the log-probabilities of the ids it carries."""
         from .engine import ScheduleStats, check_prefill_budget, kv_pool_pages, stream_schedule
 
         flags = _lib.engine_flags(dtype)
@@ -322,7 +333,7 @@ class GPT:
         if not requests:
             return
         with torch.cuda.device(self.device_gpt):
-            dev = self._engine_device(requests, S, cap, return_hidden, flags, pool)
+            dev = self._engine_device(requests, S, cap, return_hidden, flags, pool, logprobs)
             self.last_schedule_stats = stats = ScheduleStats()
             for batch in stream_schedule(requests, dev, chunk, context, stats, check, prefill_budget=prefill_budget):
                 for i, slot, n, last in batch:
@@ -331,7 +342,8 @@ class GPT:
                 self.logger.warning("generation is interrupted")
 
     def open_engine(self, slots: int, max_new_cap: int, return_hidden=True, chunk: Optional[int] = None,
-                    dtype=torch.float32, prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None):
+                    dtype=torch.float32, prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None,
+                    logprobs: bool = False):
         """A slot engine that takes requests while it decodes: ``submit(request, stream=False) -> engine.Job`` from
         any thread, ``Job.cancel()`` for one request, ``close(cancel=False)`` (or a ``with`` block) to drain it.
 
@@ -347,18 +359,18 @@ class GPT:
         ``chunk`` steps (default CTB_DECODE_CHUNK, else 24).  ``slots`` and ``dtype`` as in ``generate_continuous``
         (up to ``max_batch`` slots; a half-precision engine up to 64).  ``kv_pool_bytes`` as in
         ``generate_continuous``: ``submit`` refuses a request that does not fit in the pool alone, and a job cancelled
-        while suspended ends with the tokens it had."""
+        while suspended ends with the tokens it had.  ``logprobs`` as in ``generate_continuous``."""
         from .engine import GptEngine
 
         return self._open_slot_engine(GptEngine, slots, max_new_cap, return_hidden, chunk,
                                       flags=_lib.engine_flags(dtype), prefill_budget=prefill_budget,
-                                      kv_pool_bytes=kv_pool_bytes)
+                                      kv_pool_bytes=kv_pool_bytes, logprobs=logprobs)
 
     def _open_slot_engine(self, cls, slots, max_new_cap, return_hidden, chunk, *args, flags=0, prefill_budget=None,
-                          kv_pool_bytes=None):
+                          kv_pool_bytes=None, logprobs=False):
         """An ``engine.OpenEngine`` subclass ``cls`` that owns this handle until it is closed (``flags``: the
         ctb_gpt_engine_begin_ex precision flags; ``prefill_budget``: the engine's bound on each poll's prefill;
-        ``kv_pool_bytes``: its KV pool, None for fixed pages)."""
+        ``kv_pool_bytes``: its KV pool, None for fixed pages; ``logprobs``: outputs carry token log-probabilities)."""
         from .engine import check_prefill_budget, kv_pool_pages
 
         prefill_budget = check_prefill_budget(prefill_budget)
@@ -366,16 +378,20 @@ class GPT:
         _, S, chunk, _, cap, check = self._engine_args("open_engine", [], slots, False, False, None, chunk, None,
                                                        max_new_cap, pool)
         kw = {"slots": S} if prefill_budget is None else {"prefill_budget": prefill_budget, "slots": S}
-        engine = cls(lambda requests: self._engine_device(requests, S, cap, return_hidden, flags, pool), chunk, check,
+        engine = cls(lambda requests: self._engine_device(requests, S, cap, return_hidden, flags, pool, logprobs), chunk,
+                     check,
                      self.device_gpt, self._close_engine, *args, max_new_cap=cap, **kw)
         self._open = engine
         return engine
 
-    def _engine_device(self, requests, S, cap, return_hidden, flags, pool_pages=None):
+    def _engine_device(self, requests, S, cap, return_hidden, flags, pool_pages=None, logprobs=False):
         """The ``engine.EngineDevice`` of one slot engine; an fp32 engine with fixed pages gets the five-argument form
         that stand-in devices implement."""
         from . import engine
 
+        if logprobs:
+            return engine.EngineDevice(self, requests, S, cap, return_hidden, flags=flags, kv_pool_pages=pool_pages,
+                                       logprobs=True)
         if pool_pages is not None:
             return engine.EngineDevice(self, requests, S, cap, return_hidden, flags=flags, kv_pool_pages=pool_pages)
         if flags:

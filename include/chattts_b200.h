@@ -356,6 +356,22 @@ int ctb_gpt_engine_resume(ctb_gpt* h, int32_t slot, const void* host_buf, uint64
  * (different prefill attention kernels); CTB_ERR_POOL (paged) when the free list cannot map dst's own pages. */
 int ctb_gpt_engine_share_prompt(ctb_gpt* h, int32_t src, int32_t dst, int32_t T0, int32_t c0, void* stream);
 
+/* ---- Token log-probabilities: attach logprobs_out_dev, [S, max_new_cap, num_vq] fp32 (device), to the slot engine
+ * just begun.  From then on every sampler launch of the engine (admissions, final prefill chunks, decode steps, and the
+ * decode graphs captured after this call) is followed by k_token_logprob, which writes, for every row it sampled,
+ *   logprobs_out_dev[slot][n][q] = log softmax(z)[id]
+ * where n is the index the id is written at in ids_out, q the codebook (text requests: q = 0 only) and z the fp32
+ * head logits row the sampler read: the model's distribution at temperature 1, before the repetition penalty, top-P,
+ * top-K and the min_new_token EOS ban.  The step that samples a terminating EOS writes no id, and its entry is not
+ * part of the request's output.  The row max is taken in fp32, the denominator summed in double in a fixed order and
+ * the result rounded once to fp32, so the same logits give the same bits.  Ids, hidden states and every other output
+ * are those of the engine without the buffer.  No kernel reads the buffer: a suspended request's entries are not in
+ * its ctb_slot_image, and the caller moves them with it.  The call zeroes the buffer on `stream`.  Every
+ * ctb_gpt_engine_begin* starts without a buffer.
+ * Errors (the handle as it was): CTB_ERR_ARG for a null argument; CTB_ERR_STATE outside a slot engine, or once the
+ * engine has admitted, prefilled a chunk for or resumed a request. */
+int ctb_gpt_engine_logprobs(ctb_gpt* h, float* logprobs_out_dev, void* stream);
+
 /* Measurement hook for bench.py's roofline: launches ONE kernel kind once per layer on the
  * state left by the last generate call (kind 0 qkv, 1 attention, 2 o-proj, 3 gate/up, 4 down;
  * 5 = heads, 6 = sampler, 7 = one decode step as ONE kernel launch (k_flow / k_step), 8 = 16 decode steps in one
@@ -382,6 +398,13 @@ int ctb_gpt_embed_prompt(ctb_gpt* h, const int64_t* ids_dev, const uint8_t* text
 int ctb_sample(const float* logits_dev, int32_t rows, int32_t V, int32_t rows_per_item,
                const ctb_sampler_config* sampler, const float* q_noise_dev, const int32_t* gen_ids_dev,
                int32_t gen_stride, int32_t n_gen, int32_t step, int32_t* out_idx_dev, void* stream);
+
+/* Stand-alone token log-probability (the kernel ctb_gpt_engine_logprobs launches): for each of `rows` rows of
+ * logits_dev [rows, V] fp32, out_dev[r] = log softmax(logits_dev[r])[ids_dev[r]] (NaN for an id outside [0, V)),
+ * with the arithmetic described there.  Enqueued on `stream`.  Errors: CTB_ERR_ARG for a null argument, rows < 1 or
+ * V < 1. */
+int ctb_token_logprobs(const float* logits_dev, int32_t rows, int32_t V, const int32_t* ids_dev, float* out_dev,
+                       void* stream);
 
 /* ---- token -> waveform: replaces ChatTTS/core.py:512-539 (_decode_to_wavs) ------ */
 
