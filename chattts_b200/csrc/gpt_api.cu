@@ -1122,9 +1122,10 @@ static int prefill_reserve(ctb_gpt* h, size_t rows) {
 }
 
 // The 20 layers over the B x T0 prompt columns in h->pf_resid (positions, mask and slots in pp), the prompt's K / V
-// appended to the rows' pages.  attn(pp) launches the layer's causal attention.
+// appended to the rows' pages.  attn(pp, l) launches layer l's causal attention.  append_kv == false: the queries
+// alone, against the K / V already in the pages (the attention-map pass), which then stops after the last attention.
 template <typename Attn>
-static int prefill_layers(ctb_gpt* h, PrefillP& pp, Attn attn, cudaStream_t s) {
+static int prefill_layers(ctb_gpt* h, PrefillP& pp, Attn attn, cudaStream_t s, bool append_kv = true) {
   const ctb_gpt_config& c = h->cfg;
   const ctb_gpt_layout& L = h->lay;
   const int B = pp.B, T0 = pp.T0, M = B * T0;
@@ -1147,11 +1148,13 @@ static int prefill_layers(ctb_gpt* h, PrefillP& pp, Attn attn, cudaStream_t s) {
     CTB_LAUNCH_CHECK();
     if ((rc = tc_gemm_launch<GE_NONE>(s, h->pf_xn, d, B, T0, nqkv, d, 1, d, 1, 0, Whi + L.wqkv, wlo(L.wqkv), nullptr,
                                       nullptr, nullptr, 0, h->pf_qkv, nqkv))) return rc;
-    if (kv16) k_prefill_rope_kv<__half><<<dim3(T0, B), 256, 0, s>>>(pp);
+    if (!append_kv) k_prefill_rope_q<<<dim3(T0, B), 256, 0, s>>>(pp);
+    else if (kv16) k_prefill_rope_kv<__half><<<dim3(T0, B), 256, 0, s>>>(pp);
     else k_prefill_rope_kv<float><<<dim3(T0, B), 256, 0, s>>>(pp);
     CTB_LAUNCH_CHECK();
-    attn(pp);
+    attn(pp, l);
     CTB_LAUNCH_CHECK();
+    if (!append_kv && l == c.num_layers - 1) break;
     if ((rc = tc_gemm_launch<GE_SCALE_RES>(s, h->pf_attn, d, B, T0, d, d, 1, d, 1, 0, Whi + L.wo, wlo(L.wo), h->pf_zeros,
                                            h->pf_ones, h->pf_resid, d, h->pf_resid, d))) return rc;
     k_rms_rows<<<rms_blocks, 256, 0, s>>>(h->pf_resid, w16 ? h->pf_ones : Wl + L.ln2, h->pf_xn, M, d, c.rms_eps);
@@ -1206,7 +1209,7 @@ static int prefill(ctb_gpt* h, int B, int T, int q0, int n, const float* emb, co
       (rc = kv16 ? ensure_smem_attr((const void*)k_prefill_attn_tiled<__half>, PftSmem<__half>::BYTES)
                  : ensure_smem_attr((const void*)k_prefill_attn_tiled<float>, PftSmem<float>::BYTES)))
     return rc;
-  auto attn = [&](const PrefillP& p) {
+  auto attn = [&](const PrefillP& p, int) {
     if (tiled) {
       const dim3 tgrid((n + PFT_TILE - 1) / PFT_TILE, c.num_heads, B);
       if (kv16) k_prefill_attn_tiled<__half><<<tgrid, PFT_THREADS, PftSmem<__half>::BYTES, s>>>(p, q0);
@@ -1373,6 +1376,55 @@ extern "C" int ctb_gpt_decode(ctb_gpt* h, int32_t n_steps, void* stream) {
     } else if ((rc = enqueue_step(h, -1, true, s))) {
       return rc;
     }
+  }
+  return CTB_OK;
+}
+
+// ------------------------------------------------------------------ attention maps of a static batch
+// A query-only teacher-forced pass: columns [q0, q0 + n) of the B rows go through the prefill layers, whose attention
+// (k_attn_probs) reads the K / V the decode wrote and writes each layer's probabilities; no page is written.  Columns
+// without a map row (padded prompt columns, steps after a row's end) are computed too and get their fill rows.  The
+// pass touches only the pf_* scratch, which no decode step reads (a static batch's decode state is x, the pages,
+// seq_len / pos / active, the loop state and the k_flow arena), and runs in chunks of at most AM_ROWS (row, column)
+// pairs, so pf_* stays within that of a 2-row prompt of 1,024 columns.  It reads the rows' padding and end_idx on the
+// device, so it never synchronises.
+static constexpr int AM_ROWS = 2048;
+
+extern "C" int ctb_gpt_attention_maps(ctb_gpt* h, int32_t B, int32_t T0, int32_t q0, int32_t n, const float* emb_dev,
+                                      const uint8_t* mask_dev, float* out_dev, void* stream) {
+  if (!h || !emb_dev || !mask_dev || !out_dev) return set_err(CTB_ERR_ARG, "null argument");
+  if (!h->started || h->engine) return set_err(CTB_ERR_STATE, "attention maps: no static batch in flight (ctb_gpt_begin)");
+  if (B != h->B || T0 != h->T0) return set_err(CTB_ERR_ARG, "attention maps: B=%d T0=%d, the batch has B=%d T0=%d", B, T0, h->B, h->T0);
+  const int fed = T0 + h->steps_enqueued - 1;  // columns fed by the steps enqueued so far
+  if (n < 1 || q0 < 0 || (q0 < T0 && (q0 != 0 || n < T0)) || q0 + n > fed)
+    return set_err(CTB_ERR_ARG, "attention maps: columns [%d, %d) are not whole steps of the %d columns fed", q0, q0 + n, fed);
+  const ctb_gpt_config& c = h->cfg;
+  if (c.head_dim != 64) return set_err(CTB_ERR_ARG, "attention maps: head_dim %d (64 supported)", c.head_dim);
+  cudaStream_t s = (cudaStream_t)stream;
+  int rc;
+  // only ever raised past the 48 KB every kernel may use without the attribute
+  const int probs_smem = (AM_SMEM_FLOATS + q0 + n) * (int)sizeof(float);
+  if (probs_smem > 48 * 1024 && (rc = ensure_smem_attr((const void*)k_attn_probs, probs_smem))) return rc;
+  const int chunk = std::max(1, AM_ROWS / B), d = c.hidden_size;
+  AttnMapP ap{};
+  ap.out = out_dev; ap.L = c.num_layers; ap.B = B; ap.Hq = c.num_heads; ap.Hkv = c.num_kv_heads; ap.T0 = T0; ap.q0 = q0;
+  ap.block_table = h->block_table; ap.pages_per_row = h->pages_per_row; ap.scaling = 1.0f / sqrtf((float)c.head_dim);
+  for (int a = q0; a < q0 + n; a += chunk) {
+    const int nc = std::min(chunk, q0 + n - a);
+    if ((rc = prefill_reserve(h, (size_t)B * nc))) return rc;
+    CTB_CUDA(cudaMemcpy2DAsync(h->pf_resid, (size_t)nc * d * sizeof(float), emb_dev + (size_t)(a - q0) * d,
+                               (size_t)n * d * sizeof(float), (size_t)nc * d * sizeof(float), B,
+                               cudaMemcpyDeviceToDevice, s));
+    k_attn_map_positions<<<B, 256, 0, s>>>(mask_dev, h->end_idx, T0, a, nc, h->pf_mask, h->pf_npre);
+    CTB_LAUNCH_CHECK();
+    PrefillP pp{};
+    pp.B = B; pp.T0 = nc; pp.mask = h->pf_mask; pp.slot = nullptr;
+    ap.a = a; ap.nc = nc; ap.q = h->pf_q; ap.attn = h->pf_attn; ap.mask = h->pf_mask; ap.npre = h->pf_npre;
+    auto attn = [&](const PrefillP& p, int l) {
+      ap.kv = p.kv; ap.layer = l;
+      k_attn_probs<<<dim3(nc, c.num_heads, B), AM_THREADS, (size_t)probs_smem, s>>>(ap);
+    };
+    if ((rc = prefill_layers(h, pp, attn, s, /*append_kv=*/false))) return rc;
   }
   return CTB_OK;
 }

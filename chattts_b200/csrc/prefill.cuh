@@ -98,6 +98,147 @@ __global__ void k_prefill_rope_kv(const PrefillP p) {
   }
 }
 
+// RoPE of the queries alone, as k_prefill_rope_kv computes them, with no KV append: the attention-map pass
+// (ctb_gpt_attention_maps) reads the K / V the decode wrote and leaves them as they are.  Grid (T0, B), 256 threads.
+__global__ void k_prefill_rope_q(const PrefillP p) {
+  const int c = blockIdx.x, b = blockIdx.y;
+  if (!p.mask[(size_t)b * p.T0 + c]) return;
+  const int pos = p.npre[(size_t)b * p.T0 + c];
+  const int half = p.hd / 2, nq = p.Hq * p.hd, nkv = p.Hkv * p.hd;
+  const float* src = p.qkv + ((size_t)b * p.T0 + c) * (nq + 2 * nkv);
+  float* dst = p.q + ((size_t)b * p.T0 + c) * nq;
+  for (int i = threadIdx.x; i < p.Hq * half; i += blockDim.x) {
+    const int h = i / half, j = i % half;
+    const float v0 = src[h * p.hd + j], v1 = src[h * p.hd + j + half];
+    const float c0 = p.rope_cos[(size_t)pos * p.hd + j], s0 = p.rope_sin[(size_t)pos * p.hd + j];
+    const float c1 = p.rope_cos[(size_t)pos * p.hd + j + half], s1 = p.rope_sin[(size_t)pos * p.hd + j + half];
+    const float o0 = __fadd_rn(__fmul_rn(v0, c0), __fmul_rn(-v1, s0));
+    const float o1 = __fadd_rn(__fmul_rn(v1, c1), __fmul_rn(v0, s1));
+    dst[h * p.hd + (p.permute_qk ? 2 * j : j)] = o0;
+    dst[h * p.hd + (p.permute_qk ? 2 * j + 1 : j + half)] = o1;
+  }
+}
+
+// The attention-map pass (ctb_gpt_attention_maps) over columns [a, a + nc) of the B rows of a static batch: which
+// columns have a map row, and their positions.  mask_out / npre_out [B, nc] (k_prefill_rope_q's mask and positions):
+// column c of row b is valid when pad_b <= c < T0 + end_idx[b] (steps up to the row's end), at position c - pad_b,
+// pad_b the zeros of the row's prompt mask.  Grid B, 256 threads.
+__global__ void k_attn_map_positions(const uint8_t* __restrict__ prompt_mask, const int* __restrict__ end_idx, int T0,
+                                     int a, int nc, uint8_t* __restrict__ mask_out, int* __restrict__ npre_out) {
+  __shared__ int s_pad;
+  const int b = blockIdx.x;
+  if (threadIdx.x == 0) s_pad = 0;
+  __syncthreads();
+  int z = 0;
+  for (int c = threadIdx.x; c < T0; c += blockDim.x) z += prompt_mask[(size_t)b * T0 + c] == 0;
+  atomicAdd(&s_pad, z);
+  __syncthreads();
+  const int pad = s_pad, last = T0 + end_idx[b];
+  for (int j = threadIdx.x; j < nc; j += blockDim.x) {
+    const int c = a + j;
+    mask_out[(size_t)b * nc + j] = c >= pad && c < last;
+    npre_out[(size_t)b * nc + j] = c - pad;
+  }
+}
+
+// Attention of the map pass, and its probabilities written where the reference's GenerationOutputs.attentions has
+// them.  The output is the blocks of steps i0, i0 + 1, ... (step of column q0), each [L, B, Hq, rows, cols] fp32:
+// step 0 (columns 0 .. T0 - 1) has rows = cols = T0, step i >= 1 (column T0 + i - 1) rows = 1, cols = T0 + i.  Key
+// column k of row b holds its position k - pad_b.
+struct AttnMapP {
+  const float* q;          // [B * nc, Hq * 64] queries of the chunk's columns (RoPE applied, the pages' q / k layout)
+  float* attn;             // [B * nc, Hq * 64] attention output (zero for columns without a map row)
+  const uint8_t* mask;     // [B, nc] column has a map row (k_attn_map_positions)
+  const int* npre;         // [B, nc] its position
+  const float* kv;         // the layer's pages (fp32)
+  const int* block_table; int pages_per_row;
+  float* out;
+  int L, B, Hq, Hkv, T0, q0, a, nc, layer;
+  float scaling;
+};
+
+// Grid (nc, Hq, B), AM_THREADS threads: one CTA per (column, head, row).  A column without a map row writes its fill
+// row: a padded prompt row 1 / T0 everywhere (eager attention's fully masked row), a step after the row's end zeros
+// (the device appends no KV for a finished row).  A valid column scores its keys 0 .. t (t its position) as
+// k_prefill_attn does (the same fmaf chain over the 64 dims, then the scale), takes the max and the sum in a fixed
+// order (thread-strided partials, xor butterfly, warps in order), so the same inputs give the same bits, writes the
+// whole map row (padded key columns and keys after the query 0, the others e / sum rounded once) and the attention
+// output sum_k p_k v_k (dims split over two halves of the CTA, keys even / odd, added in that order).  Dynamic
+// shared memory: AM_SMEM_FLOATS + the call's widest row (q0 + n floats).
+constexpr int AM_THREADS = 128, AM_SMEM_FLOATS = 64 + AM_THREADS / 32 + 64;
+__global__ void __launch_bounds__(AM_THREADS) k_attn_probs(const AttnMapP p) {
+  constexpr int HD = 64, NW = AM_THREADS / 32;
+  const int j = blockIdx.x, h = blockIdx.y, b = blockIdx.z, c = p.a + j, tid = threadIdx.x;
+  const size_t row = (size_t)b * p.nc + j;
+  const int step = c < p.T0 ? 0 : c - p.T0 + 1, i0 = p.q0 < p.T0 ? 0 : p.q0 - p.T0 + 1;
+  const int rows = step ? 1 : p.T0, cols = step ? p.T0 + step : p.T0;
+  int64_t blk = 0;  // elements per (layer, row, head) of the blocks of steps i0 .. step - 1
+  if (step > 0) {
+    const int64_t j0 = i0 > 0 ? i0 : 1;
+    blk = (i0 == 0 ? (int64_t)p.T0 * p.T0 : 0) + (step - j0) * p.T0 + (j0 + step - 1) * (step - j0) / 2;
+  }
+  float* o = p.out + blk * p.L * p.B * p.Hq +
+             ((((int64_t)p.layer * p.B + b) * p.Hq + h) * rows + (step ? 0 : c)) * cols;
+  float* ao = p.attn + (row * p.Hq + h) * HD;
+  if (!p.mask[row]) {
+    const float v = step == 0 ? 1.0f / (float)p.T0 : 0.f;
+    for (int k = tid; k < cols; k += AM_THREADS) o[k] = v;
+    if (tid < HD) ao[tid] = 0.f;
+    return;
+  }
+  extern __shared__ float am_smem[];
+  float* s_q = am_smem;                // [64]
+  float* s_red = am_smem + HD;         // [NW]
+  float* s_o = s_red + NW;             // [64] the odd keys' half of the output
+  float* s_p = am_smem + AM_SMEM_FLOATS;  // [t + 1]
+  const int t = p.npre[row], pad = c - t;
+  const int hk = h / (p.Hq / p.Hkv), lane = tid & 31, warp = tid >> 5;
+  const int* bt = p.block_table + (size_t)b * p.pages_per_row;
+  if (tid < HD) s_q[tid] = p.q[(row * p.Hq + h) * HD + tid];
+  __syncthreads();
+  const float4* q4 = reinterpret_cast<const float4*>(s_q);
+  float m = -INFINITY;
+  for (int k = tid; k <= t; k += AM_THREADS) {
+    const float4* kr = reinterpret_cast<const float4*>(p.kv + kv_off(bt[k / kPageTokens], 0, hk, k % kPageTokens, p.Hkv, HD));
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < HD / 4; ++i) {
+      const float4 kk = kr[i], qq = q4[i];
+      s = fmaf(qq.x, kk.x, s); s = fmaf(qq.y, kk.y, s); s = fmaf(qq.z, kk.z, s); s = fmaf(qq.w, kk.w, s);
+    }
+    s *= p.scaling;
+    s_p[k] = s;
+    m = fmaxf(m, s);
+  }
+  m = warp_max(m);
+  if (lane == 0) s_red[warp] = m;
+  __syncthreads();
+  m = s_red[0];
+#pragma unroll
+  for (int w = 1; w < NW; ++w) m = fmaxf(m, s_red[w]);
+  __syncthreads();  // s_red is reused for the sum
+  float sum = 0.f;
+  for (int k = tid; k <= t; k += AM_THREADS) { const float e = expf(s_p[k] - m); s_p[k] = e; sum += e; }
+  sum = warp_sum(sum);
+  if (lane == 0) s_red[warp] = sum;
+  __syncthreads();  // also: every e is in s_p
+  sum = s_red[0];
+#pragma unroll
+  for (int w = 1; w < NW; ++w) sum += s_red[w];
+  for (int k = tid; k < cols; k += AM_THREADS) {
+    const int kp = k - pad;  // padded key columns and keys after the query: probability 0
+    o[k] = (kp >= 0 && kp <= t) ? __fdiv_rn(s_p[kp], sum) : 0.f;
+  }
+  // attention output: dim d = tid % 64 over keys of parity tid / 64, V read a page row at a time
+  const int d = tid & (HD - 1), par = tid >> 6;
+  float acc = 0.f;
+  for (int k = par; k <= t; k += 2)
+    acc = fmaf(s_p[k], p.kv[kv_off(bt[k / kPageTokens], 1, hk, k % kPageTokens, p.Hkv, HD) + d], acc);
+  if (par) s_o[d] = acc;
+  __syncthreads();
+  if (!par) ao[d] = (acc + s_o[d]) / sum;  // V (and the output) is never permuted
+}
+
 // Causal attention over the row's valid prompt tokens, query-parallel: grid (ceil(T0 / 8), Hq, B), 8 warps per CTA,
 // ONE WARP PER QUERY (hd == 64).  Pass 1: lane-per-key scores into the warp's shared-memory row (same fma order per score
 // as the decode kernels), warp max; pass 2: exponentials + sum; pass 3: P.V with lane = two output dims, keys in order.

@@ -39,6 +39,23 @@ def _del_all(x):
         x.clear()
 
 
+def _attention_step_shapes(T0: int, i0: int, i1: int) -> List[Tuple[int, int]]:
+    """(rows, cols) of each step's map in [i0, i1): the prompt's [T0, T0] at step 0, then [1, T0 + i]."""
+    return [(T0, T0) if i == 0 else (1, T0 + i) for i in range(i0, i1)]
+
+
+def attention_map_views(buf: torch.Tensor, L: int, B: int, H: int, T0: int, i0: int, i1: int):
+    """The entries of steps i0 .. i1 - 1 of ``GenerationOutputs.attentions``, views into ``buf``, the output of one
+    ``ctb_gpt_attention_maps`` call: per step, a tuple of ``L`` tensors ``[B, H, rows, cols]`` (one per layer)."""
+    out, off = [], 0
+    for r, c in _attention_step_shapes(T0, i0, i1):
+        size = L * B * H * r * c
+        out.append(tuple(buf.narrow(0, off, size).view(L, B, H, r, c).unbind(0)))
+        off += size
+    assert off == buf.numel()
+    return out
+
+
 class GPT:
     class Context:
         """gpt.py:103-111 - interrupt flag polled between decode chunks."""
@@ -229,6 +246,31 @@ class GPT:
         n = max_new_token - 1 if n_steps is None else n_steps
         if n > 0:
             _lib.check(lib.ctb_gpt_decode(self._handle, n, stream_ptr))
+
+    def _extend_attention_maps(self, attentions: list, steps: int, emb_d: torch.Tensor, mask_d: torch.Tensor,
+                               ids_out: torch.Tensor, infer_text: bool, stream_ptr) -> None:
+        """Append to ``attentions`` the maps of steps ``len(attentions)`` .. ``steps - 1`` of the static batch in flight:
+        ctb_gpt_attention_maps over their query columns, whose embeddings are the prompt's (step 0) and
+        ctb_gpt_embed_prompt of the ids fed at steps 1, 2, ... (step i feeds the id sampled at step i - 1)."""
+        i0 = len(attentions)
+        if steps <= i0:
+            return
+        c = self.config
+        B, T0 = int(emb_d.shape[0]), int(emb_d.shape[1])
+        L, H = c.num_hidden_layers, c.num_attention_heads
+        parts = [emb_d] if i0 == 0 else []
+        g0, g1 = max(i0, 1) - 1, steps - 1
+        if g1 > g0:
+            ids = ids_out[:, g0:g1].to(torch.int64)
+            parts.append(self.embed_prompt(ids, torch.full(ids.shape[:2], bool(infer_text), device=ids.device)))
+        emb = torch.cat(parts, 1) if len(parts) > 1 else parts[0].contiguous()
+        q0 = 0 if i0 == 0 else T0 + i0 - 1
+        floats = L * B * H * sum(r * k for r, k in _attention_step_shapes(T0, i0, steps))
+        buf = torch.empty(floats, dtype=torch.float32, device=emb_d.device)
+        _lib.check(_lib.load().ctb_gpt_attention_maps(
+            self._handle, B, T0, q0, int(emb.shape[1]), C.c_void_p(emb.data_ptr()), C.c_void_p(mask_d.data_ptr()),
+            C.c_void_p(buf.data_ptr()), stream_ptr))
+        attentions.extend(attention_map_views(buf, L, B, H, T0, i0, steps))
 
     # ------------------------------------------------------------------ continuous batching
     @torch.no_grad()
@@ -465,10 +507,19 @@ class GPT:
                  infer_text=False, return_attn=False, return_hidden=False, stream=False, show_tqdm=True,
                  ensure_non_empty=True, stream_batch=24, manual_seed: Optional[int] = None,
                  context=Context()):
-        """Generator with the reference's contract (gpt.py:315-618)."""
+        """Generator with the reference's contract (gpt.py:315-618).
+
+        ``return_attn=True`` fills ``GenerationOutputs.attentions`` as the reference with eager attention does: one
+        entry per step run, each a tuple of ``num_hidden_layers`` fp32 device tensors of softmax probabilities,
+        ``[B, heads, T0, T0]`` for the prompt (step 0) and ``[B, heads, 1, T0 + i]`` for step i, whose query is the id
+        sampled at step i - 1; columns are the reference's, left padding included.  A padded key column is 0 and a
+        padded prompt row uniform (1 / T0); a row's entries for steps after its end (``end_idx``) are 0 (SURVEY.md
+        quirk list).  They are computed by a query-only pass over the K / V the decode wrote
+        (ctb_gpt_attention_maps), so ids and hidden states are the same with or without them.  With ``stream`` every
+        yield carries the steps done so far and the list is extended in place.  The maps take
+        ``4 * L * heads * B * (T0**2 + sum(T0 + i for i in 1 .. n - 1))`` bytes of device memory for n steps: about
+        170 MB for B = 1, T0 = 100 and 500 steps."""
         self._check_free("generate")
-        if return_attn:
-            raise NotImplementedError("return_attn: attention maps never leave the fused attention kernel")
         if not self._handle:
             raise _lib.CtbError("GPT weights not loaded")
         lib = _lib.load()
@@ -510,11 +561,15 @@ class GPT:
                 _lib.check(lib.ctb_gpt_status_query(self._handle, C.byref(st), C.c_void_p(end_idx.data_ptr()),
                                                     C.c_void_p(finish.data_ptr()), stream_ptr))
 
+            attentions: List[Optional[Tuple[torch.FloatTensor, ...]]] = []
+
             def outputs():
+                if return_attn:
+                    self._extend_attention_maps(attentions, steps, emb_d, mask_d, ids_out, infer_text, stream_ptr)
                 ids64 = ids_out.to(torch.int64)
                 if inputs_ids.device != ids64.device:
                     ids64 = ids64.to(inputs_ids.device)
-                return self._prepare_generation_outputs(ids64, 0, end_idx.clone().long(), [],
+                return self._prepare_generation_outputs(ids64, 0, end_idx.clone().long(), attentions,
                                                         hid_out if return_hidden else [], infer_text)
 
             pbar = None

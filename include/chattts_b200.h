@@ -138,6 +138,22 @@ typedef struct ctb_gpt_status {
 int ctb_gpt_status_query(ctb_gpt* h, ctb_gpt_status* out, int32_t* end_idx_host, uint8_t* finish_host,
                          void* stream);
 
+/* Attention maps of the static batch in flight (the reference's return_attn=True: GenerationOutputs.attentions, eager
+ * attention's softmax probabilities of every layer at every step), for query columns [q0, q0 + n): the whole prompt
+ * (q0 = 0, n >= T0) and/or the fed tokens of steps 1, 2, ... (column T0 + i - 1 is step i's query, the id sampled at
+ * step i - 1).  A query-only pass over the K / V the decode wrote: it changes no decode state, so it may run between
+ * ctb_gpt_decode calls.  Enqueued on `stream` (it reads the mask and the rows' end_idx there); does not synchronise.
+ *   emb_dev [B, n, hidden] fp32: the embeddings of columns q0 .. q0 + n - 1 (the prompt's, and ctb_gpt_embed_prompt
+ *     of the generated ids); mask_dev [B, T0]: the ctb_gpt_begin mask.
+ *   out_dev: the blocks of the steps of those columns, in order; step 0 [L, B, Hq, T0, T0], step i >= 1
+ *     [L, B, Hq, 1, T0 + i] fp32, key columns as the reference's (left padding included).  A padded key column is 0, a
+ *     padded prompt row is uniform (1 / T0) as eager attention gives a fully masked row, and a row's steps after its
+ *     end_idx are 0 (the device appends no KV for a finished row).
+ * CTB_ERR_STATE: no static batch in flight (no ctb_gpt_begin, or a slot engine owns the handle); CTB_ERR_ARG: B / T0
+ * are not the batch's, or the columns are not whole steps among those the enqueued steps fed. */
+int ctb_gpt_attention_maps(ctb_gpt* h, int32_t B, int32_t T0, int32_t q0, int32_t n, const float* emb_dev,
+                           const uint8_t* mask_dev, float* out_dev, void* stream);
+
 /* ---- slot engine: continuous batching of audio-code generation (no reference counterpart; the reference serves
  * this with the vLLM fork behind Chat.load(use_vllm=True)).  The handle's rows become S independent slots; each holds
  * one request (one utterance) at its own point of generation, with its own sampling parameters, noise and max_new,
