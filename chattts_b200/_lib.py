@@ -94,7 +94,7 @@ class VocosConfig(C.Structure):
 #: every symbol include/chattts_b200.h declares (checked by tests/test_abi.py)
 EXPORTS = (
     "ctb_abi_version", "ctb_last_error", "ctb_launch_count", "ctb_gpt_layout_query", "ctb_gpt_create",
-    "ctb_gpt_destroy", "ctb_gpt_begin", "ctb_gpt_decode", "ctb_gpt_status_query", "ctb_gpt_attention_maps", "ctb_gpt_profile_kernel", "ctb_gpt_debug_trace", "ctb_gpt_embed_prompt", "ctb_sample",
+    "ctb_gpt_destroy", "ctb_gpt_begin", "ctb_gpt_decode", "ctb_gpt_status_query", "ctb_gpt_attention_maps", "ctb_gpt_score", "ctb_gpt_profile_kernel", "ctb_gpt_debug_trace", "ctb_gpt_embed_prompt", "ctb_sample",
     "ctb_gpt_engine_begin", "ctb_gpt_engine_admit", "ctb_gpt_engine_admit_text", "ctb_gpt_engine_status",
     "ctb_gpt_engine_cancel", "ctb_gpt_engine_begin_ex", "ctb_gpt_engine_prefill_chunk",
     "ctb_gpt_engine_begin_paged", "ctb_gpt_engine_reserve", "ctb_gpt_engine_release", "ctb_gpt_engine_pages",
@@ -148,6 +148,7 @@ def load(build_if_missing: bool = True):
         lib.ctb_gpt_debug_trace.argtypes = [vp, vp, i32]
         lib.ctb_gpt_embed_prompt.argtypes = [vp, vp, vp, i32, i32, vp, vp]
         lib.ctb_gpt_attention_maps.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, vp]
+        lib.ctb_gpt_score.argtypes = [vp, i32, i32, vp, vp, vp, vp, i32, vp, vp]
         lib.ctb_gpt_engine_begin.argtypes = [vp, i32, i32, vp, vp, vp]
         lib.ctb_gpt_engine_begin_ex.argtypes = [vp, i32, i32, i32, vp, vp, vp]
         lib.ctb_gpt_engine_admit.argtypes = [vp, i32, vp, i32, vp, vp, C.POINTER(SamplerConfig), vp, vp, vp]

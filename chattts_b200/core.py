@@ -415,23 +415,43 @@ class Chat:
         from .engine import Request
 
         temperature = params.temperature if isinstance(params.temperature, list) else [params.temperature] * self.config.gpt.num_vq
+        num_code = self.config.gpt.num_audio_tokens - 1
+        warpers, processors = gen_logits(num_code=num_code, top_P=params.top_P, top_K=params.top_K,
+                                         repetition_penalty=params.repetition_penalty)
+        return Request(emb=self._code_prompt(text, params), temperature=temperature, eos_token=num_code,
+                       max_new_token=params.max_new_token, min_new_token=params.min_new_token,
+                       logits_processors=(*processors, *warpers), manual_seed=params.manual_seed,
+                       ensure_non_empty=params.ensure_non_empty, stream_batch=params.stream_batch,
+                       noise_batch=noise_batch)
+
+    def _code_prompt(self, text, params) -> torch.Tensor:
+        """The speech-code prompt of one normalised ``text`` as ``_infer_code([text], ...)`` builds it for a batch of
+        one: ``decorate_code_prompts`` with ``params.prompt`` / ``txt_smp`` / ``spk_emb``, the ``spk_smp`` codes, the
+        embedding and ``Speaker.apply``; its valid positions ``[P, d]``."""
         input_ids, attention_mask, text_mask = self.tokenizer.encode(
             self.speaker.decorate_code_prompts([text], params.prompt, params.txt_smp, params.spk_emb),
             self.config.gpt.num_vq,
             prompt=(self.speaker.decode_prompt(params.spk_smp) if params.spk_smp is not None else None),
             device=self.device_gpt)
-        num_code = self.config.gpt.num_audio_tokens - 1
-        warpers, processors = gen_logits(num_code=num_code, top_P=params.top_P, top_K=params.top_K,
-                                         repetition_penalty=params.repetition_penalty)
         emb = self.embed(input_ids, text_mask)
         if params.spk_emb is not None:
             self.speaker.apply(emb, params.spk_emb, input_ids, self.tokenizer.spk_emb_ids, self.gpt.device_gpt)
         valid = attention_mask[0].to(torch.bool).cpu()
-        return Request(emb=emb[0][valid.to(emb.device)], temperature=temperature, eos_token=num_code,
-                       max_new_token=params.max_new_token, min_new_token=params.min_new_token,
-                       logits_processors=(*processors, *warpers), manual_seed=params.manual_seed,
-                       ensure_non_empty=params.ensure_non_empty, stream_batch=params.stream_batch,
-                       noise_batch=noise_batch)
+        return emb[0][valid.to(emb.device)]
+
+    def score(self, texts, codes, params_infer_code=None, lang=None, do_text_normalization=True,
+              do_homophone_replacement=True) -> List[torch.Tensor]:
+        """The model's log-probability of given speech codes for each text: ``codes[i]`` (``[n, num_vq]`` ids, e.g.
+        ``GenerationOutputs.ids``, or a recording's ``dvae.sample_audio(wav).T``) after the code prompt that
+        ``infer`` builds for ``texts[i]`` with ``params_infer_code`` (``prompt``, ``txt_smp``, ``spk_smp``,
+        ``spk_emb``; the normaliser as in ``infer``).  Returns per text an fp32 tensor ``[n, num_vq]`` of
+        ``log softmax(z)[code]`` (``GPT.score``).  The quantity is defined at temperature 1 on the raw head logits, so
+        the sampling fields of the params (temperature, top_P, top_K, repetition_penalty) do not enter."""
+        texts = [texts] if isinstance(texts, str) else list(texts)
+        params = params_infer_code or Chat.InferCodeParams()
+        prompts = [self._code_prompt(self.normalizer(t, do_text_normalization, do_homophone_replacement, lang), params)
+                   for t in texts]
+        return self.gpt.score(prompts, list(codes))
 
     def _refine_request(self, text, params, noise_batch=None):
         """The text request ``_refine_text([text], ...)`` would generate as a batch of one (``noise_batch`` = (B, b): as

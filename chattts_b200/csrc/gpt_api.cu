@@ -137,6 +137,12 @@ struct ctb_gpt {
   std::vector<int> pg_ref;    // [pool_pages] block-table entries that map each page (above 1: a shared prompt's)
   int pg_shared;              // pages whose count is above 1
   char* pg_stage;             // KV_STAGE_BYTES of device staging for suspend / resume (allocated by the first one)
+  // ---- teacher-forced scoring (ctb_gpt_score): built or grown by the first call that needs them, then kept
+  float *sc_head_hi[2], *sc_head_lo[2];  // tf32 hi / lo copies of head_code [num_vq * V, d] and head_text [V, d]
+  float *sc_xn, *sc_logits;   // [SCORE_ROWS, d] final-normed scored columns; [SCORE_ROWS, widest head used] logits
+  size_t sc_logits_cols;
+  int* sc_src;                // [sc_src_cap] prefill row of each scored column
+  size_t sc_src_cap;
 };
 
 static size_t kv_elem_bytes(const ctb_gpt* h) { return (h->prec & CTB_ENGINE_FP16_KV) ? 2 : 4; }
@@ -574,7 +580,8 @@ extern "C" int ctb_gpt_destroy(ctb_gpt* h) {
                   h->tc_heads_code, h->tc_heads_text, h->x_hi, h->x_lo, h->attn_hi, h->attn_lo, h->h_hi, h->h_lo, h->bar, h->trace, h->flow_arena, h->flow_epoch, h->gw_hi, h->gw_lo, h->pf_resid, h->pf_xn, h->pf_qkv, h->pf_q,
                   h->pf_attn, h->pf_gu, h->pf_h, h->pf_ones, h->pf_zeros, h->pf_npre, h->pf_nvalid,
                   h->pf_mask, h->rows, h->cfgs, h->eng_noise, h->eng_slot, h->eng_text_logits, h->eng_text_idx,
-                  h->pg_stage};
+                  h->pg_stage, h->sc_head_hi[0], h->sc_head_hi[1], h->sc_head_lo[0], h->sc_head_lo[1], h->sc_xn,
+                  h->sc_logits, h->sc_src};
   delete[] h->m_wqkv; delete[] h->m_wo; delete[] h->m_wgu; delete[] h->m_wd;
   for (void* p : ptrs) if (p) cudaFree(p);
   fp16_free(h);
@@ -1191,8 +1198,9 @@ static int prefill_first_token(ctb_gpt* h, int B, int T0, const int* nvalid, con
 // PF_ATT_MAX_T0, else k_prefill_attn_tiled.  The call that ends the prompts (q0 + n == T) then hands each row's last
 // column to its decode row and samples the first token of every row in state h->phase (all h->B rows of a static batch;
 // the admitted slots of a slot engine); an earlier chunk touches nothing but the pf_* scratch and the slot's pages.
-static int prefill(ctb_gpt* h, int B, int T, int q0, int n, const float* emb, const uint8_t* mask,
-                   const int32_t* slots, cudaStream_t s) {
+// prefill_columns is the pass alone: it leaves every column's final residual in h->pf_resid [B * n, d].
+static int prefill_columns(ctb_gpt* h, int B, int T, int q0, int n, const float* emb, const uint8_t* mask,
+                           const int32_t* slots, cudaStream_t s) {
   const ctb_gpt_config& c = h->cfg;
   const int M = B * n;
   int rc;
@@ -1221,10 +1229,16 @@ static int prefill(ctb_gpt* h, int B, int T, int q0, int n, const float* emb, co
       else k_prefill_attn<float><<<agrid, PF_ATT_WARPS * 32, smem, s>>>(p, q0);
     }
   };
-  if ((rc = prefill_layers(h, pp, attn, s))) return rc;
+  return prefill_layers(h, pp, attn, s);
+}
+
+static int prefill(ctb_gpt* h, int B, int T, int q0, int n, const float* emb, const uint8_t* mask,
+                   const int32_t* slots, cudaStream_t s) {
+  int rc;
+  if ((rc = prefill_columns(h, B, T, q0, n, emb, mask, slots, s))) return rc;
   if (q0 + n < T) return CTB_OK;
   // a chunk's k_prefill_chunk_positions puts the row's token count q0 + n in nvalid[1]
-  return prefill_first_token(h, B, n, mask ? h->pf_nvalid : h->pf_nvalid + 1, pp.slot, s);
+  return prefill_first_token(h, B, n, mask ? h->pf_nvalid : h->pf_nvalid + 1, slots ? h->eng_slot : nullptr, s);
 }
 
 // Pages for B rows of up to `tokens` tokens each: grow the pool if needed (page = 16 tokens x K|V x heads x 64 values per
@@ -1425,6 +1439,131 @@ extern "C" int ctb_gpt_attention_maps(ctb_gpt* h, int32_t B, int32_t T0, int32_t
       k_attn_probs<<<dim3(nc, c.num_heads, B), AM_THREADS, (size_t)probs_smem, s>>>(ap);
     };
     if ((rc = prefill_layers(h, pp, attn, s, /*append_kv=*/false))) return rc;
+  }
+  return CTB_OK;
+}
+
+// ------------------------------------------------------------------ teacher-forced scoring
+// One causal prefill over the B x T columns of the rows to score (prompt, then the given tokens but the last), then the
+// heads over the columns that predict a given token and k_token_logprob over their logits.  The heads run in chunks of
+// at most SCORE_ROWS columns into one logits scratch: 173 MB for the text head's 21,178 columns.
+static constexpr int SCORE_ROWS = 2048;
+
+namespace ctb {
+// The final RMSNorm (k_rms_rows' arithmetic: fp32 statistics, out = w * (x * rinv)) of prefill rows src[i] of `resid`
+// into out row i, for i < n: one warp per row of 768
+__global__ void __launch_bounds__(256) k_score_gather(const float* __restrict__ resid, const int* __restrict__ src, int n,
+                                                      const float* __restrict__ w, float* __restrict__ out, int d,
+                                                      float eps) {
+  const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (row >= n) return;
+  const float4* xr = reinterpret_cast<const float4*>(resid + (size_t)src[row] * d);
+  float4 v[6];
+  float ss = 0.f;
+#pragma unroll
+  for (int i = 0; i < 6; ++i) {
+    v[i] = xr[i * 32 + lane];
+    ss = fmaf(v[i].x, v[i].x, ss); ss = fmaf(v[i].y, v[i].y, ss); ss = fmaf(v[i].z, v[i].z, ss); ss = fmaf(v[i].w, v[i].w, ss);
+  }
+  ss = warp_sum(ss);
+  const float rinv = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(__fdiv_rn(ss, (float)d), eps)));
+#pragma unroll
+  for (int i = 0; i < 6; ++i) {
+    const float4 g = __ldg(reinterpret_cast<const float4*>(w) + i * 32 + lane);
+    float4 o;
+    o.x = __fmul_rn(g.x, __fmul_rn(v[i].x, rinv)); o.y = __fmul_rn(g.y, __fmul_rn(v[i].y, rinv));
+    o.z = __fmul_rn(g.z, __fmul_rn(v[i].z, rinv)); o.w = __fmul_rn(g.w, __fmul_rn(v[i].w, rinv));
+    reinterpret_cast<float4*>(out + (size_t)row * d)[i * 32 + lane] = o;
+  }
+}
+}  // namespace ctb
+
+// What scoring m columns with the code (text = 0) or text head needs: the head's tf32 hi / lo copies, the normed-column
+// and logits scratch, and room for m source rows
+static int score_setup(ctb_gpt* h, int text, size_t m) {
+  const ctb_gpt_config& c = h->cfg;
+  const size_t d = c.hidden_size, N = text ? (size_t)c.num_text_tokens : (size_t)c.num_vq * c.num_audio_tokens;
+  int rc;
+  if (!h->sc_head_hi[text]) {
+    if ((rc = dalloc(&h->sc_head_hi[text], N * d)) || (rc = dalloc(&h->sc_head_lo[text], N * d))) {
+      cudaFree(h->sc_head_hi[text]); cudaFree(h->sc_head_lo[text]);
+      h->sc_head_hi[text] = h->sc_head_lo[text] = nullptr;
+      return rc;
+    }
+    k_split_tf32_t<0><<<2048, 256>>>(h->W + (text ? h->lay.head_text : h->lay.head_code), h->sc_head_hi[text],
+                                     h->sc_head_lo[text], (int64_t)(N * d));
+    CTB_LAUNCH_CHECK();
+    CTB_CUDA(cudaDeviceSynchronize());
+  }
+  if (!h->sc_xn && (rc = dalloc(&h->sc_xn, (size_t)SCORE_ROWS * d))) return rc;
+  if (h->sc_logits_cols < N) {
+    cudaFree(h->sc_logits); h->sc_logits = nullptr; h->sc_logits_cols = 0;
+    if ((rc = dalloc(&h->sc_logits, (size_t)SCORE_ROWS * N))) return rc;
+    h->sc_logits_cols = N;
+  }
+  if (h->sc_src_cap < m) {
+    cudaFree(h->sc_src); h->sc_src = nullptr; h->sc_src_cap = 0;
+    if ((rc = dalloc(&h->sc_src, m))) return rc;
+    h->sc_src_cap = m;
+  }
+  return CTB_OK;
+}
+
+extern "C" int ctb_gpt_score(ctb_gpt* h, int32_t B, int32_t T, const float* emb_dev, const int32_t* n_prompt,
+                             const int32_t* n_given, const int32_t* targets_dev, int32_t infer_text, float* out_dev,
+                             void* stream) {
+  if (!h || !emb_dev || !n_prompt || !n_given || !targets_dev || !out_dev) return set_err(CTB_ERR_ARG, "null argument");
+  const ctb_gpt_config& c = h->cfg;
+  if (B < 1 || B > c.max_batch) return set_err(CTB_ERR_ARG, "score: B=%d outside [1,%d]", B, c.max_batch);
+  if (T < 8 || T > c.max_context)
+    return set_err(CTB_ERR_ARG, "score: T=%d outside [8,%d]: left-pad shorter rows to 8", T, c.max_context);
+  size_t m = 0;
+  for (int b = 0; b < B; ++b) {
+    if (n_prompt[b] < 1 || n_given[b] < 1 || (int64_t)n_prompt[b] + n_given[b] - 1 > T)
+      return set_err(CTB_ERR_ARG, "score: row %d: prompt %d + given tokens %d - 1 outside [1,%d]", b, n_prompt[b],
+                     n_given[b], T);
+    m += (size_t)n_given[b];
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  int rc;
+  if (h->engine) {  // a slot engine's pages and decode state stay as they are while any slot has work
+    std::vector<RowState> rows;
+    if ((rc = read_rows(h, rows, s))) return rc;
+    for (int b = 0; b < h->B; ++b) {
+      if ((rc = check_not_generating(rows[b], b))) return rc;
+      if (h->slot[b].chunk_T0) return set_err(CTB_ERR_STATE, "slot %d has a prompt in progress", b);
+    }
+  }
+  if ((rc = score_setup(h, infer_text ? 1 : 0, m))) return rc;
+  // the pass takes the handle as ctb_gpt_begin does: the pages and prefill scratch are the fp32 model's, so a static
+  // batch or slot engine before it is over (ctb_gpt_decode, ctb_gpt_status_query, ... CTB_ERR_STATE until the next begin)
+  h->started = 0; h->engine = 0; h->prec = 0; h->pg_pages = 0; h->use_tc = false;
+  if ((rc = kv_reserve(h, B, T, s)) || (rc = prefill_reserve(h, (size_t)B * T))) return rc;
+  std::vector<uint8_t> mask((size_t)B * T, 0);  // row b: left padded, its P + n - 1 columns at the end
+  std::vector<int> src(m);                      // the prefill row of each scored column, rows in order
+  for (int b = 0, r = 0; b < B; ++b) {
+    const int pad = T - (n_prompt[b] + n_given[b] - 1);
+    memset(mask.data() + (size_t)b * T + pad, 1, (size_t)(T - pad));
+    for (int j = 0; j < n_given[b]; ++j) src[r++] = b * T + pad + n_prompt[b] - 1 + j;
+  }
+  CTB_CUDA(cudaMemcpyAsync(h->pf_mask, mask.data(), mask.size(), cudaMemcpyHostToDevice, s));
+  CTB_CUDA(cudaMemcpyAsync(h->sc_src, src.data(), m * sizeof(int), cudaMemcpyHostToDevice, s));
+  CTB_CUDA(cudaStreamSynchronize(s));  // host temporaries
+  if ((rc = prefill_columns(h, B, T, 0, T, emb_dev, h->pf_mask, nullptr, s))) return rc;
+  const int rpi = infer_text ? 1 : c.num_vq, V = infer_text ? c.num_text_tokens : c.num_audio_tokens, N = rpi * V;
+  const int d = c.hidden_size, k = infer_text ? 1 : 0;
+  for (size_t r0 = 0; r0 < m; r0 += SCORE_ROWS) {
+    const int mc = (int)std::min((size_t)SCORE_ROWS, m - r0);
+    k_score_gather<<<(mc + 7) / 8, 256, 0, s>>>(h->pf_resid, h->sc_src + r0, mc, h->W + h->lay.final_norm, h->sc_xn, d,
+                                                c.rms_eps);
+    CTB_LAUNCH_CHECK();
+    if ((rc = tc_gemm_launch<GE_NONE>(s, h->sc_xn, d, 1, mc, N, d, 1, d, 1, 0, h->sc_head_hi[k], h->sc_head_lo[k],
+                                      nullptr, nullptr, nullptr, 0, h->sc_logits, N)))
+      return rc;
+    LogprobP lp{};
+    lp.logits = h->sc_logits; lp.V = V; lp.rows_per_item = 1; lp.idx = targets_dev + r0 * rpi; lp.out = out_dev + r0 * rpi;
+    CTB_CUDA(launch_pdl(k_token_logprob, dim3((unsigned)(mc * rpi)), dim3(LOGPROB_THREADS), 0, s, lp));
+    CTB_LAUNCH_CHECK();
   }
   return CTB_OK;
 }
@@ -2095,6 +2234,7 @@ extern "C" int ctb_gpt_debug_trace(ctb_gpt* h, unsigned long long* host_out, int
 extern "C" int ctb_gpt_status_query(ctb_gpt* h, ctb_gpt_status* out, int32_t* end_idx_host, uint8_t* finish_host,
                                     void* stream) {
   if (!h || !out) return set_err(CTB_ERR_ARG, "null argument");
+  if (!h->started) return set_err(CTB_ERR_STATE, "no static batch or slot engine in flight (ctb_gpt_begin*)");
   cudaStream_t s = (cudaStream_t)stream;
   LoopState st;
   CTB_CUDA(cudaMemcpyAsync(&st, h->st, sizeof(st), cudaMemcpyDeviceToHost, s));

@@ -56,6 +56,22 @@ def attention_map_views(buf: torch.Tensor, L: int, B: int, H: int, T0: int, i0: 
     return out
 
 
+def score_groups(widths: List[int], max_batch: int) -> List[Tuple[List[int], int]]:
+    """The ``ctb_gpt_score`` calls ``GPT.score`` makes for rows of ``widths`` columns (prompt + given tokens - 1), as
+    ``[(row indices, padded width)]``, by the slot engine's admission rule: rows of up to ``LONG_PROMPT_COLS`` columns
+    share one width (at least ``MIN_PROMPT_COLS``) in calls of at most ``ADMIT_MAX_ROWS`` (row, column) pairs and
+    ``max_batch`` rows (``engine.admission_chunks``); a longer row is scored on its own, after them."""
+    from .engine import LONG_PROMPT_COLS, MIN_PROMPT_COLS, admission_chunks
+
+    short = [i for i, w in enumerate(widths) if w <= LONG_PROMPT_COLS]
+    out = []
+    if short:
+        T = max(MIN_PROMPT_COLS, max(widths[i] for i in short))
+        for part in admission_chunks(short, T):
+            out += [(part[k: k + max_batch], T) for k in range(0, len(part), max_batch)]
+    return out + [([i], w) for i, w in enumerate(widths) if w > LONG_PROMPT_COLS]
+
+
 class GPT:
     class Context:
         """gpt.py:103-111 - interrupt flag polled between decode chunks."""
@@ -271,6 +287,73 @@ class GPT:
             self._handle, B, T0, q0, int(emb.shape[1]), C.c_void_p(emb.data_ptr()), C.c_void_p(mask_d.data_ptr()),
             C.c_void_p(buf.data_ptr()), stream_ptr))
         attentions.extend(attention_map_views(buf, L, B, H, T0, i0, steps))
+
+    # ------------------------------------------------------------------ teacher-forced scoring
+    @torch.no_grad()
+    def score(self, prompts, targets, infer_text: bool = False) -> List[torch.Tensor]:
+        """The model's log-probability of given tokens: for each row, ``log softmax(z)[token]`` of every token of
+        ``targets[i]`` after ``prompts[i]`` and the tokens before it (teacher forcing), at temperature 1 on the raw
+        head logits ``z``, the quantity ``GenerationOutputs.logprobs`` holds for sampled ids.
+
+        ``prompts``: per row, the prompt embedding ``[P, d]`` with every position valid (``Request.emb``).
+        ``targets``: per row, ids ``[n, num_vq]`` of audio codes, or ``[n]`` text ids with ``infer_text``
+        (``GenerationOutputs.ids``).  Returns per row an fp32 device tensor ``[n, num_vq]`` (``[n]`` for text).
+
+        One causal prefill pass per call of ``ctb_gpt_score`` on the fp32 model, rows grouped as the slot engine
+        admits prompts (``score_groups``).  ValueError for an id outside the vocabulary or ``P + n - 1`` over
+        ``max_context``; RuntimeError while an open engine owns the handle.  A static ``generate`` stream in flight
+        ends (resuming it raises ``CtbError``)."""
+        self._check_free("score")
+        if not self._handle:
+            raise _lib.CtbError("GPT weights not loaded")
+        prompts, targets = list(prompts), list(targets)
+        if len(prompts) != len(targets):
+            raise ValueError(f"score: {len(prompts)} prompts and {len(targets)} target rows")
+        dev, d = self.device_gpt, self.config.hidden_size
+        rpi = 1 if infer_text else self.num_vq
+        V = self.num_text_tokens if infer_text else self.num_audio_tokens
+        rows = []
+        for i, (p, t) in enumerate(zip(prompts, targets)):
+            t = torch.as_tensor(t)
+            if p.dim() != 2 or int(p.shape[1]) != d or int(p.shape[0]) < 1:
+                raise ValueError(f"score: prompt {i} has shape {tuple(p.shape)}, expected [P >= 1, {d}]")
+            if (t.dim() != 1) if infer_text else (t.dim() != 2 or int(t.shape[1]) != rpi):
+                raise ValueError(f"score: targets {i} have shape {tuple(t.shape)}, expected "
+                                 f"{'[n]' if infer_text else f'[n, {rpi}]'}")
+            P, n = int(p.shape[0]), int(t.shape[0])
+            if n and (int(t.min()) < 0 or int(t.max()) >= V):
+                raise ValueError(f"score: targets {i} hold ids outside [0, {V})")
+            if P + n - 1 > self.max_context:
+                raise ValueError(f"score: row {i}: prompt {P} + {n} tokens - 1 exceed max_context={self.max_context}")
+            rows.append((p, t.reshape(n, rpi), P, n))
+        out = [torch.empty((n, rpi) if rpi > 1 else (n,), dtype=torch.float32, device=dev) for _, _, _, n in rows]
+        live = [i for i, r in enumerate(rows) if r[3] > 0]
+        if not live:
+            return out
+        lib = _lib.load()
+        with torch.cuda.device(dev):
+            stream_ptr = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            for group, T in score_groups([rows[i][2] + rows[i][3] - 1 for i in live], self.max_batch):
+                idx = [live[g] for g in group]
+                B = len(idx)
+                emb = torch.zeros(B, T, d, dtype=torch.float32, device=dev)
+                for b, i in enumerate(idx):
+                    p, t, P, n = rows[i]
+                    c0 = T - (P + n - 1)
+                    emb[b, c0: c0 + P] = p.to(dev, torch.float32)
+                    if n > 1:
+                        ids = t[: n - 1].to(dev, torch.int64).expand(n - 1, self.num_vq)[None].contiguous()
+                        emb[b, c0 + P:] = self.embed_prompt(ids, torch.full((1, n - 1), bool(infer_text), device=dev))[0]
+                tgt = torch.cat([rows[i][1] for i in idx]).to(dev, torch.int32).contiguous()
+                res = torch.empty(tgt.shape, dtype=torch.float32, device=dev)
+                n_prompt = (C.c_int32 * B)(*[rows[i][2] for i in idx])
+                n_given = (C.c_int32 * B)(*[rows[i][3] for i in idx])
+                _lib.check(lib.ctb_gpt_score(self._handle, B, T, C.c_void_p(emb.data_ptr()), n_prompt, n_given,
+                                             C.c_void_p(tgt.data_ptr()), int(bool(infer_text)),
+                                             C.c_void_p(res.data_ptr()), stream_ptr))
+                for i, r in zip(idx, res.split([rows[i][3] for i in idx])):
+                    out[i].copy_(r.view(out[i].shape))
+        return out
 
     # ------------------------------------------------------------------ continuous batching
     @torch.no_grad()

@@ -154,6 +154,28 @@ int ctb_gpt_status_query(ctb_gpt* h, ctb_gpt_status* out, int32_t* end_idx_host,
 int ctb_gpt_attention_maps(ctb_gpt* h, int32_t B, int32_t T0, int32_t q0, int32_t n, const float* emb_dev,
                            const uint8_t* mask_dev, float* out_dev, void* stream);
 
+/* Teacher-forced scoring on the fp32 model: the log-probability of given tokens under a prompt, computed in one causal
+ * prefill pass (the prefill kernels of ctb_gpt_begin, k_prefill_attn_tiled above 1,024 columns) instead of sampled.
+ * Row b has a prompt of n_prompt[b] positions and n_given[b] given tokens; its P + n - 1 columns (the prompt, then the
+ * given tokens but the last) are the last columns of its T, left padded.  For given token j of row b, the column before
+ * it (P - 1 + j of the row) gives the raw head logits z (code heads, V = num_audio_tokens, q < num_vq; or the text
+ * head, V = num_text_tokens, q = 0) and out = log softmax(z)[token] at temperature 1, the quantity
+ * ctb_gpt_engine_logprobs returns for sampled ids, with the same kernel (k_token_logprob).
+ *   emb_dev [B, T, hidden] fp32: each row's prompt embeddings then ctb_gpt_embed_prompt of its given tokens but the
+ *     last, in its last P + n - 1 columns (the padded columns are not read into any scored value)
+ *   n_prompt, n_given [B] (host): P >= 1, n >= 1, P + n - 1 <= T
+ *   targets_dev [m, rpi] int32, m = sum of n_given, rows in order (rpi = num_vq, or 1 with infer_text); out_dev the
+ *     same shape fp32.  An id outside [0, V) gives NaN for that entry alone.
+ * Enqueued on `stream` after one synchronisation that uploads the row layout.  The pass takes the handle as
+ * ctb_gpt_begin does: a static batch in flight ends (ctb_gpt_decode, ctb_gpt_status_query and
+ * ctb_gpt_attention_maps return CTB_ERR_STATE until the next ctb_gpt_begin), and so does a slot engine with no work.
+ * Errors: CTB_ERR_ARG for a null argument, B outside [1, max_batch], T outside [8, max_context] or a row that does
+ * not fit T; CTB_ERR_STATE while a slot engine has a slot pending, running or with a prompt in progress (the handle
+ * as it was). */
+int ctb_gpt_score(ctb_gpt* h, int32_t B, int32_t T, const float* emb_dev, const int32_t* n_prompt,
+                  const int32_t* n_given, const int32_t* targets_dev, int32_t infer_text, float* out_dev,
+                  void* stream);
+
 /* ---- slot engine: continuous batching of audio-code generation (no reference counterpart; the reference serves
  * this with the vLLM fork behind Chat.load(use_vllm=True)).  The handle's rows become S independent slots; each holds
  * one request (one utterance) at its own point of generation, with its own sampling parameters, noise and max_new,
