@@ -62,6 +62,21 @@ def engine_flags(dtype) -> int:
 PREFILL_CHUNK_ALIGN = 128
 
 
+#: CTB_ABI_VERSION of include/chattts_b200.h this binding is written for
+ABI_VERSION = 4
+
+#: the decode steps ctb_gpt_step_kind reports (CTB_STEP_* in the header)
+STEP_FLOW_INK, STEP_FLOW, STEP_MEGA, STEP_FMA, STEP_WGMMA = 1, 2, 3, 4, 5
+STEP_NAMES = {STEP_FLOW_INK: "k_flow+ink", STEP_FLOW: "k_flow", STEP_MEGA: "k_step", STEP_FMA: "fma", STEP_WGMMA: "wgmma"}
+
+
+def step_kind(handle, B: int, infer_text: bool = False) -> int:
+    """ctb_gpt_step_kind: which decode step serves a static batch of ``B`` rows on ``handle`` (a STEP_* value)."""
+    kind = load().ctb_gpt_step_kind(handle, int(B), int(bool(infer_text)))
+    check(min(kind, 0))
+    return kind
+
+
 #: slot states reported by ctb_gpt_engine_status (CTB_SLOT_* in the header)
 SLOT_IDLE, SLOT_RUNNING, SLOT_FINISHED = 0, 1, 2
 
@@ -94,7 +109,7 @@ class VocosConfig(C.Structure):
 #: every symbol include/chattts_b200.h declares (checked by tests/test_abi.py)
 EXPORTS = (
     "ctb_abi_version", "ctb_last_error", "ctb_launch_count", "ctb_gpt_layout_query", "ctb_gpt_create",
-    "ctb_gpt_destroy", "ctb_gpt_begin", "ctb_gpt_decode", "ctb_gpt_status_query", "ctb_gpt_attention_maps", "ctb_gpt_score", "ctb_gpt_profile_kernel", "ctb_gpt_debug_trace", "ctb_gpt_embed_prompt", "ctb_sample",
+    "ctb_gpt_destroy", "ctb_gpt_step_kind", "ctb_gpt_begin", "ctb_gpt_decode", "ctb_gpt_status_query", "ctb_gpt_attention_maps", "ctb_gpt_score", "ctb_gpt_profile_kernel", "ctb_gpt_debug_trace", "ctb_gpt_embed_prompt", "ctb_sample",
     "ctb_gpt_engine_begin", "ctb_gpt_engine_admit", "ctb_gpt_engine_admit_text", "ctb_gpt_engine_status",
     "ctb_gpt_engine_cancel", "ctb_gpt_engine_begin_ex", "ctb_gpt_engine_prefill_chunk",
     "ctb_gpt_engine_begin_paged", "ctb_gpt_engine_reserve", "ctb_gpt_engine_release", "ctb_gpt_engine_pages",
@@ -141,6 +156,7 @@ def load(build_if_missing: bool = True):
         lib.ctb_gpt_layout_query.argtypes = [C.POINTER(GptConfig), C.POINTER(GptLayout)]
         lib.ctb_gpt_create.argtypes = [C.POINTER(GptConfig), vp, C.POINTER(vp)]
         lib.ctb_gpt_destroy.argtypes = [vp]
+        lib.ctb_gpt_step_kind.argtypes = [vp, i32, i32]
         lib.ctb_gpt_begin.argtypes = [vp, i32, i32, vp, vp, C.POINTER(SamplerConfig), vp, i32, i32, vp, vp, vp]
         lib.ctb_gpt_decode.argtypes = [vp, i32, vp]
         lib.ctb_gpt_status_query.argtypes = [vp, C.POINTER(GptStatus), vp, vp, vp]
@@ -184,7 +200,7 @@ def load(build_if_missing: bool = True):
         lib.ctb_dvae_encoder_destroy.argtypes = [vp]
         lib.ctb_dvae_encode.argtypes = [vp, vp, i64, vp, i32, C.POINTER(i32), vp, vp, vp]
         lib.ctb_dvae_encode_rows.argtypes = [vp, i32, C.POINTER(vp), C.POINTER(i64), vp, i32, C.POINTER(i32), vp, vp]
-        if lib.ctb_abi_version() != 3:
+        if lib.ctb_abi_version() != ABI_VERSION:
             raise CtbError("ABI version mismatch")
         _lib = lib
         return lib

@@ -95,6 +95,7 @@ struct ctb_gpt {
   int flow_R;        // replicas of the broadcast exchange regions (CTB_FLOW_R)
   int flow_l2_ahead;  // weight tasks prefetched one layer ahead into L2 (CTB_FLOW_L2_AHEAD)
   int flow_max_batch; // batches that use it (CTB_FLOW_MAX_BATCH, default 1)
+  bool flow_no_ink;   // CTB_FLOW_NO_INK: k_flow runs one step per launch, sampled by k_sample / k_finalize
   unsigned long long* flow_arena;
   unsigned* flow_epoch;
   int steps_enqueued;  // loop iterations enqueued since ctb_gpt_begin (host-side bound for ctb_gpt_decode)
@@ -551,6 +552,7 @@ extern "C" int ctb_gpt_create(const ctb_gpt_config* c, const float* weights_dev,
     // H100, 512-token passes: k_flow<1> 239 ms vs k_step<1> 309 ms, but at B = 2 / 3 / 4 k_step is faster (332 / 379 / 395 ms
     // vs 342 / 530 / 550 ms), so the dataflow step serves B = 1 by default
     h->flow_max_batch = getenv("CTB_FLOW_MAX_BATCH") ? std::max(0, std::min(FL_BMAX, atoi(getenv("CTB_FLOW_MAX_BATCH")))) : 1;
+    h->flow_no_ink = getenv("CTB_FLOW_NO_INK") != nullptr;
   }
 #undef TRY
   h->use_graph = getenv("CTB_NO_GRAPH") == nullptr;
@@ -985,13 +987,27 @@ static int launch_step_flow(ctb_gpt* h, int col, bool sample, cudaStream_t s, in
   }
 }
 
-// the one-kernel steps (k_flow, k_step) keep the batch's loop counters in LoopState: never used by a slot engine
-static bool use_flow(const ctb_gpt* h) { return h->flow_ok && !h->engine && !h->use_tc && h->B <= h->flow_max_batch; }
+// Which step serves a static batch of B rows (tc: the wgmma step's GEMMs are on, tc_for).  The one-kernel steps
+// (k_flow, k_step) keep the batch's loop counters in LoopState: never used by a slot engine.
+static bool tc_for(const ctb_gpt* h, int B) { return h->tc_ready && B >= h->tc_min_batch; }
+static bool flow_for(const ctb_gpt* h, int B, bool tc) { return h->flow_ok && !tc && B <= h->flow_max_batch; }
+static bool mega_for(const ctb_gpt* h, int B, bool tc) { return h->mega_ok && !tc && B <= h->mega_max_batch; }
 // decode steps of audio generation at B <= 2 sample inside k_flow and run many steps per launch
-static bool flow_ink(const ctb_gpt* h) {
-  static const bool off = getenv("CTB_FLOW_NO_INK") != nullptr;
-  return !off && use_flow(h) && !h->infer_text && h->B <= 2 && h->cfg.num_audio_tokens <= FL_VPAD &&
-         h->B * h->cfg.num_vq <= FL_SROWS && h->cfg.num_vq <= 8;
+static bool ink_for(const ctb_gpt* h, int B, bool text, bool tc) {
+  return !h->flow_no_ink && flow_for(h, B, tc) && !text && B <= 2 && h->cfg.num_audio_tokens <= FL_VPAD &&
+         B * h->cfg.num_vq <= FL_SROWS && h->cfg.num_vq <= 8;
+}
+static bool use_flow(const ctb_gpt* h) { return !h->engine && flow_for(h, h->B, h->use_tc); }
+static bool flow_ink(const ctb_gpt* h) { return !h->engine && ink_for(h, h->B, h->infer_text, h->use_tc); }
+
+extern "C" int ctb_gpt_step_kind(const ctb_gpt* h, int32_t B, int32_t infer_text) {
+  if (!h) return set_err(CTB_ERR_ARG, "null argument");
+  if (B < 1 || B > h->cfg.max_batch) return set_err(CTB_ERR_ARG, "B=%d outside [1,%d]", B, h->cfg.max_batch);
+  const bool tc = tc_for(h, B);
+  if (ink_for(h, B, infer_text != 0, tc)) return CTB_STEP_FLOW_INK;
+  if (flow_for(h, B, tc)) return CTB_STEP_FLOW;
+  if (mega_for(h, B, tc)) return CTB_STEP_MEGA;
+  return tc ? CTB_STEP_WGMMA : CTB_STEP_FMA;
 }
 
 static int launch_finalize(ctb_gpt* h, cudaStream_t s) {
@@ -1018,7 +1034,7 @@ static int enqueue_step(ctb_gpt* h, int col, bool sample, cudaStream_t s) {
   const int decode = col < 0;
   int rc;
 
-  if (use_flow(h) || (h->mega_ok && !h->engine && !h->use_tc && h->B <= h->mega_max_batch)) {
+  if (use_flow(h) || (!h->engine && mega_for(h, h->B, h->use_tc))) {
     // small batches: the whole step (input -> 20 layers -> heads) is one persistent cooperative kernel
     if ((rc = use_flow(h) ? launch_step_flow(h, col, sample, s) : launch_step_mega(h, col, sample, s))) return rc;
     if (!sample) return CTB_OK;
@@ -1312,7 +1328,7 @@ extern "C" int ctb_gpt_begin(ctb_gpt* h, int32_t B, int32_t T0, const float* emb
   cudaStream_t s = (cudaStream_t)stream;
   h->B = B; h->T0 = T0; h->max_new = max_new_token; h->infer_text = infer_text ? 1 : 0;
   h->engine = 0; h->phase = RS_RUNNING; h->prec = 0; h->pg_pages = 0;
-  h->use_tc = h->tc_ready && B >= h->tc_min_batch;
+  h->use_tc = tc_for(h, B);
   h->sampler = *sampler; h->q_noise = q_noise_dev; h->emb = emb_dev; h->mask = mask_dev;
   h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev;
   if ((rc = restart_decode(h, s)) || (rc = kv_reserve(h, B, T0 + max_new_token, s))) return rc;

@@ -1361,7 +1361,9 @@ class GptEngine(OpenEngine):
                 continue
             if job.done():
                 continue
-            cancelled = i in self.stats.cancelled
+            # a cancelled request's final yield ends its job; the stream boundaries it crossed at the same poll
+            # come before it and are ordinary yields
+            cancelled = last and i in self.stats.cancelled
             if not (job.stream or (last and final) or cancelled):
                 continue
             out = dev.empty(i) if s is None else dev.harvest(s, n)

@@ -26,7 +26,7 @@ extern "C" {
 #define CTB_ERR_STATE (-3)
 #define CTB_ERR_NOMEM (-4)
 
-#define CTB_ABI_VERSION 3
+#define CTB_ABI_VERSION 4
 
 /* ---- library ------------------------------------------------------------------- */
 int ctb_abi_version(void);
@@ -107,6 +107,23 @@ typedef struct ctb_gpt ctb_gpt;
  * kept alive by the caller for the life of the handle. */
 int ctb_gpt_create(const ctb_gpt_config* cfg, const float* weights_dev, ctb_gpt** out);
 int ctb_gpt_destroy(ctb_gpt* h);
+
+/* Which decode step serves a static batch of B rows on this handle (ctb_gpt_begin with that B and infer_text): the
+ * predicates the launch code uses, evaluated for B without touching the handle.  The choice depends on the device
+ * (the one-kernel steps need 128 SMs or more; k_flow at most 191) and on the environment at ctb_gpt_create:
+ * CTB_NO_FLOW, CTB_FLOW_MAX_BATCH, CTB_FLOW_NO_INK, CTB_NO_MEGA, CTB_MEGA_MAX_BATCH, CTB_GPT_TC, CTB_GPT_FMA.
+ *   CTB_STEP_FLOW_INK  k_flow with the sampling tail inside, up to 64 steps per launch (audio rows, B <= 2)
+ *   CTB_STEP_FLOW      k_flow, one step per launch, sampled by k_sample
+ *   CTB_STEP_MEGA      k_step, the grid-barrier one-kernel step
+ *   CTB_STEP_FMA       the per-layer FMA kernels, chained by programmatic dependent launch
+ *   CTB_STEP_WGMMA     the per-layer wgmma 3xTF32 GEMM kernels
+ * Returns one of these (all > 0), or CTB_ERR_ARG for a null handle or B outside [1, max_batch]. */
+#define CTB_STEP_FLOW_INK 1
+#define CTB_STEP_FLOW 2
+#define CTB_STEP_MEGA 3
+#define CTB_STEP_FMA 4
+#define CTB_STEP_WGMMA 5
+int ctb_gpt_step_kind(const ctb_gpt* h, int32_t B, int32_t infer_text);
 
 /* Start one generate() call.  Replaces gpt.py:343-381 (buffer set-up) and the i == 0
  * iteration (prefill + first sample).

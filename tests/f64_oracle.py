@@ -55,6 +55,8 @@ class F64Oracle:
         self.head_code = [fold_weight_norm(w(f"head_code.{q}.parametrizations.weight.original0"),
                                            w(f"head_code.{q}.parametrizations.weight.original1"))
                           for q in range(num_vq)]
+        self.head_text = fold_weight_norm(w("head_text.parametrizations.weight.original0"),
+                                          w("head_text.parametrizations.weight.original1"))
 
     def _rms(self, x, w):
         return w * (x * torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + self.eps))
@@ -117,6 +119,16 @@ class F64Oracle:
         x = torch.cat([prompt_emb.to(self.device, self.dtype), self.embed_codes(ids[: n - 1])])
         hid = self.forward(x)[T0 - 1:]
         return hid, self.logits_rows(hid)
+
+    @torch.no_grad()
+    def teacher_forced_text(self, prompt_emb: torch.Tensor, ids: torch.Tensor):
+        """``teacher_forced`` for a text request (infer_text): ``ids`` [n] the generated text ids, each fed back through
+        emb_text.  Returns (hidden states [n, d], text-head logits [n, 1, num_text]): one sampler row per step."""
+        n, T0 = int(ids.shape[0]), int(prompt_emb.shape[0])
+        x = torch.cat([prompt_emb.to(self.device, self.dtype), F.embedding(ids[: n - 1].to(self.device).long(),
+                                                                           self.emb_text)])
+        hid = self.forward(x)[T0 - 1:]
+        return hid, F.linear(hid, self.head_text)[:, None]
 
 
 def top_k_margin(logits: torch.Tensor, generated: torch.Tensor, temperature: torch.Tensor, sp: SamplerParams) -> float:

@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 import torch
 
+from chattts_b200 import _lib
 from chattts_b200.config import Config
 from chattts_b200.embed import Embed
 from chattts_b200.gpt import GPT
@@ -47,3 +48,26 @@ def release_on_teardown(*caches):
             torch.cuda.empty_cache()
 
     return _release
+
+
+# the environment variables that take a decode step away from a handle created with them
+_STEP_OFF = {_lib.STEP_FLOW_INK: ("CTB_NO_FLOW", "CTB_FLOW_NO_INK"), _lib.STEP_FLOW: ("CTB_NO_FLOW",),
+             _lib.STEP_MEGA: ("CTB_NO_MEGA",), _lib.STEP_WGMMA: ("CTB_GPT_FMA",), _lib.STEP_FMA: ()}
+
+
+def expect_step(gpt, B, want, infer_text=False):
+    """Assert that the decode step ``want`` (a _lib.STEP_* value) serves a static batch of ``B`` rows on ``gpt``'s
+    handle.  Skips, with the reason, when the device or the environment the tests started with rules that step out:
+    k_flow needs 128 .. 191 SMs and k_step at least 128 (ctb_gpt_create).  Call it with the environment as the tests
+    started, not as a test set it for a handle."""
+    got = _lib.step_kind(gpt._handle, B, infer_text)
+    if got != want:
+        sms = torch.cuda.get_device_properties(gpt.device_gpt).multi_processor_count
+        if want in (_lib.STEP_FLOW_INK, _lib.STEP_FLOW) and not 128 <= sms <= 191:
+            pytest.skip(f"k_flow needs 128..191 SMs; this device has {sms}")
+        if want == _lib.STEP_MEGA and sms < 128:
+            pytest.skip(f"k_step needs at least 128 SMs; this device has {sms}")
+        off = [k for k in _STEP_OFF[want] if k in os.environ]
+        if off:
+            pytest.skip(f"{', '.join(off)} set in the environment: no {_lib.STEP_NAMES[want]} step")
+    assert got == want, (B, infer_text, _lib.STEP_NAMES.get(got, got), _lib.STEP_NAMES[want])

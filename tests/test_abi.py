@@ -4,16 +4,19 @@ import ctypes
 import os
 import re
 
+import pytest
+
 from chattts_b200 import _lib, build
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_library_builds_and_loads():
+def test_library_builds_and_loads_abi_version_4():
+    """Version 4 added ctb_gpt_step_kind and reads CTB_FLOW_NO_INK per handle."""
     path = build.build()
     assert os.path.exists(path)
     lib = _lib.load()
-    assert lib.ctb_abi_version() == 3
+    assert lib.ctb_abi_version() == _lib.ABI_VERSION == 4
 
 
 def test_every_declared_symbol_is_exported():
@@ -51,3 +54,18 @@ def test_graft_entry_build_runs_on_cpu():
     sys.path.insert(0, ROOT)
     entry = importlib.import_module("__graft_entry__")
     entry.build()
+
+
+def test_step_kind_constants_match_header_and_bad_arguments_are_refused():
+    """ctb_gpt_step_kind: the binding's STEP_* values are the header's CTB_STEP_*, and a null handle is CTB_ERR_ARG
+    (no device call: this runs without a GPU)."""
+    hdr = open(os.path.join(ROOT, "include", "chattts_b200.h")).read()
+    declared = {m[0]: int(m[1]) for m in re.findall(r"#define\s+CTB_STEP_([A-Z_]+)\s+(\d+)", hdr)}
+    assert declared == {"FLOW_INK": _lib.STEP_FLOW_INK, "FLOW": _lib.STEP_FLOW, "MEGA": _lib.STEP_MEGA,
+                        "FMA": _lib.STEP_FMA, "WGMMA": _lib.STEP_WGMMA}
+    assert set(_lib.STEP_NAMES) == set(declared.values()) and min(declared.values()) > 0
+    lib = _lib.load()
+    assert lib.ctb_gpt_step_kind(None, 1, 0) == -1
+    assert b"null" in lib.ctb_last_error()
+    with pytest.raises(_lib.CtbError):
+        _lib.step_kind(None, 1)

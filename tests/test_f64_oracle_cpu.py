@@ -103,3 +103,23 @@ def test_top_k_margin_is_the_gap_at_the_cut():
     assert abs(top_k_margin(logits, torch.zeros(1, 0, dtype=torch.long), torch.tensor([1.0]), sp) - 1e-4) < 1e-9
     sp = SamplerParams(top_p=None, top_k=None, repetition_penalty=1.0)
     assert top_k_margin(logits, torch.zeros(1, 0, dtype=torch.long), torch.tensor([1.0]), sp) == float("inf")
+
+
+def test_text_rows_follow_the_fp32_oracle():
+    """teacher_forced_text is the oracle's infer_text loop: text ids fed back through emb_text, the text head's logits
+    sampled with the text request's noise."""
+    gs, es = _cut(synth_gpt_state(0)), synth_embed_state(1)
+    orc, ref = GPTOracle(gs, es), F64Oracle(gs, es)
+    ids, mask, tmask = synth_prompt_batch([13], seed=6)
+    steps, temp, sp = 10, torch.tensor([0.7]), SamplerParams(penalty_max_ids=21177)
+    out = orc.generate(orc.embed_prompt(ids, tmask), ids, temp, 21001, attention_mask=mask, max_new_token=steps,
+                       min_new_token=steps, sampler=sp, infer_text=True, return_hidden=True, manual_seed=5)
+    got, hid = out.ids[0], out.hiddens[0]
+    assert got.shape == (steps,)
+    h64, lg = ref.teacher_forced_text(ref.embed_prompt(ids[0]), got)
+    assert lg.shape == (steps, 1, 21178)
+    err = float((h64 - hid.double()).abs().max())
+    assert err < 1e-5, err
+    sampled, margins = sample_trace(lg, got[:, None], temp, sp, exp_noise(1, 21178, 5), 21001, steps)
+    flips = [i for i in range(steps) if int(sampled[i, 0]) != int(got[i])]
+    assert all(margins[i] < MARGIN for i in flips) and len(flips) <= 1, (flips, margins)

@@ -143,44 +143,99 @@ def test_streaming_yields_cumulative_chunks():
     assert torch.equal(outs[-1].ids[0], full.ids[0]) and torch.equal(outs[0].ids[0], full.ids[0][:24])
 
 
-@pytest.mark.parametrize("env,lengths", [({"CTB_GPT_TC": "1"}, [5, 12, 9]), ({"CTB_GPT_TC": "1"}, [16]),
-                                         ({"CTB_NO_FLOW": "1", "CTB_MEGA_MAX_BATCH": "8"}, [5, 12, 9]),
-                                         ({"CTB_NO_FLOW": "1"}, [16]), ({"CTB_NO_FLOW": "1", "CTB_NO_MEGA": "1"}, [16]),
-                                         ({"CTB_NO_FLOW": "1", "CTB_NO_MEGA": "1", "CTB_NO_GRAPH": "1", "CTB_NO_PDL": "1"}, [7, 3]),
-                                         ({"CTB_FLOW_NO_INK": "1", "CTB_FLOW_MAX_BATCH": "4"}, [7, 3]),
-                                         ({"CTB_FLOW_R": "4", "CTB_FLOW_MAX_BATCH": "4"}, [5, 12, 9, 3])])
-def test_every_decode_back_end_gives_the_same_ids(env, lengths):
-    """The step implementations - the dataflow step (flow.cuh, default for B = 1), the grid-barrier one-kernel step
-    (mega.cuh), the PDL-chained FMA kernels and the wgmma 3xTF32 GEMM step (tc_decode.cuh) - are selected by batch
-    size; each is forced here on batches it would not get by default and must reproduce the CPU oracle's ids exactly."""
-    import os
-
+def _back_end_run(lengths):
+    """The 80-step run of test_every_decode_back_end_gives_the_same_ids on a handle created with the environment as it
+    is: (the handle's GPT, its outputs)."""
     from chattts_b200.config import Config
     from chattts_b200.embed import Embed
     from chattts_b200.gpt import GPT
     from chattts_b200.synth import synth_embed_state, synth_gpt_state
 
     gs, es = synth_gpt_state(0), synth_embed_state(1)
+    embed = Embed(768, 626, 21178, 4).load_state_dict(es).to("cuda")
+    gpt = GPT(Config().gpt, embed, device="cuda", device_gpt="cuda", max_batch=len(lengths), max_context=128)
+    gpt.load_state(gs)
+    return gpt, _run(gpt, embed, lengths, 13, 21, 80)[-1]
+
+
+# CTB_NO_PDL is read once per process (the launch helper of common.cuh), so its leg runs in a child process
+_CHILD = """
+import sys
+import torch
+sys.path[:0] = [{root!r}, {tests!r}]
+from chattts_b200 import _lib
+from test_gpu_gpt import _back_end_run
+gpt, out = _back_end_run({lengths!r})
+torch.save(dict(kind=_lib.step_kind(gpt._handle, {B}), ids=[t.cpu() for t in out.ids],
+                hiddens=[t.cpu() for t in out.hiddens]), {path!r})
+"""
+
+
+def _back_end_run_in_child(env, lengths, tmp_path):
+    import os
+    import subprocess
+    import sys
+
+    tests = os.path.dirname(os.path.abspath(__file__))
+    path = str(tmp_path / "child.pt")
+    code = _CHILD.format(root=os.path.dirname(tests), tests=tests, lengths=list(lengths), B=len(lengths), path=path)
+    flags = ["-s"] if sys.flags.no_user_site else []
+    # run() kills the child if it outlives the timeout
+    r = subprocess.run([sys.executable, *flags, "-c", code], env={**os.environ, **env}, capture_output=True, text=True,
+                       timeout=600)
+    assert r.returncode == 0, r.stderr[-4000:]
+    got = torch.load(path)
+    return got["kind"], got["ids"], got["hiddens"]
+
+
+# (environment at ctb_gpt_create, prompt lengths, the decode step that must serve the batch)
+BACK_ENDS = [
+    ({"CTB_GPT_TC": "1"}, [5, 12, 9], _lib.STEP_WGMMA), ({"CTB_GPT_TC": "1"}, [16], _lib.STEP_WGMMA),
+    ({"CTB_NO_FLOW": "1", "CTB_MEGA_MAX_BATCH": "8"}, [5, 12, 9], _lib.STEP_MEGA),
+    ({"CTB_NO_FLOW": "1"}, [16], _lib.STEP_MEGA), ({"CTB_NO_FLOW": "1", "CTB_NO_MEGA": "1"}, [16], _lib.STEP_FMA),
+    ({"CTB_NO_FLOW": "1", "CTB_NO_MEGA": "1", "CTB_NO_GRAPH": "1", "CTB_NO_PDL": "1"}, [7, 3], _lib.STEP_FMA),
+    ({"CTB_FLOW_NO_INK": "1", "CTB_FLOW_MAX_BATCH": "4"}, [7, 3], _lib.STEP_FLOW),
+    ({"CTB_FLOW_R": "4", "CTB_FLOW_MAX_BATCH": "4"}, [5, 12, 9, 3], _lib.STEP_FLOW),
+    ({"CTB_FLOW_MAX_BATCH": "2"}, [7, 3], _lib.STEP_FLOW_INK)]
+
+
+@pytest.mark.parametrize("env,lengths", [(e, n) for e, n, _ in BACK_ENDS])
+def test_every_decode_back_end_gives_the_same_ids(env, lengths, tmp_path):
+    """The step implementations - the dataflow step (flow.cuh, default for B = 1) with and without its in-kernel
+    sampler, the grid-barrier one-kernel step (mega.cuh), the PDL-chained FMA kernels (and the same kernels launched
+    plainly, CTB_NO_PDL) and the wgmma 3xTF32 GEMM step (tc_decode.cuh) - are selected by batch size; each is forced
+    here on batches it would not get by default, the handle must report that it got it (ctb_gpt_step_kind), and it must
+    reproduce the CPU oracle's ids exactly."""
+    import os
+
+    from chattts_b200.synth import synth_embed_state, synth_gpt_state
+    from gpu_util import expect_step
+
+    kind = next(k for e, n, k in BACK_ENDS if (e, n) == (env, lengths))
+    gs, es = synth_gpt_state(0), synth_embed_state(1)
     orc = GPTOracle(gs, es)
     ids, mask, tmask = synth_prompt_batch(lengths, seed=13)
     ref = orc.generate(orc.embed_prompt(ids, tmask), ids, torch.tensor([0.3] * 4), 625, attention_mask=mask,
                        max_new_token=80, min_new_token=80, sampler=SamplerParams(), return_hidden=True, manual_seed=21)
-    old = {k: os.environ.get(k) for k in env}
-    os.environ.update(env)
-    try:
-        embed = Embed(768, 626, 21178, 4).load_state_dict(es).to("cuda")
-        gpt = GPT(Config().gpt, embed, device="cuda", device_gpt="cuda", max_batch=len(lengths), max_context=128)
-        gpt.load_state(gs)
-        out = _run(gpt, embed, lengths, 13, 21, 80)[-1]
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
+    if "CTB_NO_PDL" in env:
+        got, out_ids, out_hid = _back_end_run_in_child(env, lengths, tmp_path)
+        assert got == kind, (env, _lib.STEP_NAMES.get(got, got))
+    else:
+        old = {k: os.environ.get(k) for k in env}
+        os.environ.update(env)
+        try:
+            gpt, out = _back_end_run(lengths)
+        finally:
+            for k, v in old.items():
+                if v is None:
+                    os.environ.pop(k, None)
+                else:
+                    os.environ[k] = v
+        expect_step(gpt, len(lengths), kind)
+        out_ids, out_hid = out.ids, out.hiddens
     for b in range(len(lengths)):
-        assert torch.equal(out.ids[b].cpu(), ref.ids[b]), (env, b)
-        assert (out.hiddens[b].cpu() - ref.hiddens[b]).abs().max() < 1e-4
+        assert torch.equal(out_ids[b].cpu(), ref.ids[b]), (env, b)
+        assert (out_hid[b].cpu() - ref.hiddens[b]).abs().max() < 1e-4
 
 
 def test_batch_larger_than_one_tile_matches_oracle():
@@ -337,7 +392,8 @@ def test_long_context_vs_oracle(lengths, steps, greedy):
 
 def test_multi_step_launch_matches_single_step_launches():
     """The dataflow step kernel runs up to 64 decode iterations per launch with the sampling tail inside (csrc/flow.cuh);
-    CTB_FLOW_NO_INK=1 launches one step at a time with k_sample / k_finalize outside.  Same ids, same early stop."""
+    CTB_FLOW_NO_INK=1 at ctb_gpt_create launches one step at a time with k_sample / k_finalize outside.  Same ids, same
+    early stop.  tests/test_gpu_small_batch_decode.py part A runs the sampler matrix on both."""
     import os
 
     from chattts_b200.config import Config
@@ -345,14 +401,18 @@ def test_multi_step_launch_matches_single_step_launches():
     from chattts_b200.gpt import GPT
     from chattts_b200.synth import synth_embed_state, synth_gpt_state
 
+    from gpu_util import expect_step
+
     gs, es = synth_gpt_state(0), synth_embed_state(1)
-    outs = {}
+    outs, gpts = {}, {}
     for tag, env in (("ink", {"CTB_FLOW_MAX_BATCH": "2"}), ("ext", {"CTB_FLOW_NO_INK": "1", "CTB_FLOW_MAX_BATCH": "2"})):
+        old = {k: os.environ.get(k) for k in env}
         os.environ.update(env)
         try:
             embed = Embed(768, 626, 21178, 4).load_state_dict(es).to("cuda")
             gpt = GPT(Config().gpt, embed, device="cuda", device_gpt="cuda", max_batch=2, max_context=400)
             gpt.load_state(gs)
+            gpts[tag] = gpt
             ids, mask, tmask = synth_prompt_batch([16, 9], seed=3)
             warp, proc = gen_logits(num_code=625, top_P=0.7, top_K=20, repetition_penalty=1.05)
             outs[tag] = list(gpt.generate(embed(ids, tmask), ids, temperature=torch.tensor([1.5] * 4), eos_token=625,
@@ -360,8 +420,13 @@ def test_multi_step_launch_matches_single_step_launches():
                                           logits_processors=(*proc, *warp), return_hidden=True, show_tqdm=False,
                                           manual_seed=7))[-1]
         finally:
-            for k in env:
-                os.environ.pop(k, None)
+            for k, v in old.items():
+                if v is None:
+                    os.environ.pop(k, None)
+                else:
+                    os.environ[k] = v
+    expect_step(gpts["ext"], 2, _lib.STEP_FLOW)
+    expect_step(gpts["ink"], 2, _lib.STEP_FLOW_INK)
     for b in range(2):
         assert torch.equal(outs["ink"].ids[b], outs["ext"].ids[b])
         assert torch.equal(outs["ink"].hiddens[b], outs["ext"].hiddens[b])

@@ -323,3 +323,24 @@ def test_chat_engine_checks_the_speech_stage_limit_at_submit():
             eng.submit("hello", params_infer_code=Chat.InferCodeParams(max_new_token=200), skip_refine_text=False)
     finally:
         eng.close()
+
+
+def test_a_cancel_at_a_poll_that_crosses_stream_boundaries_ends_the_job_once():
+    """stream_batch 2 and 4-step chunks: every poll crosses boundaries, so the poll that stops a cancelled request also
+    yields its boundaries.  Those are ordinary yields; the job ends once, cancelled, with what it has (a second end
+    would fail the worker, and close would raise it)."""
+    def req():
+        return Request(emb=torch.zeros(5, 4), temperature=[0.3], eos_token=625, max_new_token=2000, manual_seed=1,
+                       stream_batch=2)
+
+    with GptEngine(lambda requests: SlowStub(2, requests), 4) as eng:
+        streamed, plain = eng.submit(req(), stream=True), eng.submit(req())
+        it = iter(streamed)
+        next(it)
+        streamed.cancel()
+        plain.cancel()
+        rest = [(int(o.ids[0].shape[0]), last) for o, last in it]
+        assert not any(last for _, last in rest) and all(n % 2 == 0 for n, _ in rest), rest
+        for job in (streamed, plain):
+            out = job.result(timeout=10)
+            assert job.cancelled() and out.cancelled and 0 < int(out.ids[0].shape[0]) < 2000
