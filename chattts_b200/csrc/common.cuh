@@ -172,9 +172,11 @@ __device__ __forceinline__ float philox_exp1(uint64_t seed, uint32_t c0, uint32_
   return -logf(u);
 }
 
-// order-preserving map float -> uint32 (larger float => larger key; -inf smallest)
+// order-preserving map float -> uint32 (larger float => larger key; -inf smallest).  -0.0 and +0.0 get one key, as
+// they compare equal: a -0.0 logit is kept wherever a +0.0 one is (top-k cut, greedy max), like torch's `x < kth`.
 __device__ __forceinline__ uint32_t float_key(float f) {
   uint32_t u = __float_as_uint(f);
+  if (u == 0x80000000u) u = 0u;
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 __device__ __forceinline__ float key_float(uint32_t k) {

@@ -715,8 +715,10 @@ __device__ __noinline__ int fl_sample_row(const ctb_sampler_config& c, const flo
   mx = fl_bmax(mx, sm.redf);
   FL_SK();
 
+  // as k_sample: top_k taken as given (its warper's min_tokens_to_keep is already in it), and each cut is a key
+  // threshold, so a tie group at the top-p or top-k cut is kept whole
   const bool use_p = c.top_p >= 0.f;
-  const int kk = c.top_k > 0 ? min(max(c.top_k, c.min_tokens_to_keep), V) : 0;
+  const int kk = c.top_k > 0 ? min(c.top_k, V) : 0;
   const int min_keep = min(c.min_tokens_to_keep, V);
   uint32_t thr_key = 0;
   // greedy replaces thr_key by the arg-max key below, so the top-p / top-k threshold is dead work there (uniform branch)

@@ -106,8 +106,12 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) k_sample(const SampleP p) {
   for (int v = tid; v < V; v += SAMPLE_THREADS) mx = fmaxf(mx, s_x[v]);
   mx = block_max_f(mx, s_redf);
 
+  // top_k is taken as given: TopKLogitsWarper has already folded its own min_tokens_to_keep into it, and
+  // c.min_tokens_to_keep is top-p's alone.  Both cuts are key thresholds, so a tie group at either cut is kept whole:
+  // top-p keeps every token equal to the smallest kept one, where HF removes by position in its sorted row (an order
+  // among equal values no deterministic kernel can reproduce; only the number HF removes is defined).
   const bool use_p = c.top_p >= 0.f;
-  const int kk = c.top_k > 0 ? min(max(c.top_k, c.min_tokens_to_keep), V) : 0;
+  const int kk = c.top_k > 0 ? min(c.top_k, V) : 0;
   const int min_keep = min(c.min_tokens_to_keep, V);
   uint32_t thr_key = 0;  // keep x iff float_key(x) >= thr_key
 

@@ -79,12 +79,17 @@ int ctb_gpt_layout_query(const ctb_gpt_config* cfg, ctb_gpt_layout* out);
 
 /* Sampling tail: gpt.py:487-508 + processors.py:18-58 + HF TopP/TopK warpers.
  * Order: temperature -> repetition penalty -> top-p -> top-k -> [greedy mask] ->
- * (step < min_new: EOS ban) -> softmax -> argmax(p / q)  (== torch.multinomial). */
+ * (step < min_new: EOS ban) -> softmax -> argmax(p / q)  (== torch.multinomial).
+ * Ties: the top-p and top-k cuts are value thresholds, so every token equal to the smallest kept value is kept.  At
+ * the top-p cut HF removes tied tokens by their position in torch.sort's output, an order among equal values that is
+ * not defined; the kept set here contains HF's and differs from it only in tokens equal to the cut value.  -0.0 and
+ * +0.0 are equal values. */
 typedef struct ctb_sampler_config {
   float temperature[8];     /* per codebook (row r uses temperature[r % rows_per_item]) */
   float top_p;              /* <0: warper absent (gen_logits top_P=None) */
-  int32_t top_k;            /* <=0: warper absent */
-  int32_t min_tokens_to_keep; /* 3 (processors.py:45,47) */
+  int32_t top_k;            /* <=0: warper absent; else the number kept, used as given: HF's TopKLogitsWarper has
+                               already taken max(top_k, its own min_tokens_to_keep) */
+  int32_t min_tokens_to_keep; /* top-p's (TopPLogitsWarper.min_tokens_to_keep; 3 at processors.py:45) */
   int32_t penalty_on;       /* 0: no CustomRepetitionPenaltyLogitsProcessorRepeat (penalty == 1) */
   float penalty_lut[32];    /* penalty ** count for count = 0..past_window, built by the host
                                with the same torch.pow call as processors.py:28 */
