@@ -115,7 +115,7 @@ EXPORTS = (
     "ctb_gpt_engine_begin_paged", "ctb_gpt_engine_reserve", "ctb_gpt_engine_release", "ctb_gpt_engine_pages",
     "ctb_gpt_engine_suspend_bytes",
     "ctb_gpt_engine_suspend", "ctb_gpt_engine_resume", "ctb_gpt_engine_share_prompt", "ctb_gpt_engine_logprobs",
-    "ctb_token_logprobs",
+    "ctb_token_logprobs", "ctb_gpt_engine_top_logprobs", "ctb_token_top_logprobs", "ctb_gpt_score_ex",
     "ctb_dvae_blob_floats", "ctb_vocos_blob_floats", "ctb_decoder_create", "ctb_decoder_destroy",
     "ctb_dvae_decode", "ctb_vocos_decode", "ctb_decode_rows",
     "ctb_dvae_encoder_blob_floats", "ctb_dvae_encoder_create", "ctb_dvae_encoder_destroy", "ctb_dvae_encode",
@@ -183,6 +183,9 @@ def load(build_if_missing: bool = True):
         lib.ctb_gpt_engine_share_prompt.argtypes = [vp, i32, i32, i32, i32, vp]
         lib.ctb_gpt_engine_logprobs.argtypes = [vp, vp, vp]
         lib.ctb_token_logprobs.argtypes = [vp, i32, i32, vp, vp, vp]
+        lib.ctb_gpt_engine_top_logprobs.argtypes = [vp, i32, vp, vp, vp]
+        lib.ctb_token_top_logprobs.argtypes = [vp, i32, i32, i32, vp, vp, vp]
+        lib.ctb_gpt_score_ex.argtypes = [vp, i32, i32, vp, vp, vp, vp, i32, vp, i32, vp, vp, vp]
         lib.ctb_sample.argtypes = [vp, i32, i32, i32, C.POINTER(SamplerConfig), vp, vp, i32, i32, i32, vp, vp]
         lib.ctb_dvae_blob_floats.argtypes = [C.POINTER(ConvStackConfig)]
         lib.ctb_dvae_blob_floats.restype = i64

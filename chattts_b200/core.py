@@ -440,17 +440,24 @@ class Chat:
         return emb[0][valid.to(emb.device)]
 
     def score(self, texts, codes, params_infer_code=None, lang=None, do_text_normalization=True,
-              do_homophone_replacement=True) -> List[torch.Tensor]:
+              do_homophone_replacement=True, top_logprobs: int = 0) -> list:
         """The model's log-probability of given speech codes for each text: ``codes[i]`` (``[n, num_vq]`` ids, e.g.
         ``GenerationOutputs.ids``, or a recording's ``dvae.sample_audio(wav).T``) after the code prompt that
         ``infer`` builds for ``texts[i]`` with ``params_infer_code`` (``prompt``, ``txt_smp``, ``spk_smp``,
         ``spk_emb``; the normaliser as in ``infer``).  Returns per text an fp32 tensor ``[n, num_vq]`` of
         ``log softmax(z)[code]`` (``GPT.score``).  The quantity is defined at temperature 1 on the raw head logits, so
-        the sampling fields of the params (temperature, top_P, top_K, repetition_penalty) do not enter."""
+        the sampling fields of the params (temperature, top_P, top_K, repetition_penalty) do not enter.
+        ``top_logprobs=N`` (1..20) makes each entry ``(lp, top_ids, top_lp)``: the codes the model expected most at
+        every frame, ``[n, num_vq, N]``, and their log-probabilities (``GPT.score(top_logprobs=N)``)."""
+        from .engine import check_top_logprobs
+
+        check_top_logprobs(top_logprobs)
         texts = [texts] if isinstance(texts, str) else list(texts)
         params = params_infer_code or Chat.InferCodeParams()
         prompts = [self._code_prompt(self.normalizer(t, do_text_normalization, do_homophone_replacement, lang), params)
                    for t in texts]
+        if top_logprobs:
+            return self.gpt.score(prompts, list(codes), top_logprobs=top_logprobs)
         return self.gpt.score(prompts, list(codes))
 
     def _refine_request(self, text, params, noise_batch=None):
@@ -477,7 +484,7 @@ class Chat:
 
     def open_engine(self, slots: Optional[int] = None, max_new_cap: int = 2048, use_decoder: bool = True,
                     dtype=torch.float32, prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None,
-                    logprobs: bool = False):
+                    logprobs: bool = False, top_logprobs: int = 0):
         """A long-lived slot engine (``GPT.open_engine``) that synthesises texts submitted from any thread while it
         decodes: ``engine.submit(text, params_infer_code=None, stream=False, skip_refine_text=True, ...) -> Job``,
         ``Job.cancel()`` for one text, ``close(cancel=False)`` or a ``with`` block to drain it (``close(cancel=True)``
@@ -495,14 +502,22 @@ class Chat:
         token under the model's head logits at temperature 1 (``GPT.generate_continuous(logprobs=True)``): the
         ``[n, num_vq]`` tensor of its code request for a one-sentence job, a list of such tensors in take order with
         ``takes``, and in sentence order with ``split_text=True`` (neither the reference stage nor refinements are
-        included).  The waveforms are the same as without it.  None on an engine opened without it."""
+        included).  The waveforms are the same as without it.  None on an engine opened without it.
+
+        ``top_logprobs=N`` (1..20): every finished job also has ``Job.top_logprobs``, with the same structure: per code
+        request a CPU pair ``(ids, lp)`` of ``[n, num_vq, N]`` tensors, the N codes with the largest head logits at
+        each frame and their log-probabilities (``GPT.generate_continuous(top_logprobs=N)``).  Independent of
+        ``logprobs``; the waveforms are the same as without it.  None on an engine opened without it."""
+        from .engine import check_top_logprobs
+
+        check_top_logprobs(top_logprobs)
         flags = _lib.engine_flags(dtype)
         check_prefill_budget(prefill_budget)
         assert self.has_loaded(use_decoder=use_decoder)
         return self.gpt._open_slot_engine(ChatEngine, self.gpt.max_batch if slots is None else slots, max_new_cap,
                                           use_decoder, None, self, use_decoder, flags=flags,
                                           prefill_budget=prefill_budget, kv_pool_bytes=kv_pool_bytes,
-                                          logprobs=logprobs)
+                                          logprobs=logprobs, top_logprobs=top_logprobs)
 
     def interrupt(self):
         self.context.set(True)
@@ -700,6 +715,7 @@ class _Paragraph:
     def __init__(self, n: int, stream_params, sink=None, takes: bool = False, split: bool = False):
         self.n, self.sink, self.takes, self.split = n, sink, takes, split
         self.logprobs: Optional[list] = None  # an engine with logprobs: each sentence's, once its code request ends
+        self.top_logprobs: Optional[list] = None  # an engine with top_logprobs: each sentence's (ids, lp), likewise
         self.windows = ([StreamWindows(stream_params.stream_speed, stream_params.pass_first_n_batches)
                          for _ in range(n)] if stream_params is not None else None)
         self.ref = None
@@ -726,6 +742,8 @@ class _Paragraph:
         job = self.job
         if done and self.logprobs is not None:
             job.logprobs = self.logprobs if self.takes or self.split else self.logprobs[0]
+        if done and self.top_logprobs is not None:
+            job.top_logprobs = self.top_logprobs if self.takes or self.split else self.top_logprobs[0]
         if self.windows is not None:
             for j, c in enumerate(out):
                 item = (c, done and j == len(out) - 1)
@@ -1007,11 +1025,18 @@ class ChatEngine(OpenEngine):
                 continue  # a refinement, or the reference stage, whose audio only becomes the speaker sample
             else:
                 k = para.order[requests[i]]
-                if last and getattr(dev, "lp_out", None) is not None:  # an engine opened with logprobs
-                    if para.logprobs is None:
-                        para.logprobs = [None] * para.n
+                lp_on = getattr(dev, "lp_out", None) is not None  # an engine opened with logprobs
+                top_on = getattr(dev, "top_ids_out", None) is not None  # with top_logprobs
+                if last and (lp_on or top_on):
                     out = dev.empty(i) if s is None else dev.harvest(s, n, copy=False)
-                    para.logprobs[k] = out.logprobs[0].cpu()
+                    if lp_on:
+                        if para.logprobs is None:
+                            para.logprobs = [None] * para.n
+                        para.logprobs[k] = out.logprobs[0].cpu()
+                    if top_on:
+                        if para.top_logprobs is None:
+                            para.top_logprobs = [None] * para.n
+                        para.top_logprobs[k] = tuple(t.cpu() for t in out.top_logprobs[0])
                 if para.windows is not None:
                     ws = para.windows[k].windows(n, last)
                     wjobs += [((para, k), s, n, a, b, flush, last and j == len(ws) - 1) for j, (a, b, flush) in

@@ -122,6 +122,9 @@ struct ctb_gpt {
   uint64_t graph_kernels_text;
   float* eng_logprobs;        // [S, max_new, num_vq] token log-probabilities (ctb_gpt_engine_logprobs), or nullptr
   int eng_served;             // 1 once the engine has admitted, chunked or resumed a request
+  int eng_top_n;              // N of the top log-probability buffers (ctb_gpt_engine_top_logprobs), 0 without them
+  int32_t* eng_top_ids;       // [S, max_new, num_vq, N] the N most likely ids of every sampled row
+  float* eng_top_lp;          // [S, max_new, num_vq, N] their log-probabilities
   std::vector<SlotRecord> slot;  // [S] host-side record of each slot
   // ---- half-precision slot engine (ctb_gpt_engine_begin_ex)
   int prec;                   // CTB_ENGINE_FP16_* bits of the current engine (0 for fp32 engines and generate())
@@ -792,6 +795,24 @@ static int launch_logprob(ctb_gpt* h, const SampleP& sp, cudaStream_t s) {
   return CTB_OK;
 }
 
+static int launch_top_logprobs(const TopLogprobP& tp, int rows, cudaStream_t s) {
+  const int smem = tp.V * (int)sizeof(float);
+  { int rc = ensure_smem_attr((const void*)k_token_top_logprobs, smem); if (rc) return rc; }
+  CTB_CUDA(launch_pdl(k_token_top_logprobs, dim3(rows), dim3(LOGPROB_THREADS), (size_t)smem, s, tp));
+  CTB_LAUNCH_CHECK();
+  return CTB_OK;
+}
+
+// the N most likely ids and their log-probabilities for the rows the k_sample<true> launch `sp` just served, at the
+// index k_finalize_rows writes the sampled id
+static int launch_top_logprobs(ctb_gpt* h, const SampleP& sp, cudaStream_t s) {
+  TopLogprobP tp{};
+  tp.st = sp.st; tp.check_finished = sp.check_finished; tp.logits = sp.logits; tp.V = sp.V;
+  tp.rows_per_item = sp.rows_per_item; tp.rstate = sp.rstate; tp.want = sp.want; tp.n_top = h->eng_top_n;
+  tp.ids = h->eng_top_ids; tp.lp = h->eng_top_lp; tp.max_new = h->max_new; tp.num_vq = h->cfg.num_vq;
+  return launch_top_logprobs(tp, sp.rows, s);
+}
+
 static int launch_sampler(ctb_gpt* h, const StepCtx& x, cudaStream_t s) {
   const ctb_gpt_config& c = h->cfg;
   const int rpi = h->infer_text ? 1 : c.num_vq;
@@ -805,12 +826,13 @@ static int launch_sampler(ctb_gpt* h, const StepCtx& x, cudaStream_t s) {
   sp.noise_stride = (int)noise_stride(h);
   int rc = launch_sample(sp, s);
   if (!rc && h->eng_logprobs) rc = launch_logprob(h, sp, s);
+  if (!rc && h->eng_top_n) rc = launch_top_logprobs(h, sp, s);
   if (rc || !h->eng_text) return rc;
   // text rows: one row per slot over the text head's logits, as a batch of one samples them
   sp.logits = h->eng_text_logits; sp.rows = h->B; sp.V = c.num_text_tokens; sp.rows_per_item = 1;
   sp.out_idx = h->eng_text_idx; sp.want = h->phase | WANT_TEXT;
-  if ((rc = launch_sample(sp, s)) || !h->eng_logprobs) return rc;
-  return launch_logprob(h, sp, s);
+  if ((rc = launch_sample(sp, s)) || (h->eng_logprobs && (rc = launch_logprob(h, sp, s)))) return rc;
+  return h->eng_top_n ? launch_top_logprobs(h, sp, s) : CTB_OK;
 }
 
 // npad 16 for B <= 16, 32 for B <= 32, 64 for B <= 64 (a 64-row scratch only: tc_rows == 64)
@@ -1525,9 +1547,10 @@ static int score_setup(ctb_gpt* h, int text, size_t m) {
   return CTB_OK;
 }
 
-extern "C" int ctb_gpt_score(ctb_gpt* h, int32_t B, int32_t T, const float* emb_dev, const int32_t* n_prompt,
-                             const int32_t* n_given, const int32_t* targets_dev, int32_t infer_text, float* out_dev,
-                             void* stream) {
+// ctb_gpt_score (n_top == 0) and ctb_gpt_score_ex
+static int score_pass(ctb_gpt* h, int32_t B, int32_t T, const float* emb_dev, const int32_t* n_prompt, const int32_t* n_given,
+                      const int32_t* targets_dev, int32_t infer_text, float* out_dev, int32_t n_top, int32_t* top_ids_dev,
+                      float* top_lp_dev, void* stream) {
   if (!h || !emb_dev || !n_prompt || !n_given || !targets_dev || !out_dev) return set_err(CTB_ERR_ARG, "null argument");
   const ctb_gpt_config& c = h->cfg;
   if (B < 1 || B > c.max_batch) return set_err(CTB_ERR_ARG, "score: B=%d outside [1,%d]", B, c.max_batch);
@@ -1580,8 +1603,29 @@ extern "C" int ctb_gpt_score(ctb_gpt* h, int32_t B, int32_t T, const float* emb_
     lp.logits = h->sc_logits; lp.V = V; lp.rows_per_item = 1; lp.idx = targets_dev + r0 * rpi; lp.out = out_dev + r0 * rpi;
     CTB_CUDA(launch_pdl(k_token_logprob, dim3((unsigned)(mc * rpi)), dim3(LOGPROB_THREADS), 0, s, lp));
     CTB_LAUNCH_CHECK();
+    if (n_top) {
+      TopLogprobP tp{};
+      tp.logits = h->sc_logits; tp.V = V; tp.rows_per_item = 1; tp.n_top = n_top;
+      tp.ids = top_ids_dev + r0 * rpi * n_top; tp.lp = top_lp_dev + r0 * rpi * n_top;
+      if ((rc = launch_top_logprobs(tp, mc * rpi, s))) return rc;
+    }
   }
   return CTB_OK;
+}
+
+extern "C" int ctb_gpt_score(ctb_gpt* h, int32_t B, int32_t T, const float* emb_dev, const int32_t* n_prompt,
+                             const int32_t* n_given, const int32_t* targets_dev, int32_t infer_text, float* out_dev,
+                             void* stream) {
+  return score_pass(h, B, T, emb_dev, n_prompt, n_given, targets_dev, infer_text, out_dev, 0, nullptr, nullptr, stream);
+}
+
+extern "C" int ctb_gpt_score_ex(ctb_gpt* h, int32_t B, int32_t T, const float* emb_dev, const int32_t* n_prompt,
+                                const int32_t* n_given, const int32_t* targets_dev, int32_t infer_text, float* out_dev,
+                                int32_t n_top, int32_t* top_ids_dev, float* top_lp_dev, void* stream) {
+  if (!top_ids_dev || !top_lp_dev) return set_err(CTB_ERR_ARG, "null argument");
+  if (n_top < 1 || n_top > TOP_LOGPROBS_MAX) return set_err(CTB_ERR_ARG, "N=%d outside [1,%d]", n_top, TOP_LOGPROBS_MAX);
+  return score_pass(h, B, T, emb_dev, n_prompt, n_given, targets_dev, infer_text, out_dev, n_top, top_ids_dev,
+                    top_lp_dev, stream);
 }
 
 // ------------------------------------------------------------------ slot engine (continuous batching)
@@ -1635,6 +1679,7 @@ static int engine_begin(ctb_gpt* h, int32_t S, int32_t max_new_cap, int32_t flag
   h->q_noise = h->eng_noise; h->emb = nullptr; h->mask = nullptr;
   h->ids_out = ids_out_dev; h->hiddens_out = hiddens_out_dev; h->eng_text = 0; h->pg_pages = 0;
   h->eng_logprobs = nullptr; h->eng_served = 0;
+  h->eng_top_n = 0; h->eng_top_ids = nullptr; h->eng_top_lp = nullptr;
   if ((rc = restart_decode(h, s)) ||
       (rc = pool_pages ? kv_pool_paged(h, S, pool_pages, s) : kv_reserve(h, S, c.max_context, s)))
     return rc;
@@ -1791,6 +1836,24 @@ extern "C" int ctb_gpt_engine_logprobs(ctb_gpt* h, float* logprobs_out_dev, void
                            (cudaStream_t)stream));
   h->eng_logprobs = logprobs_out_dev;
   // decode graphs captured so far (steps of the idle engine) lack the k_token_logprob nodes
+  if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
+  if (h->graph_exec_text) { cudaGraphExecDestroy(h->graph_exec_text); h->graph_exec_text = nullptr; }
+  return CTB_OK;
+}
+
+extern "C" int ctb_gpt_engine_top_logprobs(ctb_gpt* h, int32_t n_top, int32_t* ids_out_dev, float* lp_out_dev,
+                                           void* stream) {
+  if (!h || !ids_out_dev || !lp_out_dev) return set_err(CTB_ERR_ARG, "null argument");
+  if (n_top < 1 || n_top > TOP_LOGPROBS_MAX) return set_err(CTB_ERR_ARG, "N=%d outside [1,%d]", n_top, TOP_LOGPROBS_MAX);
+  if (int rc = check_engine(h)) return rc;
+  if (h->eng_served)
+    return set_err(CTB_ERR_STATE, "the engine has served a request: attach the top log-probability buffers right after begin");
+  const size_t n = (size_t)h->B * h->max_new * h->cfg.num_vq * n_top;
+  cudaStream_t s = (cudaStream_t)stream;
+  CTB_CUDA(cudaMemsetAsync(ids_out_dev, 0, n * sizeof(int32_t), s));
+  CTB_CUDA(cudaMemsetAsync(lp_out_dev, 0, n * sizeof(float), s));
+  h->eng_top_n = n_top; h->eng_top_ids = ids_out_dev; h->eng_top_lp = lp_out_dev;
+  // decode graphs captured so far (steps of the idle engine) lack the k_token_top_logprobs nodes
   if (h->graph_exec) { cudaGraphExecDestroy(h->graph_exec); h->graph_exec = nullptr; }
   if (h->graph_exec_text) { cudaGraphExecDestroy(h->graph_exec_text); h->graph_exec_text = nullptr; }
   return CTB_OK;
@@ -2290,4 +2353,15 @@ extern "C" int ctb_token_logprobs(const float* logits_dev, int32_t rows, int32_t
   CTB_CUDA(launch_pdl(k_token_logprob, dim3(rows), dim3(LOGPROB_THREADS), 0, (cudaStream_t)stream, lp));
   CTB_LAUNCH_CHECK();
   return CTB_OK;
+}
+
+extern "C" int ctb_token_top_logprobs(const float* logits_dev, int32_t rows, int32_t V, int32_t n_top, int32_t* ids_out_dev,
+                                      float* lp_out_dev, void* stream) {
+  if (!logits_dev || !ids_out_dev || !lp_out_dev) return set_err(CTB_ERR_ARG, "null argument");
+  if (n_top < 1 || n_top > TOP_LOGPROBS_MAX) return set_err(CTB_ERR_ARG, "N=%d outside [1,%d]", n_top, TOP_LOGPROBS_MAX);
+  if (rows < 1 || V < n_top) return set_err(CTB_ERR_ARG, "bad shape: rows=%d, V=%d, N=%d", rows, V, n_top);
+  if ((size_t)V * 4 > 200 * 1024) return set_err(CTB_ERR_ARG, "V=%d: a row does not fit in shared memory", V);
+  TopLogprobP tp{};
+  tp.logits = logits_dev; tp.V = V; tp.rows_per_item = 1; tp.n_top = n_top; tp.ids = ids_out_dev; tp.lp = lp_out_dev;
+  return launch_top_logprobs(tp, rows, (cudaStream_t)stream);
 }

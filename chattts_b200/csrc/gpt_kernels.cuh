@@ -761,6 +761,25 @@ struct LogprobP {
 constexpr int LOGPROB_THREADS = 256;
 __global__ void k_token_logprob(const LogprobP p);
 
+// k_token_top_logprobs: the n_top ids of a logits row with the largest z (z descending, the smaller id first among equal
+// z) and their log softmax(z), with k_token_logprob's row max and denominator.  Launched beside k_token_logprob with the
+// same rows, rows_per_item, want and st; each served row writes its n_top entries at
+// [((b * max_new + n_gen(b)) * num_vq + q) * n_top + k].  rstate == nullptr (ctb_token_top_logprobs, scoring): every
+// row, at [r * n_top + k].  Dynamic shared memory: V floats (the row).
+struct TopLogprobP {
+  const LoopState* st; int check_finished;
+  const float* logits;   // [rows, V]
+  int V, rows_per_item;
+  const RowState* rstate;
+  int want;
+  int n_top;             // 1..TOP_LOGPROBS_MAX
+  int32_t* ids;          // slot engine: [B, max_new, num_vq, n_top]; stand-alone: [rows, n_top]
+  float* lp;             // same shape as ids
+  int max_new, num_vq;
+};
+constexpr int TOP_LOGPROBS_MAX = 20;
+__global__ void k_token_top_logprobs(const TopLogprobP p);
+
 struct FinalP {
   LoopState* st;
   int B, rows_per_item, num_vq, max_new, eos;

@@ -402,6 +402,82 @@ __global__ void __launch_bounds__(LOGPROB_THREADS) k_token_logprob(const Logprob
   }
 }
 
+namespace {
+
+// One 64-bit key per column, larger = earlier in the top order: float_key(z) (one key for -0.0 and +0.0, which compare
+// equal) above 0x7fffffff - v (the smaller id first among equal z).  Every key is > 0 and < ~0ull.
+__device__ __forceinline__ unsigned long long top_key(float z, int v) {
+  return ((unsigned long long)float_key(z) << 32) | (uint32_t)(0x7fffffff - v);
+}
+
+// the largest key below `below` among this thread's columns of s_z[0, V), 0 if none
+__device__ __forceinline__ unsigned long long top_scan(const float* s_z, int V, unsigned long long below) {
+  unsigned long long best = 0ull;
+  for (int v = threadIdx.x; v < V; v += LOGPROB_THREADS) {
+    const unsigned long long k = top_key(s_z[v], v);
+    if (k < below && k > best) best = k;
+  }
+  return best;
+}
+
+}  // namespace
+
+// Top log-probabilities (ctb_gpt_engine_top_logprobs, ctb_token_top_logprobs, ctb_gpt_score_ex): one CTA per logits row.
+// The row goes to shared memory as k_token_logprob's max pass reads it; max and den are then k_token_logprob's (same
+// CTA size, helpers and summation order), so an entry equals that kernel's value for its id bit for bit.  Selection:
+// n_top rounds of a block arg-max over the column keys.  Each thread holds the best key of its columns below the last
+// chosen one; only the thread that owned the round's winner rescans its columns, so a round is one rescan of V / 256
+// columns and one CTA reduction, and the result depends on the keys alone.
+__global__ void __launch_bounds__(LOGPROB_THREADS) k_token_top_logprobs(const TopLogprobP p) {
+  pdl_trigger();
+  pdl_wait();
+  if (p.check_finished && ldg_cg(&p.st->all_finished)) return;
+  const int row = blockIdx.x, V = p.V;
+  const int item = row / p.rows_per_item, q = row % p.rows_per_item;
+  if (p.rstate != nullptr && !row_wanted(p.rstate + item, p.want)) return;  // CTA-uniform: the rows k_sample served
+  extern __shared__ float s_z[];  // [V]
+  __shared__ double s_redd[LOGPROB_THREADS / 32];
+  __shared__ float s_redf[LOGPROB_THREADS / 32];
+  __shared__ unsigned long long s_best[2][LOGPROB_THREADS / 32];
+  const float* lg = p.logits + (size_t)row * V;
+  float mx = -INFINITY;
+  for (int v = threadIdx.x; v < V; v += LOGPROB_THREADS) {
+    const float z = ldg_cg(&lg[v]);
+    s_z[v] = z;
+    mx = fmaxf(mx, z);
+  }
+  mx = block_max_f<LOGPROB_THREADS>(mx, s_redf);  // its barriers also publish s_z
+  double den = 0.0;
+  for (int v = threadIdx.x; v < V; v += LOGPROB_THREADS) den += (double)expf(s_z[v] - mx);
+  den = block_sum_d<LOGPROB_THREADS>(den, s_redd);
+  const double lden = log(den);
+  const size_t base = p.rstate == nullptr
+      ? (size_t)row * p.n_top
+      : (((size_t)item * p.max_new + ldg_cg(&p.rstate[item].n_gen)) * p.num_vq + q) * p.n_top;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned long long mine = top_scan(s_z, V, ~0ull);
+  for (int k = 0; k < p.n_top; ++k) {
+    unsigned long long w = mine;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long ow = __shfl_xor_sync(0xffffffffu, w, o);
+      w = ow > w ? ow : w;
+    }
+    // two buffers: round k + 2 writes this one only after every thread has passed round k + 1's barrier
+    if (lane == 0) s_best[k & 1][warp] = w;
+    __syncthreads();
+    w = 0ull;
+#pragma unroll
+    for (int i = 0; i < LOGPROB_THREADS / 32; ++i) w = s_best[k & 1][i] > w ? s_best[k & 1][i] : w;
+    if (threadIdx.x == 0) {
+      const int id = w ? 0x7fffffff - (int)(uint32_t)w : -1;  // w == 0: fewer than n_top columns
+      p.ids[base + k] = id;
+      p.lp[base + k] = id >= 0 ? (float)((double)(s_z[id] - mx) - lden) : __int_as_float(0x7fc00000);
+    }
+    if (mine == w && w) mine = top_scan(s_z, V, w);
+  }
+}
+
 template __global__ void k_sample<false>(const SampleP p);
 template __global__ void k_sample<true>(const SampleP p);
 

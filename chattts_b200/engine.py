@@ -88,6 +88,16 @@ def check_prefill_budget(budget: Optional[int]) -> Optional[int]:
     return int(budget)
 
 
+TOP_LOGPROBS_MAX = 20  # the most alternatives per token ctb_gpt_engine_top_logprobs and ctb_gpt_score_ex return
+
+
+def check_top_logprobs(n) -> int:
+    """``top_logprobs`` as an int in [0, 20] (0: off); ValueError otherwise."""
+    if isinstance(n, bool) or not isinstance(n, int) or not 0 <= n <= TOP_LOGPROBS_MAX:
+        raise ValueError(f"top_logprobs={n!r}: an int in [0, {TOP_LOGPROBS_MAX}] (0: off)")
+    return n
+
+
 def kv_pool_pages(gpt_config, kv_pool_bytes: Optional[int], flags: int) -> Optional[int]:
     """The pages (16 tokens of K and V of every layer; page 0 is the zero page) a pool of ``kv_pool_bytes`` holds on an
     engine of precision ``flags``, or None for None.  ValueError when it holds fewer than two."""
@@ -821,12 +831,15 @@ class SlotImage:
     ``EngineDevice.resume`` restores it into a slot.  ``row(hidden)`` and ``outputs(n)`` read its first tokens' ids and
     hidden states, as the slot held them, once the copies that filled it are complete (``ready``).  ``logprobs``: the
     slot's log-probabilities [n_gen, num_vq] in pinned host memory (an engine with logprobs; they are not part of the
-    device image), else None."""
+    device image), else None.  ``top``: likewise its top log-probabilities, (ids, lp) [n_gen, num_vq, N] (an engine
+    with top_logprobs), else None."""
+
+    top: Optional[Tuple[torch.Tensor, torch.Tensor]] = None
 
     def __init__(self, buf: torch.Tensor, text: bool, device, num_vq: int, hidden_size: int, stream,
-                 logprobs: Optional[torch.Tensor] = None):
+                 logprobs: Optional[torch.Tensor] = None, top: Optional[Tuple[torch.Tensor, torch.Tensor]] = None):
         self.buf, self.text, self.device, self.num_vq, self.hidden_size = buf, text, device, num_vq, hidden_size
-        self.logprobs = logprobs
+        self.logprobs, self.top = logprobs, top
         self.ready = torch.cuda.Event()
         self.ready.record(stream)  # after the copies that fill the image
         self.header = _lib.SlotImage.from_address(buf.data_ptr())
@@ -852,10 +865,15 @@ class SlotImage:
         ids = self.row(False)[:n].to(torch.int64)
         lp = [] if self.logprobs is None else [self.logprobs[:n, 0] if self.text else self.logprobs[:n]]
         lp = [t.to(self.device) for t in lp]
+        top = []
+        if self.top is not None:
+            i, v = (t[:n, 0] if self.text else t[:n] for t in self.top)
+            top = [(i.to(self.device, torch.int64), v.to(self.device))]
         if self.text:
-            return GPT.GenerationOutputs(ids=[ids[:, 0].contiguous()], attentions=[], hiddens=[], logprobs=lp)
+            return GPT.GenerationOutputs(ids=[ids[:, 0].contiguous()], attentions=[], hiddens=[], logprobs=lp,
+                                         top_logprobs=top)
         hid = [self.row(True)[:n]] if return_hidden else []
-        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid, logprobs=lp)
+        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid, logprobs=lp, top_logprobs=top)
 
 
 class EngineDevice:
@@ -863,10 +881,15 @@ class EngineDevice:
     ``kv_pool_pages`` (``kv_pool_pages()``) makes a paged engine (ctb_gpt_engine_begin_paged) with the pool interface
     ``_poll_cycles`` describes; None keeps every slot's fixed pages.  ``logprobs`` attaches a buffer of token
     log-probabilities (ctb_gpt_engine_logprobs) beside ``ids_out``: outputs then carry them (``GenerationOutputs
-    .logprobs``), and suspended requests take theirs along in their ``SlotImage``."""
+    .logprobs``), and suspended requests take theirs along in their ``SlotImage``.  ``top_logprobs`` (N > 0) attaches
+    the two buffers of ctb_gpt_engine_top_logprobs, the N most likely ids of every sampled row and their
+    log-probabilities, which outputs (``GenerationOutputs.top_logprobs``) and suspended requests carry in the same way."""
+
+    top_ids_out: Optional[torch.Tensor] = None  # [S, max_new_cap, num_vq, N] int32 with top_logprobs
+    top_lp_out: Optional[torch.Tensor] = None   # [S, max_new_cap, num_vq, N] fp32
 
     def __init__(self, gpt, requests: Sequence[Request], slots: int, max_new_cap: int, return_hidden: bool = True,
-                 flags: int = 0, kv_pool_pages: Optional[int] = None, logprobs: bool = False):
+                 flags: int = 0, kv_pool_pages: Optional[int] = None, logprobs: bool = False, top_logprobs: int = 0):
         self.gpt, self.requests, self.slots = gpt, requests, slots
         self.max_context = gpt.max_context
         self.lib = _lib.load()
@@ -879,6 +902,10 @@ class EngineDevice:
                         if return_hidden else None)
         self.lp_out = (torch.zeros(slots, max_new_cap, gpt.num_vq, dtype=torch.float32, device=dev) if logprobs
                        else None)
+        top_n = check_top_logprobs(top_logprobs)
+        shape = (slots, max_new_cap, gpt.num_vq, top_n)
+        self.top_ids_out = torch.zeros(shape, dtype=torch.int32, device=dev) if top_n else None
+        self.top_lp_out = torch.zeros(shape, dtype=torch.float32, device=dev) if top_n else None
         hid = C.c_void_p(self.hid_out.data_ptr()) if self.hid_out is not None else None
         self.pool_pages = kv_pool_pages
         if kv_pool_pages is None:
@@ -890,6 +917,9 @@ class EngineDevice:
                 self.stream))
         if self.lp_out is not None:
             _lib.check(self.lib.ctb_gpt_engine_logprobs(gpt._handle, C.c_void_p(self.lp_out.data_ptr()), self.stream))
+        if top_n:
+            _lib.check(self.lib.ctb_gpt_engine_top_logprobs(gpt._handle, top_n, C.c_void_p(self.top_ids_out.data_ptr()),
+                                                            C.c_void_p(self.top_lp_out.data_ptr()), self.stream))
         # the images of suspended requests, by id, while anything holds them (a cancelled one's ends with its outputs)
         self._images: "weakref.WeakValueDictionary[int, SlotImage]" = weakref.WeakValueDictionary()
         self._resumed: List[SlotImage] = []  # read by the device until the next status read
@@ -1006,14 +1036,20 @@ class EngineDevice:
         buf = torch.empty(nbytes.value, dtype=torch.uint8, pin_memory=True)
         _lib.check(self.lib.ctb_gpt_engine_suspend(self.gpt._handle, slot, C.c_void_p(buf.data_ptr()), nbytes.value,
                                                    self.stream))
-        lp = None
-        if self.lp_out is not None:  # the header is written: n_gen is known on the host
-            n = _lib.SlotImage.from_address(buf.data_ptr()).n_gen
+        lp = top = None
+        n = _lib.SlotImage.from_address(buf.data_ptr()).n_gen  # the header is written: n_gen is known on the host
+        if self.lp_out is not None:
             lp = torch.empty(n, self.gpt.num_vq, dtype=torch.float32, pin_memory=True)
             with torch.cuda.stream(self._torch_stream):
                 lp.copy_(self.lp_out[slot, :n], non_blocking=True)
+        if self.top_ids_out is not None:
+            top = tuple(torch.empty(t[slot, :n].shape, dtype=t.dtype, pin_memory=True)
+                        for t in (self.top_ids_out, self.top_lp_out))
+            with torch.cuda.stream(self._torch_stream):
+                for h, t in zip(top, (self.top_ids_out, self.top_lp_out)):
+                    h.copy_(t[slot, :n], non_blocking=True)
         image = SlotImage(buf, self._text[slot], self.dev, self.gpt.num_vq, self.gpt.config.hidden_size,
-                          self._torch_stream, lp)
+                          self._torch_stream, lp, top)
         self._images[id(image)] = image
         return image
 
@@ -1024,6 +1060,10 @@ class EngineDevice:
         if self.lp_out is not None:
             with torch.cuda.stream(self._torch_stream):
                 self.lp_out[slot, :image.logprobs.shape[0]].copy_(image.logprobs, non_blocking=True)
+        if self.top_ids_out is not None:
+            with torch.cuda.stream(self._torch_stream):
+                for t, h in zip((self.top_ids_out, self.top_lp_out), image.top):
+                    t[slot, :h.shape[0]].copy_(h, non_blocking=True)
         self._text[slot] = image.text
         self._images.pop(id(image), None)
         self._resumed.append(image)  # the copies read it until the stream passes them
@@ -1064,13 +1104,17 @@ class EngineDevice:
             return slot.outputs(n, self.hid_out is not None)
         text = self._text[slot]
         lp = [] if self.lp_out is None else [(self.lp_out[slot, :n, 0] if text else self.lp_out[slot, :n]).clone()]
+        top = []
+        if self.top_ids_out is not None:
+            i, v = (t[slot, :n, 0] if text else t[slot, :n] for t in (self.top_ids_out, self.top_lp_out))
+            top = [(i.to(torch.int64), v.clone())]
         if text:
             return GPT.GenerationOutputs(ids=[self.ids_out[slot, :n, 0].to(torch.int64)], attentions=[], hiddens=[],
-                                         logprobs=lp)
+                                         logprobs=lp, top_logprobs=top)
         ids = self.ids_out[slot, :n].to(torch.int64)
         hid = ([self.hid_out[slot, :n].clone() if copy else self.hid_out[slot, :n]] if self.hid_out is not None
                else [])
-        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid, logprobs=lp)
+        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid, logprobs=lp, top_logprobs=top)
 
     def empty(self, index: Optional[int] = None):
         """The outputs of request ``index`` (default: a code request) when it ended empty (a seeded request whose
@@ -1080,13 +1124,18 @@ class EngineDevice:
         text = index is not None and self.requests[index].infer_text
         lp = ([] if self.lp_out is None else
               [torch.zeros((0,) if text else (0, self.gpt.num_vq), dtype=torch.float32, device=self.dev)])
+        top = []
+        if self.top_ids_out is not None:
+            shape = (0, self.top_ids_out.shape[3]) if text else (0, self.gpt.num_vq, self.top_ids_out.shape[3])
+            top = [(torch.zeros(shape, dtype=torch.int64, device=self.dev),
+                    torch.zeros(shape, dtype=torch.float32, device=self.dev))]
         if text:
             return GPT.GenerationOutputs(ids=[torch.zeros(0, dtype=torch.int64, device=self.dev)], attentions=[],
-                                         hiddens=[], logprobs=lp)
+                                         hiddens=[], logprobs=lp, top_logprobs=top)
         ids = torch.zeros(0, self.gpt.num_vq, dtype=torch.int64, device=self.dev)
         hid = ([torch.zeros(0, self.gpt.config.hidden_size, dtype=torch.float32, device=self.dev)]
                if self.hid_out is not None else [])
-        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid, logprobs=lp)
+        return GPT.GenerationOutputs(ids=[ids], attentions=[], hiddens=hid, logprobs=lp, top_logprobs=top)
 
 
 _END = object()  # closes a streaming job's iterator
@@ -1135,6 +1184,7 @@ class Job:
         self.spk_smp: Optional[str] = None  # Chat.open_engine paragraphs: the speaker sampled from sentence 0
         self.refined: Optional[List[Optional[str]]] = None  # refined paragraphs: each sentence's text once refined
         self.logprobs = None  # Chat.open_engine(logprobs=True): the speech tokens' log-probabilities once it has ended
+        self.top_logprobs = None  # Chat.open_engine(top_logprobs=N): their N most likely ids and log p, likewise
 
     def cancel(self) -> None:
         self._engine._source.cancel(self)
@@ -1349,7 +1399,7 @@ class GptEngine(OpenEngine):
             out = value[0] if isinstance(value, tuple) else value
             cur = torch.cuda.current_stream(self.device)
             cur.wait_event(event)
-            for t in [*out.ids, *out.hiddens, *out.logprobs]:
+            for t in [*out.ids, *out.hiddens, *out.logprobs, *(t for pair in out.top_logprobs for t in pair)]:
                 t.record_stream(cur)
         return value
 

@@ -96,12 +96,17 @@ class GPT:
         # a slot engine opened with logprobs=True: per item, log p of each returned id under the model's logits at
         # temperature 1 ([n, num_vq] fp32 for codes, [n] for text), aligned with ``ids``; otherwise empty
         logprobs: List[torch.Tensor] = field(default_factory=list)
+        # a slot engine opened with top_logprobs=N: per item, (ids, lp) of the N most likely ids at each returned token
+        # under the same logits, z descending (int64 and fp32, [n, num_vq, N] for codes, [n, N] for text), aligned
+        # with ``ids``; otherwise empty
+        top_logprobs: List[Tuple[torch.Tensor, torch.Tensor]] = field(default_factory=list)
 
         def destroy(self):
             _del_all(self.ids)
             _del_all(self.attentions)
             _del_all(self.hiddens)
             _del_all(self.logprobs)
+            _del_all(self.top_logprobs)
 
     def __init__(self, gpt_config: Union[dict, GPTConfig], embed: Embed, use_flash_attn=False, use_vllm=False,
                  device=torch.device("cuda"), device_gpt=torch.device("cuda"),
@@ -290,7 +295,7 @@ class GPT:
 
     # ------------------------------------------------------------------ teacher-forced scoring
     @torch.no_grad()
-    def score(self, prompts, targets, infer_text: bool = False) -> List[torch.Tensor]:
+    def score(self, prompts, targets, infer_text: bool = False, top_logprobs: int = 0) -> list:
         """The model's log-probability of given tokens: for each row, ``log softmax(z)[token]`` of every token of
         ``targets[i]`` after ``prompts[i]`` and the tokens before it (teacher forcing), at temperature 1 on the raw
         head logits ``z``, the quantity ``GenerationOutputs.logprobs`` holds for sampled ids.
@@ -302,7 +307,15 @@ class GPT:
         One causal prefill pass per call of ``ctb_gpt_score`` on the fp32 model, rows grouped as the slot engine
         admits prompts (``score_groups``).  ValueError for an id outside the vocabulary or ``P + n - 1`` over
         ``max_context``; RuntimeError while an open engine owns the handle.  A static ``generate`` stream in flight
-        ends (resuming it raises ``CtbError``)."""
+        ends (resuming it raises ``CtbError``).
+
+        ``top_logprobs=N`` (1..20; ctb_gpt_score_ex) makes each row ``(lp, top_ids, top_lp)``: besides ``lp`` as above,
+        the N ids with the largest ``z`` at every scored position (z descending, the smaller id first among equal z;
+        int64 ``[n, num_vq, N]``, ``[n, N]`` for text) and their log-probabilities (fp32, same shape), the quantity
+        ``GenerationOutputs.top_logprobs`` holds.  ``lp`` is bit-equal to that of a call without it."""
+        from .engine import check_top_logprobs
+
+        top_n = check_top_logprobs(top_logprobs)
         self._check_free("score")
         if not self._handle:
             raise _lib.CtbError("GPT weights not loaded")
@@ -327,9 +340,13 @@ class GPT:
                 raise ValueError(f"score: row {i}: prompt {P} + {n} tokens - 1 exceed max_context={self.max_context}")
             rows.append((p, t.reshape(n, rpi), P, n))
         out = [torch.empty((n, rpi) if rpi > 1 else (n,), dtype=torch.float32, device=dev) for _, _, _, n in rows]
+        top_shape = [((n, rpi, top_n) if rpi > 1 else (n, top_n)) for _, _, _, n in rows]
+        top_ids = [torch.empty(t, dtype=torch.int64, device=dev) for t in top_shape] if top_n else []
+        top_lp = [torch.empty(t, dtype=torch.float32, device=dev) for t in top_shape] if top_n else []
+        result = list(zip(out, top_ids, top_lp)) if top_n else out
         live = [i for i, r in enumerate(rows) if r[3] > 0]
         if not live:
-            return out
+            return result
         lib = _lib.load()
         with torch.cuda.device(dev):
             stream_ptr = C.c_void_p(torch.cuda.current_stream().cuda_stream)
@@ -348,12 +365,24 @@ class GPT:
                 res = torch.empty(tgt.shape, dtype=torch.float32, device=dev)
                 n_prompt = (C.c_int32 * B)(*[rows[i][2] for i in idx])
                 n_given = (C.c_int32 * B)(*[rows[i][3] for i in idx])
-                _lib.check(lib.ctb_gpt_score(self._handle, B, T, C.c_void_p(emb.data_ptr()), n_prompt, n_given,
-                                             C.c_void_p(tgt.data_ptr()), int(bool(infer_text)),
-                                             C.c_void_p(res.data_ptr()), stream_ptr))
+                if not top_n:
+                    _lib.check(lib.ctb_gpt_score(self._handle, B, T, C.c_void_p(emb.data_ptr()), n_prompt, n_given,
+                                                 C.c_void_p(tgt.data_ptr()), int(bool(infer_text)),
+                                                 C.c_void_p(res.data_ptr()), stream_ptr))
+                else:
+                    t_ids = torch.empty(*tgt.shape, top_n, dtype=torch.int32, device=dev)
+                    t_lp = torch.empty(*tgt.shape, top_n, dtype=torch.float32, device=dev)
+                    _lib.check(lib.ctb_gpt_score_ex(self._handle, B, T, C.c_void_p(emb.data_ptr()), n_prompt, n_given,
+                                                    C.c_void_p(tgt.data_ptr()), int(bool(infer_text)),
+                                                    C.c_void_p(res.data_ptr()), top_n, C.c_void_p(t_ids.data_ptr()),
+                                                    C.c_void_p(t_lp.data_ptr()), stream_ptr))
+                    sizes = [rows[i][3] for i in idx]
+                    for i, a, b in zip(idx, t_ids.split(sizes), t_lp.split(sizes)):
+                        top_ids[i].copy_(a.view(top_shape[i]))
+                        top_lp[i].copy_(b.view(top_shape[i]))
                 for i, r in zip(idx, res.split([rows[i][3] for i in idx])):
                     out[i].copy_(r.view(out[i].shape))
-        return out
+        return result
 
     # ------------------------------------------------------------------ continuous batching
     @torch.no_grad()
@@ -361,7 +390,7 @@ class GPT:
                             stream=False, return_attn=False, context=None, chunk: Optional[int] = None,
                             max_new_cap: Optional[int] = None, dtype=torch.float32,
                             prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None,
-                            logprobs: bool = False):
+                            logprobs: bool = False, top_logprobs: int = 0):
         """Generate audio codes or text for many utterances on a slot engine (chattts_b200.engine): up to ``slots``
         requests (default: ``max_batch``, at most the number of requests) decode together, and a waiting request takes
         the place of a finished one at the next poll (every ``chunk`` steps, default CTB_DECODE_CHUNK or 32).  Each
@@ -405,9 +434,16 @@ class GPT:
 
         ``logprobs=True`` fills ``GenerationOutputs.logprobs``: for each returned id, its log-probability under the
         head logits the sampler read, at temperature 1 and before the repetition penalty, top-P, top-K and the EOS ban
-        (ctb_gpt_engine_logprobs).  Ids and hidden states are the same with or without it."""
-        from .engine import ScheduleStats, check_prefill_budget, kv_pool_pages, schedule
+        (ctb_gpt_engine_logprobs).  Ids and hidden states are the same with or without it.
 
+        ``top_logprobs=N`` (1..20; 0 is off) fills ``GenerationOutputs.top_logprobs``: for each returned token, the N
+        ids with the largest head logits ``z`` (z descending, the smaller id first among equal z) and their
+        log-probabilities, of the distribution ``logprobs`` uses (ctb_gpt_engine_top_logprobs).  Where the sampled id
+        is among them its entry equals its ``logprobs`` value bit for bit.  Independent of ``logprobs``; ids, hidden
+        states and log-probabilities are the same with or without it."""
+        from .engine import ScheduleStats, check_prefill_budget, check_top_logprobs, kv_pool_pages, schedule
+
+        check_top_logprobs(top_logprobs)
         flags = _lib.engine_flags(dtype)
         prefill_budget = check_prefill_budget(prefill_budget)
         pool = kv_pool_pages(self.config, kv_pool_bytes, flags)
@@ -420,7 +456,7 @@ class GPT:
         if not requests:
             return
         with torch.cuda.device(self.device_gpt):
-            dev = self._engine_device(requests, S, cap, return_hidden, flags, pool, logprobs)
+            dev = self._engine_device(requests, S, cap, return_hidden, flags, pool, logprobs, top_logprobs)
             self.last_schedule_stats = stats = ScheduleStats()  # admissions, decode steps (tools/bench_continuous.py)
             for i, slot, n in schedule(requests, dev, chunk, context, stats, check, prefill_budget):
                 yield i, (dev.empty(i) if slot is None else dev.harvest(slot, n))
@@ -432,7 +468,7 @@ class GPT:
                                    chunk: Optional[int] = None, infer_text=False, return_attn=False,
                                    max_new_cap: Optional[int] = None, dtype=torch.float32,
                                    prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None,
-                                   logprobs: bool = False):
+                                   logprobs: bool = False, top_logprobs: int = 0):
         """Streaming form of ``generate_continuous``: generator of ``(request_index, GenerationOutputs, last)``.
 
         For each request the yields are exactly those ``generate(stream=True, stream_batch=r.stream_batch)`` makes for
@@ -446,9 +482,10 @@ class GPT:
         ``ids`` are copies.  ``hiddens`` are views into the engine's buffer, like the narrowed views ``generate``
         hands out: they stay valid until this generator is resumed (copy them to keep them).  ``dtype``,
         ``prefill_budget`` and ``kv_pool_bytes`` as in ``generate_continuous``: none changes a request's yields.
-        ``logprobs`` as there: each yield carries copies of the log-probabilities of the ids it carries."""
-        from .engine import ScheduleStats, check_prefill_budget, kv_pool_pages, stream_schedule
+        ``logprobs`` and ``top_logprobs`` as there: each yield carries copies of the rows of the ids it carries."""
+        from .engine import ScheduleStats, check_prefill_budget, check_top_logprobs, kv_pool_pages, stream_schedule
 
+        check_top_logprobs(top_logprobs)
         flags = _lib.engine_flags(dtype)
         prefill_budget = check_prefill_budget(prefill_budget)
         pool = kv_pool_pages(self.config, kv_pool_bytes, flags)
@@ -458,7 +495,7 @@ class GPT:
         if not requests:
             return
         with torch.cuda.device(self.device_gpt):
-            dev = self._engine_device(requests, S, cap, return_hidden, flags, pool, logprobs)
+            dev = self._engine_device(requests, S, cap, return_hidden, flags, pool, logprobs, top_logprobs)
             self.last_schedule_stats = stats = ScheduleStats()
             for batch in stream_schedule(requests, dev, chunk, context, stats, check, prefill_budget=prefill_budget):
                 for i, slot, n, last in batch:
@@ -468,7 +505,7 @@ class GPT:
 
     def open_engine(self, slots: int, max_new_cap: int, return_hidden=True, chunk: Optional[int] = None,
                     dtype=torch.float32, prefill_budget: Optional[int] = None, kv_pool_bytes: Optional[int] = None,
-                    logprobs: bool = False):
+                    logprobs: bool = False, top_logprobs: int = 0):
         """A slot engine that takes requests while it decodes: ``submit(request, stream=False) -> engine.Job`` from
         any thread, ``Job.cancel()`` for one request, ``close(cancel=False)`` (or a ``with`` block) to drain it.
 
@@ -484,36 +521,42 @@ class GPT:
         ``chunk`` steps (default CTB_DECODE_CHUNK, else 24).  ``slots`` and ``dtype`` as in ``generate_continuous``
         (up to ``max_batch`` slots; a half-precision engine up to 64).  ``kv_pool_bytes`` as in
         ``generate_continuous``: ``submit`` refuses a request that does not fit in the pool alone, and a job cancelled
-        while suspended ends with the tokens it had.  ``logprobs`` as in ``generate_continuous``."""
+        while suspended ends with the tokens it had.  ``logprobs`` and ``top_logprobs`` as in
+        ``generate_continuous``."""
         from .engine import GptEngine
 
         return self._open_slot_engine(GptEngine, slots, max_new_cap, return_hidden, chunk,
                                       flags=_lib.engine_flags(dtype), prefill_budget=prefill_budget,
-                                      kv_pool_bytes=kv_pool_bytes, logprobs=logprobs)
+                                      kv_pool_bytes=kv_pool_bytes, logprobs=logprobs, top_logprobs=top_logprobs)
 
     def _open_slot_engine(self, cls, slots, max_new_cap, return_hidden, chunk, *args, flags=0, prefill_budget=None,
-                          kv_pool_bytes=None, logprobs=False):
+                          kv_pool_bytes=None, logprobs=False, top_logprobs=0):
         """An ``engine.OpenEngine`` subclass ``cls`` that owns this handle until it is closed (``flags``: the
         ctb_gpt_engine_begin_ex precision flags; ``prefill_budget``: the engine's bound on each poll's prefill;
-        ``kv_pool_bytes``: its KV pool, None for fixed pages; ``logprobs``: outputs carry token log-probabilities)."""
-        from .engine import check_prefill_budget, kv_pool_pages
+        ``kv_pool_bytes``: its KV pool, None for fixed pages; ``logprobs``: outputs carry token log-probabilities;
+        ``top_logprobs``: and the N most likely ids at each token)."""
+        from .engine import check_prefill_budget, check_top_logprobs, kv_pool_pages
 
+        check_top_logprobs(top_logprobs)
         prefill_budget = check_prefill_budget(prefill_budget)
         pool = kv_pool_pages(self.config, kv_pool_bytes, flags)
         _, S, chunk, _, cap, check = self._engine_args("open_engine", [], slots, False, False, None, chunk, None,
                                                        max_new_cap, pool)
         kw = {"slots": S} if prefill_budget is None else {"prefill_budget": prefill_budget, "slots": S}
-        engine = cls(lambda requests: self._engine_device(requests, S, cap, return_hidden, flags, pool, logprobs), chunk,
-                     check,
+        engine = cls(lambda requests: self._engine_device(requests, S, cap, return_hidden, flags, pool, logprobs,
+                                                          top_logprobs), chunk, check,
                      self.device_gpt, self._close_engine, *args, max_new_cap=cap, **kw)
         self._open = engine
         return engine
 
-    def _engine_device(self, requests, S, cap, return_hidden, flags, pool_pages=None, logprobs=False):
+    def _engine_device(self, requests, S, cap, return_hidden, flags, pool_pages=None, logprobs=False, top_logprobs=0):
         """The ``engine.EngineDevice`` of one slot engine; an fp32 engine with fixed pages gets the five-argument form
         that stand-in devices implement."""
         from . import engine
 
+        if top_logprobs:
+            return engine.EngineDevice(self, requests, S, cap, return_hidden, flags=flags, kv_pool_pages=pool_pages,
+                                       logprobs=logprobs, top_logprobs=top_logprobs)
         if logprobs:
             return engine.EngineDevice(self, requests, S, cap, return_hidden, flags=flags, kv_pool_pages=pool_pages,
                                        logprobs=True)

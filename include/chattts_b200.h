@@ -198,6 +198,15 @@ int ctb_gpt_score(ctb_gpt* h, int32_t B, int32_t T, const float* emb_dev, const 
                   const int32_t* n_given, const int32_t* targets_dev, int32_t infer_text, float* out_dev,
                   void* stream);
 
+/* ctb_gpt_score, and for every scored position the n_top ids with the largest z and their log softmax(z), as
+ * ctb_gpt_engine_top_logprobs describes (same kernel, k_token_top_logprobs, over the same logits rows):
+ *   top_ids_dev [m, rpi, n_top] int32, top_lp_dev [m, rpi, n_top] fp32.
+ * out_dev is bit-equal to ctb_gpt_score's.  Errors: those of ctb_gpt_score; CTB_ERR_ARG for a null top buffer or n_top
+ * outside [1, 20]. */
+int ctb_gpt_score_ex(ctb_gpt* h, int32_t B, int32_t T, const float* emb_dev, const int32_t* n_prompt,
+                     const int32_t* n_given, const int32_t* targets_dev, int32_t infer_text, float* out_dev,
+                     int32_t n_top, int32_t* top_ids_dev, float* top_lp_dev, void* stream);
+
 /* ---- slot engine: continuous batching of audio-code generation (no reference counterpart; the reference serves
  * this with the vLLM fork behind Chat.load(use_vllm=True)).  The handle's rows become S independent slots; each holds
  * one request (one utterance) at its own point of generation, with its own sampling parameters, noise and max_new,
@@ -432,6 +441,20 @@ int ctb_gpt_engine_share_prompt(ctb_gpt* h, int32_t src, int32_t dst, int32_t T0
  * engine has admitted, prefilled a chunk for or resumed a request. */
 int ctb_gpt_engine_logprobs(ctb_gpt* h, float* logprobs_out_dev, void* stream);
 
+/* ---- Top log-probabilities: attach ids_out_dev [S, max_new_cap, num_vq, n_top] int32 and lp_out_dev (same shape,
+ * fp32), both device, to the slot engine just begun.  From then on every sampler launch of the engine (where
+ * ctb_gpt_engine_logprobs' kernel runs, after it when both are attached) is followed by k_token_top_logprobs, which
+ * writes, for every row it sampled, at [slot][n][q][k] for k < n_top:
+ *   ids_out_dev = the k-th id of z's order (z descending, the smaller id first among equal z)
+ *   lp_out_dev  = (float)((double)(z[id] - max) - log(den))
+ * with z, n and q as in ctb_gpt_engine_logprobs, and max and den computed as k_token_logprob computes them: an entry
+ * whose id is the sampled one equals that call's value bit for bit.  Ids, hidden states and log-probabilities are those
+ * of the engine without the buffers; no kernel reads them, and a suspended request's entries are not in its
+ * ctb_slot_image.  The call zeroes both buffers on `stream`.  Every ctb_gpt_engine_begin* starts without them.
+ * Errors (the handle as it was): CTB_ERR_ARG for a null argument or n_top outside [1, 20]; CTB_ERR_STATE outside a
+ * slot engine, or once the engine has admitted, prefilled a chunk for or resumed a request. */
+int ctb_gpt_engine_top_logprobs(ctb_gpt* h, int32_t n_top, int32_t* ids_out_dev, float* lp_out_dev, void* stream);
+
 /* Measurement hook for bench.py's roofline: launches ONE kernel kind once per layer on the
  * state left by the last generate call (kind 0 qkv, 1 attention, 2 o-proj, 3 gate/up, 4 down;
  * 5 = heads, 6 = sampler, 7 = one decode step as ONE kernel launch (k_flow / k_step), 8 = 16 decode steps in one
@@ -465,6 +488,13 @@ int ctb_sample(const float* logits_dev, int32_t rows, int32_t V, int32_t rows_pe
  * V < 1. */
 int ctb_token_logprobs(const float* logits_dev, int32_t rows, int32_t V, const int32_t* ids_dev, float* out_dev,
                        void* stream);
+
+/* Stand-alone top log-probabilities (the kernel ctb_gpt_engine_top_logprobs launches): for each of `rows` rows of
+ * logits_dev [rows, V] fp32, ids_out_dev [rows, n_top] int32 and lp_out_dev [rows, n_top] fp32 as described there.
+ * Enqueued on `stream`.  Errors: CTB_ERR_ARG for a null argument, n_top outside [1, 20], rows < 1, V < n_top or a row
+ * over 200 KiB (V > 51,200). */
+int ctb_token_top_logprobs(const float* logits_dev, int32_t rows, int32_t V, int32_t n_top, int32_t* ids_out_dev,
+                           float* lp_out_dev, void* stream);
 
 /* ---- token -> waveform: replaces ChatTTS/core.py:512-539 (_decode_to_wavs) ------ */
 
